@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Benchmark of the sam_road tiled-inference hot path on B200 (contract: see the task brief / DESIGN.md).
+"""Benchmark of the sam_road tiled-inference hot path on one or more H100s (see DESIGN.md).
 
-    python bench.py --gpus 1 --steps 20 --warmup 3                # this framework (CUDA, sm_100a)
+    python bench.py --gpus 1 --steps 20 --warmup 3                # this framework (CUDA, sm_90a)
     python bench.py --workload c4                                 # another BASELINE configuration
     python bench.py --impl reference --steps 3 --warmup 1         # reference algorithm on host CPU cores
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
+    python bench.py --dump-outputs DIR                            # also save the last timed step's outputs
 
 Default workload (BASELINE.json configs[1], `toponet_vitb_512_cityscale`): one "step" is one pass of the
 hot path over one INFER_BATCH_SIZE=64 batch of synthetic 512x512 RGB tiles per GPU: ViT-B encoder + naive
@@ -18,6 +19,7 @@ Printed JSON (one line, rank 0):
   e2e_scene  whole scenes through the drop-in `infer_one_img` (uint8 scene in host memory -> nodes, edges
              and the two uint8 masks in host memory): tiles/s = tiles of the scene / wall time
   roofline   dominant kernel class: algorithmic FLOPs / CUDA-event duration vs MEASURED_PEAKS.json
+             (when present, otherwise the H100 SXM data sheet)
   cpu_baseline  the CPU oracle (port of the reference algorithm) timed on this box's host cores
 """
 from __future__ import annotations
@@ -80,13 +82,14 @@ def load_peaks():
         p = json.load(open(path))
         return dict(tflops=float(p["bf16_tflops_sustained"]), tflops_burst=float(p["bf16_tflops"]),
                     hbm=float(p["hbm_gbs"]), source="measured (MEASURED_PEAKS.json, sustained)")
-    return dict(tflops=1400.0, tflops_burst=1590.0, hbm=6650.0,
-                source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): dense FP16 tensor 989 TFLOP/s, HBM3 3.35 TB/s -- not measured
+    return dict(tflops=989.0, tflops_burst=989.0, hbm=3350.0,
+                source="H100 SXM data sheet (dense FP16, 700 W), not measured")
 
 
 def load_ncu_metrics():
-    """Per-kernel-class ncu numbers (DRAM bytes per launch, tensor-pipe %) written by tools/ncu_extract.py
-    from the `--set full` captures of tools/gpu/profile_r02.sh, stamped with the digest of the kernel sources
+    """Per-kernel-class profiler numbers (DRAM bytes per launch, tensor-pipe %) from profiles/ncu_metrics.json when
+    such a capture is present, stamped with the digest of the kernel sources
     they were taken from.  Returned only when that digest is the one of the library being run."""
     path = os.path.join(ROOT, "profiles", "ncu_metrics.json")
     dig = os.path.join(ROOT, "sam_road_b200", "_build", "digest.txt")
@@ -330,6 +333,23 @@ def run_scenes(args, w, wl, dev, rank, world, barrier):
     return out
 
 
+def dump_outputs(out_dir, scores, feat, topo_scores):
+    """What the last timed step returned to its caller, as float32 .npy files (< 64 MB in all): mask
+    scores and image embeddings of 8 tiles drawn with a fixed seed (the whole batch is > 64 MB), and
+    every topology score."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    g = torch.Generator().manual_seed(1234)
+    sel = torch.randperm(scores.shape[0], generator=g)[:8].sort().values
+    arrays = {"mask_scores": scores[sel.to(scores.device)], "img_features": feat[sel.to(feat.device)],
+              "tile_index": sel}
+    if topo_scores is not None:
+        arrays["topo_scores"] = topo_scores
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def run_native(args, w, wl):
     import torch
     import torch.distributed as dist
@@ -357,7 +377,7 @@ def run_native(args, w, wl):
     net.eval().to(dev)
 
     # R distinct resident input batches: R * B * P^2 * 3 B of uint8 tiles; the step's own activations
-    # (>1 GB at 64 tiles of 512^2) exceed the 126 MB L2 many times over, so no explicit flush is needed.
+    # (>1 GB at 64 tiles of 512^2) exceed the 50 MB L2 many times over, so no explicit flush is needed.
     R = 3
     tiles = [synth.make_tiles(B, P, seed=100 * rank + r).to(dev) for r in range(R)]
     topo_host = [synth.make_topo_inputs(B, P, NP, seed=100 * rank + r, ragged=False) for r in range(R)] if NP else None
@@ -387,10 +407,10 @@ def run_native(args, w, wl):
                 ex_sc.publish(sl)
                 if NP:
                     ex_ts.publish(sl)
-            return scores, ts
+            return scores, feat, ts
         scores, feat = net.infer_masks_and_img_features(tiles[r])
         ts = net.infer_toponet(feat, *topo[r]) if NP else None
-        return scores, ts
+        return scores, feat, ts
 
     def drain():
         for ex in (ex_sc, ex_ts):
@@ -416,12 +436,14 @@ def run_native(args, w, wl):
         barrier()
         e0.record()
         for i in range(args.steps):
-            step(args.warmup + i)
+            last = step(args.warmup + i)
         drain()                                            # the last steps' gathers belong to the timed region
         e1.record()
         barrier()
     launches = int(lib.samroad_launch_count(0))
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last)
     buf = C.create_string_buffer(1 << 16)
     _lib.check(lib.samroad_timing_read(handle, buf, len(buf)), "timing_read")
     kernels = json.loads(buf.value.decode())
@@ -533,7 +555,7 @@ def run_native(args, w, wl):
         "config": {"workload": w["name"], "workload_key": wl, "what": w["note"], "tiles_per_step_per_gpu": B,
                    "patch_size": P, "points_per_tile": NP, "pairs_per_point": 16, "input_dtype": "uint8",
                    "l2_policy": f"{R} rotating resident input batches and >1 GB of activations per step "
-                                "(> 126 MB L2); no explicit flush",
+                                "(> 50 MB L2); no explicit flush",
                    "parallelism": f"tile-sharded dp{world}" +
                                   (" + all-gather of mask scores and topology scores, double-buffered, overlapped with "
                                    "the next step" if world > 1 else ""),
@@ -613,7 +635,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--debug-gemm-mode", type=int, default=0,
                     help="A/B only: samroad_debug_disable_2cta_gemm bit mask (16 = no snake traversal)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (seeded sample, float32 .npy) to DIR")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "native":
+        ap.error("--dump-outputs writes what the native path computed; it needs --impl native")
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
     w = WORKLOADS[args.workload]
     with _JsonStdout() as out:
         _OUT = out

@@ -1,6 +1,6 @@
 /* samroad_b200.h -- C ABI of libsamroad_b200.so
  *
- * B200-native (sm_100a) implementation of the tiled-inference hot path of htcr/sam_road.
+ * H100-native (sm_90a) implementation of the tiled-inference hot path of htcr/sam_road.
  * Every entry point replaces one piece of the reference's Python interface (file:line cited per
  * function, relative to the reference repository root).  The reference has no FFI of its own (it is
  * pure PyTorch, SURVEY.md §2.2); the binding a maintainer adds is the ctypes stub shown in
@@ -230,23 +230,17 @@ int samroad_op_attention(const void* qkv16, const float* qkv_bias, const float* 
                          const float* rel_w, int B, int s, int win, int heads, int head_dim,
                          void* out16, void* stream);
 
-/* Test hook (bit mask): bit 0 routes samroad_op_attention / the encoder through the fp32 SIMT
- * attention kernel (the independent on-device checker of the tcgen05 kernel); bit 1 selects the
- * tcgen05 variant that evaluates 1 in 4 softmax exponentials as a polynomial on the FMA pipe; bit 2
- * starts softmax group 1 half a block late; bit 3 disables the groups' turn-taking on the MUFU (A/B
- * timing, tools/att_trace.py).  Not for production use. */
+/* Test hook: bit 0 routes samroad_op_attention / the encoder through the fp32 SIMT attention
+ * kernel (the independent on-device checker of the tensor-core kernel).  Not for production use. */
 void samroad_debug_force_simt_attention(int on);
-/* Test hook (bit mask): bit 0 routes every GEMM through the 1-CTA kernels (the 2-CTA cta_group::2
- * kernel is then checked against them); bit 1 routes the in-place fp32 shortcut GEMMs through the
- * register-path epilogue instead of the TMA one; bit 2 selects the TMA load+store variant of that
- * epilogue (bit-identical to the register path) instead of the default TMA reduce-add; bit 4 makes
- * every encoder kernel walk the token rows in ascending order (no snake traversal). */
+/* Test hook (bit mask): bit 4 makes every encoder kernel walk the token rows in ascending order (no
+ * snake traversal).  Bits 0-2 selected GEMM variants of an earlier multi-kernel GEMM path; there is
+ * one GEMM kernel now and they are ignored. */
 void samroad_debug_disable_2cta_gemm(int off);
-/* Test hook: direction in which the next op-level row-streaming kernel (LayerNorm, 2-CTA GEMM, encoder
- * attention) walks the token rows (1 = descending; the encoder alternates it from kernel to kernel). */
+/* Test hook: direction in which the next op-level row-streaming kernel (LayerNorm) walks the token
+ * rows (1 = descending; the encoder alternates it from kernel to kernel). */
 void samroad_debug_set_traverse_reverse(int on);
-/* Debug hook: device buffer of 256 int64 receiving clock64 stamps of CTA 0's first work unit in the
- * tcgen05 attention kernel (softmax warp phases, MMA issue times); NULL disables. */
+/* Kept for ABI compatibility: the attention kernel records no phase trace, and the call does nothing. */
 void samroad_debug_attention_trace(void* dev_buf);
 
 #ifdef __cplusplus

@@ -92,7 +92,7 @@ def load() -> C.CDLL:
     if not LIB_PATH.exists():
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -m sam_road_b200.build` "
-            "(nvcc, sm_100a). sam_road_b200 has no CPU or PyTorch fallback path.")
+            "(nvcc, sm_90a). sam_road_b200 has no CPU or PyTorch fallback path.")
     lib = C.CDLL(str(LIB_PATH))
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol

@@ -1,4 +1,4 @@
-"""Build libsamroad_b200.so in-tree with nvcc for sm_100a (no torch extension machinery: the
+"""Build libsamroad_b200.so in-tree with nvcc for sm_90a (H100) (no torch extension machinery: the
 library is a plain C-ABI shared object loaded through ctypes, see _lib.py and include/samroad_b200.h).
 
     python -m sam_road_b200.build [--force]
@@ -20,7 +20,7 @@ LIB_PATH = PKG_DIR / "libsamroad_b200.so"
 
 SOURCES = ["common.cu", "gemm_ops.cu", "kernels.cu", "attention.cu", "toponet.cu", "sam_decoder.cu", "graph.cu", "model.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -45,7 +45,7 @@ def _digest() -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every .cu for sm_100a and link the shared library. Returns its path."""
+    """Compile every .cu for sm_90a and link the shared library. Returns its path."""
     stamp = OBJ_DIR / "digest.txt"
     dig = _digest()
     if not force and LIB_PATH.exists() and stamp.exists() and stamp.read_text() == dig:

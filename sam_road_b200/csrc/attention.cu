@@ -10,11 +10,11 @@
 // math, and a padded token (y >= s or x >= s) has x = 0 so q = k = v = qkv bias (SURVEY.md §8a P1):
 // such tokens are real softmax keys but their query rows are never written.
 //
-// v1: fp32 SIMT flash-style kernel (one thread = one query row, keys streamed through shared memory
-// in chunks of 32 with an online softmax).  It is the straightforward, easily-audited statement of
-// the math and the on-device checker for the tensor-core version.
-#include "attention_tc.cuh"
-#include "attention_tc80.cuh"
+// Two kernels: the tensor-core kernel (attention_mma.cuh) on the hot path, and an fp32 SIMT
+// flash-style kernel (one thread = one query row, keys streamed through shared memory in chunks of 32
+// with an online softmax) -- the straightforward, easily-audited statement of the math and the
+// on-device checker for the tensor-core version.
+#include "attention_mma.cuh"
 #include "common.cuh"
 #include "ops.h"
 
@@ -200,167 +200,17 @@ static int launch_attention_simt(const __half* qkv, const float* qkv_bias, const
   return 0;
 }
 
-// ------------------------------------------------------------------------------------------------
-// rel-pos table packing for the tensor-core kernel: tab[r] = rel_pos_h[r] for r < 2K-1,
-// rel_pos_w[r - rows/2] for rows/2 <= r < rows/2 + 2K-1, 0 otherwise; fp16 [rows, 64]
-// ------------------------------------------------------------------------------------------------
-__global__ void pack_rel_table_kernel(const float* __restrict__ rel_h, const float* __restrict__ rel_w,
-                                      int win, int hd, int ld, int rows, __half* __restrict__ tab) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= rows * ld) return;
-  const int r = idx / ld, c = idx % ld, L = 2 * win - 1;
-  float v = 0.f;
-  if (c < hd) {
-    if (r < L) v = rel_h[r * hd + c];
-    else if (r >= rows / 2 && r < rows / 2 + L) v = rel_w[(r - rows / 2) * hd + c];
-  }
-  tab[idx] = __float2half_rn(v);
-}
-
-// fp16 [rows, ld] with ld = 64 (head_dim 64) or 128 (head_dim 80, columns 80.. zero)
-int pack_rel_table(const float* rel_h, const float* rel_w, int win, int hd, __half* tab,
-                   cudaStream_t st) {
-  const int rows = rel_table_rows(win);
-  const int ld = hd == 64 ? 64 : 128;
-  pack_rel_table_kernel<<<(rows * ld + 255) / 256, 256, 0, st>>>(rel_h, rel_w, win, hd, ld, rows, tab);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
-  return 0;
-}
-
 static bool g_force_simt = false;
-static bool g_no_stagger = true;    // A/B hook (bit 2 set): start group 1 half a block late
-static bool g_alternate = true;     // A/B hook (bit 3 set): no turn-taking on the MUFU
-static bool g_poly = false;         // A/B hook: 1 in 4 softmax exponentials as a polynomial on the FMA pipe
-static long long* g_att_trace = nullptr;
-void attention_set_trace(long long* p) { g_att_trace = p; }
-void attention_force_simt(int mode) { g_force_simt = (mode & 1) != 0; g_poly = (mode & 2) != 0; g_no_stagger = (mode & 4) == 0; g_alternate = (mode & 8) == 0; }
-
-template <bool kWindow, int WIN>
-static int launch_attention_tc(const __half* qkv, const float* qkv_bias, const __half* tab, int B,
-                               int s, int heads, __half* out, cudaStream_t st) {
-  const int D = heads * 64;
-  const int T = s * s;
-  CUtensorMap tmQKV, tmTab;
-  if (kWindow) {
-    const uint64_t dims[4] = {static_cast<uint64_t>(3 * D), static_cast<uint64_t>(s),
-                              static_cast<uint64_t>(s), static_cast<uint64_t>(B)};
-    const uint64_t strides[3] = {static_cast<uint64_t>(3 * D), static_cast<uint64_t>(s) * 3 * D,
-                                 static_cast<uint64_t>(T) * 3 * D};
-    const uint32_t box[4] = {64, static_cast<uint32_t>(WIN), static_cast<uint32_t>(WIN), 1};
-    if (int rc = make_tmap_f16_4d(&tmQKV, qkv, dims, strides, box)) return rc;
-  } else {
-    if (int rc = make_tmap_f16_2d(&tmQKV, qkv, static_cast<uint64_t>(B) * T, 3 * D, 3 * D, 128))
-      return rc;
-  }
-  const int rows = rel_table_rows(WIN);
-  static_assert(atc_table_rows(WIN) == (4 * WIN - 2 <= 64 ? 64 : (4 * WIN - 2 <= 128 ? 128 : 256)), "table rows");
-  if (int rc = make_tmap_f16_2d(&tmTab, tab, rows, 64, 64, rows)) return rc;
-  auto kern = g_poly ? attention_tc_kernel<kWindow, WIN, true> : attention_tc_kernel<kWindow, WIN, false>;
-  static uint64_t attr_devs = 0;          // one bit per CUDA device: function attributes are per device
-  if (first_use_on_device(&attr_devs)) {
-    SRB_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<kWindow, WIN, false>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, AtcSmem<kWindow, atc_table_bytes(WIN)>::kBytes));
-    SRB_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<kWindow, WIN, true>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, AtcSmem<kWindow, atc_table_bytes(WIN)>::kBytes));
-  }
-  AtcParams p;
-  p.qkv_bias = qkv_bias; p.out = out; p.B = B; p.s = s; p.heads = heads; p.D = D;
-  p.nwin = kWindow ? (s + WIN - 1) / WIN : 1;
-  p.scale_log2e = 0.125f * 1.4426950408889634f;
-  const int units = kWindow ? B * p.nwin * p.nwin * heads : B * (T / 256) * heads;
-  p.num_units = units;
-  p.trace = g_att_trace;
-  p.no_stagger = g_no_stagger ? 1 : 0;
-  p.alternate = g_alternate ? 1 : 0;
-  p.reverse = traverse_reverse() ? 1 : 0;
-  const int grid = units < device_sm_count() ? units : device_sm_count();   // persistent CTAs
-  kern<<<grid, kAtcThreads, AtcSmem<kWindow, atc_table_bytes(WIN)>::kBytes, st>>>(tmQKV, tmTab, p);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
-  return 0;
-}
-
-template <bool kWindow, int WIN>
-static int launch_attention_tc80(const __half* qkv, const float* qkv_bias, const __half* tab, int B,
-                                 int s, int heads, __half* out, cudaStream_t st) {
-  const int D = heads * kAtc80HD;
-  const int T = s * s;
-  using SM = Atc80Smem<kWindow, WIN>;
-  CUtensorMap tmQKV, tmTab;
-  if (kWindow) {
-    const uint64_t dims[4] = {static_cast<uint64_t>(3 * D), static_cast<uint64_t>(s),
-                              static_cast<uint64_t>(s), static_cast<uint64_t>(B)};
-    const uint64_t strides[3] = {static_cast<uint64_t>(3 * D), static_cast<uint64_t>(s) * 3 * D,
-                                 static_cast<uint64_t>(T) * 3 * D};
-    const uint32_t box[4] = {64, static_cast<uint32_t>(WIN), static_cast<uint32_t>(WIN), 1};
-    if (int rc = make_tmap_f16_4d(&tmQKV, qkv, dims, strides, box)) return rc;
-  } else {
-    if (int rc = make_tmap_f16_2d(&tmQKV, qkv, static_cast<uint64_t>(B) * T, 3 * D, 3 * D, 128))
-      return rc;
-  }
-  if (int rc = make_tmap_f16_2d(&tmTab, tab, SM::NTAB, 128, 128, SM::NTAB)) return rc;
-  auto kern = attention_tc80_kernel<kWindow, WIN>;
-  static uint64_t attr_devs = 0;          // one bit per CUDA device: function attributes are per device
-  if (first_use_on_device(&attr_devs)) {
-    SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes));
-  }
-  AtcParams p;
-  p.qkv_bias = qkv_bias; p.out = out; p.B = B; p.s = s; p.heads = heads; p.D = D;
-  p.nwin = kWindow ? (s + WIN - 1) / WIN : 1;
-  p.scale_log2e = 0.11180339887498948f * 1.4426950408889634f;      // 80^-0.5 * log2(e)
-  p.num_units = kWindow ? B * p.nwin * p.nwin * heads : B * (T / 128) * heads;
-  p.trace = nullptr; p.no_stagger = 1; p.alternate = 0; p.reverse = traverse_reverse() ? 1 : 0;
-  const int grid = p.num_units < device_sm_count() ? p.num_units : device_sm_count();
-  kern<<<grid, kAtc80Threads, SM::kBytes, st>>>(tmQKV, tmTab, p);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
-  return 0;
-}
+void attention_force_simt(int mode) { g_force_simt = (mode & 1) != 0; }
 
 int encoder_attention(const __half* qkv, const float* qkv_bias, const float* rel_h,
-                      const float* rel_w, const __half* rel_tab, int B, int s, int win, int heads,
-                      int hd, __half* out, cudaStream_t st) {
+                      const float* rel_w, int B, int s, int win, int heads, int hd, __half* out,
+                      cudaStream_t st) {
   SRB_REQUIRE(win > 0 && win <= s && s <= 64, "attention: win=%d s=%d unsupported", win, s);
   if (B <= 0) return 0;
-  // tensor-core path: head_dim 64; window 14 on any grid, global on 16x16 / 32x32 token grids
-  const bool tc_ok = hd == 64 && !g_force_simt &&
-                     ((win == 14 && s > 14) || (win == s && (s == 16 || s == 32 || s == 64)));
-  if (tc_ok) {
-    const __half* tab = rel_tab;
-    if (!tab) {
-      static __half* scratch_dev[64] = {nullptr};   // op-level calls without a pre-packed table (per device)
-      int dev = 0;
-      SRB_CUDA_OK(cudaGetDevice(&dev));
-      SRB_REQUIRE(dev >= 0 && dev < 64, "attention: device index %d", dev);
-      __half*& scratch = scratch_dev[dev];
-      if (!scratch) SRB_CUDA_OK(cudaMalloc(&scratch, 256 * 64 * sizeof(__half)));
-      SRB_TRY_RC(pack_rel_table(rel_h, rel_w, win, hd, scratch, st));
-      tab = scratch;
-    }
-    if (win == 14 && win < s) return launch_attention_tc<true, 14>(qkv, qkv_bias, tab, B, s, heads, out, st);
-    if (s == 16) return launch_attention_tc<false, 16>(qkv, qkv_bias, tab, B, s, heads, out, st);
-    if (s == 64) return launch_attention_tc<false, 64>(qkv, qkv_bias, tab, B, s, heads, out, st);
-    return launch_attention_tc<false, 32>(qkv, qkv_bias, tab, B, s, heads, out, st);
-  }
-  // head_dim 80 (ViT-H): tensor-core kernel with two K-blocks per operand tile
-  const bool tc80_ok = hd == 80 && !g_force_simt &&
-                       ((win == 14 && s > 14) || (win == s && (s == 16 || s == 32)));
-  if (tc80_ok) {
-    const __half* tab = rel_tab;
-    if (!tab) {
-      static __half* scratch80_dev[64] = {nullptr};
-      int dev = 0;
-      SRB_CUDA_OK(cudaGetDevice(&dev));
-      SRB_REQUIRE(dev >= 0 && dev < 64, "attention: device index %d", dev);
-      __half*& scratch80 = scratch80_dev[dev];
-      if (!scratch80) SRB_CUDA_OK(cudaMalloc(&scratch80, 128 * 128 * sizeof(__half)));
-      SRB_TRY_RC(pack_rel_table(rel_h, rel_w, win, hd, scratch80, st));
-      tab = scratch80;
-    }
-    if (win == 14 && win < s) return launch_attention_tc80<true, 14>(qkv, qkv_bias, tab, B, s, heads, out, st);
-    if (s == 16) return launch_attention_tc80<false, 16>(qkv, qkv_bias, tab, B, s, heads, out, st);
-    return launch_attention_tc80<false, 32>(qkv, qkv_bias, tab, B, s, heads, out, st);
+  if (!g_force_simt) {
+    if (hd == 64) return launch_attention_mma<64>(qkv, qkv_bias, rel_h, rel_w, B, s, win, heads, out, st);
+    if (hd == 80) return launch_attention_mma<80>(qkv, qkv_bias, rel_h, rel_w, B, s, win, heads, out, st);
   }
   if (hd == 64) return launch_attention_simt<64>(qkv, qkv_bias, rel_h, rel_w, B, s, win, heads, out, st);
   if (hd == 80) return launch_attention_simt<80>(qkv, qkv_bias, rel_h, rel_w, B, s, win, heads, out, st);

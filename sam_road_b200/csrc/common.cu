@@ -28,11 +28,11 @@ uint64_t launch_count(bool reset) {
 int device_sm_count() {
   static int cached[64] = {0};     // per device: a process may drive several GPUs
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;   // H100 SXM
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      return 148;
+      return 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -174,9 +174,9 @@ int stream_wait_value32_geq(void* addr, uint32_t value, cudaStream_t st) {
   return 0;
 }
 
-// Traversal direction of the next row-streaming kernel (LayerNorm, 2-CTA GEMMs, encoder attention):
+// Traversal direction of the next row-streaming kernel (LayerNorm):
 // the encoder alternates it from kernel to kernel so that each kernel starts on the rows its
-// producer wrote last, i.e. on what is still in the 126 MB L2 (activations are 100-400 MB).
+// producer wrote last, i.e. on what is still in the 50 MB L2 (activations are 100-400 MB).
 static bool g_traverse_reverse = false;
 static bool g_traverse_snake_off = false;     // A/B hook
 void set_traverse_snake_enabled(bool on) { g_traverse_snake_off = !on; }

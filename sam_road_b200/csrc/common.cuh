@@ -1,10 +1,10 @@
-// sam_road_b200 :: common device/host helpers for sm_100a.
+// sam_road_b200 :: common device/host helpers for sm_90a.
 //
-// Thin inline-PTX wrappers for the Blackwell primitives the hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld),
+// Thin inline-PTX wrappers for the Hopper primitives the hot path uses:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors),
 // plus small math helpers shared by the kernels.  Nothing here is a port of
 // reference code: the reference (htcr/sam_road) ships no CUDA at all
-// (SURVEY.md §2.2); these are the building blocks of the B200-native path.
+// (SURVEY.md §2.2); these are the building blocks of the native path.
 #pragma once
 
 #include <cuda.h>
@@ -70,6 +70,14 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// Element-wise fp32x2 add / fma, each lane rounded as its scalar counterpart.
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 // exact-erf GELU (reference: sam/segment_anything/modeling/common.py:18 nn.GELU default,
 // model.py:285).  erff() is accurate to ~1 ulp; the output is rounded to fp16 afterwards.
 __device__ __forceinline__ float gelu_erf(float x) {
@@ -93,20 +101,25 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
   return fmaf(-a, e, fmaxf(x, 0.0f));
 }
 
-// Two elements per instruction on the packed fp32x2 pipe (FFMA2): the polynomial is evaluated in
-// t = -min(|x|, 5.6) (odd coefficients negated) so that no packed negation is needed.  Same
-// coefficients, same rounding per lane as gelu_erf_fast -> bit-identical results.
+// Two elements at a time: the polynomial is evaluated in t = -min(|x|, 5.6) (odd coefficients
+// negated).  Same coefficients, same rounding per lane as gelu_erf_fast -> bit-identical results.
 __device__ __forceinline__ float2 gelu_erf_fast2(float2 x) {
   const float2 na = make_float2(fminf(x.x, -x.x), fminf(x.y, -x.y));
   const float2 t = make_float2(fmaxf(na.x, -5.6f), fmaxf(na.y, -5.6f));
-  float2 l = __ffma2_rn(make_float2(0.0038648627f, 0.0038648627f), t, make_float2(0.044072032f, 0.044072032f));
-  l = __ffma2_rn(l, t, make_float2(-0.46802717f, -0.46802717f));
-  l = __ffma2_rn(l, t, make_float2(1.1473644f, 1.1473644f));
-  l = __ffma2_rn(l, t, make_float2(-1.0004811f, -1.0004811f));
+  float2 l = ffma2(make_float2(0.0038648627f, 0.0038648627f), t, make_float2(0.044072032f, 0.044072032f));
+  l = ffma2(l, t, make_float2(-0.46802717f, -0.46802717f));
+  l = ffma2(l, t, make_float2(1.1473644f, 1.1473644f));
+  l = ffma2(l, t, make_float2(-1.0004811f, -1.0004811f));
   float2 e;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(l.x));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(l.y));
-  return __ffma2_rn(na, e, make_float2(fmaxf(x.x, 0.0f), fmaxf(x.y, 0.0f)));
+  return ffma2(na, e, make_float2(fmaxf(x.x, 0.0f), fmaxf(x.y, 0.0f)));
+}
+
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
 }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __expf(-x)); }
@@ -237,231 +250,115 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* t
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads -- SASS: UTCHMMA / LDTM
+// wgmma (warpgroup MMA, sm_90a) -- SASS: HGMMA
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t tmem_base, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 fp16 (=128 B).
-// 8-row swizzle atoms are 1024 B apart (SBO); LBO is unused for swizzled K-major layouts.
-// Field layout: cute::UMMA::SmemDescriptor (cute/arch/mma_sm100_desc.hpp).
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 fp16 (=128 B) as
+// written by a 128B-swizzled TMA box.  8-row swizzle atoms are 1024 B apart (SBO); LBO is unused
+// for swizzled K-major layouts.  Advancing 16 elements (32 B) along K inside the atom is +2 on the
+// start-address field.
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);        // start address >> 4
-  d |= static_cast<uint64_t>(0) << 16;                           // leading byte offset (unused)
+  d |= static_cast<uint64_t>(1) << 16;                           // leading byte offset (unused)
   d |= static_cast<uint64_t>(1024u >> 4) << 32;                  // stride byte offset = 1024 B
-  d |= static_cast<uint64_t>(1) << 46;                           // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                           // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                           // SWIZZLE_128B
   return d;
 }
-
-// Instruction descriptor for kind::f16, fp16 A/B (K-major), fp32 accumulate.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4)                                   // C format = F32
-         | (0u << 7) | (0u << 10)                    // A, B format = F16
-         | (0u << 15) | (0u << 16)                   // A, B K-major
-         | (static_cast<uint32_t>(N >> 3) << 17)     // N >> 3
-         | (static_cast<uint32_t>(M >> 4) << 24);    // M >> 4
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-// Same, but B operand MN-major (used for P·V where V is stored [keys][hd] row-major).
-__host__ __device__ constexpr uint32_t umma_idesc_f16_bmn(int M, int N) {
-  return umma_idesc_f16(M, N) | (1u << 16);
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator accesses across the asynchronous MMA
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// register budget of a warpgroup (all its warps execute it): producers give registers to consumers
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
+// Accumulator fragment of wgmma m64nNk16 (f32): register i of thread (warp w of the warpgroup, lane l)
+// holds row 16*w + l/4 + 8*((i>>1)&1), column 8*(i>>2) + 2*(l&3) + (i&1).
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b,
+                                             uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t"
       "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns (lane i of the warp reads TMEM lane
-// base+i).  A warp may only touch lanes [32*(warp_id%4), +32).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 32 columns without the wait (issue several, then tmem_ld_wait once)
-__device__ __forceinline__ void tmem_ld_32x32_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 16 columns, no wait
-__device__ __forceinline__ void tmem_ld_32x16_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM, 32 lanes x 32 columns
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]),
-      "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]),
-      "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-      "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-      "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// 2^x on the FMA/ALU pipes (Cody-Waite split + degree-3 polynomial, rel. error 1.0e-4 < fp16 ulp/2):
-// used for a quarter of the softmax exponentials to take load off the MUFU pipe, the attention
-// kernel's busiest unit (ncu: sm__inst_executed_pipe_xu ~60 %).
-__device__ __forceinline__ float ex2_poly3(float x) {
-  x = fmaxf(x, -125.0f);
-  const float t = x + 12582912.0f;            // 1.5 * 2^23: the low mantissa bits hold round(x)
-  const float f = x - (t - 12582912.0f);      // in [-0.5, 0.5]
-  float p = fmaf(0.05592203512787819f, f, 0.24264007806777954f);
-  p = fmaf(p, f, 0.6931210160255432f);
-  p = fmaf(p, f, 0.9999244809150696f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-// three-input maximum (FMNMX3, sm_100)
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-// Two at a time on the packed fp32x2 pipe (same coefficients and rounding per lane as ex2_poly3).
-__device__ __forceinline__ float2 ex2_poly3_2(float2 x) {
-  x = make_float2(fmaxf(x.x, -125.0f), fmaxf(x.y, -125.0f));
-  const float2 t = __fadd2_rn(x, make_float2(12582912.0f, 12582912.0f));
-  const float2 r = __fadd2_rn(t, make_float2(-12582912.0f, -12582912.0f));
-  const float2 f = __ffma2_rn(r, make_float2(-1.0f, -1.0f), x);
-  float2 p = __ffma2_rn(make_float2(0.05592203512787819f, 0.05592203512787819f), f,
-                        make_float2(0.24264007806777954f, 0.24264007806777954f));
-  p = __ffma2_rn(p, f, make_float2(0.6931210160255432f, 0.6931210160255432f));
-  p = __ffma2_rn(p, f, make_float2(0.9999244809150696f, 0.9999244809150696f));
-  return make_float2(__int_as_float(__float_as_int(p.x) + (__float_as_int(t.x) << 23)),
-                     __int_as_float(__float_as_int(p.y) + (__float_as_int(t.y) << 23)));
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// 2-CTA (cta_group::2) variants: a cluster of two CTAs on one TPC issues one UMMA of M = 256; each
-// CTA stages half of A and half of B, so L2 -> SM operand traffic per FLOP halves.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load whose completion bytes are credited to the LEADER CTA's mbarrier (peer bit cleared)
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* tm, uint64_t* bar,
-                                                int32_t c0, int32_t c1) {
-  const uint32_t mbar = smem_u32(bar) & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(mbar), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the mbarrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}\n"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t tmem_base, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                                uint32_t idesc, uint32_t accumulate) {
+// D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b,
+                                             uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t"
       "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-// arrive (once all prior MMAs of this thread retired) on the barrier at this offset in both CTAs
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
+
 
 // ----------------------------------------------------------------------------------------------
 // host: TMA descriptor construction (driver entry point fetched at run time; no -lcuda needed)

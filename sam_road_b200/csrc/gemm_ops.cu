@@ -2,23 +2,12 @@
 #include <cstring>
 
 #include "gemm_tc.cuh"
-#include "gemm_tc2.cuh"
-#include "gemm_tc2r.cuh"
 #include "ops.h"
 
 namespace srb {
 
-// 128x256 tiles (3-stage ring, all 512 TMEM columns) when N allows and the grid still fills the GPU,
-// otherwise 128x128 tiles (5-stage ring).
-// 2-CTA 256x256 tiles for the big streaming GEMMs (halves L2->SM operand traffic)
-static bool g_disable_2cta = false;
-static bool g_disable_tma_resid = false;
-static int g_resid_variant = 0;
-void gemm_disable_2cta(int mode) { g_disable_2cta = (mode & 1) != 0; g_disable_tma_resid = (mode & 2) != 0; g_resid_variant = (mode >> 2) & 3; }
-static inline bool use_2cta(int M, int N) {
-  if (g_disable_2cta || N % 256 != 0) return false;
-  return static_cast<long>((M + 255) / 256) * (N / 256) >= device_sm_count() / 2;
-}
+// 128x256 tiles (3-stage ring) when N allows and the grid still fills the GPU, otherwise 128x128
+// tiles (5-stage ring).
 
 static inline bool use_bn256(int M, int N) {
   if (N % 256 != 0) return false;
@@ -30,7 +19,6 @@ int gemm_f16out(const __half* A, int lda, const __half* W, int ldw, int M, int N
                 const float* bias, int act, __half* out, int ldo, cudaStream_t st) {
   EpiF16::Params p{out, bias, ldo, act};
   SRB_REQUIRE(ldo % 8 == 0, "gemm_f16out: ldo=%d must be a multiple of 8", ldo);
-  if (use_2cta(M, N)) return launch_gemm_tc2<EpiF16>(A, lda, W, ldw, M, N, K, p, st);
   if (use_bn256(M, N)) return launch_gemm_tc<256, 3, EpiF16>(A, lda, W, ldw, M, N, K, p, st);
   return launch_gemm_tc<128, 5, EpiF16>(A, lda, W, ldw, M, N, K, p, st);
 }
@@ -40,22 +28,6 @@ int gemm_f32out(const __half* A, int lda, const __half* W, int ldw, int M, int N
                 int ldo, cudaStream_t st) {
   EpiF32::Params p{out, bias, resid, pos, ldo, pos_rows > 0 ? pos_rows : 1, N};
   SRB_REQUIRE(ldo % 4 == 0, "gemm_f32out: ldo=%d must be a multiple of 4", ldo);
-  if (use_2cta(M, N)) {
-    // in-place shortcut add (attention proj, MLP lin2): residual streamed through TMA
-    if (!g_disable_tma_resid && resid == out && resid != nullptr && pos == nullptr && bias != nullptr &&
-        (reinterpret_cast<uintptr_t>(out) & 15u) == 0)
-    {
-      // default: shortcut add performed by the TMA reduce in L2; variant 1 (test hook) streams the
-      // shortcut through smem instead and is bit-identical to the register-path epilogue
-      if (g_resid_variant == 1) return launch_gemm_tc2_resid<4, 3, false>(A, lda, W, ldw, M, N, K, bias, out, ldo, st);
-      return launch_gemm_tc2_resid<5, 2, true>(A, lda, W, ldw, M, N, K, bias, out, ldo, st);
-    }
-    // out = A.W^T + b + pos[m % pos_rows] (patch embedding + pos_embed): addend streamed by TMA
-    if (!g_disable_tma_resid && resid == nullptr && pos != nullptr && bias != nullptr && pos_rows % 32 == 0 &&
-        (reinterpret_cast<uintptr_t>(out) & 15u) == 0 && (reinterpret_cast<uintptr_t>(pos) & 15u) == 0)
-      return launch_gemm_tc2_resid<4, 3, false>(A, lda, W, ldw, M, N, K, bias, out, ldo, st, pos, N, pos_rows);
-    return launch_gemm_tc2<EpiF32>(A, lda, W, ldw, M, N, K, p, st);
-  }
   if (use_bn256(M, N)) return launch_gemm_tc<256, 3, EpiF32>(A, lda, W, ldw, M, N, K, p, st);
   return launch_gemm_tc<128, 5, EpiF32>(A, lda, W, ldw, M, N, K, p, st);
 }

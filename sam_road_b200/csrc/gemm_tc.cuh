@@ -1,21 +1,24 @@
-// sam_road_b200 :: tcgen05 GEMM  C[M,N] = A[M,K] * W[N,K]^T  (+ fused epilogue)
+// sam_road_b200 :: wgmma GEMM  C[M,N] = A[M,K] * W[N,K]^T  (+ fused epilogue)
 //
 // One kernel template covers every dense contraction of the hot path (SURVEY.md §2.4 K2, K5, K9,
-// K10, K11, K12, K16): fp16 operands (both K-major), fp32 accumulation in TMEM.
+// K10, K11, K12, K16): fp16 operands (both K-major), fp32 accumulation in registers.
 //
-//   warp 0      : TMA producer   (cp.async.bulk.tensor, 128B-swizzled 128x64 / BNx64 boxes)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128 x BN x 16)
-//   warps 2..9  : epilogue       (tcgen05.ld 32x32b -> registers -> fused math -> global); two warps
-//                 per TMEM lane quarter split the tile's columns.  Streaming epilogues (EpiF16 /
-//                 EpiF32) transpose each 32x32 fp32 block through a per-warp smem scratch so that
-//                 global loads/stores are row-contiguous (8 lanes x 16 B per row) instead of one
-//                 row per lane; row-statistics epilogues (EpiLN, EpiDecFinal) keep one row per
-//                 thread and use four warps.
+//   warpgroup 0     : TMA producer (one thread; cp.async.bulk.tensor, 128B-swizzled 128x64 / BNx64
+//                     boxes), registers handed to the consumers with setmaxnreg
+//   warpgroups 1, 2 : consumers.  Each issues wgmma m64 x BN x 16 for its 64 rows of the 128-row
+//                     tile, then stages its fp32 accumulators in shared memory and runs the fused
+//                     epilogue over them: warp w of consumer g reads rows 32*(2g + (w&1)) .. +31 (one
+//                     row per lane) and columns half (w>>1) of the tile.  Streaming epilogues (EpiF16)
+//                     transpose each 32x32 fp32 block through a per-warp smem scratch so that global
+//                     stores are row-contiguous (8 lanes x 16 B per row); row-statistics epilogues
+//                     (EpiLN, EpiDecFinal) keep one row per thread.
 //
-// Persistent CTAs (grid = min(#tiles, #SMs)), STAGES-deep smem ring between TMA and MMA, and a
-// two-deep TMEM accumulator ring between MMA and epilogue so the epilogue of tile i overlaps the
-// main loop of tile i+1.  Tile order is n-fastest so the CTAs running concurrently share the same
-// A rows (L2 reuse); the weights (<= 4.7 MB per layer) stay L2-resident.
+// Persistent CTAs (grid = min(#tiles, #SMs)) and a STAGES-deep smem ring between TMA and the MMAs.
+// The accumulator staging area reuses the ring (an m128 x n256 fp32 tile needs 130 KB, and a second
+// buffer of that size does not fit next to the ring in 227 KB), so the producer starts the next
+// tile's loads once the epilogue has read the accumulators.  Tile order is n-fastest so the CTAs
+// running concurrently share the same A rows (L2 reuse); the weights (<= 4.7 MB per layer) stay
+// L2-resident.
 //
 // Reference semantics implemented by the epilogues:
 //   nn.Linear (+bias)                       image_encoder.py:212-213,227,238; common.py:21-26
@@ -35,7 +38,7 @@ namespace srb {
 
 constexpr int kGemmBM = 128;
 constexpr int kGemmBK = 64;
-constexpr int kGemmThreads = 320;
+constexpr int kGemmThreads = 384;
 constexpr int kGemmEpiWarps = 8;
 constexpr int kGemmScratchFloats = 32 * 36;   // per epilogue warp: 32x32 fp32 block, rows padded to 36
 
@@ -47,27 +50,29 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   return x;
 }
 
-// One accumulator row (this thread's TMEM lane) of the current tile.
-struct TmemRow {
-  uint32_t taddr;
+// One accumulator row (this lane's row of the tile, starting at the warp's first column) in the
+// shared-memory staging area.
+struct AccRow {
+  const float* p;
   __device__ __forceinline__ void load(int chunk, float (&v)[32]) const {
-    uint32_t r[32];
-    tmem_ld_32x32(taddr + static_cast<uint32_t>(chunk) * 32u, r);
-    tmem_ld_wait();
+    const float4* s = reinterpret_cast<const float4*>(p + chunk * 32);
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < 8; ++i) {
+      const float4 x = s[i];
+      v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
+    }
   }
 };
 
 // ------------------------------------------------------------------------------------------------
-// Streaming epilogues.  A warp owns 32 tile rows (its TMEM lane quarter) x n_cols columns.  Per
+// Streaming epilogues.  A warp owns 32 tile rows (a row quarter of the tile) x n_cols columns.  Per
 // 32-column chunk: lane r holds row r's 32 accumulators -> scratch[r][0..31] (row pitch 36 floats,
 // float4 accesses, conflict-free) -> re-read as "lane l holds columns 4*(l&7).. of row 4*j + (l>>3)", j = 0..7 ->
 // bias / activation / residual in that layout -> 8 lanes cover 128 (fp32) or 64 (fp16) contiguous
 // bytes of a row per store instruction.
 // ------------------------------------------------------------------------------------------------
 template <class F>
-__device__ __forceinline__ void epi_stream_chunks(int n_cols, const TmemRow& row, float* scratch,
+__device__ __forceinline__ void epi_stream_chunks(int n_cols, const AccRow& row, float* scratch,
                                                   int lane, F&& body) {
   const int nchunks = n_cols >> 5;
   const int cc = (lane & 7) * 4, rsub = lane >> 3;
@@ -98,10 +103,10 @@ struct EpiF16 {
     int act;
   };
   static __device__ __forceinline__ void run(const Params& p, int m0, int M, int n_base, int n_cols,
-                                             const TmemRow& row, float* scratch, int lane) {
+                                             const AccRow& row, float* scratch, int lane) {
     if (p.act >= ACT_PROBE_SKIP) {          // timing ablations (tools/gemm_probe.py), never a result
       if (p.act == ACT_PROBE_SKIP) return;
-      if (p.act == ACT_PROBE_TMEM) {
+      if (p.act == ACT_PROBE_ACC) {
         float acc = 0.f;
         for (int c = 0; c < (n_cols >> 5); ++c) {
           float v[32];
@@ -157,7 +162,7 @@ struct EpiF32 {
   // 128 B contiguous per lane and chunk, and the residual of chunk c+1 prefetched into registers
   // while chunk c is processed, keeps more bytes in flight than the transposed scheme.
   static __device__ __forceinline__ void run(const Params& p, int m0, int M, int n_base, int n_cols,
-                                             const TmemRow& row, float* /*scratch*/, int lane) {
+                                             const AccRow& row, float* /*scratch*/, int lane) {
     const int nchunks = n_cols >> 5;
     const int m = m0 + lane;
     const bool valid = m < M;
@@ -205,8 +210,8 @@ struct EpiF32 {
 // ------------------------------------------------------------------------------------------------
 // Epilogue 3: grouped row LayerNorm.  x = acc + bias + resid; per group of `group` consecutive
 // columns: y = (x - mean) / sqrt(var + eps) * gamma[n % group] + beta[n % group]; y = act(y).
-// The tile must hold whole groups (BN % group == 0).  Three TMEM passes (mean, var, write) keep the
-// exact two-pass variance of torch.  All eight epilogue warps work: the two warps of a TMEM lane
+// The tile must hold whole groups (BN % group == 0).  Three accumulator passes (mean, var, write) keep the
+// exact two-pass variance of torch.  All eight epilogue warps work: the two warps of a row
 // quarter split the tile's columns; when a group fits into one half they are independent, when it
 // spans the tile (neck: group = BN = 256) they combine their partial sums through their smem scratch
 // and a 64-thread named barrier.  Outputs (each optional): fp16 row-major, fp32 row-major, fp32 NCHW
@@ -230,7 +235,7 @@ struct EpiLN {
     int n_total;
   };
   static __device__ __forceinline__ void load_x(const Params& p, int m, bool valid, int n0,
-                                                int chunk, const TmemRow& row, float (&v)[32]) {
+                                                int chunk, const AccRow& row, float (&v)[32]) {
     row.load(chunk, v);
     if (p.bias) {
       const float4* b4 = reinterpret_cast<const float4*>(p.bias + n0);
@@ -251,7 +256,7 @@ struct EpiLN {
     }
   }
   static __device__ __forceinline__ void run(const Params& p, int m0, int M, int n_base, int n_cols,
-                                             const TmemRow& row, float* scratch, int lane) {
+                                             const AccRow& row, float* scratch, int lane) {
     const int m = m0 + lane;
     const bool valid = m < M;
     if (n_cols <= 0) return;
@@ -260,7 +265,7 @@ struct EpiLN {
     const int cpg = span >> 5;                         // chunks per group (mine)
     const int ngroups = n_cols / span;
     const float inv_g = 1.0f / static_cast<float>(p.group);
-    // partner warp of the same lane quarter (warps 2+q and 6+q): scratch 4 warps away
+    // partner warp of the same row quarter: its scratch is 4 slots away
     const int half = (n_base / n_cols) & 1;
     const float* partner = scratch + (half ? -4 : 4) * kGemmScratchFloats;
     const int pair_bar = 1 + ((m0 >> 5) & 3);
@@ -349,7 +354,7 @@ struct EpiLN {
 // d = di*2 + dj (see decoder weight packing in pack.cu).
 // ------------------------------------------------------------------------------------------------
 struct EpiDecFinal {
-  static constexpr bool kSplitCols = true;     // warps 2-5: sub-pixels d3 = 0,1; warps 6-9: d3 = 2,3
+  static constexpr bool kSplitCols = true;     // column half 0: sub-pixels d3 = 0,1; half 1: d3 = 2,3
   struct Params {
     // [B, P, P, 2] fp32 seen as 4-D (x: 2P floats | di: 2 | h: 2 | k: B*P/4), image row = 4k + 2h + di;
     // box {64 floats, 2, 1, 4}: the 2 x 16 output pixels x 8 rows one warp produces per tile and half
@@ -368,7 +373,7 @@ struct EpiDecFinal {
   // as the dense TMA box and written with one 4-D TMA store per output (whole 128 B lines, where the
   // old direct epilogue scattered 16 B pieces).
   static __device__ __forceinline__ void run(const Params& p, int m0, int M, int n_base, int n_cols,
-                                             const TmemRow& row, float* scratch, int lane) {
+                                             const AccRow& row, float* scratch, int lane) {
     const int half = n_base >> 6;
     const int m = m0 + lane;
     const int d2 = m & 3, d1 = (m >> 2) & 3;
@@ -390,18 +395,18 @@ struct EpiDecFinal {
 #pragma unroll
       for (int ci = 0; ci < 32; ci += 2) {
         const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias3 + ci));
-        const float2 hh = gelu_erf_fast2(__fadd2_rn(make_float2(v[ci], v[ci + 1]), bb));
+        const float2 hh = gelu_erf_fast2(fadd2(make_float2(v[ci], v[ci + 1]), bb));
         const float4* wp = reinterpret_cast<const float4*>(p.w4 + ci * 8);
         const float4 w0 = __ldg(wp), w1 = __ldg(wp + 1), w2 = __ldg(wp + 2), w3 = __ldg(wp + 3);
         const float2 h0 = make_float2(hh.x, hh.x), h1 = make_float2(hh.y, hh.y);
-        o[0] = __ffma2_rn(h0, make_float2(w0.x, w0.y), o[0]);
-        o[1] = __ffma2_rn(h0, make_float2(w0.z, w0.w), o[1]);
-        o[2] = __ffma2_rn(h0, make_float2(w1.x, w1.y), o[2]);
-        o[3] = __ffma2_rn(h0, make_float2(w1.z, w1.w), o[3]);
-        o[0] = __ffma2_rn(h1, make_float2(w2.x, w2.y), o[0]);
-        o[1] = __ffma2_rn(h1, make_float2(w2.z, w2.w), o[1]);
-        o[2] = __ffma2_rn(h1, make_float2(w3.x, w3.y), o[2]);
-        o[3] = __ffma2_rn(h1, make_float2(w3.z, w3.w), o[3]);
+        o[0] = ffma2(h0, make_float2(w0.x, w0.y), o[0]);
+        o[1] = ffma2(h0, make_float2(w0.z, w0.w), o[1]);
+        o[2] = ffma2(h0, make_float2(w1.x, w1.y), o[2]);
+        o[3] = ffma2(h0, make_float2(w1.z, w1.w), o[3]);
+        o[0] = ffma2(h1, make_float2(w2.x, w2.y), o[0]);
+        o[1] = ffma2(h1, make_float2(w2.z, w2.w), o[1]);
+        o[2] = ffma2(h1, make_float2(w3.x, w3.y), o[2]);
+        o[3] = ffma2(h1, make_float2(w3.z, w3.w), o[3]);
       }
 #pragma unroll
       for (int di = 0; di < 2; ++di) {
@@ -441,9 +446,26 @@ struct GemmSmem {
   static constexpr int kABytes = kGemmBM * kGemmBK * 2;
   static constexpr int kBBytes = BN * kGemmBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kAccPitch = BN + 4;                       // floats; conflict-free row reads
+  static_assert(kGemmBM * kAccPitch * 4 <= STAGES * kStageBytes, "accumulators must fit the ring");
   static constexpr int kBarOffset = STAGES * kStageBytes;
   static constexpr int kScratchOffset = kBarOffset + 256;
   static constexpr int kTotal = kScratchOffset + kGemmEpiWarps * kGemmScratchFloats * 4 + 1024;
+};
+
+template <int BN>
+struct WgmmaTile;
+template <>
+struct WgmmaTile<128> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    wgmma_m64n128k16(d, a, b, acc);
+  }
+};
+template <>
+struct WgmmaTile<256> {
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) {
+    wgmma_m64n256k16(d, a, b, acc);
+  }
 };
 
 template <int BN, int STAGES, class Epi>
@@ -455,18 +477,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // ordered (tap, channel) and k-block kb reads the channel block of the tap-shifted 128-pixel slab;
   // out-of-image taps arrive as TMA zero fill.  (neck conv, image_encoder.py:96-103)
   using SM = GemmSmem<BN, STAGES>;
+  static_assert(Epi::kSplitCols, "the consumer warps split every tile into two column halves");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
 
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* accfree_bar = empty_bar + STAGES;     // the epilogue has read the staged accumulators
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
 
   const int num_m = (M + kGemmBM - 1) / kGemmBM;
   const int num_n = (N + BN - 1) / BN;
@@ -478,27 +500,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kGemmEpiWarps);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], Epi::kSplitCols ? 8 : 4);
-    }
+    mbar_init(accfree_bar, kGemmEpiWarps);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 2 * BN);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
       int stage = 0;
-      uint32_t phase = 0;
+      uint32_t phase = 0, accphase = 0;
+      bool first = true;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile / num_n, n_blk = tile % num_n;
+        if (!first) {                      // the ring holds the previous tile's accumulators
+          mbar_wait(accfree_bar, accphase);
+          accphase ^= 1u;
+        }
+        first = false;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u);
           uint8_t* sa = smem + stage * SM::kStageBytes;
@@ -518,74 +540,69 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(kGemmBM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[as], aphase ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(as * BN);
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem + stage * SM::kStageBytes);
-          const uint64_t adesc = umma_desc_k128(a_addr);
-          const uint64_t bdesc = umma_desc_k128(a_addr + SM::kABytes);
-#pragma unroll
-          for (int k = 0; k < kGemmBK / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the 128B swizzle atom: +2 in addr>>4 units
-            umma_f16_ss(tmem_d, adesc + static_cast<uint64_t>(2 * k),
-                        bdesc + static_cast<uint64_t>(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(&tfull_bar[as]);
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
-      }
-    }
   } else {
-    // ===================== epilogue warps (2..9) =====================
-    const int q = warp & 3;            // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;  // which half of the tile's columns (streaming epilogues)
-    if (Epi::kSplitCols || half == 0) {
-      float* scratch = reinterpret_cast<float*>(smem + SM::kScratchOffset) +
-                       (warp - 2) * kGemmScratchFloats;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / num_n, n_blk = tile % num_n;
-        mbar_wait(&tfull_bar[as], aphase);
-        tc_fence_after_sync();
-        const int m0 = m_blk * kGemmBM + q * 32;
-        const int n_tile = min(BN, N - n_blk * BN);        // valid columns of this tile
-        int col0 = 0, n_cols = n_tile;
-        if (Epi::kSplitCols) {
-          col0 = half * (BN / 2);
-          n_cols = max(0, min(BN / 2, n_tile - col0));
-        }
-        TmemRow row{tmem_base + (static_cast<uint32_t>(q * 32) << 16) +
-                    static_cast<uint32_t>(as * BN + col0)};
-        Epi::run(ep, m0, M, n_blk * BN + col0, n_cols, row, scratch, lane);
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[as]);
-        as ^= 1;
-        if (as == 0) aphase ^= 1u;
+    // ===================== consumers: MMA + epilogue =====================
+    setmaxnreg_inc<232>();
+    const int g = wg - 1;                      // consumer index: tile rows 64g .. 64g+63
+    const int w = warp & 3;                    // warp inside the warpgroup
+    const int q = 2 * g + (w & 1);             // epilogue row quarter
+    const int half = w >> 1;                   // epilogue column half
+    float* scratch = reinterpret_cast<float*>(smem + SM::kScratchOffset) + (half * 4 + q) * kGemmScratchFloats;
+    float* accs = reinterpret_cast<float*>(smem);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m_blk = tile / num_n, n_blk = tile % num_n;
+      float d[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_k; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * SM::kStageBytes);
+        const uint64_t adesc = wgmma_desc_k128(a_addr + g * (64 * kGemmBK * 2));
+        const uint64_t bdesc = wgmma_desc_k128(a_addr + SM::kABytes);
+        wgmma_fence_operand(d);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kGemmBK / 16; ++k)
+          WgmmaTile<BN>::mma(d, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k),
+                             (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                       // the previous k-block's MMAs have read their stage
+        wgmma_fence_operand(d);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
-      if constexpr (std::is_same<Epi, EpiDecFinal>::value) EpiDecFinal::drain(lane);
+      wgmma_wait<0>();
+      wgmma_fence_operand(d);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      // both consumers are done with the ring: stage the accumulators there
+      named_bar_sync(5, 256);
+      {
+        const int r0 = 64 * g + 16 * w + (lane >> 2);
+        const int c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(accs + r0 * SM::kAccPitch + 8 * j + c0) = make_float2(d[4 * j], d[4 * j + 1]);
+          *reinterpret_cast<float2*>(accs + (r0 + 8) * SM::kAccPitch + 8 * j + c0) =
+              make_float2(d[4 * j + 2], d[4 * j + 3]);
+        }
+      }
+      named_bar_sync(6 + g, 128);             // this consumer's 64 rows are staged
+      const int m0 = m_blk * kGemmBM + q * 32;
+      const int n_tile = min(BN, N - n_blk * BN);          // valid columns of this tile
+      const int col0 = half * (BN / 2);
+      const int n_cols = max(0, min(BN / 2, n_tile - col0));
+      AccRow row{accs + (q * 32 + lane) * SM::kAccPitch + col0};
+      Epi::run(ep, m0, M, n_blk * BN + col0, n_cols, row, scratch, lane);
+      fence_proxy_async_smem();               // generic accesses before the next TMA writes
+      __syncwarp();
+      if (lane == 0) mbar_arrive(accfree_bar);
     }
+    if constexpr (std::is_same<Epi, EpiDecFinal>::value) EpiDecFinal::drain(lane);
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 2 * BN);
 }
 
 // ------------------------------------------------------------------------------------------------

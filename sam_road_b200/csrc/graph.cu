@@ -1,7 +1,7 @@
 // sam_road_b200 :: graph.cu -- the middle and the tail of inferencer.infer_one_img on the device.
 //
 // The reference runs three pieces of host code between / after its two model passes (SURVEY.md §8f
-// rows 1-2); at B200 tile rates they are the critical path of a scene, so they live here:
+// rows 1-2); at GPU tile rates they are the critical path of a scene, so they live here:
 //   * keypoint extraction   graph_extraction.extract_graph_points  graph_extraction.py:24-28,130-139
 //                           graph_utils.nms_points                 graph_utils.py:572-591
 //   * pair-query build      inferencer.py:126-197 (rtree box query + KDTree kNN per tile)

@@ -38,7 +38,6 @@ struct BlockW {
   __half* qkv_w;  float* qkv_b;
   __half* proj_w; float* proj_b;
   float *rel_h, *rel_w;
-  __half* rel_tab;   // packed [rel_pos_h ; rel_pos_w] fp16 table for the tensor-core attention
   __half* lin1_w; float* lin1_b;
   __half* lin2_w; float* lin2_b;
   int win;   // attention window (14) or s for global blocks
@@ -383,7 +382,7 @@ extern "C" int samroad_create(const SamRoadCfg* cfg, int device, samroad_handle_
   SRB_CUDA_OK(cudaSetDevice(device));
   cudaDeviceProp prop;
   SRB_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  SRB_REQUIRE(prop.major == 10, "device %d is sm_%d%d; this library is built for sm_100a only",
+  SRB_REQUIRE(prop.major == 9 && prop.minor == 0, "device %d is sm_%d%d; this library is built for sm_90a only",
               device, prop.major, prop.minor);
   samroad_ctx* h = new samroad_ctx();
   h->cfg = *cfg;
@@ -500,18 +499,6 @@ extern "C" int samroad_finalize_weights(samroad_handle_t h) {
     b.proj_b = P.f32(K("attn.proj.bias"), {D});
     b.rel_h = P.f32(K("attn.rel_pos_h"), {rel_rows, hd});
     b.rel_w = P.f32(K("attn.rel_pos_w"), {rel_rows, hd});
-    b.rel_tab = nullptr;
-    if (P.ok && (hd == 64 || hd == 80)) {   // fp16 table [rows, 64 | 128] of the tensor-core attention
-      void* d = nullptr;
-      if (cudaMalloc(&d, 128 * 128 * sizeof(__half)) != cudaSuccess) {
-        P.fail("cudaMalloc of rel-pos table failed");
-      } else {
-        h->weight_allocs.push_back(d);
-        b.rel_tab = static_cast<__half*>(d);
-        if (pack_rel_table(b.rel_h, b.rel_w, b.win, static_cast<int>(hd), b.rel_tab, nullptr) != 0)
-          P.fail("pack_rel_table failed: %s", get_last_error());
-      }
-    }
     b.lin1_w = P.linear_w(K("mlp.lin1.weight"), 4 * D, D);
     b.lin1_b = P.f32(K("mlp.lin1.bias"), {4 * D});
     b.lin2_w = P.linear_w(K("mlp.lin2.weight"), D, 4 * D);
@@ -766,7 +753,7 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
           gemm_f16out(w.XN, D, b.qkv_w, D, M, 3 * D, D, b.qkv_b, ACT_NONE, w.QKV, 3 * D, st));
     turn();
     SRB_T(b.win == s ? KT_ATTN_GLOBAL : KT_ATTN_WINDOW, att_flops, Md * 4 * Dd * 2,
-          encoder_attention(w.QKV, b.qkv_b, b.rel_h, b.rel_w, b.rel_tab, B, s, b.win,
+          encoder_attention(w.QKV, b.qkv_b, b.rel_h, b.rel_w, B, s, b.win,
                             h->cfg.num_heads, h->hd, w.ATT, st));
     turn();
     SRB_T(KT_GEMM_PROJ, 2 * Md * Dd * Dd, Md * Dd * 2 + Md * Dd * 8,
@@ -892,7 +879,7 @@ extern "C" int samroad_toponet(samroad_handle_t h, const float* image_embeddings
           topo_pair_features(w.PST, h->tp_off_w, h->tp_pair_b, points, pts_dtype, pairs, pairs_dtype, B,
                              N, Ns, Np, zero_off, w.X32, w.X16, st));
   if (fused) {
-    // all three encoder layers + output_proj in one persistent tcgen05 kernel
+    // all three encoder layers + output_proj in one persistent wgmma kernel
     TopoFusedParams fp;
     for (int l = 0; l < 3; ++l) {
       const TopoLayerW& t = h->tp_layers[l];
@@ -1124,14 +1111,11 @@ extern "C" int samroad_op_layernorm(const float* x, const float* gamma, const fl
 extern "C" int samroad_op_attention(const void* qkv16, const float* qkv_bias, const float* rel_h,
                                     const float* rel_w, int B, int s, int win, int heads,
                                     int head_dim, void* out16, void* stream) {
-  return encoder_attention(static_cast<const __half*>(qkv16), qkv_bias, rel_h, rel_w, nullptr, B, s,
+  return encoder_attention(static_cast<const __half*>(qkv16), qkv_bias, rel_h, rel_w, B, s,
                            win, heads, head_dim, static_cast<__half*>(out16),
                            static_cast<cudaStream_t>(stream));
 }
 extern "C" void samroad_debug_force_simt_attention(int on) { attention_force_simt(on); }
 extern "C" void samroad_debug_set_traverse_reverse(int on) { set_traverse_reverse(on != 0); }
-extern "C" void samroad_debug_attention_trace(void* dev_buf) { attention_set_trace(static_cast<long long*>(dev_buf)); }
-extern "C" void samroad_debug_disable_2cta_gemm(int off) {
-  gemm_disable_2cta(off);
-  set_traverse_snake_enabled((off & 16) == 0);
-}
+extern "C" void samroad_debug_attention_trace(void* /*dev_buf*/) {}
+extern "C" void samroad_debug_disable_2cta_gemm(int off) { set_traverse_snake_enabled((off & 16) == 0); }

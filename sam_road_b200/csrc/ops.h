@@ -13,10 +13,8 @@ enum Act : int {
   ACT_GELU_SCALAR = 4,         // same function, one element per instruction (A/B timing only)
   // tools/gemm_probe.py only: epilogue ablations that do NOT produce the result
   ACT_PROBE_SKIP = 100,        // release the accumulator untouched (main-loop ceiling)
-  ACT_PROBE_TMEM = 101,        // TMEM loads only
-  ACT_PROBE_NOSTORE = 102,     // full GELU epilogue without the global stores
-  ACT_PROBE_NOTMA = 0x80,      // flag (2-CTA fp16 epilogue): everything but the TMA store (no output)
-  ACT_PROBE_DIRECT = 0x40      // flag (2-CTA fp16 epilogue): registers -> st.global instead of smem + TMA store
+  ACT_PROBE_ACC = 101,         // accumulator reads only
+  ACT_PROBE_NOSTORE = 102      // full GELU epilogue without the global stores
 };
 
 void set_last_error(const char* fmt, ...);
@@ -44,7 +42,6 @@ int gemm_dec_final(const __half* A, int lda, const __half* W, int ldw, int M, in
                    const float* bias3, const float* w4, const float* bias4, int s, int P,
                    float* scores, float* logits, cudaStream_t st);
 // plain SIMT fp32-accumulate GEMM used only by the on-device unit tests as an independent checker
-void gemm_disable_2cta(int mode);   // test hook: bit 0 forces the 1-CTA kernels, bit 1 the register-path fp32 epilogue
 int gemm_ref_simt(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
                   float* out, int ldo, cudaStream_t st);
 
@@ -65,18 +62,11 @@ int convert_f32_f16(const float* x, long n, __half* out, cudaStream_t st);
 // qkv: [B*s*s, 3*D] fp16, columns (q|k|v) x head x hd ; out: [B*s*s, D] fp16.
 // win == s means global attention; otherwise window attention over zero-padded LN output, whose pad
 // tokens have q=k=v=bias (image_encoder.py:168-172,227).  rel_h/rel_w: [2*win-1, hd] fp32.
-// rel_tab (optional): fp16 [64 or 128, 64] = [rel_pos_h ; rel_pos_w ; 0] as packed by
-// pack_rel_table(); when null the launcher packs it on the fly into a per-device scratch.
 int encoder_attention(const __half* qkv, const float* qkv_bias, const float* rel_h,
-                      const float* rel_w, const __half* rel_tab, int B, int s, int win, int heads,
-                      int hd, __half* out, cudaStream_t st);
-// rows of the packed table for a window size: each half holds 2*win-1 rows (64 / 128 / 256 rows in all)
-inline int rel_table_rows(int win) { return 4 * win - 2 <= 64 ? 64 : (4 * win - 2 <= 128 ? 128 : 256); }
-int pack_rel_table(const float* rel_h, const float* rel_w, int win, int hd, __half* tab,
-                   cudaStream_t st);
-// force the SIMT v1 attention kernel (tests use it as the independent on-device checker)
-void attention_force_simt(int mode);   // bit 0: SIMT kernel, bit 1: tcgen05 kernel with 1-in-4 polynomial exps, bit 2: half-block stagger, bit 3: no MUFU turn-taking
-void attention_set_trace(long long* device_buffer_128);   // debug: per-phase clock64 stamps of CTA 0
+                      const float* rel_w, int B, int s, int win, int heads, int hd, __half* out,
+                      cudaStream_t st);
+// force the SIMT attention kernel (tests use it as the independent on-device checker)
+void attention_force_simt(int mode);   // bit 0: SIMT kernel
 
 // ---- TopoNet pieces (toponet.cu) -----------------------------------------------------------------------------
 // points dtype: 0 = float32, 1 = int64, 2 = int32 ; pairs dtype: 1 = int64, 2 = int32

@@ -2,7 +2,7 @@
 // sam/segment_anything/modeling/{mask_decoder.py:112-149, transformer.py:62-240,
 // prompt_encoder.py:128-205}).
 //   * image side ([B*T,256] tokens): k/v/q projections, the image->token out_proj + norm4 and the
-//     ConvTranspose upscaler run on the tcgen05 GEMM (gemm_ops.cu) with fused LN / GELU epilogues;
+//     ConvTranspose upscaler run on the wgmma GEMM (gemm_ops.cu) with fused LN / GELU epilogues;
 //   * token side (4 output tokens per image): the tokens of ALL images form one [4B, 256] fp32 matrix; every
 //     linear layer is one small fp32 GEMM over it (weights read once for the whole batch instead of once
 //     per image), self-attention / token->image attention (online softmax over T keys) / LayerNorm are

@@ -4,27 +4,24 @@
 // Per layer (torch TransformerEncoderLayer, d=128, 4 heads, ff=128, relu, LN eps 1e-5, eval mode):
 //   qkv = x W_in^T + b_in -> per-sample 16x16 masked attention per head -> x = LN1(x + att W_o^T + b_o)
 //   -> x = LN2(x + relu(x W_1^T + b_1) W_2^T + b_2)
-// The four GEMMs run on tcgen05 (UMMA 128x128x16, fp16 operands, fp32 in TMEM); everything between
-// them stays on chip:
-//   TMEM  cols [0,384)   GEMM accumulators (q|k|v, later out_proj / lin1 / lin2 in [0,128))
-//         cols [384,512) the fp32 residual stream x of the tile (one token per lane)
+// Everything between the GEMMs stays on chip:
+//   registers  the fp32 residual stream x (a token thread keeps its 32 columns of the row)
 //   smem  A buffer 32 KB  current fp16 GEMM A operand (x -> attention output -> x' -> hidden -> x'')
-//         KV buffer 66 KB k and v of the tile as fp16 rows
+//         KV buffer 66 KB k and v of the tile as fp16 rows; after the attention, the fp32 [128][132]
+//                         staging area of the out_proj / linear2 results
 //         weight ring 3 x 32 KB  the 18 [128x128] weight chunks streamed by TMA in consumption order
-// Warps: 0 = TMA producer, 1 = MMA issuer + TMEM allocator, 2..17 = 512 token threads, FOUR per token
-// (warps w, w+4, w+8, w+12 share a TMEM lane quarter): epilogues, attention, LayerNorm, output_proj.
-// Part p owns columns 32p..32p+31 = head p, and two of the eight 32-column chunks of k|v; a thread
-// keeps its 32 columns of the row in registers through a whole LayerNorm (one TMEM read, one write).
-// LayerNorm statistics and the output dot product are combined through a small smem exchange, always
-// summed in part order.  The 16 x 16 x 32 attention of a (sample, head) is far too small for a UMMA
-// tile and runs on warp-level mma.sync: a warp owns two samples of its head; q (bias, 1/sqrt(32),
-// fp16) is staged in the warp's own rows of the A buffer, k / v fragments come from the k|v rows by
-// ldmatrix / ldmatrix.trans, softmax in fp32 on the S fragments, P (fp16) feeds the PV mma from
-// registers.  The token work, not the GEMMs, bounds this kernel, and it is bound by latency (one tile
-// in flight per CTA, phases separated by the MMA round trips): four warps per scheduler hide twice
-// the latency of two (one -> two threads per token was 1.58x in round 1, two -> four 1.34x, attention
-// on mma.sync another 1.36x).  Key-padding semantics (SURVEY.md §8a P4): masked keys are excluded from
-// the softmax; masked slots report output_proj.bias.
+// Warps 0..15 = 512 token threads in four warpgroups, warp 16 = TMA producer.  Warpgroup g owns
+// columns 32g..32g+31 = head g: it computes them for every GEMM on wgmma (two m64 x n32 x k16 per
+// k-step, A and the weight chunk read from 128B-swizzled smem), and as token threads its warp q holds
+// rows 32q..32q+31 (one per lane) of the same columns.  So the accumulators reach the token threads
+// through a warpgroup-local smem exchange, and only the A operand, which every warpgroup reads whole,
+// needs the 512-thread barrier.  LayerNorm statistics and the output dot product are combined across
+// the four warpgroups through a small smem exchange per row quarter, always summed in part order.
+// The 16 x 16 x 32 attention of a (sample, head) runs on warp-level mma.sync: a warp owns two
+// samples of its head; q (bias, 1/sqrt(32), fp16) is staged in the warp's own rows of the A buffer,
+// k / v fragments come from the k|v rows by ldmatrix / ldmatrix.trans, softmax in fp32 on the S
+// fragments, P (fp16) feeds the PV mma from registers.  Key-padding semantics (SURVEY.md §8a P4):
+// masked keys are excluded from the softmax; masked slots report output_proj.bias.
 #pragma once
 
 #include "common.cuh"
@@ -32,17 +29,22 @@
 
 namespace srb {
 
-constexpr int kTtcThreads = 576;          // 2 + 16 warps
+constexpr int kTtcThreads = 544;          // 16 token warps + 1 producer warp
 constexpr int kTtcTokenThreads = 512;
 constexpr int kTtcWStages = 3;
 constexpr int kTtcOffA = 0;                       // 2 k-blocks x 16 KB
 constexpr int kTtcOffKV = 32768;                  // 128 rows x 528 B (k|v fp16, padded: ldmatrix rows hit 32 banks)
 constexpr int kTtcKVStride = 528;
+constexpr int kTtcStgPitch = 132;                 // fp32 staging rows (overlays the KV buffer)
+static_assert(128 * kTtcStgPitch * 4 <= 68608, "staging must fit the KV buffer");
 constexpr int kTtcOffW = kTtcOffKV + 68608;       // 3 x 32 KB
 constexpr int kTtcOffBar = kTtcOffW + kTtcWStages * 32768;
 constexpr int kTtcOffXch = kTtcOffBar + 256;      // 3 slots x 4 parts x 128 floats: partial sums of the parts
 constexpr int kTtcSmemBytes = kTtcOffXch + 3 * 2048 + 1024;
-constexpr int kTtcChunksPerLayer = 6;             // Wq, Wk, Wv, Wo, W1, W2
+constexpr int kTtcChunksPerLayer = 6;             // Wq, Wk, Wv, Wo, W1, W2 as packed
+// consumption order of a layer's chunks: k and v first, q last (q is written into the A buffer,
+// which may only happen once every warpgroup has finished the in_proj GEMMs)
+__host__ __device__ constexpr int ttc_chunk(int i) { return i == 0 ? 1 : (i == 1 ? 2 : (i == 2 ? 0 : i)); }
 
 struct TtcLayerParams {
   const float* in_b;    // [384]
@@ -98,15 +100,36 @@ __device__ __forceinline__ void ttc_mma_16816(float (&d)[4], const uint32_t (&a)
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// Everything the token threads exchange through shared memory stays inside a TMEM lane quarter: the four
-// threads of a row (one per part) sit in the four warps of the same quarter, and a warp's two samples
-// are rows of its own quarter.  So the barriers are per quarter (ids 1..4, 128 threads each), and the
-// quarters only meet at the a_ready mbarrier of the next GEMM.
+
+// named barriers: 1 = all 512 token threads, 2..5 = row quarter q (its warps in the four warpgroups),
+// 6..9 = warpgroup g
+__device__ __forceinline__ void ttc_bar_all() { asm volatile("bar.sync 1, 512;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync_quarter(int quarter) {
-  asm volatile("bar.sync %0, 128;" ::"r"(quarter + 1) : "memory");
+  asm volatile("bar.sync %0, 128;" ::"r"(quarter + 2) : "memory");
+}
+__device__ __forceinline__ void ttc_bar_group(int g) {
+  asm volatile("bar.sync %0, 128;" ::"r"(g + 6) : "memory");
 }
 
-__global__ void __launch_bounds__(kTtcThreads, 1)   // 18 warps: 5 on two of the sub-partitions -> 96 registers
+// D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t desc_a, uint64_t desc_b,
+                                             uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1, 0, 0;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+
+__global__ void __launch_bounds__(kTtcThreads, 1)
 toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -114,35 +137,28 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
   uint8_t* sA = smem + kTtcOffA;
   uint8_t* sKV = smem + kTtcOffKV;
   uint8_t* sW = smem + kTtcOffW;
+  float* stg = reinterpret_cast<float*>(sKV);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kTtcOffBar);
-  uint64_t* a_ready = bars + 2;     // 512 token threads: new A operand written
-  uint64_t* acc_ready = bars + 3;   // MMA commit: GEMM result in TMEM
-  uint64_t* w_full = bars + 4;      // [3]
-  uint64_t* w_empty = bars + 7;     // [3]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
+  uint64_t* w_full = bars;          // [3]
+  uint64_t* w_empty = bars + 3;     // [3]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 16 && lane == 0) {
     tma_prefetch_desc(&tmW);
-    mbar_init(a_ready, kTtcTokenThreads);
-    mbar_init(acc_ready, 1);
-    for (int i = 0; i < kTtcWStages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 1); }
+    for (int i = 0; i < kTtcWStages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 4); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 16) {
     // =========================== TMA producer ===========================
     if (lane == 0) {
       int wc = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        for (int ch = 0; ch < 3 * kTtcChunksPerLayer; ++ch, ++wc) {
+        for (int i = 0; i < 3 * kTtcChunksPerLayer; ++i, ++wc) {
+          const int ch = (i / kTtcChunksPerLayer) * kTtcChunksPerLayer + ttc_chunk(i % kTtcChunksPerLayer);
           const int st = wc % kTtcWStages;
           mbar_wait(&w_empty[st], ((wc / kTtcWStages) & 1) ^ 1u);
           mbar_arrive_expect_tx(&w_full[st], 32768);
@@ -151,142 +167,141 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(128, 128);
-      int wc = 0, ac = 0;   // weight chunks consumed, a_ready completions consumed
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        for (int l = 0; l < 3; ++l) {
-          for (int gemm = 0; gemm < 4; ++gemm) {          // 0: in_proj (3 chunks), 1: out, 2: lin1, 3: lin2
-            // every GEMM reads an A operand the token threads have just written (the first one of a
-            // tile: the pair features) and overwrites accumulator columns they read in the previous
-            // step: each waits for their a_ready arrival
-            mbar_wait(a_ready, ac & 1);
-            ++ac;
-            tc_fence_after_sync();
-            const int nch = gemm == 0 ? 3 : 1;
-            for (int j = 0; j < nch; ++j, ++wc) {
-              const int st = wc % kTtcWStages;
-              mbar_wait(&w_full[st], (wc / kTtcWStages) & 1);
-              tc_fence_after_sync();
-              const uint32_t abase = smem_u32(sA), wbase = smem_u32(sW + st * 32768);
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                const uint64_t adesc = umma_desc_k128(abase + (k >> 2) * 16384) + 2 * (k & 3);
-                const uint64_t bdesc = umma_desc_k128(wbase + (k >> 2) * 16384) + 2 * (k & 3);
-                umma_f16_ss(tmem_base + j * 128, adesc, bdesc, idesc, k != 0 ? 1u : 0u);
-              }
-              umma_commit(&w_empty[st]);
-            }
-            umma_commit(acc_ready);
-          }
-        }
-      }
-    }
-  } else {
-    // =========================== token threads ===========================
-    const int quarter = warp & 3;
-    const int part = (warp - 2) >> 2;                 // 0..3: columns 32*part .. 32*part+31, head `part`
-    const int row = quarter * 32 + lane;
-    const uint32_t tlane = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t tAcc = tmem_base + tlane;          // cols [0,384)
-    const uint32_t tRes = tmem_base + tlane + 384;    // cols [384,512)
-    const int sw = row & 7;
-    uint8_t* myA = sA + row * 128;
-    float* xch = reinterpret_cast<float*>(smem + kTtcOffXch);   // [3][4 parts][128 rows]
-    int ti = 0, rc = 0;                               // tiles, acc_ready completions consumed
+    return;
+  }
 
-    auto write_a_chunk = [&](int c, const float (&v)[32]) {   // 32 fp32 -> fp16 into the swizzled A buffer
-      uint8_t* dst = myA + (c >> 1) * 16384;
+  // =========================== token threads / MMA warpgroups ===========================
+  const int quarter = warp & 3;
+  const int part = warp >> 2;                       // warpgroup; columns 32*part .. +31, head `part`
+  const int row = quarter * 32 + lane;
+  const int sw = row & 7;
+  uint8_t* myA = sA + row * 128;
+  float* xch = reinterpret_cast<float*>(smem + kTtcOffXch);   // [3][4 parts][128 rows]
+  // accumulator fragment coordinates (wgmma m64nN): rows fr0 (+8) (+64 for the second product),
+  // columns 8j + fc (+1) of this warpgroup's 32
+  const int fr0 = quarter * 16 + (lane >> 2), fc = 2 * (lane & 3);
+  int ti = 0, wc = 0;
+
+  auto write_a_chunk = [&](int c, const float (&v)[32]) {   // 32 fp32 -> fp16 into the swizzled A buffer
+    uint8_t* dst = myA + (c >> 1) * 16384;
 #pragma unroll
-      for (int q4 = 0; q4 < 4; ++q4) {
-        uint4 u;
-        u.x = pack_half2(v[q4 * 8 + 0], v[q4 * 8 + 1]);
-        u.y = pack_half2(v[q4 * 8 + 2], v[q4 * 8 + 3]);
-        u.z = pack_half2(v[q4 * 8 + 4], v[q4 * 8 + 5]);
-        u.w = pack_half2(v[q4 * 8 + 6], v[q4 * 8 + 7]);
-        *reinterpret_cast<uint4*>(dst + ((((c & 1) * 4 + q4) ^ sw) << 4)) = u;
+    for (int q4 = 0; q4 < 4; ++q4) {
+      uint4 u;
+      u.x = pack_half2(v[q4 * 8 + 0], v[q4 * 8 + 1]);
+      u.y = pack_half2(v[q4 * 8 + 2], v[q4 * 8 + 3]);
+      u.z = pack_half2(v[q4 * 8 + 4], v[q4 * 8 + 5]);
+      u.w = pack_half2(v[q4 * 8 + 6], v[q4 * 8 + 7]);
+      *reinterpret_cast<uint4*>(dst + ((((c & 1) * 4 + q4) ^ sw) << 4)) = u;
+    }
+  };
+  // fp16 pair (columns 32h + 8j + fc, +1) of tile row r into the swizzled A buffer
+  auto a_pair = [&](int r, int h, int j) -> uint32_t* {
+    return reinterpret_cast<uint32_t*>(sA + (h >> 1) * 16384 + r * 128 + ((((h & 1) * 4 + j) ^ (r & 7)) << 4) + fc * 2);
+  };
+  // the four parts' partials of the same row, summed in part order (slot: 0 sum, 1 var, 2 dot): every
+  // thread of a row gets the same value
+  auto combine = [&](int slot, float mine) -> float {
+    float* x = xch + slot * 512 + row;
+    x[part * 128] = mine;
+    named_bar_sync_quarter(quarter);
+    return ((x[0] + x[128]) + x[256]) + x[384];
+  };
+  auto ldg32 = [&](const float* src, float (&v)[32]) {     // 32 consecutive floats (128 B aligned)
+    const float4* s4 = reinterpret_cast<const float4*>(src);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float4 t = __ldg(s4 + i);
+      v[4 * i + 0] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+    }
+  };
+  // this warpgroup's 32 output columns of the next weight chunk for all 128 rows: acc[h] = rows 64h..
+  auto gemm = [&](float (&acc)[2][16]) {
+    const int st = wc % kTtcWStages;
+    mbar_wait(&w_full[st], (wc / kTtcWStages) & 1);
+    const uint32_t abase = smem_u32(sA), wbase = smem_u32(sW + st * 32768) + part * 32 * 128;
+    wgmma_fence_operand(acc[0]);
+    wgmma_fence_operand(acc[1]);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const uint64_t bdesc = wgmma_desc_k128(wbase + (k >> 2) * 16384) + 2 * (k & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        wgmma_m64n32k16(acc[h], wgmma_desc_k128(abase + (k >> 2) * 16384 + h * 8192) + 2 * (k & 3), bdesc,
+                        k != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(acc[0]);
+    wgmma_fence_operand(acc[1]);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&w_empty[st]);
+    ++wc;
+  };
+  // accumulators -> fp32 staging rows (this warpgroup's columns), then visible to its token threads
+  auto stage = [&](const float (&acc)[2][16]) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int r = h * 64 + fr0, c = part * 32 + 8 * j + fc;
+        *reinterpret_cast<float2*>(stg + r * kTtcStgPitch + c) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+        *reinterpret_cast<float2*>(stg + (r + 8) * kTtcStgPitch + c) =
+            make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
       }
-    };
-    auto ld_chunk = [&](uint32_t taddr, float (&v)[32]) {
-      uint32_t r[32];
-      tmem_ld_32x32(taddr, r);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-    };
-    auto st_chunk = [&](uint32_t taddr, const float (&v)[32]) {
-      uint32_t r[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(v[i]);
-      tmem_st_32x32(taddr, r);
-    };
-    // the four parts' partials of the same row, summed in part order (slot: 0 sum, 1 var, 2 dot): every
-    // thread of a row gets the same value
-    auto combine = [&](int slot, float mine) -> float {
-      float* x = xch + slot * 512 + row;
-      x[part * 128] = mine;
-      named_bar_sync_quarter(quarter);
-      return ((x[0] + x[128]) + x[256]) + x[384];
-    };
-    auto ldg32 = [&](const float* src, float (&v)[32]) {     // 32 consecutive floats (128 B aligned)
-      const float4* s4 = reinterpret_cast<const float4*>(src);
+    ttc_bar_group(part);
+  };
+  float res[32];                                    // residual stream: row `row`, columns 32*part ..
+  // x = LayerNorm(res + acc + bias) ; res <- x ; optionally A buffer <- fp16(x); returns x.w_out
+  // (this part's 32 columns; exact two-pass statistics over the whole row).  acc is in the staging rows.
+  auto residual_layernorm = [&](const float* bias, const float* gamma, const float* beta,
+                                bool write_a, const float* wdot) -> float {
+    const int c = part;
+    float r[32];
+    float sum = 0.f;
+    {
+      float bv[32];
+      ldg32(bias + c * 32, bv);
+      const float4* s4 = reinterpret_cast<const float4*>(stg + row * kTtcStgPitch + c * 32);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float4 t = __ldg(s4 + i);
-        v[4 * i + 0] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+        const float4 a = s4[i];
+        r[4 * i + 0] = res[4 * i + 0] + (a.x + bv[4 * i + 0]);
+        r[4 * i + 1] = res[4 * i + 1] + (a.y + bv[4 * i + 1]);
+        r[4 * i + 2] = res[4 * i + 2] + (a.z + bv[4 * i + 2]);
+        r[4 * i + 3] = res[4 * i + 3] + (a.w + bv[4 * i + 3]);
       }
-    };
-    // x = LayerNorm(res + acc + bias) ; res <- x ; optionally A buffer <- fp16(x); returns x.w_out
-    // (this part's 32 columns, held in registers; exact two-pass statistics over the whole row)
-    auto residual_layernorm = [&](const float* bias, const float* gamma, const float* beta,
-                                  bool write_a, const float* wdot) -> float {
-      const int c = part;
-      float r[32];
-      float sum = 0.f;
-      {
-        uint32_t ua[32], ur[32];
-        tmem_ld_32x32_nowait(tAcc + c * 32, ua);
-        tmem_ld_32x32_nowait(tRes + c * 32, ur);
-        float bv[32];
-        ldg32(bias + c * 32, bv);
-        tmem_ld_wait();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          r[i] = __uint_as_float(ur[i]) + (__uint_as_float(ua[i]) + bv[i]);
-          sum += r[i];
-        }
+      for (int i = 0; i < 32; ++i) sum += r[i];
+    }
+    const float mean = combine(0, sum) * (1.0f / 128.0f);
+    float var = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float d = r[i] - mean;
+      var = fmaf(d, d, var);
+    }
+    const float rstd = rsqrtf(combine(1, var) * (1.0f / 128.0f) + 1e-5f);
+    float dot = 0.f;
+    {
+      float gv[32], bt[32];
+      ldg32(gamma + c * 32, gv);
+      ldg32(beta + c * 32, bt);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) r[i] = (r[i] - mean) * rstd * gv[i] + bt[i];
+      if (wdot) {
+        ldg32(wdot + c * 32, gv);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) dot = fmaf(r[i], gv[i], dot);
       }
-      const float mean = combine(0, sum) * (1.0f / 128.0f);
-      float var = 0.f;
+    }
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const float d = r[i] - mean;
-        var = fmaf(d, d, var);
-      }
-      const float rstd = rsqrtf(combine(1, var) * (1.0f / 128.0f) + 1e-5f);
-      float dot = 0.f;
-      {
-        float gv[32], bt[32];
-        ldg32(gamma + c * 32, gv);
-        ldg32(beta + c * 32, bt);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) r[i] = (r[i] - mean) * rstd * gv[i] + bt[i];
-        if (wdot) {
-          ldg32(wdot + c * 32, gv);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) dot = fmaf(r[i], gv[i], dot);
-        }
-      }
-      st_chunk(tRes + c * 32, r);
-      if (write_a) write_a_chunk(c, r);
-      tmem_st_wait();
-      return dot;
-    };
+    for (int i = 0; i < 32; ++i) res[i] = r[i];
+    if (write_a) write_a_chunk(c, r);
+    return dot;
+  };
 
-    // source / target rows and offset of this thread's pair token in tile `t` (index -> address chain
-    // of the gather; issued one tile ahead so that only the pst loads themselves are exposed)
+  // source / target rows and offset of this thread's pair token in tile `t` (index -> address chain
+  // of the gather; issued one tile ahead so that only the pst loads themselves are exposed)
     float nx_ox = 0.f, nx_oy = 0.f;
     size_t nx_ps = 0, nx_pt = 0;
     auto pair_lookup = [&](int t) {
@@ -306,7 +321,7 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
         }
       }
     };
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++ti) {
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++ti) {
       const long tok = static_cast<long>(tile) * 128 + row;
       const bool tok_ok = tok < p.tokens;
       // key-validity bits of this token's sample (16 consecutive tokens)
@@ -322,11 +337,11 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
         my_valid = tok_ok && p.valid[tok];
       }
 
-      // ---- pair features of this token -> TMEM residual (fp32) and A buffer (fp16) ----
-      {
-        if (ti == 0) pair_lookup(tile);              // later tiles: looked up during the previous tile
-        const float ox = nx_ox, oy = nx_oy;
-        const size_t ps = nx_ps, pt = nx_pt;
+    // ---- pair features of this token -> residual (fp32 registers) and A buffer (fp16) ----
+    {
+      if (ti == 0) pair_lookup(tile);              // later tiles: looked up during the previous tile
+      const float ox = nx_ox, oy = nx_oy;
+      const size_t ps = nx_ps, pt = nx_pt;
         {
           const int c = part;
           float v[32];
@@ -348,69 +363,63 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
             v[4 * i + 2] = tok_ok ? fmaxf(x2, 0.f) : 0.f;
             v[4 * i + 3] = tok_ok ? fmaxf(x3, 0.f) : 0.f;
           }
-          st_chunk(tRes + c * 32, v);
+#pragma unroll
+          for (int i = 0; i < 32; ++i) res[i] = v[i];
           write_a_chunk(c, v);
         }
-        tmem_st_wait();
-        tc_fence_before_sync();
-        fence_proxy_async_smem();
-        mbar_arrive(a_ready);
-      }
+    }
+    fence_proxy_async_smem();
+    ttc_bar_all();
 
-      float dot = 0.f;
+    float dot = 0.f;
 #pragma unroll 1
-      for (int l = 0; l < 3; ++l) {
-        const TtcLayerParams& L = p.layer[l];
-        // ================= qkv: k, v -> smem (fp16 rows), attention per head =================
-        mbar_wait(acc_ready, rc & 1); ++rc;
-        tc_fence_after_sync();
-        {                                            // parts 0,1: k (cols 128..255), parts 2,3: v (cols 256..383)
-          uint32_t kv[2][32];
-          tmem_ld_32x32_nowait(tAcc + 128 + (part * 2 + 0) * 32, kv[0]);
-          tmem_ld_32x32_nowait(tAcc + 128 + (part * 2 + 1) * 32, kv[1]);
-          tmem_ld_wait();
+    for (int l = 0; l < 3; ++l) {
+      const TtcLayerParams& L = p.layer[l];
+      float acc[2][16];
+      // ================= in_proj: k, v of head `part` -> smem (fp16 rows, bias added) =================
+#pragma unroll 1
+      for (int kv = 0; kv < 2; ++kv) {
+        gemm(acc);
+        const int c = kv * 4 + part;               // 32-column chunk of the k|v rows
+        const float* bias = L.in_b + 128 + c * 32;
 #pragma unroll
-          for (int cc = 0; cc < 2; ++cc) {
-            const int c = part * 2 + cc;
-            uint8_t* dst = sKV + row * kTtcKVStride + ((c * 64) ^ (((row >> 4) & 1) << 6));
-            const float4* b4 = reinterpret_cast<const float4*>(L.in_b + 128 + c * 32);
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4) {
-              const float4 b0 = __ldg(b4 + 2 * q4), b1 = __ldg(b4 + 2 * q4 + 1);
-              const uint32_t* v = kv[cc] + q4 * 8;
-              uint4 u;
-              u.x = pack_half2(__uint_as_float(v[0]) + b0.x, __uint_as_float(v[1]) + b0.y);
-              u.y = pack_half2(__uint_as_float(v[2]) + b0.z, __uint_as_float(v[3]) + b0.w);
-              u.z = pack_half2(__uint_as_float(v[4]) + b1.x, __uint_as_float(v[5]) + b1.y);
-              u.w = pack_half2(__uint_as_float(v[6]) + b1.z, __uint_as_float(v[7]) + b1.w);
-              *reinterpret_cast<uint4*>(dst + q4 * 16) = u;
+          for (int j = 0; j < 4; ++j) {
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + fc));
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int r = h * 64 + fr0 + 8 * e;
+              const int sxs = ((r >> 4) & 1) << 6;
+              *reinterpret_cast<uint32_t*>(sKV + r * kTtcKVStride + ((c * 64) ^ sxs) + (8 * j + fc) * 2) =
+                  pack_half2(acc[h][4 * j + 2 * e] + bb.x, acc[h][4 * j + 2 * e + 1] + bb.y);
             }
           }
-        }
-        {
-          // ---- attention of head `part` for the warp's two samples on mma.sync (16 queries x 16 keys x
-          // 32 dims per sample): q (bias added, scaled, fp16) is staged in the warp's own rows of the A
-          // buffer -- the 64 B chunk (row, h) the attention output overwrites afterwards --, k and v come
-          // straight from their smem rows through ldmatrix, P stays in registers (S fragments -> A
-          // fragments), O is normalised and stored as the out_proj A operand.
-          const int h = part;
-          {
-            uint32_t q[32];
-            tmem_ld_32x32_nowait(tAcc + h * 32, q);  // in flight across the barrier
-            named_bar_sync_quarter(quarter);         // the k and v rows of this quarter's samples are in smem
-            tmem_ld_wait();
-            float qs[32];
-            const float4* b4 = reinterpret_cast<const float4*>(L.in_b + h * 32);
+      }
+      // ================= in_proj: q of head `part` -> A buffer (bias, 1/sqrt(32), fp16) =================
+      gemm(acc);
+      ttc_bar_all();                               // every warpgroup has read the A operand
+      {
+        const float* bias = L.in_b + part * 32;
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {            // torch MHA scales q by 1/sqrt(head_dim)
-              const float4 bb = __ldg(b4 + i);
-              qs[4 * i + 0] = (__uint_as_float(q[4 * i + 0]) + bb.x) * 0.17677669529663687f;
-              qs[4 * i + 1] = (__uint_as_float(q[4 * i + 1]) + bb.y) * 0.17677669529663687f;
-              qs[4 * i + 2] = (__uint_as_float(q[4 * i + 2]) + bb.z) * 0.17677669529663687f;
-              qs[4 * i + 3] = (__uint_as_float(q[4 * i + 3]) + bb.w) * 0.17677669529663687f;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + fc));
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {            // torch MHA scales q by 1/sqrt(head_dim)
+              const int r = h * 64 + fr0 + 8 * e;
+              *a_pair(r, part, j) = pack_half2((acc[h][4 * j + 2 * e] + bb.x) * 0.17677669529663687f,
+                                               (acc[h][4 * j + 2 * e + 1] + bb.y) * 0.17677669529663687f);
             }
-            write_a_chunk(h, qs);
           }
+      }
+      ttc_bar_group(part);                         // q, k, v of head `part` are in smem
+      {
+        // ---- attention of head `part` for the warp's two samples on mma.sync (16 queries x 16 keys x
+        // 32 dims per sample): k and v come straight from their smem rows through ldmatrix, P stays in
+        // registers (S fragments -> A fragments), O is normalised and stored as the out_proj A operand.
+        const int h = part;
           __syncwarp();
           const int g8 = lane >> 2, t4 = lane & 3;   // fragment coordinates: row g8 (+8), column pair t4
           const int mi = lane >> 3, rr = lane & 7;   // ldmatrix: this lane addresses row rr of matrix mi
@@ -505,55 +514,55 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
             }
           }
         }
-        tc_fence_before_sync();
-        fence_proxy_async_smem();
-        mbar_arrive(a_ready);
-        // ================= out_proj + residual + LayerNorm1 =================
-        mbar_wait(acc_ready, rc & 1); ++rc;
-        tc_fence_after_sync();
-        residual_layernorm(L.out_b, L.n1_g, L.n1_b, true, nullptr);
-        tc_fence_before_sync();
-        fence_proxy_async_smem();
-        mbar_arrive(a_ready);
-        // ================= linear1 + relu =================
-        mbar_wait(acc_ready, rc & 1); ++rc;
-        tc_fence_after_sync();
-        {
-          const int c = part;
-          float v[32], bv[32];
-          ldg32(L.l1_b + c * 32, bv);
-          ld_chunk(tAcc + c * 32, v);
+      fence_proxy_async_smem();
+      ttc_bar_all();
+      // ================= out_proj + residual + LayerNorm1 =================
+      gemm(acc);
+      ttc_bar_all();                               // A operand read by every warpgroup
+      stage(acc);
+      residual_layernorm(L.out_b, L.n1_g, L.n1_b, true, nullptr);
+      fence_proxy_async_smem();
+      ttc_bar_all();
+      // ================= linear1 + relu =================
+      gemm(acc);
+      ttc_bar_all();
+      {
+        const float* bias = L.l1_b + part * 32;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i] + bv[i], 0.f);
-          write_a_chunk(c, v);
-        }
-        tc_fence_before_sync();
-        fence_proxy_async_smem();
-        mbar_arrive(a_ready);
-        if (l == 2) pair_lookup(tile + static_cast<int>(gridDim.x));   // next tile's indices, off the critical path
-        // ================= linear2 + residual + LayerNorm2 =================
-        mbar_wait(acc_ready, rc & 1); ++rc;
-        tc_fence_after_sync();
-        dot = residual_layernorm(L.l2_b, L.n2_g, L.n2_b, l < 2, l == 2 ? p.out_w : nullptr);
-        tc_fence_before_sync();
-        fence_proxy_async_smem();
-        if (l < 2) mbar_arrive(a_ready);   // after the last layer the next tile's pair features arrive
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + fc));
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int r = h * 64 + fr0 + 8 * e;
+              *a_pair(r, part, j) = pack_half2(fmaxf(acc[h][4 * j + 2 * e] + bb.x, 0.f),
+                                               fmaxf(acc[h][4 * j + 2 * e + 1] + bb.y, 0.f));
+            }
+          }
       }
-      // ================= output_proj + sigmoid =================
-      dot = combine(2, dot);
-      if (tok_ok && part == 0) {
-        const float b = __ldg(p.out_b);
-        const float lg = my_valid ? dot + b : b;
-        if (p.logits) p.logits[tok] = lg;
-        if (p.scores) p.scores[tok] = 1.0f / (1.0f + expf(-lg));
+      fence_proxy_async_smem();
+      ttc_bar_all();
+      if (l == 2) pair_lookup(tile + static_cast<int>(gridDim.x));   // next tile's indices, off the critical path
+      // ================= linear2 + residual + LayerNorm2 =================
+      gemm(acc);
+      ttc_bar_all();
+      stage(acc);
+      dot = residual_layernorm(L.l2_b, L.n2_g, L.n2_b, l < 2, l == 2 ? p.out_w : nullptr);
+      if (l < 2) {
+        fence_proxy_async_smem();
+        ttc_bar_all();
       }
-      tc_fence_before_sync();
+    }
+    // ================= output_proj + sigmoid =================
+    dot = combine(2, dot);
+    if (tok_ok && part == 0) {
+      const float b = __ldg(p.out_b);
+      const float lg = my_valid ? dot + b : b;
+      if (p.logits) p.logits[tok] = lg;
+      if (p.scores) p.scores[tok] = 1.0f / (1.0f + expf(-lg));
     }
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace srb

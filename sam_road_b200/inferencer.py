@@ -290,10 +290,9 @@ def infer_scenes(net, images, config, device: Optional[torch.device] = None,
     a background thread pulls the next images from the `images` iterable -- file reads and PNG decoding in the
     CLI -- while the GPU works on the current scene.  Results are infer_one_img's, in order.
 
-    The scenes themselves run back to back on one stream.  Enqueueing the next scene's encoder pass on a second
-    stream under the current scene's graph stage was measured and is NOT done: the encoder kernels are
-    persistent (they hold every SM for 0.2-0.5 ms at a time), so the ~60 small kernels and the read-backs of
-    the graph stage queue behind them, and a C2 scene went from 86.5 to 96.4 ms (DESIGN.md §8)."""
+    The scenes themselves run back to back on one stream.  The next scene's encoder pass is not enqueued on a
+    second stream under the current scene's graph stage: the encoder GEMMs are persistent (one CTA per SM), so
+    the ~60 small kernels and the read-backs of the graph stage would queue behind them."""
     import queue
     import threading
     device = _resolve_device(net, device)

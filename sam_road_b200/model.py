@@ -9,7 +9,7 @@ Mirrors the reference's model-level interface (reference model.py):
 with the same state_dict key set (SURVEY.md §8b), argument meaning and output shapes/dtypes.
 
 Host side is Python/PyTorch only as plumbing (parameters, device memory, streams); all model math
-runs in the hand-written sm_100a kernels behind the C ABI (include/samroad_b200.h).  There is no
+runs in the hand-written sm_90a kernels behind the C ABI (include/samroad_b200.h).  There is no
 PyTorch / CPU fallback: without the shared library or a CUDA device the calls raise.
 """
 from __future__ import annotations
@@ -176,7 +176,7 @@ except Exception:  # lightning is absent in this image; inference needs nothing 
 
 
 class SAMRoad(_Base):
-    """B200-native SAMRoad (inference only)."""
+    """H100-native SAMRoad (inference only)."""
 
     def __init__(self, config):
         super().__init__()
@@ -257,7 +257,7 @@ class SAMRoad(_Base):
     def _handle(self, device: torch.device) -> int:
         if device.type != "cuda":
             raise RuntimeError(
-                f"sam_road_b200.SAMRoad runs on CUDA (sm_100a) only; got input on '{device}'. "
+                f"sam_road_b200.SAMRoad runs on CUDA (sm_90a) only; got input on '{device}'. "
                 "There is no CPU path.")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         lib = _lib.load()

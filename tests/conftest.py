@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200, sm_100a)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a)")
     config.addinivalue_line("markers", "slow: long-running CPU test")
 
 

@@ -115,10 +115,10 @@ def test_encode_and_topo_parity(name, patch, version, B, lora):
 
 
 def test_benched_configuration_b64_composition():
-    """The configuration bench.py times: ViT-B @512, B = 64 tiles in ONE call -- 2-CTA GEMMs, TMA
-    reduce-add shortcut epilogues, snake traversal, persistent attention CTAs running dozens of units.
+    """The configuration bench.py times: ViT-B @512, B = 64 tiles in ONE call -- persistent GEMM CTAs
+    running many tiles each, snake traversal, thousands of attention CTAs.
     (a) 4 of the 64 tiles against the oracle at the 1e-3 tolerance; (b) the same 4 tiles from a B = 4
-    call with every GEMM on the 1-CTA kernels and ascending traversal (debug mode 1|16), which must agree
+    call with ascending traversal (debug mode 1|16), which must agree
     with the B = 64 result to rounding (different tile shapes / epilogues round differently; how the
     variants relate bit-wise is recorded in the report); (c) a tile's result must not depend on where it
     sits in the batch: permuting the batch permutes the output bit for bit."""
@@ -221,7 +221,7 @@ def test_toponet_versions(topo):
 def test_toponet_dense_c4():
     """BASELINE config 4 (toponet_vitb_512_cityscale_8x8): dense TopoNet path -- 1024 keypoints per 512
     tile, every one of them a query with 16 neighbour slots (16 384 sequences of 16 per tile), ragged
-    validity as inferencer.py:156-176 builds it.  Fused tcgen05 kernel against the oracle."""
+    validity as inferencer.py:156-176 builds it.  Layered TopoNet path against the oracle."""
     cfg = _config(512)
     spec, sd, net = _build(cfg, seed=5)
     g = torch.Generator().manual_seed(12)

@@ -1,4 +1,4 @@
-"""Op-level determinism / correctness probe of the tcgen05 encoder attention: the same QKV through the
+"""Op-level determinism / correctness probe of the tensor-core encoder attention: the same QKV through the
 kernel several times, ascending and descending unit order, against the SIMT kernel.
     python tools/attention_probe.py"""
 import json

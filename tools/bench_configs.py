@@ -2,7 +2,7 @@
 C1/C3 tile shape (ViT-B @256), C4 (ViT-B @512, dense TopoNet: 1024 keypoints x 16 pairs per tile) and
 C5 (ViT-H @256, encoder + mask head).  Device-resident inputs, CUDA events, seeded random weights.
 
-    python tools/bench_configs.py [--steps 5] > profiles/r01_other_configs.json
+    python tools/bench_configs.py [--steps 5] > other_configs.json
 """
 import argparse
 import json
@@ -56,7 +56,7 @@ def main():
     a = ap.parse_args()
     out = [run("vitb_256 (C1/C3 tile shape) + TopoNet 64 keypoints", cfg(256), 256, 64, a.steps),
            run("vitb_512 dense TopoNet (C4: 1024 keypoints x 16 pairs)", cfg(512), 64, 1024, a.steps),
-           run("vith_256 encoder + mask head (C5; head_dim 80 tcgen05 attention)",
+           run("vith_256 encoder + mask head (C5; head_dim 80 tensor-core attention)",
                cfg(256, "vit_h"), 64, 0, a.steps)]
     print(json.dumps(out, indent=1))
 
