@@ -206,7 +206,8 @@ void attention_force_simt(int mode) { g_force_simt = (mode & 1) != 0; }
 int encoder_attention(const __half* qkv, const float* qkv_bias, const float* rel_h,
                       const float* rel_w, int B, int s, int win, int heads, int hd, __half* out,
                       cudaStream_t st) {
-  SRB_REQUIRE(win > 0 && win <= s && s <= 64, "attention: win=%d s=%d unsupported", win, s);
+  // win > s is one padded window (a window block on a grid smaller than its window)
+  SRB_REQUIRE(win > 0 && win <= 64 && s > 0 && s <= 64, "attention: win=%d s=%d unsupported", win, s);
   if (B <= 0) return 0;
   if (!g_force_simt) {
     if (hd == 64) return launch_attention_mma<64>(qkv, qkv_bias, rel_h, rel_w, B, s, win, heads, out, st);

@@ -45,23 +45,33 @@ int gemm_ln(const __half* A, int lda, const __half* W, int ldw, int M, int N, in
   return launch_gemm_tc<128, 5, EpiLN>(A, lda, W, ldw, M, N, K, p, st, conv_s);
 }
 
-int gemm_dec_final(const __half* A, int lda, const __half* W, int ldw, int M, int K,
-                   const float* bias3, const float* w4, const float* bias4, int s, int P,
-                   float* scores, float* logits, cudaStream_t st) {
-  EpiDecFinal::Params p;
+template <bool kPerToken>
+static int launch_dec_final(const __half* A, int lda, const __half* W, int ldw, int M, int K,
+                            const float* bias3, const float* w4, const float* bias4, int s, int P,
+                            float* scores, float* logits, cudaStream_t st) {
+  typename EpiDecFinal<kPerToken>::Params p;
   memset(&p, 0, sizeof(p));
-  SRB_REQUIRE(P == 16 * s && M % (16 * s * s) == 0, "gemm_dec_final: M=%d s=%d P=%d inconsistent", M, s, P);
   const int B = M / (16 * s * s);
   const uint64_t rowb = static_cast<uint64_t>(P) * 2 * sizeof(float);
   const uint64_t dims[4] = {static_cast<uint64_t>(P) * 2, 2, 2, static_cast<uint64_t>(B) * P / 4};
   const uint64_t strides[3] = {rowb, 2 * rowb, 4 * rowb};
-  const uint32_t box[4] = {64, 2, 1, 4};
+  const uint32_t box[4] = {kPerToken ? 32u : 64u, 2, 1, 4};
   if (scores) { if (int rc = make_tmap_f32_4d_dense(&p.tm_scores, scores, dims, strides, box)) return rc; }
   if (logits) { if (int rc = make_tmap_f32_4d_dense(&p.tm_logits, logits, dims, strides, box)) return rc; }
   p.has_scores = scores != nullptr;
   p.has_logits = logits != nullptr;
   p.bias3 = bias3; p.w4 = w4; p.bias4 = bias4; p.s = s; p.P = P;
-  return launch_gemm_tc<128, 5, EpiDecFinal>(A, lda, W, ldw, M, 128, K, p, st);
+  return launch_gemm_tc<128, 5, EpiDecFinal<kPerToken>>(A, lda, W, ldw, M, 128, K, p, st);
+}
+
+int gemm_dec_final(const __half* A, int lda, const __half* W, int ldw, int M, int K,
+                   const float* bias3, const float* w4, const float* bias4, int s, int P,
+                   float* scores, float* logits, cudaStream_t st) {
+  SRB_REQUIRE(P == 16 * s && M % (16 * s * s) == 0, "gemm_dec_final: M=%d s=%d P=%d inconsistent", M, s, P);
+  // a warp stores two consecutive tokens: one 32-pixel box when they are always row neighbours (s
+  // even), one 16-pixel box per token otherwise (a pair can wrap to the next row or image)
+  if (s % 2 == 0) return launch_dec_final<false>(A, lda, W, ldw, M, K, bias3, w4, bias4, s, P, scores, logits, st);
+  return launch_dec_final<true>(A, lda, W, ldw, M, K, bias3, w4, bias4, s, P, scores, logits, st);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -352,12 +352,19 @@ struct EpiLN {
 // + b4[co]; writes logits and sigmoid scores straight into NHWC [B, P, P, 2].
 // Row index r of the GEMM encodes the pixel hierarchy: r = ((b*s*s + i*s + j)*4 + d1)*4 + d2,
 // d = di*2 + dj (see decoder weight packing in pack.cu).
+//
+// kPerToken = false (even s): a warp's two tokens (i, j), (i, j+1) are horizontally adjacent and leave
+// in one 32-pixel-wide box.  kPerToken = true (odd s): the warp's first token has an even index, so a
+// pair can straddle a row end ((i, s-1) with (i+1, 0)) or an image boundary; each token is staged
+// separately and stored with a 16-pixel-wide box at its own (b, i, j).
 // ------------------------------------------------------------------------------------------------
+template <bool kPerToken>
 struct EpiDecFinal {
   static constexpr bool kSplitCols = true;     // column half 0: sub-pixels d3 = 0,1; half 1: d3 = 2,3
   struct Params {
     // [B, P, P, 2] fp32 seen as 4-D (x: 2P floats | di: 2 | h: 2 | k: B*P/4), image row = 4k + 2h + di;
     // box {64 floats, 2, 1, 4}: the 2 x 16 output pixels x 8 rows one warp produces per tile and half
+    // (kPerToken: box {32 floats, 2, 1, 4}, one token's 16 pixels)
     CUtensorMap tm_scores, tm_logits;
     int has_scores, has_logits;
     const float* bias3;   // [32]
@@ -410,7 +417,9 @@ struct EpiDecFinal {
       }
 #pragma unroll
       for (int di = 0; di < 2; ++di) {
-        const int off = (k * 2 + di) * 64 + (tl * 16 + (xq * 2 + cc) * 2) * 2;
+        // even s: [k 4][di 2][64 floats = 2 tokens x 16 px x 2]; odd s: [token 2][k 4][di 2][32 floats]
+        const int off = kPerToken ? tl * 256 + (k * 2 + di) * 32 + ((xq * 2 + cc) * 2) * 2
+                                  : (k * 2 + di) * 64 + (tl * 16 + (xq * 2 + cc) * 2) * 2;
         const float4 lg = make_float4(o[di * 2].x, o[di * 2].y, o[di * 2 + 1].x, o[di * 2 + 1].y);
         if (p.has_logits) *reinterpret_cast<float4*>(sL + off) = lg;
         if (p.has_scores)
@@ -423,12 +432,17 @@ struct EpiDecFinal {
     if (lane == 0 && m0 < M) {
       const int pix0 = m0 >> 4;                                 // first of the warp's two tokens
       const int ss = p.s * p.s;
-      const int b = pix0 / ss;
-      const int ij = pix0 - b * ss;
-      const int i = ij / p.s, j = ij - i * p.s;
-      const int c0 = j * 32, c3 = (b * p.P + i * 16) >> 2;
-      if (p.has_scores) tma_store_4d(&p.tm_scores, sS, c0, 0, half, c3);
-      if (p.has_logits) tma_store_4d(&p.tm_logits, sL, c0, 0, half, c3);
+#pragma unroll
+      for (int t = 0; t < (kPerToken ? 2 : 1); ++t) {
+        const int pix = pix0 + t;
+        if (kPerToken && pix >= (M >> 4)) break;                // B*s*s odd: the last warp has one token
+        const int b = pix / ss;
+        const int ij = pix - b * ss;
+        const int i = ij / p.s, j = ij - i * p.s;
+        const int c0 = j * 32, c3 = (b * p.P + i * 16) >> 2;
+        if (p.has_scores) tma_store_4d(&p.tm_scores, sS + t * 256, c0, 0, half, c3);
+        if (p.has_logits) tma_store_4d(&p.tm_logits, sL + t * 256, c0, 0, half, c3);
+      }
       bulk_commit_group();
     }
     (void)n_cols;
@@ -601,7 +615,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       __syncwarp();
       if (lane == 0) mbar_arrive(accfree_bar);
     }
-    if constexpr (std::is_same<Epi, EpiDecFinal>::value) EpiDecFinal::drain(lane);
+    if constexpr (std::is_same<Epi, EpiDecFinal<false>>::value || std::is_same<Epi, EpiDecFinal<true>>::value)
+      Epi::drain(lane);
   }
 }
 

@@ -460,8 +460,10 @@ extern "C" int samroad_finalize_weights(samroad_handle_t h) {
   for (int i = 0; i < c.depth && P.ok; ++i) {
     BlockW& b = h->blocks[i];
     const bool glob = is_global_block(c, i);
-    b.win = glob ? static_cast<int>(s) : (c.window_size < s ? c.window_size : static_cast<int>(s));
-    // window blocks keep their 14x14 rel-pos tables even when s < 14 is never the case here
+    // A window block keeps its window size even when it exceeds the grid (s < 14, PATCH_SIZE < 224):
+    // the s x s tokens are then padded to one window, whose pad tokens are softmax keys
+    // (image_encoder.py:168-172), and the rel-pos tables have 2*window-1 rows.
+    b.win = glob ? static_cast<int>(s) : c.window_size;
     const int64_t rel_rows = glob ? 2 * s - 1 : 2 * c.window_size - 1;
     auto K = [&](const char* suffix) { return fmt_key("image_encoder.blocks.%d.", i) + suffix; };
     b.ln1_g = P.f32(K("norm1.weight"), {D});
@@ -503,9 +505,8 @@ extern "C" int samroad_finalize_weights(samroad_handle_t h) {
     b.lin1_b = P.f32(K("mlp.lin1.bias"), {4 * D});
     b.lin2_w = P.linear_w(K("mlp.lin2.weight"), D, 4 * D);
     b.lin2_b = P.f32(K("mlp.lin2.bias"), {D});
-    if (!glob && c.window_size > s)
-      P.fail("window_size=%d larger than the %lld-token feature map is not supported",
-             c.window_size, (long long)s);
+    if (!glob && c.window_size > 64)
+      P.fail("window_size=%d unsupported (at most 64)", c.window_size);
   }
 
   // ---- neck (image_encoder.py:88-104) ----

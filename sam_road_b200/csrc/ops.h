@@ -61,7 +61,8 @@ int convert_f32_f16(const float* x, long n, __half* out, cudaStream_t st);
 // ---- encoder attention (attention.cu) --------------------------------------------------------------------
 // qkv: [B*s*s, 3*D] fp16, columns (q|k|v) x head x hd ; out: [B*s*s, D] fp16.
 // win == s means global attention; otherwise window attention over zero-padded LN output, whose pad
-// tokens have q=k=v=bias (image_encoder.py:168-172,227).  rel_h/rel_w: [2*win-1, hd] fp32.
+// tokens have q=k=v=bias (image_encoder.py:168-172,227); win > s is a single padded window.
+// rel_h/rel_w: [2*win-1, hd] fp32.
 int encoder_attention(const __half* qkv, const float* qkv_bias, const float* rel_h,
                       const float* rel_w, int B, int s, int win, int heads, int hd, __half* out,
                       cudaStream_t st);

@@ -26,7 +26,9 @@ def _stats(t):
 @pytest.mark.parametrize("name,patch,lora", [("vitb_256", 256, 0), ("vitb_512", 512, 0),
                                              ("vitb_256_lora4", 256, 4), ("vitb_256_samdec", 256, 0),
                                              ("vith_256", 256, 0), ("vitl_256", 256, 0),
-                                             ("vitb_1024", 1024, 0)])
+                                             ("vitb_1024", 1024, 0),
+                                             ("vitb_400", 400, 0),            # odd 25x25 grid
+                                             ("vitb_192_samdec", 192, 0)])    # 12x12 grid < 14x14 window
 def test_model_against_reference_golden(name, patch, lora):
     g = np.load(os.path.join(GOLD, f"{name}.npz"))
     cfg = _cfg(patch, lora=lora, samdec=name.endswith("samdec"),
@@ -66,6 +68,27 @@ def test_toponet_versions_against_reference_golden(topo):
         b = O.infer_toponet(sd, spec, feat, pts.float() + 0.25, prs, val)
     assert np.abs(a.numpy() - g[f"{topo}_int"]).max() < TOL
     assert np.abs(b.numpy() - g[f"{topo}_float"]).max() < TOL
+
+
+@pytest.mark.parametrize("n_pairs", [1, 5, 15])
+def test_toponet_npairs_against_reference_golden(n_pairs):
+    """n_pairs != 16 (the layered CUDA TopoNet path) with pairs / valid covering fewer samples than
+    there are points (Ns = 13, N = 20); inputs as tools/make_golden.py:toponet_npairs_inputs."""
+    g = np.load(os.path.join(GOLD, "toponet_npairs.npz"))
+    cfg = _cfg(256)
+    sd = synth.make_state_dict(cfg, seed=5)
+    spec = O.ModelSpec.from_config(cfg)
+    gen = torch.Generator().manual_seed(78)
+    feat = torch.randn(2, 256, 16, 16, generator=gen)
+    pts, prs, val = synth.make_topo_inputs(2, 256, 20, seed=10 + n_pairs, max_nbr=n_pairs)
+    prs, val = prs[:, :13].contiguous(), val[:, :13].contiguous()
+    val[1, 3] = False
+    with torch.no_grad():
+        a = O.infer_toponet(sd, spec, feat, pts, prs, val)
+        b = O.infer_toponet(sd, spec, feat, pts.float() + 0.25, prs, val)
+    assert a.shape == g[f"np{n_pairs}_int"].shape == (2, 13, n_pairs, 1)
+    assert np.abs(a.numpy() - g[f"np{n_pairs}_int"]).max() < TOL
+    assert np.abs(b.numpy() - g[f"np{n_pairs}_float"]).max() < TOL
 
 
 def test_tile_grid_and_keypoints_against_reference_golden():

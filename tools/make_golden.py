@@ -97,6 +97,45 @@ def toponet_fixture():
     np.savez_compressed(os.path.join(OUT, "toponet_versions.npz"), **out)
 
 
+TOPO_NPAIRS = (1, 5, 15)
+TOPO_NPAIRS_NS = 13          # samples kept: fewer than the 20 points, not a multiple of 8
+
+
+def toponet_npairs_inputs(n_pairs):
+    """Inputs of toponet_npairs.npz: 2 images x 20 points, n_pairs neighbour slots, pairs / valid sliced
+    to the first TOPO_NPAIRS_NS samples (Ns != N), sample 3 of image 1 all-invalid."""
+    g = torch.Generator().manual_seed(78)
+    feat = torch.randn(2, 256, 16, 16, generator=g)
+    pts, prs, val = synth.make_topo_inputs(2, 256, 20, seed=10 + n_pairs, max_nbr=n_pairs)
+    prs, val = prs[:, :TOPO_NPAIRS_NS].contiguous(), val[:, :TOPO_NPAIRS_NS].contiguous()
+    val[1, 3] = False
+    return feat, pts, prs, val
+
+
+def toponet_npairs_fixture():
+    out = {}
+    cfg = _cfg(256)
+    torch.manual_seed(0)
+    net = ref_loader.load_reference_model(cfg)
+    sd = synth.make_state_dict(cfg, seed=5)
+    net.load_state_dict(sd, strict=True)
+    spec = O.ModelSpec.from_config(cfg)
+    for n_pairs in TOPO_NPAIRS:
+        feat, pts, prs, val = toponet_npairs_inputs(n_pairs)
+        with torch.no_grad():
+            ref = net.infer_toponet(feat, pts, prs, val)
+            ref_f = net.infer_toponet(feat, pts.float() + 0.25, prs, val)
+            ora = O.infer_toponet(sd, spec, feat, pts, prs, val)
+            ora_f = O.infer_toponet(sd, spec, feat, pts.float() + 0.25, prs, val)
+        assert ref.shape == (2, TOPO_NPAIRS_NS, n_pairs, 1), ref.shape
+        err = max((ref - ora).abs().max().item(), (ref_f - ora_f).abs().max().item())
+        assert err < ORACLE_TOL, f"toponet n_pairs={n_pairs}: oracle disagrees with the reference: {err}"
+        out[f"np{n_pairs}_int"] = ref.numpy()
+        out[f"np{n_pairs}_float"] = ref_f.numpy()
+        print(f"toponet[n_pairs={n_pairs}, Ns={TOPO_NPAIRS_NS}, N=20]: oracle-vs-reference max-abs {err:.2e}")
+    np.savez_compressed(os.path.join(OUT, "toponet_npairs.npz"), **out)
+
+
 def _extract_functions(path, names):
     """exec selected top-level function definitions of a reference file (it cannot be imported as a
     whole here: rtree / igraph / shapely / tcod are absent) -- the source is read where it lies."""
@@ -147,6 +186,14 @@ def tileloop_fixture():
     print(f"tileloop: {len(pts_ref)} graph points, tile grids identical")
 
 
+def shape_fixtures():
+    # PATCH_SIZE 400: odd 25x25 token grid, windows padded to 28, 3x3 neck conv through im2col
+    model_fixture("vitb_400", _cfg(400), seed=8, n_points=24)
+    # PATCH_SIZE 192: 12x12 grid smaller than the 14x14 window (one padded window), SAM mask decoder
+    model_fixture("vitb_192_samdec", _cfg(192, samdec=True), seed=9, n_points=16)
+    toponet_npairs_fixture()
+
+
 def main():
     assert ref_loader.available(), "needs /root/reference"
     os.makedirs(OUT, exist_ok=True)
@@ -154,6 +201,9 @@ def main():
     if "--only-new" in sys.argv:      # fixtures added in round 2 (the round-1 files stay byte-identical)
         model_fixture("vitl_256", _cfg(256, version="vit_l"), seed=6, n_points=16)
         model_fixture("vitb_1024", _cfg(1024), seed=7, n_points=40)
+        return
+    if "--shapes" in sys.argv:        # tile sizes and pair counts outside the benched configs
+        shape_fixtures()
         return
     model_fixture("vitb_256", _cfg(256), seed=0, n_points=24)
     model_fixture("vitb_512", _cfg(512), seed=1, n_points=40)
@@ -164,6 +214,7 @@ def main():
     model_fixture("vitb_1024", _cfg(1024), seed=7, n_points=40)
     toponet_fixture()
     tileloop_fixture()
+    shape_fixtures()
 
 
 if __name__ == "__main__":
