@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define SAMROAD_ABI_VERSION 2
+#define SAMROAD_ABI_VERSION 3
 
 typedef struct samroad_ctx* samroad_handle_t;
 
@@ -209,14 +209,14 @@ int samroad_abi_version(void);
 
 /* ---- op-level entry points (unit tests and composition; all pointers device, fp16 = IEEE half) ---- */
 
-/* out16[M,N] = act(A[M,K] W[N,K]^T + bias)      act: 0 none, 1 GELU(erf), 2 ReLU */
+/* out16[M,N] = act(A[M,K] W[N,K]^T + bias)      act: 0 none, 1 GELU(erf), 2 ReLU; others are rejected */
 int samroad_op_gemm_f16(const void* A, int lda, const void* W, int ldw, int M, int N, int K,
                         const float* bias, int act, void* out16, int ldo, void* stream);
 /* out32[M,N] = A W^T + bias + resid + pos[m % pos_rows]   (bias/resid/pos may be NULL) */
 int samroad_op_gemm_f32(const void* A, int lda, const void* W, int ldw, int M, int N, int K,
                         const float* bias, const float* resid, const float* pos, int pos_rows,
                         float* out32, int ldo, void* stream);
-/* grouped LayerNorm epilogue, see gemm_tc.cuh EpiLN */
+/* grouped LayerNorm epilogue, see gemm_tc.cuh EpiLN (act as for samroad_op_gemm_f16) */
 int samroad_op_gemm_ln(const void* A, int lda, const void* W, int ldw, int M, int N, int K,
                        const float* bias, const float* resid, const float* gamma,
                        const float* beta, float eps, int group, int act, void* out16, float* out32,
@@ -233,15 +233,9 @@ int samroad_op_attention(const void* qkv16, const float* qkv_bias, const float* 
 /* Test hook: bit 0 routes samroad_op_attention / the encoder through the fp32 SIMT attention
  * kernel (the independent on-device checker of the tensor-core kernel).  Not for production use. */
 void samroad_debug_force_simt_attention(int on);
-/* Test hook (bit mask): bit 4 makes every encoder kernel walk the token rows in ascending order (no
- * snake traversal).  Bits 0-2 selected GEMM variants of an earlier multi-kernel GEMM path; there is
- * one GEMM kernel now and they are ignored. */
+/* Test hook (bit mask): bit 4 (16) makes the encoder's LayerNorms walk the token rows ascending
+ * (by default those of even blocks walk them descending).  Other bits are ignored. */
 void samroad_debug_disable_2cta_gemm(int off);
-/* Test hook: direction in which the next op-level row-streaming kernel (LayerNorm) walks the token
- * rows (1 = descending; the encoder alternates it from kernel to kernel). */
-void samroad_debug_set_traverse_reverse(int on);
-/* Kept for ABI compatibility: the attention kernel records no phase trace, and the call does nothing. */
-void samroad_debug_attention_trace(void* dev_buf);
 
 #ifdef __cplusplus
 }

@@ -13,7 +13,7 @@ _PKG = Path(__file__).resolve().parent
 LIB_PATH = _PKG / "libsamroad_b200.so"
 
 F32, I64, I32, U8, F64 = 0, 1, 2, 3, 4
-ABI_VERSION = 2
+ABI_VERSION = 3
 TOPO_NORMAL, TOPO_NO_OFFSET, TOPO_NO_TRANSFORMER = 0, 1, 2
 ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
 
@@ -76,8 +76,6 @@ SIGNATURES = {
     "samroad_op_layernorm": (_i, [_vp, _vp, _vp, _f, _i, _i, _vp, _vp]),
     "samroad_debug_force_simt_attention": (None, [_i]),
     "samroad_debug_disable_2cta_gemm": (None, [_i]),
-    "samroad_debug_set_traverse_reverse": (None, [_i]),
-    "samroad_debug_attention_trace": (None, [_vp]),
     "samroad_op_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
 }
 

@@ -45,28 +45,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
 
@@ -78,31 +59,12 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
   return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
-// exact-erf GELU (reference: sam/segment_anything/modeling/common.py:18 nn.GELU default,
-// model.py:285).  erff() is accurate to ~1 ulp; the output is rounded to fp16 afterwards.
-__device__ __forceinline__ float gelu_erf(float x) {
-  return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
-}
-
 // Fast erf-GELU for GEMM epilogues: gelu(x) = relu(x) - |x| * 0.5*erfc(|x|/sqrt2), with
 // log2(0.5*erfc(a/sqrt2)) fitted by a degree-4 polynomial on [0, 5.6] (clamped beyond, where the term
 // is < 1e-7).  4 FMA + 1 MUFU.EX2 + 3 ALU; max abs error 6.1e-6 (fit + error scan in DESIGN.md "GELU"):
 // 1 % of the half-ulp of the fp16 value the result is rounded to at |gelu| ~ 1, and below the fp16
-// half-ulp everywhere above |gelu| = 0.016.
-__device__ __forceinline__ float gelu_erf_fast(float x) {
-  const float a = fabsf(x);
-  const float ac = fminf(a, 5.6f);
-  float l = fmaf(0.0038648627f, ac, -0.044072032f);
-  l = fmaf(l, ac, -0.46802717f);
-  l = fmaf(l, ac, -1.1473644f);
-  l = fmaf(l, ac, -1.0004811f);
-  float e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(l));
-  return fmaf(-a, e, fmaxf(x, 0.0f));
-}
-
-// Two elements at a time: the polynomial is evaluated in t = -min(|x|, 5.6) (odd coefficients
-// negated).  Same coefficients, same rounding per lane as gelu_erf_fast -> bit-identical results.
+// half-ulp everywhere above |gelu| = 0.016.  Two elements at a time; the polynomial is evaluated in
+// t = -min(|x|, 5.6) (odd coefficients negated).
 __device__ __forceinline__ float2 gelu_erf_fast2(float2 x) {
   const float2 na = make_float2(fminf(x.x, -x.x), fminf(x.y, -x.y));
   const float2 t = make_float2(fmaxf(na.x, -5.6f), fmaxf(na.y, -5.6f));
@@ -162,21 +124,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// non-blocking probe (mbarrier.try_wait may suspend the thread for a system-dependent time before it
-// returns false, which is poison for a loop that polls several barriers)
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
@@ -197,21 +144,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       "r"(c0), "r"(c1)
       : "memory");
 }
-// TMA store (shared::cta -> global) through a bulk async-group; the smem source may be reused once
-// cp.async.bulk.wait_group.read has retired the group.
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int32_t c0,
-                                             int32_t c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-// TMA reduce-add (fp32): global[tile] += smem[tile], performed at L2.
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* tm, const void* smem_src,
-                                                  int32_t c0, int32_t c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, const void* smem_src, int32_t c0,
                                              int32_t c1, int32_t c2, int32_t c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
@@ -229,15 +161,6 @@ __device__ __forceinline__ void bulk_wait_group_read() {
 template <int N>
 __device__ __forceinline__ void bulk_wait_group() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar,
-                                            int32_t c0, int32_t c1, int32_t c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)),
-      "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar,
                                             int32_t c0, int32_t c1, int32_t c2, int32_t c3) {
@@ -368,17 +291,10 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_
 int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                      uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols = 64);
 
-// 2D fp32 row-major tensor, box [box_rows][32 cols] (= 128 B inner), 128B swizzle.
-int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                     uint64_t ld_elems, uint32_t box_rows);
-
 // 4D fp16 view [d3][d2][d1][d0] (d0 contiguous; strides in elements for d1..d3), box {b0,b1,b2,b3},
 // 128B swizzle (b0 * 2 bytes must be 128).  Out-of-bounds elements read as zero.
 int make_tmap_f16_4d(CUtensorMap* out, const void* base, const uint64_t dims[4],
                      const uint64_t strides_elems[3], const uint32_t box[4]);
-void set_traverse_reverse(bool r);   // next row-streaming kernel walks its tiles / units / rows backwards
-bool traverse_reverse();
-void set_traverse_snake_enabled(bool on);   // A/B hook: false = every kernel ascending
 int make_tmap_f32_4d_dense(CUtensorMap* out, const void* base, const uint64_t dims[4],
                            const uint64_t strides_bytes[3], const uint32_t box[4]);
 

@@ -17,6 +17,8 @@ static inline bool use_bn256(int M, int N) {
 
 int gemm_f16out(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
                 const float* bias, int act, __half* out, int ldo, cudaStream_t st) {
+  SRB_REQUIRE(act == ACT_NONE || act == ACT_GELU || act == ACT_RELU,
+              "gemm_f16out: act=%d must be 0 (none), 1 (GELU) or 2 (ReLU)", act);
   EpiF16::Params p{out, bias, ldo, act};
   SRB_REQUIRE(ldo % 8 == 0, "gemm_f16out: ldo=%d must be a multiple of 8", ldo);
   if (use_bn256(M, N)) return launch_gemm_tc<256, 3, EpiF16>(A, lda, W, ldw, M, N, K, p, st);
@@ -36,6 +38,8 @@ int gemm_ln(const __half* A, int lda, const __half* W, int ldw, int M, int N, in
             const float* bias, const float* resid, const float* gamma, const float* beta, float eps,
             int group, int act, __half* out16, float* out32, float* out_nchw, int tokens, int ldo,
             cudaStream_t st, int conv_s) {
+  SRB_REQUIRE(act == ACT_NONE || act == ACT_GELU || act == ACT_RELU,
+              "gemm_ln: act=%d must be 0 (none), 1 (GELU) or 2 (ReLU)", act);
   SRB_REQUIRE(group == 64 || group == 128 || group == 256, "gemm_ln: group=%d must be 64, 128 or 256", group);
   SRB_REQUIRE(N % group == 0, "gemm_ln: N=%d not a multiple of group=%d", N, group);
   EpiLN::Params p{out16, out32, out_nchw, bias, resid, gamma, beta, eps, ldo, group, act,

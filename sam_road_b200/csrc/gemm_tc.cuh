@@ -29,8 +29,6 @@
 //   ConvTranspose2d(k=2,s=2) as GEMM        model.py:286-295 (SURVEY.md §8a P7)
 #pragma once
 
-#include <type_traits>
-
 #include "common.cuh"
 #include "ops.h"
 
@@ -42,13 +40,6 @@ constexpr int kGemmThreads = 384;
 constexpr int kGemmEpiWarps = 8;
 constexpr int kGemmScratchFloats = 32 * 36;   // per epilogue warp: 32x32 fp32 block, rows padded to 36
 
-
-__device__ __forceinline__ float apply_act(float x, int act) {
-  if (act == ACT_GELU || act == ACT_GELU_SCALAR) return gelu_erf_fast(x);
-  if (act == ACT_RELU) return fmaxf(x, 0.0f);
-  if (act == ACT_SIGMOID) return sigmoidf_(x);
-  return x;
-}
 
 // One accumulator row (this lane's row of the tile, starting at the warp's first column) in the
 // shared-memory staging area.
@@ -95,7 +86,6 @@ __device__ __forceinline__ void epi_stream_chunks(int n_cols, const AccRow& row,
 
 // Epilogue 1: out16[m,n] = act(acc + bias[n])                       (qkv, MLP lin1, TopoNet lin)
 struct EpiF16 {
-  static constexpr bool kSplitCols = true;
   struct Params {
     __half* out;          // [M, ldo]
     const float* bias;    // [N] or null
@@ -104,38 +94,21 @@ struct EpiF16 {
   };
   static __device__ __forceinline__ void run(const Params& p, int m0, int M, int n_base, int n_cols,
                                              const AccRow& row, float* scratch, int lane) {
-    if (p.act >= ACT_PROBE_SKIP) {          // timing ablations (tools/gemm_probe.py), never a result
-      if (p.act == ACT_PROBE_SKIP) return;
-      if (p.act == ACT_PROBE_ACC) {
-        float acc = 0.f;
-        for (int c = 0; c < (n_cols >> 5); ++c) {
-          float v[32];
-          row.load(c, v);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) acc += v[i];
-        }
-        if (acc == 1234.5678f) p.out[0] = __float2half(acc);
-        return;
-      }
-    }
-    const bool probe_nostore = p.act == ACT_PROBE_NOSTORE;
-    const int act = probe_nostore ? ACT_GELU : p.act;
     epi_stream_chunks(n_cols, row, scratch, lane, [&](int c, int rr, int cc, float4 x) {
       const int n = n_base + c * 32 + cc;
       if (p.bias) {
         const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n));
         x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
       }
-      if (act == ACT_GELU) {
+      if (p.act == ACT_GELU) {
         const float2 g0 = gelu_erf_fast2(make_float2(x.x, x.y));
         const float2 g1 = gelu_erf_fast2(make_float2(x.z, x.w));
         x = make_float4(g0.x, g0.y, g1.x, g1.y);
-      } else if (act != ACT_NONE) {
-        x.x = apply_act(x.x, act); x.y = apply_act(x.y, act);
-        x.z = apply_act(x.z, act); x.w = apply_act(x.w, act);
+      } else if (p.act == ACT_RELU) {
+        x = make_float4(fmaxf(x.x, 0.0f), fmaxf(x.y, 0.0f), fmaxf(x.z, 0.0f), fmaxf(x.w, 0.0f));
       }
       const int m = m0 + rr;
-      if (m < M && !(probe_nostore && x.x != 1234.5678f)) {
+      if (m < M) {
         uint2 u;
         u.x = pack_half2(x.x, x.y);
         u.y = pack_half2(x.z, x.w);
@@ -143,12 +116,12 @@ struct EpiF16 {
       }
     });
   }
+  static __device__ __forceinline__ void drain(int /*lane*/) {}
 };
 
 // Epilogue 2: out32[m,n] = acc + bias[n] + resid[m,n] + pos[m % pos_rows, n]
 //             (patch-embed + pos_embed, attention proj + shortcut, MLP lin2 + shortcut; plain f32)
 struct EpiF32 {
-  static constexpr bool kSplitCols = true;
   struct Params {
     float* out;           // [M, ldo]
     const float* bias;    // [N] or null
@@ -205,6 +178,7 @@ struct EpiF32 {
       }
     }
   }
+  static __device__ __forceinline__ void drain(int /*lane*/) {}
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -218,7 +192,6 @@ struct EpiF32 {
 // ([b, n, tok] with tok = m % tokens, b = m / tokens) for the API-visible embeddings.
 // ------------------------------------------------------------------------------------------------
 struct EpiLN {
-  static constexpr bool kSplitCols = true;
   struct Params {
     __half* out16;        // [M, ldo] or null
     float* out32;         // [M, ldo] or null
@@ -310,7 +283,7 @@ struct EpiLN {
           const float2 bt = __ldg(reinterpret_cast<const float2*>(p.beta + gi + i));
           float2 y = make_float2((v[i] - mean) * rstd * gm.x + bt.x, (v[i + 1] - mean) * rstd * gm.y + bt.y);
           if (p.act == ACT_GELU) y = gelu_erf_fast2(y);
-          else if (p.act != ACT_NONE) y = make_float2(apply_act(y.x, p.act), apply_act(y.y, p.act));
+          else if (p.act == ACT_RELU) y = make_float2(fmaxf(y.x, 0.0f), fmaxf(y.y, 0.0f));
           v[i] = y.x; v[i + 1] = y.y;
         }
         if (valid) {
@@ -342,6 +315,7 @@ struct EpiLN {
       }
     }
   }
+  static __device__ __forceinline__ void drain(int /*lane*/) {}
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -351,7 +325,7 @@ struct EpiLN {
 // Per chunk: h = GELU(acc + b3) ; ConvT(32->2,k2,s2): out[co, di, dj] = sum_ci h[ci] W4[ci,co,di,dj]
 // + b4[co]; writes logits and sigmoid scores straight into NHWC [B, P, P, 2].
 // Row index r of the GEMM encodes the pixel hierarchy: r = ((b*s*s + i*s + j)*4 + d1)*4 + d2,
-// d = di*2 + dj (see decoder weight packing in pack.cu).
+// d = di*2 + dj.
 //
 // kPerToken = false (even s): a warp's two tokens (i, j), (i, j+1) are horizontally adjacent and leave
 // in one 32-pixel-wide box.  kPerToken = true (odd s): the warp's first token has an even index, so a
@@ -360,7 +334,6 @@ struct EpiLN {
 // ------------------------------------------------------------------------------------------------
 template <bool kPerToken>
 struct EpiDecFinal {
-  static constexpr bool kSplitCols = true;     // column half 0: sub-pixels d3 = 0,1; half 1: d3 = 2,3
   struct Params {
     // [B, P, P, 2] fp32 seen as 4-D (x: 2P floats | di: 2 | h: 2 | k: B*P/4), image row = 4k + 2h + di;
     // box {64 floats, 2, 1, 4}: the 2 x 16 output pixels x 8 rows one warp produces per tile and half
@@ -491,7 +464,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // ordered (tap, channel) and k-block kb reads the channel block of the tap-shifted 128-pixel slab;
   // out-of-image taps arrive as TMA zero fill.  (neck conv, image_encoder.py:96-103)
   using SM = GemmSmem<BN, STAGES>;
-  static_assert(Epi::kSplitCols, "the consumer warps split every tile into two column halves");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
@@ -615,16 +587,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       __syncwarp();
       if (lane == 0) mbar_arrive(accfree_bar);
     }
-    if constexpr (std::is_same<Epi, EpiDecFinal<false>>::value || std::is_same<Epi, EpiDecFinal<true>>::value)
-      Epi::drain(lane);
+    Epi::drain(lane);
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // host launcher
 // ------------------------------------------------------------------------------------------------
-int device_sm_count();
-
 template <int BN, int STAGES, class Epi>
 int launch_gemm_tc(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
                    const typename Epi::Params& ep, cudaStream_t stream, int conv_s = 0) {

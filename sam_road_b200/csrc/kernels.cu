@@ -59,10 +59,10 @@ layernorm_f16_kernel(const float* __restrict__ x, const float* __restrict__ gamm
 }
 
 int layernorm_f16(const float* x, const float* gamma, const float* beta, float eps, int M, int D,
-                  __half* out, cudaStream_t st) {
+                  __half* out, bool reverse, cudaStream_t st) {
   SRB_REQUIRE(D % 128 == 0 && D <= 128 * kLNMaxVec, "layernorm: D=%d unsupported", D);
   if (M <= 0) return 0;
-  layernorm_f16_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, gamma, beta, eps, M, D, out, traverse_reverse() ? 1 : 0);
+  layernorm_f16_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, gamma, beta, eps, M, D, out, reverse ? 1 : 0);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch();
   return 0;

@@ -43,14 +43,6 @@ struct BlockW {
   int win;   // attention window (14) or s for global blocks
 };
 
-struct TopoLayerW {
-  __half* in_w;  float* in_b;
-  __half* out_w; float* out_b;
-  __half* l1_w;  float* l1_b;
-  __half* l2_w;  float* l2_b;
-  float *n1_g, *n1_b, *n2_g, *n2_b;
-};
-
 }  // namespace
 
 // Per-kernel-class CUDA-event timing (bench.py roofline): events are recorded on the launching
@@ -119,8 +111,10 @@ struct samroad_ctx {
   // toponet
   __half* tp_feat_w = nullptr; float* tp_feat_b = nullptr;
   __half* tp_st_w = nullptr; float* tp_off_w = nullptr; float* tp_pair_b = nullptr;
-  TopoLayerW tp_layers[3];
-  __half* tp_chunks = nullptr;   // fused-kernel weight chunks [18*128, 128]
+  TopoLayerParams tp_layers[3];
+  // fp16 layer weights [18*128, 128]: per layer Wq, Wk, Wv, Wo, W1, W2 as [128, 128] blocks, so that
+  // in_proj_weight (Wq|Wk|Wv), out_proj, linear1 and linear2 are each one contiguous [N, 128] operand
+  __half* tp_chunks = nullptr;
   float* tp_out_w = nullptr; float* tp_out_b = nullptr;
 
   // activation workspace (grown on demand); TopoNet has its own so that the encoder of the next scene
@@ -146,6 +140,9 @@ namespace {
 
 constexpr float kPixelMean[3] = {123.675f, 116.28f, 103.53f};   // model.py:229
 constexpr float kPixelStd[3] = {58.395f, 57.12f, 57.375f};      // model.py:230
+
+// test hook (bit 4 of samroad_debug_disable_2cta_gemm): every encoder LayerNorm walks its rows ascending
+bool g_ln_ascending = false;
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -645,29 +642,9 @@ extern "C" int samroad_finalize_weights(samroad_handle_t h) {
   }
   h->tp_pair_b = P.f32("topo_net.pair_proj.bias", {128});
   if (c.toponet_version != SAMROAD_TOPO_NO_TRANSFORMER) {
-    for (int l = 0; l < 3; ++l) {
-      TopoLayerW& t = h->tp_layers[l];
-      auto K = [&](const char* suffix) {
-        return fmt_key("topo_net.transformer_encoder.layers.%d.", l) + suffix;
-      };
-      t.in_w = P.linear_w(K("self_attn.in_proj_weight"), 384, 128);
-      t.in_b = P.f32(K("self_attn.in_proj_bias"), {384});
-      t.out_w = P.linear_w(K("self_attn.out_proj.weight"), 128, 128);
-      t.out_b = P.f32(K("self_attn.out_proj.bias"), {128});
-      t.l1_w = P.linear_w(K("linear1.weight"), 128, 128);
-      t.l1_b = P.f32(K("linear1.bias"), {128});
-      t.l2_w = P.linear_w(K("linear2.weight"), 128, 128);
-      t.l2_b = P.f32(K("linear2.bias"), {128});
-      t.n1_g = P.f32(K("norm1.weight"), {128});
-      t.n1_b = P.f32(K("norm1.bias"), {128});
-      t.n2_g = P.f32(K("norm2.weight"), {128});
-      t.n2_b = P.f32(K("norm2.bias"), {128});
-    }
-  }
-  if (c.toponet_version != SAMROAD_TOPO_NO_TRANSFORMER && P.ok) {
-    // fused-kernel operand: per layer Wq, Wk, Wv (= in_proj rows), Wo, W1, W2 as [128,128] chunks
     std::vector<__half> chunks(static_cast<size_t>(18) * 128 * 128);
-    for (int l = 0; l < 3; ++l) {
+    for (int l = 0; l < 3 && P.ok; ++l) {
+      TopoLayerParams& t = h->tp_layers[l];
       auto K = [&](const char* suffix) {
         return fmt_key("topo_net.transformer_encoder.layers.%d.", l) + suffix;
       };
@@ -676,10 +653,18 @@ extern "C" int samroad_finalize_weights(samroad_handle_t h) {
                                   P.get(K("linear1.weight"), {128, 128}),
                                   P.get(K("linear2.weight"), {128, 128})};
       size_t off = static_cast<size_t>(l) * 6 * 128 * 128;
-      for (int t = 0; t < 4 && P.ok; ++t) {
-        for (size_t i = 0; i < src[t]->data.size(); ++i) chunks[off + i] = __float2half_rn(src[t]->data[i]);
-        off += src[t]->data.size();
+      for (int i = 0; i < 4 && P.ok; ++i) {
+        for (size_t j = 0; j < src[i]->data.size(); ++j) chunks[off + j] = __float2half_rn(src[i]->data[j]);
+        off += src[i]->data.size();
       }
+      t.in_b = P.f32(K("self_attn.in_proj_bias"), {384});
+      t.out_b = P.f32(K("self_attn.out_proj.bias"), {128});
+      t.l1_b = P.f32(K("linear1.bias"), {128});
+      t.l2_b = P.f32(K("linear2.bias"), {128});
+      t.n1_g = P.f32(K("norm1.weight"), {128});
+      t.n1_b = P.f32(K("norm1.bias"), {128});
+      t.n2_g = P.f32(K("norm2.weight"), {128});
+      t.n2_b = P.f32(K("norm2.bias"), {128});
     }
     h->tp_chunks = P.upload(chunks);
   }
@@ -728,13 +713,12 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
   SRB_T(KT_GEMM_PATCH, 2 * Md * Dd * 768, Md * 768 * 2 + Md * Dd * 4,
         gemm_f32out(w.XN, 768, h->pe_w, 768, M, D, 768, h->pe_b, nullptr, h->pos, T, w.X, D, st));
 
-  // transformer blocks (image_encoder.py:166-182).  The seven kernels of a block stream the same
-  // M x D token rows; they walk them in alternating directions (snake) so that every kernel starts on
-  // the rows its producer wrote last, which are the ones still in L2.
-  bool snake = true;    // the patch embedding ran ascending
-  auto turn = [&]() { set_traverse_reverse(snake); snake = !snake; };
+  // transformer blocks (image_encoder.py:166-182).  Both LayerNorms of block i walk the token rows
+  // descending when i is even and ascending when i is odd (all ascending under the test hook); the
+  // effect of this order on L2 reuse has not been measured on the H100.
   for (int i = 0; i < h->cfg.depth; ++i) {
     const BlockW& b = h->blocks[i];
+    const bool ln_reverse = i % 2 == 0 && !g_ln_ascending;
     // algorithmic attention FLOPs: real query/key tokens only (SURVEY.md §8d)
     double att_flops = 0;
     {
@@ -747,30 +731,21 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
         }
       att_flops *= static_cast<double>(B) * h->cfg.num_heads;
     }
-    turn();
-    SRB_T(KT_LAYERNORM, 0, Md * Dd * 6, layernorm_f16(w.X, b.ln1_g, b.ln1_b, 1e-6f, M, D, w.XN, st));
-    turn();
+    SRB_T(KT_LAYERNORM, 0, Md * Dd * 6, layernorm_f16(w.X, b.ln1_g, b.ln1_b, 1e-6f, M, D, w.XN, ln_reverse, st));
     SRB_T(KT_GEMM_QKV, 2 * Md * 3 * Dd * Dd, Md * Dd * 2 + Md * 3 * Dd * 2,
           gemm_f16out(w.XN, D, b.qkv_w, D, M, 3 * D, D, b.qkv_b, ACT_NONE, w.QKV, 3 * D, st));
-    turn();
     SRB_T(b.win == s ? KT_ATTN_GLOBAL : KT_ATTN_WINDOW, att_flops, Md * 4 * Dd * 2,
           encoder_attention(w.QKV, b.qkv_b, b.rel_h, b.rel_w, B, s, b.win,
                             h->cfg.num_heads, h->hd, w.ATT, st));
-    turn();
     SRB_T(KT_GEMM_PROJ, 2 * Md * Dd * Dd, Md * Dd * 2 + Md * Dd * 8,
           gemm_f32out(w.ATT, D, b.proj_w, D, M, D, D, b.proj_b, w.X, nullptr, 0, w.X, D, st));
-    turn();
-    SRB_T(KT_LAYERNORM, 0, Md * Dd * 6, layernorm_f16(w.X, b.ln2_g, b.ln2_b, 1e-6f, M, D, w.XN, st));
-    turn();
+    SRB_T(KT_LAYERNORM, 0, Md * Dd * 6, layernorm_f16(w.X, b.ln2_g, b.ln2_b, 1e-6f, M, D, w.XN, ln_reverse, st));
     SRB_T(KT_GEMM_LIN1, 2 * Md * 4 * Dd * Dd, Md * Dd * 2 + Md * 4 * Dd * 2,
           gemm_f16out(w.XN, D, b.lin1_w, D, M, 4 * D, D, b.lin1_b, ACT_GELU, w.H, 4 * D, st));
-    turn();
     SRB_T(KT_GEMM_LIN2, 2 * Md * 4 * Dd * Dd, Md * 4 * Dd * 2 + Md * Dd * 8,
           gemm_f32out(w.H, 4 * D, b.lin2_w, 4 * D, M, D, 4 * D, b.lin2_b, w.X, nullptr, 0, w.X, D,
                       st));
   }
-
-  set_traverse_reverse(false);
 
   // neck (image_encoder.py:88-104,114): 1x1 conv -> LN2d -> 3x3 conv -> LN2d
   SRB_T(KT_NECK, 0, Md * Dd * 6, convert_f32_f16(w.X, static_cast<long>(M) * D, w.XN, st));
@@ -875,40 +850,36 @@ extern "C" int samroad_toponet(samroad_handle_t h, const float* image_embeddings
                     256, st));
   SRB_T(KT_TOPO_PAIR, 0, tokd * 2, topo_fix_valid(valid, rows, Np, w.VF, st));
   const bool fused = !no_tf && Np == 16;
-  if (!fused)
-    SRB_T(KT_TOPO_PAIR, tokd * 128 * 6, tokd * 128 * (8 + 6),
-          topo_pair_features(w.PST, h->tp_off_w, h->tp_pair_b, points, pts_dtype, pairs, pairs_dtype, B,
-                             N, Ns, Np, zero_off, w.X32, w.X16, st));
+  const TopoPairInputs pin{w.PST, h->tp_off_w, h->tp_pair_b, points, pairs, pts_dtype, pairs_dtype, N,
+                           Ns * Np, zero_off};
   if (fused) {
     // all three encoder layers + output_proj in one persistent wgmma kernel
-    TopoFusedParams fp;
-    for (int l = 0; l < 3; ++l) {
-      const TopoLayerW& t = h->tp_layers[l];
-      fp.in_b[l] = t.in_b; fp.out_b[l] = t.out_b; fp.l1_b[l] = t.l1_b; fp.l2_b[l] = t.l2_b;
-      fp.n1_g[l] = t.n1_g; fp.n1_b[l] = t.n1_b; fp.n2_g[l] = t.n2_g; fp.n2_b[l] = t.n2_b;
-    }
-    fp.out_w = h->tp_out_w; fp.out_b_final = h->tp_out_b;
-    TopoPairInputs pin{w.PST, h->tp_off_w, h->tp_pair_b, points, pairs, pts_dtype, pairs_dtype, N,
-                       Ns * Np, zero_off};
     SRB_T(KT_TOPO_GEMM, tokd * 2 * 128 * (384 + 128 * 3) * 3 + tokd * 4 * 16 * 128 * 3 + tokd * 128 * 6,
           tokd * 1024 * 2 + tokd * 8,
-          topo_transformer_fused(pin, h->tp_chunks, fp, w.VF, tok, topo_logits, topo_scores, st));
+          topo_transformer_fused(pin, h->tp_chunks, h->tp_layers, h->tp_out_w, h->tp_out_b, w.VF, tok,
+                                 topo_logits, topo_scores, st));
     return 0;
   }
+  SRB_T(KT_TOPO_PAIR, tokd * 128 * 6, tokd * 128 * (8 + 6), topo_pair_features(pin, tok, w.X32, w.X16, st));
   if (!no_tf) {
     for (int l = 0; l < 3; ++l) {
-      const TopoLayerW& t = h->tp_layers[l];
+      const TopoLayerParams& t = h->tp_layers[l];
+      // this layer's [Wq|Wk|Wv], Wo, W1, W2 in tp_chunks
+      const __half* in_w = h->tp_chunks + static_cast<size_t>(l) * 6 * 128 * 128;
+      const __half* out_w = in_w + 3 * 128 * 128;
+      const __half* l1_w = in_w + 4 * 128 * 128;
+      const __half* l2_w = in_w + 5 * 128 * 128;
       SRB_T(KT_TOPO_GEMM, 2 * tokd * 384 * 128, tokd * 512 * 2,
-            gemm_f16out(w.X16, 128, t.in_w, 128, tok, 384, 128, t.in_b, ACT_NONE, w.QKV16, 384, st));
+            gemm_f16out(w.X16, 128, in_w, 128, tok, 384, 128, t.in_b, ACT_NONE, w.QKV16, 384, st));
       SRB_T(KT_TOPO_ATTN, 4 * tokd * Np * 128, tokd * 512 * 2,
             topo_attention(w.QKV16, w.VF, rows, Np, w.ATT16, st));
       SRB_T(KT_TOPO_GEMM, 2 * tokd * 128 * 128, tokd * 128 * (2 + 4 + 4 + 2),
-            gemm_ln(w.ATT16, 128, t.out_w, 128, tok, 128, 128, t.out_b, w.X32, t.n1_g, t.n1_b, 1e-5f,
+            gemm_ln(w.ATT16, 128, out_w, 128, tok, 128, 128, t.out_b, w.X32, t.n1_g, t.n1_b, 1e-5f,
                     128, ACT_NONE, w.X16, w.X32, nullptr, 1, 128, st));
       SRB_T(KT_TOPO_GEMM, 2 * tokd * 128 * 128, tokd * 128 * 4,
-            gemm_f16out(w.X16, 128, t.l1_w, 128, tok, 128, 128, t.l1_b, ACT_RELU, w.H16, 128, st));
+            gemm_f16out(w.X16, 128, l1_w, 128, tok, 128, 128, t.l1_b, ACT_RELU, w.H16, 128, st));
       SRB_T(KT_TOPO_GEMM, 2 * tokd * 128 * 128, tokd * 128 * (2 + 4 + 4 + 2),
-            gemm_ln(w.H16, 128, t.l2_w, 128, tok, 128, 128, t.l2_b, w.X32, t.n2_g, t.n2_b, 1e-5f, 128,
+            gemm_ln(w.H16, 128, l2_w, 128, tok, 128, 128, t.l2_b, w.X32, t.n2_g, t.n2_b, 1e-5f, 128,
                     ACT_NONE, w.X16, w.X32, nullptr, 1, 128, st));
     }
   }
@@ -1106,7 +1077,7 @@ extern "C" int samroad_op_gemm_ref(const void* A, int lda, const void* W, int ld
 }
 extern "C" int samroad_op_layernorm(const float* x, const float* gamma, const float* beta,
                                     float eps, int M, int D, void* out16, void* stream) {
-  return layernorm_f16(x, gamma, beta, eps, M, D, static_cast<__half*>(out16),
+  return layernorm_f16(x, gamma, beta, eps, M, D, static_cast<__half*>(out16), false,
                        static_cast<cudaStream_t>(stream));
 }
 extern "C" int samroad_op_attention(const void* qkv16, const float* qkv_bias, const float* rel_h,
@@ -1117,6 +1088,4 @@ extern "C" int samroad_op_attention(const void* qkv16, const float* qkv_bias, co
                            static_cast<cudaStream_t>(stream));
 }
 extern "C" void samroad_debug_force_simt_attention(int on) { attention_force_simt(on); }
-extern "C" void samroad_debug_set_traverse_reverse(int on) { set_traverse_reverse(on != 0); }
-extern "C" void samroad_debug_attention_trace(void* /*dev_buf*/) {}
-extern "C" void samroad_debug_disable_2cta_gemm(int off) { set_traverse_snake_enabled((off & 16) == 0); }
+extern "C" void samroad_debug_disable_2cta_gemm(int off) { g_ln_ascending = (off & 16) != 0; }

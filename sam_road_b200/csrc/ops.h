@@ -8,14 +8,7 @@
 
 namespace srb {
 
-enum Act : int {
-  ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SIGMOID = 3,
-  ACT_GELU_SCALAR = 4,         // same function, one element per instruction (A/B timing only)
-  // tools/gemm_probe.py only: epilogue ablations that do NOT produce the result
-  ACT_PROBE_SKIP = 100,        // release the accumulator untouched (main-loop ceiling)
-  ACT_PROBE_ACC = 101,         // accumulator reads only
-  ACT_PROBE_NOSTORE = 102      // full GELU epilogue without the global stores
-};
+enum Act : int { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2 };
 
 void set_last_error(const char* fmt, ...);
 const char* get_last_error();
@@ -46,8 +39,9 @@ int gemm_ref_simt(const __half* A, int lda, const __half* W, int ldw, int M, int
                   float* out, int ldo, cudaStream_t st);
 
 // ---- elementwise / data-movement kernels (kernels.cu) ------------------------------------------------
+// reverse: walk the rows from the last to the first
 int layernorm_f16(const float* x, const float* gamma, const float* beta, float eps, int M, int D,
-                  __half* out, cudaStream_t st);
+                  __half* out, bool reverse, cudaStream_t st);
 // rgb: [B,P,P,3] fp32 (dtype 0) or uint8 (dtype 1); out: [B*(P/16)^2, 768] fp16, k = ky*48+kx*3+c
 int im2col_patch16(const void* rgb, int dtype, int B, int P, const float* mean, const float* inv_std,
                    __half* out, cudaStream_t st);
@@ -73,22 +67,8 @@ void attention_force_simt(int mode);   // bit 0: SIMT kernel
 // points dtype: 0 = float32, 1 = int64, 2 = int32 ; pairs dtype: 1 = int64, 2 = int32
 int topo_sample_features(const float* feat_nchw, int B, int C, int s, int P, const void* points,
                          int pts_dtype, int N, __half* out, cudaStream_t st);
-int topo_pair_features(const float* pst, const float* w_off, const float* bias, const void* points,
-                       int pts_dtype, const void* pairs, int pairs_dtype, int B, int N, int Ns,
-                       int Np, int zero_offset, float* x32, __half* x16, cudaStream_t st);
-int topo_fix_valid(const uint8_t* valid, int rows, int Np, uint8_t* out, cudaStream_t st);
-int topo_attention(const __half* qkv, const uint8_t* valid, int rows, int Np, __half* out,
-                   cudaStream_t st);
-int topo_output(const float* x32, const uint8_t* valid_fixed, const float* w, const float* b,
-                int tokens, float* logits, float* scores, cudaStream_t st);
-
-// fused 3-layer transformer + output_proj for n_pairs == 16 (toponet_tc.cuh)
-struct TopoFusedParams {
-  const float *in_b[3], *out_b[3], *l1_b[3], *l2_b[3], *n1_g[3], *n1_b[3], *n2_g[3], *n2_b[3];
-  const float* out_w;        // [128]
-  const float* out_b_final;  // [1]
-};
-struct TopoPairInputs {       // what topo_pair_features reads; the fused kernel forms x itself
+// pair features (model.py:96-120): x = relu(Ws f[src] + Wt f[tgt] + Wo (pt[tgt] - pt[src]) + bias)
+struct TopoPairInputs {
   const float* pst;          // [B*N, 256] per-point projections (Ws f | Wt f)
   const float* w_off;        // [128][2]
   const float* bias;         // [128]
@@ -96,9 +76,26 @@ struct TopoPairInputs {       // what topo_pair_features reads; the fused kernel
   const void* pairs;         // [B, Ns, Np, 2]
   int pts_dtype, pairs_dtype, N, tokens_per_b, zero_offset;
 };
-int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, const TopoFusedParams& fp,
-                           const uint8_t* valid_fixed, int tokens, float* logits, float* scores,
-                           cudaStream_t st);
+int topo_pair_features(const TopoPairInputs& in, int tokens, float* x32, __half* x16, cudaStream_t st);
+int topo_fix_valid(const uint8_t* valid, int rows, int Np, uint8_t* out, cudaStream_t st);
+int topo_attention(const __half* qkv, const uint8_t* valid, int rows, int Np, __half* out,
+                   cudaStream_t st);
+int topo_output(const float* x32, const uint8_t* valid_fixed, const float* w, const float* b,
+                int tokens, float* logits, float* scores, cudaStream_t st);
+
+// fp32 parameters of one post-norm encoder layer (torch TransformerEncoderLayer, d = 128)
+struct TopoLayerParams {
+  const float* in_b;    // [384]
+  const float* out_b;   // [128]
+  const float* l1_b;    // [128]
+  const float* l2_b;    // [128]
+  const float *n1_g, *n1_b, *n2_g, *n2_b;   // [128]
+};
+// fused 3-layer transformer + output_proj for n_pairs == 16 (toponet_tc.cuh).  w_chunks: per layer
+// Wq, Wk, Wv, Wo, W1, W2 as [128, 128] fp16 blocks; out_w [128], out_b [1].
+int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, const TopoLayerParams* layers,
+                           const float* out_w, const float* out_b, const uint8_t* valid_fixed, int tokens,
+                           float* logits, float* scores, cudaStream_t st);
 
 // ---- SAM mask-decoder path (sam_decoder.cu), USE_SAM_DECODER: True --------------------------------
 struct SamAttnW { const float *qw, *qb, *kw, *kb, *vw, *vb, *ow, *ob; };

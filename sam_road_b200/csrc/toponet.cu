@@ -15,16 +15,6 @@
 
 namespace srb {
 
-__device__ __forceinline__ float load_coord(const void* p, int dtype, size_t idx) {
-  if (dtype == 0) return static_cast<const float*>(p)[idx];
-  if (dtype == 1) return static_cast<float>(static_cast<const long long*>(p)[idx]);
-  return static_cast<float>(static_cast<const int*>(p)[idx]);
-}
-__device__ __forceinline__ long long load_index(const void* p, int dtype, size_t idx) {
-  if (dtype == 1) return static_cast<const long long*>(p)[idx];
-  return static_cast<long long>(static_cast<const int*>(p)[idx]);
-}
-
 // ------------------------------------------------------------------------------------------------
 // Bilinear sampling of image_embeddings [B,C,s,s] fp32 at pixel-space points (x,y):
 //   g = pt / P * 2 - 1 (model.py:47) ; grid_sample unnormalise: u = ((g + 1) * s - 1) / 2 ;
@@ -76,38 +66,21 @@ int topo_sample_features(const float* feat_nchw, int B, int C, int s, int P, con
 //   pst: [B*N, 256] fp32, columns 0..127 = Ws f, 128..255 = Wt f.   One block (128 thr) per token.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
-topo_pair_kernel(const float* __restrict__ pst, const float* __restrict__ w_off,
-                 const float* __restrict__ bias, const void* points, int pts_dtype,
-                 const void* pairs, int pairs_dtype, int N, int tokens_per_b, int zero_offset,
-                 float* __restrict__ x32, __half* __restrict__ x16) {
+topo_pair_kernel(const TopoPairInputs in, float* __restrict__ x32, __half* __restrict__ x16) {
   const size_t tok = blockIdx.x;
-  const int b = static_cast<int>(tok / tokens_per_b);
-  // indices are clamped into [0, N): an out-of-range pair (an IndexError in the reference) must not
-  // become an out-of-bounds read here
-  const long long src = min(max(load_index(pairs, pairs_dtype, tok * 2 + 0), 0LL), static_cast<long long>(N) - 1);
-  const long long tgt = min(max(load_index(pairs, pairs_dtype, tok * 2 + 1), 0LL), static_cast<long long>(N) - 1);
-  const size_t ps = static_cast<size_t>(b) * N + src, pt = static_cast<size_t>(b) * N + tgt;
-  float ox = 0.f, oy = 0.f;
-  if (!zero_offset) {
-    ox = load_coord(points, pts_dtype, pt * 2 + 0) - load_coord(points, pts_dtype, ps * 2 + 0);
-    oy = load_coord(points, pts_dtype, pt * 2 + 1) - load_coord(points, pts_dtype, ps * 2 + 1);
-  }
+  const PairToken pr = resolve_pair(in, tok);
   const int c = threadIdx.x;
-  float v = pst[ps * 256 + c] + pst[pt * 256 + 128 + c];
-  v += __ldg(w_off + c * 2 + 0) * ox + __ldg(w_off + c * 2 + 1) * oy + __ldg(bias + c);
+  float v = __ldg(in.pst + pr.ps * 256 + c) + __ldg(in.pst + pr.pt * 256 + 128 + c);
+  v += __ldg(in.w_off + c * 2 + 0) * pr.ox + __ldg(in.w_off + c * 2 + 1) * pr.oy + __ldg(in.bias + c);
   v = fmaxf(v, 0.f);
   x32[tok * 128 + c] = v;
   x16[tok * 128 + c] = __float2half_rn(v);
 }
 
-int topo_pair_features(const float* pst, const float* w_off, const float* bias, const void* points,
-                       int pts_dtype, const void* pairs, int pairs_dtype, int B, int N, int Ns,
-                       int Np, int zero_offset, float* x32, __half* x16, cudaStream_t st) {
-  SRB_REQUIRE(pairs_dtype == 1 || pairs_dtype == 2, "topo_pair: pairs dtype %d", pairs_dtype);
-  const long tokens = static_cast<long>(B) * Ns * Np;
+int topo_pair_features(const TopoPairInputs& in, int tokens, float* x32, __half* x16, cudaStream_t st) {
+  SRB_REQUIRE(in.pairs_dtype == 1 || in.pairs_dtype == 2, "topo_pair: pairs dtype %d", in.pairs_dtype);
   if (tokens <= 0) return 0;
-  topo_pair_kernel<<<static_cast<unsigned>(tokens), 128, 0, st>>>(
-      pst, w_off, bias, points, pts_dtype, pairs, pairs_dtype, N, Ns * Np, zero_offset, x32, x16);
+  topo_pair_kernel<<<static_cast<unsigned>(tokens), 128, 0, st>>>(in, x32, x16);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch();
   return 0;
@@ -247,9 +220,9 @@ int topo_output(const float* x32, const uint8_t* valid_fixed, const float* w, co
 // per-point projections pst; weights = 18 chunks [128x128] fp16 in consumption order (per layer:
 // Wq, Wk, Wv, Wo, W1, W2)
 // ------------------------------------------------------------------------------------------------
-int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, const TopoFusedParams& fp,
-                           const uint8_t* valid_fixed, int tokens, float* logits, float* scores,
-                           cudaStream_t st) {
+int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, const TopoLayerParams* layers,
+                           const float* out_w, const float* out_b, const uint8_t* valid_fixed, int tokens,
+                           float* logits, float* scores, cudaStream_t st) {
   if (tokens <= 0) return 0;
   SRB_REQUIRE(in.pairs_dtype == 1 || in.pairs_dtype == 2, "topo fused: pairs dtype %d", in.pairs_dtype);
   CUtensorMap tmW;
@@ -260,16 +233,9 @@ int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, con
                                      kTtcSmemBytes));
   }
   TtcParams p;
-  for (int l = 0; l < 3; ++l) {
-    p.layer[l].in_b = fp.in_b[l]; p.layer[l].out_b = fp.out_b[l];
-    p.layer[l].l1_b = fp.l1_b[l]; p.layer[l].l2_b = fp.l2_b[l];
-    p.layer[l].n1_g = fp.n1_g[l]; p.layer[l].n1_b = fp.n1_b[l];
-    p.layer[l].n2_g = fp.n2_g[l]; p.layer[l].n2_b = fp.n2_b[l];
-  }
-  p.pst = in.pst; p.w_off = in.w_off; p.pair_b = in.bias; p.points = in.points; p.pairs = in.pairs;
-  p.pts_dtype = in.pts_dtype; p.pairs_dtype = in.pairs_dtype; p.N = in.N;
-  p.tokens_per_b = in.tokens_per_b; p.zero_offset = in.zero_offset;
-  p.valid = valid_fixed; p.out_w = fp.out_w; p.out_b = fp.out_b_final;
+  for (int l = 0; l < 3; ++l) p.layer[l] = layers[l];
+  p.in = in;
+  p.valid = valid_fixed; p.out_w = out_w; p.out_b = out_b;
   p.logits = logits; p.scores = scores; p.tokens = tokens;
   p.num_tiles = (tokens + 127) / 128;
   const int grid = p.num_tiles < device_sm_count() ? p.num_tiles : device_sm_count();

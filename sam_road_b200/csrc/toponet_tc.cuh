@@ -46,24 +46,9 @@ constexpr int kTtcChunksPerLayer = 6;             // Wq, Wk, Wv, Wo, W1, W2 as p
 // which may only happen once every warpgroup has finished the in_proj GEMMs)
 __host__ __device__ constexpr int ttc_chunk(int i) { return i == 0 ? 1 : (i == 1 ? 2 : (i == 2 ? 0 : i)); }
 
-struct TtcLayerParams {
-  const float* in_b;    // [384]
-  const float* out_b;   // [128]
-  const float* l1_b;    // [128]
-  const float* l2_b;    // [128]
-  const float *n1_g, *n1_b, *n2_g, *n2_b;   // [128]
-};
-
 struct TtcParams {
-  TtcLayerParams layer[3];
-  // pair features (model.py:96-120), computed in the kernel: x = relu(PS[b,src] + PT[b,tgt] +
-  // Wo (pt[tgt] - pt[src]) + bias) with the per-point projections pst [B*N, 256] (Ws f | Wt f)
-  const float* pst;
-  const float* w_off;     // [128][2]
-  const float* pair_b;    // [128]
-  const void* points;     // [B, N, 2] (x, y)
-  const void* pairs;      // [B, Ns, Np, 2] indices into N
-  int pts_dtype, pairs_dtype, N, tokens_per_b, zero_offset;
+  TopoLayerParams layer[3];
+  TopoPairInputs in;      // the kernel forms the pair features itself
   const uint8_t* valid;   // [tokens] fixed validity (all-invalid rows already flipped), or null
   const float* out_w;     // [128]
   const float* out_b;     // [1]
@@ -73,14 +58,39 @@ struct TtcParams {
   int num_tiles;
 };
 
-__device__ __forceinline__ float ttc_load_coord(const void* p, int dtype, size_t idx) {
+// ------------------------------------------------------------------------------------------------
+// Pair-token gather, shared with topo_pair_kernel (toponet.cu)
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float load_coord(const void* p, int dtype, size_t idx) {
   if (dtype == 0) return static_cast<const float*>(p)[idx];
   if (dtype == 1) return static_cast<float>(static_cast<const long long*>(p)[idx]);
   return static_cast<float>(static_cast<const int*>(p)[idx]);
 }
-__device__ __forceinline__ long long ttc_load_index(const void* p, int dtype, size_t idx) {
+__device__ __forceinline__ long long load_index(const void* p, int dtype, size_t idx) {
   if (dtype == 1) return static_cast<const long long*>(p)[idx];
   return static_cast<long long>(static_cast<const int*>(p)[idx]);
+}
+
+// Rows of a pair token's source and target point in pst / points (b * N + index) and its offset
+// pt[tgt] - pt[src] (zero for TOPONET_VERSION 'no_offset').
+struct PairToken {
+  size_t ps, pt;
+  float ox, oy;
+};
+__device__ __forceinline__ PairToken resolve_pair(const TopoPairInputs& in, size_t tok) {
+  const size_t b = tok / in.tokens_per_b;
+  // indices are clamped into [0, N): an out-of-range pair (an IndexError in the reference) must not
+  // become an out-of-bounds read here
+  const long long nm1 = static_cast<long long>(in.N) - 1;
+  PairToken r;
+  r.ps = b * in.N + min(max(load_index(in.pairs, in.pairs_dtype, tok * 2 + 0), 0LL), nm1);
+  r.pt = b * in.N + min(max(load_index(in.pairs, in.pairs_dtype, tok * 2 + 1), 0LL), nm1);
+  r.ox = r.oy = 0.f;
+  if (!in.zero_offset) {
+    r.ox = load_coord(in.points, in.pts_dtype, r.pt * 2 + 0) - load_coord(in.points, in.pts_dtype, r.ps * 2 + 0);
+    r.oy = load_coord(in.points, in.pts_dtype, r.pt * 2 + 1) - load_coord(in.points, in.pts_dtype, r.ps * 2 + 1);
+  }
+  return r;
 }
 
 // warp-level MMA for the 16 x 16 attention of one sample and head (far too small for a UMMA tile)
@@ -302,25 +312,12 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
 
   // source / target rows and offset of this thread's pair token in tile `t` (index -> address chain
   // of the gather; issued one tile ahead so that only the pst loads themselves are exposed)
-    float nx_ox = 0.f, nx_oy = 0.f;
-    size_t nx_ps = 0, nx_pt = 0;
-    auto pair_lookup = [&](int t) {
-      const long tk = static_cast<long>(t) * 128 + row;
-      nx_ox = nx_oy = 0.f;
-      nx_ps = nx_pt = 0;
-      if (t < p.num_tiles && tk < p.tokens) {
-        const size_t b = static_cast<size_t>(tk) / p.tokens_per_b;
-        const long long nm1 = static_cast<long long>(p.N) - 1;    // clamp: no out-of-bounds gather on bad indices
-        nx_ps = b * p.N + min(max(ttc_load_index(p.pairs, p.pairs_dtype, static_cast<size_t>(tk) * 2 + 0), 0LL), nm1);
-        nx_pt = b * p.N + min(max(ttc_load_index(p.pairs, p.pairs_dtype, static_cast<size_t>(tk) * 2 + 1), 0LL), nm1);
-        if (!p.zero_offset) {
-          nx_ox = ttc_load_coord(p.points, p.pts_dtype, nx_pt * 2 + 0) -
-                  ttc_load_coord(p.points, p.pts_dtype, nx_ps * 2 + 0);
-          nx_oy = ttc_load_coord(p.points, p.pts_dtype, nx_pt * 2 + 1) -
-                  ttc_load_coord(p.points, p.pts_dtype, nx_ps * 2 + 1);
-        }
-      }
-    };
+  PairToken nx{0, 0, 0.f, 0.f};
+  auto pair_lookup = [&](int t) {
+    const long tk = static_cast<long>(t) * 128 + row;
+    nx = PairToken{0, 0, 0.f, 0.f};
+    if (t < p.num_tiles && tk < p.tokens) nx = resolve_pair(p.in, static_cast<size_t>(tk));
+  };
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++ti) {
       const long tok = static_cast<long>(tile) * 128 + row;
       const bool tok_ok = tok < p.tokens;
@@ -340,15 +337,15 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
     // ---- pair features of this token -> residual (fp32 registers) and A buffer (fp16) ----
     {
       if (ti == 0) pair_lookup(tile);              // later tiles: looked up during the previous tile
-      const float ox = nx_ox, oy = nx_oy;
-      const size_t ps = nx_ps, pt = nx_pt;
+      const float ox = nx.ox, oy = nx.oy;
+      const size_t ps = nx.ps, pt = nx.pt;
         {
           const int c = part;
           float v[32];
-          const float4* a4 = reinterpret_cast<const float4*>(p.pst + ps * 256 + c * 32);
-          const float4* b4 = reinterpret_cast<const float4*>(p.pst + pt * 256 + 128 + c * 32);
-          const float4* w4 = reinterpret_cast<const float4*>(p.w_off + c * 64);
-          const float4* c4 = reinterpret_cast<const float4*>(p.pair_b + c * 32);
+          const float4* a4 = reinterpret_cast<const float4*>(p.in.pst + ps * 256 + c * 32);
+          const float4* b4 = reinterpret_cast<const float4*>(p.in.pst + pt * 256 + 128 + c * 32);
+          const float4* w4 = reinterpret_cast<const float4*>(p.in.w_off + c * 64);
+          const float4* c4 = reinterpret_cast<const float4*>(p.in.bias + c * 32);
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const float4 a = a4[i], bb = b4[i], w0 = __ldg(w4 + 2 * i), w1 = __ldg(w4 + 2 * i + 1),
@@ -374,7 +371,7 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
     float dot = 0.f;
 #pragma unroll 1
     for (int l = 0; l < 3; ++l) {
-      const TtcLayerParams& L = p.layer[l];
+      const TopoLayerParams& L = p.layer[l];
       float acc[2][16];
       // ================= in_proj: k, v of head `part` -> smem (fp16 rows, bias added) =================
 #pragma unroll 1

@@ -28,7 +28,21 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, n), f"{n} declared in include/samroad_b200.h but not exported"
     assert set(_lib.SIGNATURES) == set(names), set(_lib.SIGNATURES) ^ set(names)
     bound = _lib.load()
-    assert bound.samroad_abi_version() == 2
+    # the version is written in the header and in _lib.py; the library must report both
+    src = open(os.path.join(ROOT, "include", "samroad_b200.h")).read()
+    header_version = int(re.search(r"#define SAMROAD_ABI_VERSION (\d+)", src).group(1))
+    assert bound.samroad_abi_version() == _lib.ABI_VERSION == header_version
+
+
+@pytest.mark.parametrize("act", [3, 100])
+def test_gemm_rejects_unknown_activation(act):
+    # the activation is checked before any CUDA call, so this needs no GPU
+    lib = _lib.load()
+    rc = lib.samroad_op_gemm_f16(None, 64, None, 64, 128, 128, 64, None, act, None, 128, None)
+    assert rc != 0 and f"act={act}" in _lib.last_error()
+    rc = lib.samroad_op_gemm_ln(None, 64, None, 64, 128, 128, 64, None, None, None, None, 1e-6, 128, act,
+                                None, None, None, 1, 128, None)
+    assert rc != 0 and f"act={act}" in _lib.last_error()
 
 
 def test_cfg_struct_matches_header():

@@ -116,11 +116,11 @@ def test_encode_and_topo_parity(name, patch, version, B, lora):
 
 def test_benched_configuration_b64_composition():
     """The configuration bench.py times: ViT-B @512, B = 64 tiles in ONE call -- persistent GEMM CTAs
-    running many tiles each, snake traversal, thousands of attention CTAs.
+    running many tiles each, LayerNorms alternating their row order, thousands of attention CTAs.
     (a) 4 of the 64 tiles against the oracle at the 1e-3 tolerance; (b) the same 4 tiles from a B = 4
-    call with ascending traversal (debug bit 16), which must agree with the B = 64 result to rounding
-    (a different grid fill can pick other GEMM tile shapes); (c) the traversal order (snake or
-    ascending) must not change any bit, at B = 64 and at B = 4; (d) a tile's result must not depend on
+    call with every LayerNorm walking its rows ascending (debug bit 16), which must agree with the
+    B = 64 result to rounding (a different grid fill can pick other GEMM tile shapes); (c) the
+    LayerNorm row order (alternating or ascending) must not change any bit, at B = 64 and at B = 4; (d) a tile's result must not depend on
     where it sits in the batch: permuting the batch permutes the output bit for bit."""
     from sam_road_b200 import _lib
     lib = _lib.load()
