@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define SAMROAD_ABI_VERSION 3
+#define SAMROAD_ABI_VERSION 4
 
 typedef struct samroad_ctx* samroad_handle_t;
 
@@ -85,8 +85,8 @@ int samroad_encode_masks_scene(samroad_handle_t h, const uint8_t* scene, int H, 
 /* SAMRoad.infer_toponet (model.py:498-508) = BilinearSampler (model.py:34-58) + TopoNet.forward
  * (model.py:88-148).  image_embeddings: device fp32 [B,256,s,s]; points [B,N,2] (x,y) pixels,
  * SAMROAD_F32 / I64 / I32; pairs [B,Ns,Np,2] indices into N, SAMROAD_I64 / I32; valid [B,Ns,Np]
- * bytes (0/1).  Outputs fp32 [B,Ns,Np] (either may be NULL).  Slots masked by `valid` report
- * output_proj.bias, mirroring torch's eval fast path (SURVEY.md §8a P4). */
+ * bytes (0/1), Np = MAX_NEIGHBOR_QUERIES in 1..32.  Outputs fp32 [B,Ns,Np] (either may be NULL).
+ * Slots masked by `valid` report output_proj.bias, mirroring torch's eval fast path (SURVEY.md §8a P4). */
 int samroad_toponet(samroad_handle_t h, const float* image_embeddings, const void* points,
                     int pts_dtype, const void* pairs, int pairs_dtype, const uint8_t* valid, int B,
                     int N, int Ns, int Np, float* topo_logits, float* topo_scores, void* stream);
@@ -150,16 +150,21 @@ int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* keypoint_mask
 /* Pair-query construction of inferencer.py:126-197 for every tile of the scene: the box query
  * (rtree.intersection, inclusive bounds, ascending point index) and the per-tile kNN
  * (KDTree.query(k=MAX_NEIGHBOR_QUERIES+1, distance_upper_bound=NEIGHBOR_RADIUS) minus self: strictly
- * closer than the radius, ascending distance, equal distances in ascending index).  points_xy: device
- * int64 [N,2]; tile_xy_host: host int32 [n_tiles,2] tile origins (x0,y0) in tile-list order.
- * Writes the number of points of every tile to tile_counts_host (the caller pads each batch to its
- * own maximum, inferencer.py:179-185).  Synchronises the stream. */
+ * closer than the radius, ascending distance, equal distances in ascending index) for
+ * max_nbr = MAX_NEIGHBOR_QUERIES in 1..32.  points_xy: device int64 [N,2]; tile_xy_host: host int32
+ * [n_tiles,2] tile origins (x0,y0) in tile-list order.  Writes the number of points of every tile to
+ * tile_counts_host (the caller pads each batch to its own maximum, inferencer.py:179-185).  The plan
+ * serves fill / aggregate calls with any K <= max_nbr.  Synchronises the stream. */
+int samroad_pair_queries_plan_k(samroad_graph_t g, const int64_t* points_xy, int N,
+                                const int32_t* tile_xy_host, int n_tiles, int P, double radius,
+                                int max_nbr, int32_t* tile_counts_host, void* stream);
+/* samroad_pair_queries_plan_k with max_nbr = 16. */
 int samroad_pair_queries_plan(samroad_graph_t g, const int64_t* points_xy, int N,
                               const int32_t* tile_xy_host, int n_tiles, int P, double radius,
                               int32_t* tile_counts_host, void* stream);
 /* Padded batch tensors for tiles [tile_begin, tile_begin+B): points int32 [B,nmax,2] relative to the
  * tile origin, pairs int32 [B,nmax,K,2], valid bytes [B,nmax,K] (device) -- the inputs of
- * samroad_toponet (inferencer.py:164-197).  Asynchronous. */
+ * samroad_toponet (inferencer.py:164-197).  K may not exceed the planned max_nbr.  Asynchronous. */
 int samroad_pair_queries_fill(samroad_graph_t g, int tile_begin, int B, int nmax, int K,
                               int32_t* points, int32_t* pairs, uint8_t* valid, void* stream);
 
@@ -168,7 +173,8 @@ int samroad_pair_queries_fill(samroad_graph_t g, int tile_begin, int B, int nmax
  * the tile's batch was skipped, inferencer.py:188-189).  Per directed (src,tgt) the scores are added in
  * float32 in (tile, sample, pair) order, averaged and compared with `> threshold`; surviving edges are
  * written in first-occurrence order as int64 [n,2] global point indices.  *bad_score != 0 when a score
- * fell outside [0,1] (the reference asserts).  Synchronises the stream. */
+ * fell outside [0,1] (the reference asserts).  K may not exceed the planned max_nbr.  Synchronises the
+ * stream. */
 int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scores,
                             const int64_t* tile_score_offset_host, int K, float threshold,
                             int64_t* edges, int cap, int* n_edges, int* bad_score, void* stream);

@@ -13,7 +13,7 @@ _PKG = Path(__file__).resolve().parent
 LIB_PATH = _PKG / "libsamroad_b200.so"
 
 F32, I64, I32, U8, F64 = 0, 1, 2, 3, 4
-ABI_VERSION = 3
+ABI_VERSION = 4
 TOPO_NORMAL, TOPO_NO_OFFSET, TOPO_NO_TRANSFORMER = 0, 1, 2
 ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
 
@@ -53,6 +53,7 @@ SIGNATURES = {
     "samroad_extract_graph_points": (_i, [_vp, _vp, _vp, _i, _i, _d, _d, _d, _d, ARGSORT_FN, _vp, _vp, _i,
                                           _ip, _vp, _vp]),
     "samroad_pair_queries_plan": (_i, [_vp, _vp, _i, _vp, _i, _i, _d, _vp, _vp]),
+    "samroad_pair_queries_plan_k": (_i, [_vp, _vp, _i, _vp, _i, _i, _d, _i, _vp, _vp]),
     "samroad_pair_queries_fill": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "samroad_aggregate_edges": (_i, [_vp, _vp, _vp, _i, _f, _vp, _i, _ip, _ip, _vp]),
     "samroad_encode_masks_host": (_i, [_vp, _vp, _i, _i, _vp, _vp]),

@@ -81,6 +81,8 @@ struct samroad_graph_ctx {
   int N = 0, n_tiles = 0, P = 0;
   long total = 0;
   int d2lt = 0;                           // neighbours satisfy d^2 < d2lt
+  int max_nbr = 0;                        // K the plan was made for (fill / aggregate take K <= max_nbr)
+  int nbr_stride = 16;                    // row length of nbr: 16 for max_nbr <= 16, else 32
   // aggregation
   DevBuf adj_deg, adj_off, adj_src, adj_tgt, adj_sum, adj_cnt, adj_first, eflags, tile_soff;
 };
@@ -854,9 +856,10 @@ tile_fill_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restri
   }
 }
 
-// KDTree.query(k = K+1, distance_upper_bound = R) minus self (inferencer.py:159-163): the (up to) 16
+// KDTree.query(k = K+1, distance_upper_bound = R) minus self (inferencer.py:159-163): the (up to) KN
 // nearest other points of the same tile with d < R, ascending distance; equal distances in ascending
-// index.  Brute force per tile (a tile holds a few hundred points).
+// index; nbr rows are KN long.  Brute force per tile (a tile holds a few hundred points).
+template <int KN>
 __global__ void __launch_bounds__(128)
 knn_kernel(const int32_t* __restrict__ pts, const int* __restrict__ cnt, const int* __restrict__ off,
            const int32_t* __restrict__ members, int d2lt, int32_t* __restrict__ nbr) {
@@ -868,9 +871,9 @@ knn_kernel(const int32_t* __restrict__ pts, const int* __restrict__ cnt, const i
   const int j = blockIdx.y * 128 + threadIdx.x;
   int px = 0, py = 0;
   if (j < n) { const int gi = members[base + j]; px = pts[2 * gi]; py = pts[2 * gi + 1]; }
-  int bd[16], bi[16];
+  int bd[KN], bi[KN];
 #pragma unroll
-  for (int k = 0; k < 16; ++k) { bd[k] = INT_MAX; bi[k] = -1; }
+  for (int k = 0; k < KN; ++k) { bd[k] = INT_MAX; bi[k] = -1; }
   for (int c0 = 0; c0 < n; c0 += 128) {
     const int c = c0 + threadIdx.x;
     if (c < n) { const int gi = members[base + c]; sx[threadIdx.x] = pts[2 * gi]; sy[threadIdx.x] = pts[2 * gi + 1]; }
@@ -881,11 +884,11 @@ knn_kernel(const int32_t* __restrict__ pts, const int* __restrict__ cnt, const i
         const int lc = c0 + q;
         const int dx = sx[q] - px, dy = sy[q] - py;
         const int d2 = dx * dx + dy * dy;
-        if (lc == j || d2 >= d2lt || d2 >= bd[15]) continue;
+        if (lc == j || d2 >= d2lt || d2 >= bd[KN - 1]) continue;
         int cd = d2, ci = lc;
         bool ins = false;
 #pragma unroll
-        for (int k = 0; k < 16; ++k) {
+        for (int k = 0; k < KN; ++k) {
           if (ins || cd < bd[k]) {
             const int td = bd[k], ti = bi[k];
             bd[k] = cd; bi[k] = ci; cd = td; ci = ti;
@@ -898,12 +901,13 @@ knn_kernel(const int32_t* __restrict__ pts, const int* __restrict__ cnt, const i
   }
   if (j < n) {
 #pragma unroll
-    for (int k = 0; k < 16; ++k) nbr[(static_cast<size_t>(base) + j) * 16 + k] = bi[k];
+    for (int k = 0; k < KN; ++k) nbr[(static_cast<size_t>(base) + j) * KN + k] = bi[k];
   }
 }
 
 // padded batch tensors (inferencer.py:164-185): points relative to the tile origin, pairs (src, tgt or src),
-// prefix-valid mask; rows beyond the tile's point count are zero (np.pad)
+// prefix-valid mask; rows beyond the tile's point count are zero (np.pad).  nbr rows are NS long.
+template <int NS>
 __global__ void fill_batch_kernel(const int32_t* __restrict__ pts, const int32_t* __restrict__ txy,
                                   const int* __restrict__ cnt, const int* __restrict__ off,
                                   const int32_t* __restrict__ members, const int32_t* __restrict__ nbr,
@@ -920,7 +924,7 @@ __global__ void fill_batch_kernel(const int32_t* __restrict__ pts, const int32_t
   int src = 0, tgt = 0;
   uint8_t v = 0;
   if (j < n) {
-    const int nb = nbr[(static_cast<size_t>(off[t]) + j) * 16 + k];
+    const int nb = nbr[(static_cast<size_t>(off[t]) + j) * NS + k];
     v = nb >= 0 ? 1 : 0;
     src = j;
     tgt = nb >= 0 ? nb : j;
@@ -943,16 +947,20 @@ __global__ void fill_batch_kernel(const int32_t* __restrict__ pts, const int32_t
 
 }  // namespace
 
-extern "C" int samroad_pair_queries_plan(samroad_graph_t g, const int64_t* points_xy, int N,
-                                         const int32_t* tile_xy_host, int n_tiles, int P, double radius,
-                                         int32_t* tile_counts_host, void* stream) {
+extern "C" int samroad_pair_queries_plan_k(samroad_graph_t g, const int64_t* points_xy, int N,
+                                           const int32_t* tile_xy_host, int n_tiles, int P, double radius,
+                                           int max_nbr, int32_t* tile_counts_host, void* stream) {
   SRB_REQUIRE(g && tile_xy_host && tile_counts_host, "samroad_pair_queries_plan: null argument");
+  SRB_REQUIRE(max_nbr >= 1 && max_nbr <= 32, "samroad_pair_queries_plan: MAX_NEIGHBOR_QUERIES=%d must be in 1..32",
+              max_nbr);
   SRB_REQUIRE(N >= 0 && n_tiles > 0 && P > 0, "samroad_pair_queries_plan: bad sizes N=%d tiles=%d P=%d", N, n_tiles, P);
   SRB_REQUIRE(N == 0 || points_xy != nullptr, "samroad_pair_queries_plan: null points");
   SRB_REQUIRE(radius >= 0.0 && radius < 30000.0, "samroad_pair_queries_plan: radius %.3f", radius);
   SRB_CUDA_OK(cudaSetDevice(g->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   g->N = N; g->n_tiles = n_tiles; g->P = P;
+  g->max_nbr = max_nbr;
+  g->nbr_stride = max_nbr <= 16 ? 16 : 32;
   g->d2lt = static_cast<int>(std::ceil(radius * radius));        // d < R  <=>  d^2 < R^2  on integer d^2
   g->h_cnt.assign(n_tiles, 0);
   g->h_off.assign(n_tiles + 1, 0);
@@ -981,36 +989,50 @@ extern "C" int samroad_pair_queries_plan(samroad_graph_t g, const int64_t* point
     if (g->h_cnt[t] > max_cnt) max_cnt = g->h_cnt[t];
   }
   g->total = g->h_off[n_tiles];
-  SRB_REQUIRE(g->total * 16 < 2147483647L, "samroad_pair_queries_plan: %ld (tile, point) instances is too many", g->total);
+  SRB_REQUIRE(g->total * g->max_nbr < 2147483647L, "samroad_pair_queries_plan: %ld (tile, point) instances is too many", g->total);
   SRB_CUDA_OK(cudaMemcpyAsync(g->t_off.p, g->h_off.data(), sizeof(int) * (n_tiles + 1), cudaMemcpyHostToDevice, st));
   if (g->total == 0) { SRB_CUDA_OK(cudaStreamSynchronize(st)); return 0; }
   if (int rc = g->members.ensure(sizeof(int32_t) * static_cast<size_t>(g->total))) return rc;
-  if (int rc = g->nbr.ensure(sizeof(int32_t) * 16 * static_cast<size_t>(g->total))) return rc;
+  if (int rc = g->nbr.ensure(sizeof(int32_t) * g->nbr_stride * static_cast<size_t>(g->total))) return rc;
   tile_fill_kernel<<<n_tiles, 256, 0, st>>>(g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P, g->t_off.as<int>(),
                                             g->members.as<int32_t>());
-  knn_kernel<<<dim3(n_tiles, (max_cnt + 127) / 128), 128, 0, st>>>(g->pts32.as<int32_t>(), g->t_cnt.as<int>(),
-                                                                   g->t_off.as<int>(), g->members.as<int32_t>(),
-                                                                   g->d2lt, g->nbr.as<int32_t>());
+  const dim3 knn_grid(n_tiles, (max_cnt + 127) / 128);
+  if (g->nbr_stride == 16)
+    knn_kernel<16><<<knn_grid, 128, 0, st>>>(g->pts32.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
+                                             g->members.as<int32_t>(), g->d2lt, g->nbr.as<int32_t>());
+  else
+    knn_kernel<32><<<knn_grid, 128, 0, st>>>(g->pts32.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
+                                             g->members.as<int32_t>(), g->d2lt, g->nbr.as<int32_t>());
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(2);
   SRB_CUDA_OK(cudaStreamSynchronize(st));    // h_off was copied from pageable memory
   return 0;
 }
 
+extern "C" int samroad_pair_queries_plan(samroad_graph_t g, const int64_t* points_xy, int N,
+                                         const int32_t* tile_xy_host, int n_tiles, int P, double radius,
+                                         int32_t* tile_counts_host, void* stream) {
+  return samroad_pair_queries_plan_k(g, points_xy, N, tile_xy_host, n_tiles, P, radius, 16, tile_counts_host,
+                                     stream);
+}
+
 extern "C" int samroad_pair_queries_fill(samroad_graph_t g, int tile_begin, int B, int nmax, int K,
                                          int32_t* points, int32_t* pairs, uint8_t* valid, void* stream) {
   SRB_REQUIRE(g && points && pairs && valid, "samroad_pair_queries_fill: null argument");
-  SRB_REQUIRE(K >= 1 && K <= 16, "samroad_pair_queries_fill: MAX_NEIGHBOR_QUERIES=%d must be in 1..16", K);
+  SRB_REQUIRE(K >= 1 && K <= 32, "samroad_pair_queries_fill: MAX_NEIGHBOR_QUERIES=%d must be in 1..32", K);
   SRB_REQUIRE(tile_begin >= 0 && B >= 0 && tile_begin + B <= g->n_tiles,
               "samroad_pair_queries_fill: tiles [%d,%d) outside the planned %d", tile_begin, tile_begin + B, g->n_tiles);
   if (B == 0 || nmax <= 0) return 0;
+  SRB_REQUIRE(K <= g->max_nbr, "samroad_pair_queries_fill: MAX_NEIGHBOR_QUERIES=%d but the pair queries were "
+              "planned for %d", K, g->max_nbr);
   for (int b = 0; b < B; ++b)
     SRB_REQUIRE(g->h_cnt[tile_begin + b] <= nmax, "samroad_pair_queries_fill: tile %d has %d points > nmax=%d",
                 tile_begin + b, g->h_cnt[tile_begin + b], nmax);
   SRB_CUDA_OK(cudaSetDevice(g->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long total = static_cast<long>(B) * nmax * K;
-  fill_batch_kernel<<<blocks_for(total), 256, 0, st>>>(
+  auto* fill = g->nbr_stride == 16 ? fill_batch_kernel<16> : fill_batch_kernel<32>;
+  fill<<<blocks_for(total), 256, 0, st>>>(
       g->pts32.as<int32_t>(), g->tile_xy.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
       g->members.as<int32_t>(), g->nbr.as<int32_t>(), tile_begin, B, nmax, K, points, pairs, valid);
   SRB_CUDA_OK(cudaGetLastError());
@@ -1070,7 +1092,8 @@ __device__ __forceinline__ int lower_bound_i32(const int32_t* a, int n, int v) {
 // float32 sum is bit-identical.  The lanes own the source's adjacency slots (slot = lane + 32 d) and keep
 // sum / count / first occurrence in registers; a tile's K (target, score) pairs are loaded by K lanes at
 // once and broadcast one by one.  first[] records the key's first occurrence in the loop (dict order).
-template <int DPL>
+// nbr rows are NS long.
+template <int DPL, int NS>
 __global__ void __launch_bounds__(256)
 aggregate_warp_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restrict__ txy, int n_tiles, int P,
                       const int* __restrict__ cnt, const int* __restrict__ off, const int32_t* __restrict__ members,
@@ -1101,7 +1124,7 @@ aggregate_warp_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __r
     int Tk = -1;
     float vk = 0.f;
     if (lane < K) {
-      const int nb = nbr[(static_cast<size_t>(base) + j) * 16 + lane];
+      const int nb = nbr[(static_cast<size_t>(base) + j) * NS + lane];
       if (nb >= 0) {
         Tk = members[base + nb];
         vk = scores[so + static_cast<int64_t>(j) * K + lane];
@@ -1133,6 +1156,7 @@ aggregate_warp_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __r
 
 // Fallback for sources with more than 128 points within the neighbour radius (tiny NMS radii): one thread per
 // source, slots in global memory.  Same order of additions.
+template <int NS>
 __global__ void __launch_bounds__(128)
 aggregate_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restrict__ txy, int n_tiles, int P,
                  const int* __restrict__ cnt, const int* __restrict__ off, const int32_t* __restrict__ members,
@@ -1152,7 +1176,7 @@ aggregate_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restri
     const int j = lower_bound_i32(members + base, cnt[t], S);
     const float* sc = scores + so + static_cast<int64_t>(j) * K;
     for (int k = 0; k < K; ++k) {
-      const int nb = nbr[(static_cast<size_t>(base) + j) * 16 + k];
+      const int nb = nbr[(static_cast<size_t>(base) + j) * NS + k];
       if (nb < 0) break;                                     // prefix-valid
       const int T = members[base + nb];
       float v = sc[k];
@@ -1164,6 +1188,18 @@ aggregate_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restri
       if (first[slot] < 0) first[slot] = (base + j) * K + k;
     }
   }
+}
+
+template <int NS, typename... Args>
+void launch_aggregate(int max_deg, int N, cudaStream_t st, Args... args) {
+  if (max_deg <= 32)
+    aggregate_warp_kernel<1, NS><<<blocks_for(32L * N, 256), 256, 0, st>>>(args...);
+  else if (max_deg <= 64)
+    aggregate_warp_kernel<2, NS><<<blocks_for(32L * N, 256), 256, 0, st>>>(args...);
+  else if (max_deg <= 128)
+    aggregate_warp_kernel<4, NS><<<blocks_for(32L * N, 256), 256, 0, st>>>(args...);
+  else
+    aggregate_kernel<NS><<<blocks_for(N, 128), 128, 0, st>>>(args...);
 }
 
 __global__ void edge_select_kernel(const float* __restrict__ sum, const float* __restrict__ num,
@@ -1180,13 +1216,15 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
                                        int K, float threshold, int64_t* edges, int cap, int* n_edges,
                                        int* bad_score, void* stream) {
   SRB_REQUIRE(g && n_edges && tile_score_offset_host, "samroad_aggregate_edges: null argument");
-  SRB_REQUIRE(K >= 1 && K <= 16, "samroad_aggregate_edges: K=%d must be in 1..16", K);
+  SRB_REQUIRE(K >= 1 && K <= 32, "samroad_aggregate_edges: MAX_NEIGHBOR_QUERIES=%d must be in 1..32", K);
   SRB_CUDA_OK(cudaSetDevice(g->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   *n_edges = 0;
   if (bad_score) *bad_score = 0;
   const int N = g->N;
   if (N == 0 || g->total == 0) return 0;
+  SRB_REQUIRE(K <= g->max_nbr, "samroad_aggregate_edges: MAX_NEIGHBOR_QUERIES=%d but the pair queries were "
+              "planned for %d", K, g->max_nbr);
   SRB_REQUIRE(topo_scores != nullptr, "samroad_aggregate_edges: null scores");
   const int32_t* pts = g->pts32.as<int32_t>();
   if (int rc = g->adj_deg.ensure(sizeof(int) * static_cast<size_t>(N))) return rc;
@@ -1223,14 +1261,10 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
       g->members.as<int32_t>(), g->nbr.as<int32_t>(), topo_scores, g->tile_soff.as<int64_t>(), K,           \
       g->adj_off.as<int>(), g->adj_tgt.as<int32_t>(), g->adj_sum.as<float>(), g->adj_cnt.as<float>(),       \
       g->adj_first.as<int32_t>(), tot + 8
-  if (max_deg <= 32)
-    aggregate_warp_kernel<1><<<blocks_for(32L * N, 256), 256, 0, st>>>(SRB_AGG_ARGS);
-  else if (max_deg <= 64)
-    aggregate_warp_kernel<2><<<blocks_for(32L * N, 256), 256, 0, st>>>(SRB_AGG_ARGS);
-  else if (max_deg <= 128)
-    aggregate_warp_kernel<4><<<blocks_for(32L * N, 256), 256, 0, st>>>(SRB_AGG_ARGS);
+  if (g->nbr_stride == 16)
+    launch_aggregate<16>(max_deg, N, st, SRB_AGG_ARGS);
   else
-    aggregate_kernel<<<blocks_for(N, 128), 128, 0, st>>>(SRB_AGG_ARGS);
+    launch_aggregate<32>(max_deg, N, st, SRB_AGG_ARGS);
 #undef SRB_AGG_ARGS
   edge_select_kernel<<<blocks_for(nnz), 256, 0, st>>>(g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
                                                       g->adj_first.as<int32_t>(), nnz, threshold,

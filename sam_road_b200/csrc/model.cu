@@ -825,7 +825,7 @@ extern "C" int samroad_toponet(samroad_handle_t h, const float* image_embeddings
               "samroad_toponet: points dtype %d", pts_dtype);
   SRB_REQUIRE(pairs_dtype == SAMROAD_I64 || pairs_dtype == SAMROAD_I32,
               "samroad_toponet: pairs dtype %d", pairs_dtype);
-  SRB_REQUIRE(Np >= 1 && Np <= 16, "samroad_toponet: n_pairs=%d must be in 1..16", Np);
+  SRB_REQUIRE(Np >= 1 && Np <= 32, "samroad_toponet: n_pairs=%d must be in 1..32", Np);
   if (B <= 0 || Ns <= 0) return 0;
   SRB_REQUIRE(N > 0, "samroad_toponet: N=%d points but Ns=%d samples", N, Ns);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -849,14 +849,14 @@ extern "C" int samroad_toponet(samroad_handle_t h, const float* image_embeddings
         gemm_f32out(w.PF16, 128, h->tp_st_w, 128, pts, 256, 128, nullptr, nullptr, nullptr, 0, w.PST,
                     256, st));
   SRB_T(KT_TOPO_PAIR, 0, tokd * 2, topo_fix_valid(valid, rows, Np, w.VF, st));
-  const bool fused = !no_tf && Np == 16;
+  const bool fused = !no_tf && (Np == 16 || Np == 32);
   const TopoPairInputs pin{w.PST, h->tp_off_w, h->tp_pair_b, points, pairs, pts_dtype, pairs_dtype, N,
                            Ns * Np, zero_off};
   if (fused) {
     // all three encoder layers + output_proj in one persistent wgmma kernel
-    SRB_T(KT_TOPO_GEMM, tokd * 2 * 128 * (384 + 128 * 3) * 3 + tokd * 4 * 16 * 128 * 3 + tokd * 128 * 6,
+    SRB_T(KT_TOPO_GEMM, tokd * 2 * 128 * (384 + 128 * 3) * 3 + tokd * 4 * Np * 128 * 3 + tokd * 128 * 6,
           tokd * 1024 * 2 + tokd * 8,
-          topo_transformer_fused(pin, h->tp_chunks, h->tp_layers, h->tp_out_w, h->tp_out_b, w.VF, tok,
+          topo_transformer_fused(pin, h->tp_chunks, h->tp_layers, h->tp_out_w, h->tp_out_b, w.VF, tok, Np,
                                  topo_logits, topo_scores, st));
     return 0;
   }

@@ -91,11 +91,11 @@ struct TopoLayerParams {
   const float* l2_b;    // [128]
   const float *n1_g, *n1_b, *n2_g, *n2_b;   // [128]
 };
-// fused 3-layer transformer + output_proj for n_pairs == 16 (toponet_tc.cuh).  w_chunks: per layer
-// Wq, Wk, Wv, Wo, W1, W2 as [128, 128] fp16 blocks; out_w [128], out_b [1].
+// fused 3-layer transformer + output_proj for n_pairs Np == 16 or 32 (toponet_tc.cuh).  w_chunks: per
+// layer Wq, Wk, Wv, Wo, W1, W2 as [128, 128] fp16 blocks; out_w [128], out_b [1].
 int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, const TopoLayerParams* layers,
                            const float* out_w, const float* out_b, const uint8_t* valid_fixed, int tokens,
-                           float* logits, float* scores, cudaStream_t st);
+                           int Np, float* logits, float* scores, cudaStream_t st);
 
 // ---- SAM mask-decoder path (sam_decoder.cu), USE_SAM_DECODER: True --------------------------------
 struct SamAttnW { const float *qw, *qb, *kw, *kb, *vw, *vb, *ow, *ob; };

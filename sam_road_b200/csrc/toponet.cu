@@ -105,10 +105,12 @@ int topo_fix_valid(const uint8_t* valid, int rows, int Np, uint8_t* out, cudaStr
 }
 
 // ------------------------------------------------------------------------------------------------
-// Self-attention inside each sample (sequence of Np <= 16 pairs, 4 heads x 32), key-padding mask.
+// Self-attention inside each sample (sequence of Np <= KMAX pairs, 4 heads x 32), key-padding mask.
 //   qkv: [rows*Np, 384] fp16 (q | k | v), torch MHA scales q by 1/sqrt(32).
 //   One thread per (sample, head, query); a 128-thread block covers 128/(4*Np) samples.
+//   KMAX = 16 for Np <= 16, 32 above.
 // ------------------------------------------------------------------------------------------------
+template <int KMAX>
 __global__ void __launch_bounds__(128)
 topo_attention_kernel(const __half* __restrict__ qkv, const uint8_t* __restrict__ valid, int rows,
                       int Np, __half* __restrict__ out) {
@@ -127,10 +129,10 @@ topo_attention_kernel(const __half* __restrict__ qkv, const uint8_t* __restrict_
     q[c] = f.x; q[c + 1] = f.y;
   }
   const float scale = 0.17677669529663687f;   // 1/sqrt(32)
-  float sc[16];
+  float sc[KMAX];
   float mx = -INFINITY;
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
+  for (int j = 0; j < KMAX; ++j) {
     sc[j] = -INFINITY;
     if (j < Np && valid[tok0 + j]) {
       const __half* kp = qkv + (tok0 + j) * 384 + 128 + head * 32;
@@ -150,7 +152,7 @@ topo_attention_kernel(const __half* __restrict__ qkv, const uint8_t* __restrict_
   for (int c = 0; c < 32; ++c) o[c] = 0.f;
   float l = 0.f;
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
+  for (int j = 0; j < KMAX; ++j) {
     if (j < Np && sc[j] > -INFINITY) {
       const float p = __expf(sc[j] - mx);
       l += p;
@@ -172,11 +174,11 @@ topo_attention_kernel(const __half* __restrict__ qkv, const uint8_t* __restrict_
 
 int topo_attention(const __half* qkv, const uint8_t* valid, int rows, int Np, __half* out,
                    cudaStream_t st) {
-  SRB_REQUIRE(Np >= 1 && Np <= 16, "topo_attention: n_pairs=%d must be in 1..16", Np);
+  SRB_REQUIRE(Np >= 1 && Np <= 32, "topo_attention: n_pairs=%d must be in 1..32", Np);
   if (rows <= 0) return 0;
   const int per_block = 128 / (4 * Np);
-  topo_attention_kernel<<<(rows + per_block - 1) / per_block, 128, 0, st>>>(qkv, valid, rows, Np,
-                                                                           out);
+  auto* kernel = Np <= 16 ? topo_attention_kernel<16> : topo_attention_kernel<32>;
+  kernel<<<(rows + per_block - 1) / per_block, 128, 0, st>>>(qkv, valid, rows, Np, out);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch();
   return 0;
@@ -216,21 +218,23 @@ int topo_output(const float* x32, const uint8_t* valid_fixed, const float* w, co
 }
 
 // ------------------------------------------------------------------------------------------------
-// fused transformer launcher (n_pairs == 16): pair features are formed in the kernel from the
+// fused transformer launcher (n_pairs == 16 or 32): pair features are formed in the kernel from the
 // per-point projections pst; weights = 18 chunks [128x128] fp16 in consumption order (per layer:
 // Wq, Wk, Wv, Wo, W1, W2)
 // ------------------------------------------------------------------------------------------------
 int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, const TopoLayerParams* layers,
                            const float* out_w, const float* out_b, const uint8_t* valid_fixed, int tokens,
-                           float* logits, float* scores, cudaStream_t st) {
+                           int Np, float* logits, float* scores, cudaStream_t st) {
+  SRB_REQUIRE(Np == 16 || Np == 32, "topo fused: n_pairs=%d must be 16 or 32", Np);
   if (tokens <= 0) return 0;
   SRB_REQUIRE(in.pairs_dtype == 1 || in.pairs_dtype == 2, "topo fused: pairs dtype %d", in.pairs_dtype);
   CUtensorMap tmW;
   if (int rc = make_tmap_f16_2d(&tmW, w_chunks, 18 * 128, 128, 128, 128)) return rc;
-  static uint64_t attr_devs = 0;          // one bit per CUDA device: function attributes are per device
-  if (first_use_on_device(&attr_devs)) {
-    SRB_CUDA_OK(cudaFuncSetAttribute(toponet_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     kTtcSmemBytes));
+  // one bit per CUDA device and instantiation: function attributes are per device and function
+  static uint64_t attr_devs[2] = {0, 0};
+  auto* kernel = Np == 16 ? toponet_tc_kernel<16> : toponet_tc_kernel<32>;
+  if (first_use_on_device(&attr_devs[Np == 32])) {
+    SRB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTtcSmemBytes));
   }
   TtcParams p;
   for (int l = 0; l < 3; ++l) p.layer[l] = layers[l];
@@ -239,7 +243,7 @@ int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, con
   p.logits = logits; p.scores = scores; p.tokens = tokens;
   p.num_tiles = (tokens + 127) / 128;
   const int grid = p.num_tiles < device_sm_count() ? p.num_tiles : device_sm_count();
-  toponet_tc_kernel<<<grid, kTtcThreads, kTtcSmemBytes, st>>>(tmW, p);
+  kernel<<<grid, kTtcThreads, kTtcSmemBytes, st>>>(tmW, p);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch();
   return 0;

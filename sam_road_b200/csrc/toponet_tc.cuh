@@ -1,8 +1,9 @@
 // sam_road_b200 :: fused TopoNet transformer (model.py:74-86,135-146): all three post-norm encoder
-// layers + output_proj for a tile of 128 pair tokens (8 samples x 16 pairs) in ONE persistent kernel.
+// layers + output_proj for a tile of 128 pair tokens (8 samples x 16 pairs, or 4 samples x 32 pairs)
+// in ONE persistent kernel, templated on the pairs per sample.
 //
 // Per layer (torch TransformerEncoderLayer, d=128, 4 heads, ff=128, relu, LN eps 1e-5, eval mode):
-//   qkv = x W_in^T + b_in -> per-sample 16x16 masked attention per head -> x = LN1(x + att W_o^T + b_o)
+//   qkv = x W_in^T + b_in -> per-sample masked attention per head -> x = LN1(x + att W_o^T + b_o)
 //   -> x = LN2(x + relu(x W_1^T + b_1) W_2^T + b_2)
 // Everything between the GEMMs stays on chip:
 //   registers  the fp32 residual stream x (a token thread keeps its 32 columns of the row)
@@ -17,10 +18,11 @@
 // through a warpgroup-local smem exchange, and only the A operand, which every warpgroup reads whole,
 // needs the 512-thread barrier.  LayerNorm statistics and the output dot product are combined across
 // the four warpgroups through a small smem exchange per row quarter, always summed in part order.
-// The 16 x 16 x 32 attention of a (sample, head) runs on warp-level mma.sync: a warp owns two
-// samples of its head; q (bias, 1/sqrt(32), fp16) is staged in the warp's own rows of the A buffer,
-// k / v fragments come from the k|v rows by ldmatrix / ldmatrix.trans, softmax in fp32 on the S
-// fragments, P (fp16) feeds the PV mma from registers.  Key-padding semantics (SURVEY.md §8a P4):
+// The attention of a (sample, head) runs on warp-level mma.sync: with 16 pairs a warp owns two
+// samples of its head (16 x 16 x 32 each), with 32 pairs exactly one (32 x 32 x 32 as two 16-query
+// row blocks); either way they are the warp's own 32 token rows.  q (bias, 1/sqrt(32), fp16) is
+// staged in those rows of the A buffer, k / v fragments come from the k|v rows by ldmatrix /
+// ldmatrix.trans, softmax in fp32 on the S fragments, P (fp16) feeds the PV mma from registers.  Key-padding semantics (SURVEY.md §8a P4):
 // masked keys are excluded from the softmax; masked slots report output_proj.bias.
 #pragma once
 
@@ -93,7 +95,7 @@ __device__ __forceinline__ PairToken resolve_pair(const TopoPairInputs& in, size
   return r;
 }
 
-// warp-level MMA for the 16 x 16 attention of one sample and head (far too small for a UMMA tile)
+// warp-level MMA for the attention of one sample and head (far too small for a wgmma tile)
 __device__ __forceinline__ void ttc_ldmatrix_x4(uint32_t (&r)[4], uint32_t saddr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr) : "memory");
@@ -139,8 +141,11 @@ __device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t desc_a,
 }
 
 
+template <int kPairs>
 __global__ void __launch_bounds__(kTtcThreads, 1)
 toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
+  static_assert(kPairs == 16 || kPairs == 32, "a sample is 16 or 32 pair tokens");
+  constexpr uint32_t kAllKeys = kPairs == 32 ? 0xffffffffu : 0xffffu;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
@@ -321,16 +326,16 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++ti) {
       const long tok = static_cast<long>(tile) * 128 + row;
       const bool tok_ok = tok < p.tokens;
-      // key-validity bits of this token's sample (16 consecutive tokens)
-      uint32_t kmask = 0xffffu;
+      // key-validity bits of this token's sample (kPairs consecutive tokens)
+      uint32_t kmask = kAllKeys;
       bool my_valid = true;
       if (p.valid) {
         kmask = 0;
-        const long s0 = static_cast<long>(tile) * 128 + (row & ~15);
+        const long s0 = static_cast<long>(tile) * 128 + (row & ~(kPairs - 1));
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
+        for (int j = 0; j < kPairs; ++j)
           if (s0 + j < p.tokens && p.valid[s0 + j]) kmask |= 1u << j;
-        if (kmask == 0) kmask = 0xffffu;            // tail rows beyond `tokens`
+        if (kmask == 0) kmask = kAllKeys;           // tail rows beyond `tokens`
         my_valid = tok_ok && p.valid[tok];
       }
 
@@ -412,7 +417,7 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
           }
       }
       ttc_bar_group(part);                         // q, k, v of head `part` are in smem
-      {
+      if constexpr (kPairs == 16) {
         // ---- attention of head `part` for the warp's two samples on mma.sync (16 queries x 16 keys x
         // 32 dims per sample): k and v come straight from their smem rows through ldmatrix, P stays in
         // registers (S fragments -> A fragments), O is normalised and stored as the out_proj A operand.
@@ -510,7 +515,112 @@ toponet_tc_kernel(const __grid_constant__ CUtensorMap tmW, TtcParams p) {
                   pack_half2(oacc[j][2] * inv1, oacc[j][3] * inv1);
             }
           }
+      } else {
+        // ---- attention of head `part` for the warp's one sample (32 queries x 32 keys x 32 dims) on
+        // mma.sync, as two 16-query row blocks.  Keys 0-15 and 16-31 are two 16-row blocks of the k|v
+        // rows; the second sits at odd (row >> 4), so its columns are XOR 64 B.  Every lane holds the
+        // sample's key mask.
+        const int h = part;
+        __syncwarp();
+        const int g8 = lane >> 2, t4 = lane & 3;     // fragment coordinates: row g8 (+8), column pair t4
+        const int mi = lane >> 3, rr = lane & 7;     // ldmatrix: this lane addresses row rr of matrix mi
+        const uint32_t sA_h = smem_u32(sA) + (h >> 1) * 16384;
+        const uint32_t sKV_a = smem_u32(sKV);
+        const int r0 = quarter * 32;                 // first tile row of the sample
+#pragma unroll
+        for (int qb = 0; qb < 2; ++qb) {
+          const int q0 = r0 + qb * 16;               // first query row of the block
+          // S = Q K^T : four 8-key column tiles, two 16-dim k-steps
+          float sacc[4][4];
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) sacc[nt][i] = 0.f;
+#pragma unroll
+          for (int ks = 0; ks < 2; ++ks) {
+            uint32_t qa[4];
+            {   // matrices: (rows 0-7 | 8-15) x (dims ks*16 + 0-7 | 8-15)
+              const int qr = q0 + (mi & 1) * 8 + rr;
+              const int piece = (h & 1) * 4 + ks * 2 + (mi >> 1);
+              ttc_ldmatrix_x4(qa, sA_h + qr * 128 + ((piece ^ (qr & 7)) << 4));
+            }
+#pragma unroll
+            for (int kb = 0; kb < 2; ++kb) {   // keys kb*16 + (0-7 | 8-15) x (dims ks*16 + 0-7 | 8-15)
+              uint32_t kf[4];
+              const int kr = r0 + kb * 16 + (mi >> 1) * 8 + rr;
+              ttc_ldmatrix_x4(kf, sKV_a + kr * kTtcKVStride + ((h * 64) ^ (kb << 6)) + (ks * 16 + (mi & 1) * 8) * 2);
+              ttc_mma_16816(sacc[2 * kb + 0], qa, kf[0], kf[1]);
+              ttc_mma_16816(sacc[2 * kb + 1], qa, kf[2], kf[3]);
+            }
+          }
+          // masked softmax of rows g8 (values [nt][0..1]) and g8 + 8 ([nt][2..3]); keys nt*8 + 2*t4 (+1)
+          float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const bool on = (kmask >> (nt * 8 + 2 * t4 + e)) & 1u;
+              sacc[nt][e] = on ? sacc[nt][e] : -INFINITY;
+              sacc[nt][2 + e] = on ? sacc[nt][2 + e] : -INFINITY;
+              mx0 = fmaxf(mx0, sacc[nt][e]);
+              mx1 = fmaxf(mx1, sacc[nt][2 + e]);
+            }
+          mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+          mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+          mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+          mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+          float l0 = 0.f, l1 = 0.f;
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              sacc[nt][e] = __expf(sacc[nt][e] - mx0);           // exp(-inf) = 0 for masked keys
+              sacc[nt][2 + e] = __expf(sacc[nt][2 + e] - mx1);
+              l0 += sacc[nt][e];
+              l1 += sacc[nt][2 + e];
+            }
+          l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+          l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+          l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+          l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+          uint32_t pa[2][4];                         // A fragments of P for keys kk*16 + 0..15
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk) {
+            pa[kk][0] = pack_half2(sacc[2 * kk][0], sacc[2 * kk][1]);
+            pa[kk][1] = pack_half2(sacc[2 * kk][2], sacc[2 * kk][3]);
+            pa[kk][2] = pack_half2(sacc[2 * kk + 1][0], sacc[2 * kk + 1][1]);
+            pa[kk][3] = pack_half2(sacc[2 * kk + 1][2], sacc[2 * kk + 1][3]);
+          }
+          // O = P V : four 8-dim column tiles, two 16-key k-steps
+          float oacc[4][4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) oacc[j][i] = 0.f;
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+            for (int dh = 0; dh < 2; ++dh) {
+              uint32_t vb[4];   // transposed matrices: (keys kk*16 + 0-7 | 8-15) x (dims dh*16 + 0-7 | 8-15)
+              const int vr = r0 + kk * 16 + (mi & 1) * 8 + rr;
+              ttc_ldmatrix_x4_trans(vb, sKV_a + vr * kTtcKVStride + ((256 + h * 64) ^ (kk << 6)) +
+                                            (dh * 16 + (mi >> 1) * 8) * 2);
+              ttc_mma_16816(oacc[dh * 2 + 0], pa[kk], vb[0], vb[1]);
+              ttc_mma_16816(oacc[dh * 2 + 1], pa[kk], vb[2], vb[3]);
+            }
+          const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+          __syncwarp();                              // every lane's Q fragments of this block are loaded
+          const int ra = q0 + g8, rb = q0 + g8 + 8;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {              // attention output columns h*32 + j*8 + 2*t4 (+1)
+            const int piece = (h & 1) * 4 + j;
+            *reinterpret_cast<uint32_t*>(sA + (h >> 1) * 16384 + ra * 128 + ((piece ^ (ra & 7)) << 4) + t4 * 4) =
+                pack_half2(oacc[j][0] * inv0, oacc[j][1] * inv0);
+            *reinterpret_cast<uint32_t*>(sA + (h >> 1) * 16384 + rb * 128 + ((piece ^ (rb & 7)) << 4) + t4 * 4) =
+                pack_half2(oacc[j][2] * inv1, oacc[j][3] * inv1);
+          }
         }
+      }
       fence_proxy_async_smem();
       ttc_bar_all();
       // ================= out_proj + residual + LayerNorm1 =================

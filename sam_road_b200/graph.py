@@ -111,9 +111,10 @@ class SceneGraph:
 
     # ---- pair queries -------------------------------------------------------------------------------
     def plan_pair_queries(self, points_xy: torch.Tensor, tile_xy: np.ndarray, patch_size: int,
-                          neighbor_radius: float) -> np.ndarray:
+                          neighbor_radius: float, max_nbr: int = 16) -> np.ndarray:
         """Box query + kNN for every tile (inferencer.py:148-176).  points_xy: int64 [N,2] on the device;
-        tile_xy: host int [n_tiles,2] origins in tile-list order.  Returns the per-tile point counts."""
+        tile_xy: host int [n_tiles,2] origins in tile-list order; max_nbr: MAX_NEIGHBOR_QUERIES (1..32),
+        the largest K fill_batch / aggregate_edges may then use.  Returns the per-tile point counts."""
         if points_xy.dtype != torch.int64 or points_xy.dim() != 2 or points_xy.shape[1] != 2 or \
                 points_xy.device != self.device:
             raise ValueError("points_xy must be an int64 [N,2] tensor on the graph's device")
@@ -121,10 +122,10 @@ class SceneGraph:
         txy = np.ascontiguousarray(tile_xy, dtype=np.int32).reshape(-1, 2)
         counts = np.zeros(txy.shape[0], dtype=np.int32)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().samroad_pair_queries_plan(
+            _lib.check(_lib.load().samroad_pair_queries_plan_k(
                 self._h, pts.data_ptr(), int(pts.shape[0]), txy.ctypes.data, int(txy.shape[0]),
-                int(patch_size), float(neighbor_radius), counts.ctypes.data, _lib.current_stream_ptr()),
-                "samroad_pair_queries_plan")
+                int(patch_size), float(neighbor_radius), int(max_nbr), counts.ctypes.data,
+                _lib.current_stream_ptr()), "samroad_pair_queries_plan")
         self._counts = counts
         return counts
 

@@ -214,7 +214,7 @@ def _scene_finish(j: _SceneJob, nms_tie_order: Optional[str], timings: Optional[
         if timings is not None:
             torch.cuda.synchronize(device)
         return time.perf_counter()
-    counts = gx.plan_pair_queries(points_d, tile_xy, P, R)
+    counts = gx.plan_pair_queries(points_d, tile_xy, P, R, K)
     t_plan = _mark()
     # layout of the scene-wide score buffer: per batch [n, nmax_of_the_batch, K] (inferencer.py:179-185
     # pads every batch to its own maximum); batches with no point at all are skipped (188-189)

@@ -98,6 +98,7 @@ def toponet_fixture():
 
 
 TOPO_NPAIRS = (1, 5, 15)
+TOPO_NPAIRS_WIDE = (17, 24, 32)
 TOPO_NPAIRS_NS = 13          # samples kept: fewer than the 20 points, not a multiple of 8
 
 
@@ -112,7 +113,7 @@ def toponet_npairs_inputs(n_pairs):
     return feat, pts, prs, val
 
 
-def toponet_npairs_fixture():
+def toponet_npairs_fixture(npairs=TOPO_NPAIRS, name="toponet_npairs"):
     out = {}
     cfg = _cfg(256)
     torch.manual_seed(0)
@@ -120,7 +121,7 @@ def toponet_npairs_fixture():
     sd = synth.make_state_dict(cfg, seed=5)
     net.load_state_dict(sd, strict=True)
     spec = O.ModelSpec.from_config(cfg)
-    for n_pairs in TOPO_NPAIRS:
+    for n_pairs in npairs:
         feat, pts, prs, val = toponet_npairs_inputs(n_pairs)
         with torch.no_grad():
             ref = net.infer_toponet(feat, pts, prs, val)
@@ -133,7 +134,7 @@ def toponet_npairs_fixture():
         out[f"np{n_pairs}_int"] = ref.numpy()
         out[f"np{n_pairs}_float"] = ref_f.numpy()
         print(f"toponet[n_pairs={n_pairs}, Ns={TOPO_NPAIRS_NS}, N=20]: oracle-vs-reference max-abs {err:.2e}")
-    np.savez_compressed(os.path.join(OUT, "toponet_npairs.npz"), **out)
+    np.savez_compressed(os.path.join(OUT, f"{name}.npz"), **out)
 
 
 def _extract_functions(path, names):
@@ -192,6 +193,7 @@ def shape_fixtures():
     # PATCH_SIZE 192: 12x12 grid smaller than the 14x14 window (one padded window), SAM mask decoder
     model_fixture("vitb_192_samdec", _cfg(192, samdec=True), seed=9, n_points=16)
     toponet_npairs_fixture()
+    toponet_npairs_fixture(TOPO_NPAIRS_WIDE, "toponet_npairs_wide")
 
 
 def main():
@@ -204,6 +206,9 @@ def main():
         return
     if "--shapes" in sys.argv:        # tile sizes and pair counts outside the benched configs
         shape_fixtures()
+        return
+    if "--wide-pairs" in sys.argv:    # MAX_NEIGHBOR_QUERIES 17..32
+        toponet_npairs_fixture(TOPO_NPAIRS_WIDE, "toponet_npairs_wide")
         return
     model_fixture("vitb_256", _cfg(256), seed=0, n_points=24)
     model_fixture("vitb_512", _cfg(512), seed=1, n_points=40)
