@@ -27,6 +27,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdio>
+#include <cstring>
 #include <thread>
 #include <vector>
 
@@ -40,6 +41,10 @@ namespace {
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
   int ensure(size_t bytes) {
     if (bytes <= cap) return 0;
     if (p) {
@@ -53,28 +58,40 @@ struct DevBuf {
     cap = want;
     return 0;
   }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
   template <typename T> T* as() const { return static_cast<T*>(p); }
 };
+
+// Every count written on the device and read back by the host, one field each.  The entry points that
+// use them clear them all on entry.
+struct Counters {
+  int cand[2];       // candidates per mask
+  int sort_total;    // counting sort: scan total
+  int order_err;     // visiting order: 1 = host index out of range, 2 = not non-increasing
+  int n_mortal;      // entries of an NMS pass that can be suppressed
+  int survivors;     // entries an NMS pass keeps
+  int bad_score;     // aggregation: a score outside [0, 1]
+  int n_edges;
+  int max_deg;       // most points within the neighbour radius of one point
+  int nnz;           // (src, tgt) slots of the aggregation
+};
+
+constexpr size_t kPinBytes = 256;
 
 }  // namespace
 
 struct samroad_graph_ctx {
   int device = 0;
+  DevBuf counters;                        // one Counters
   // keypoint extraction
-  DevBuf blk_cnt, blk_off, totals;        // compaction scratch
+  DevBuf blk_cnt, blk_off;                // compaction scratch
   DevBuf cand_pix[2], cand_score[2];      // candidates of the two masks, np.where order
   DevBuf order, sorted_pix, immune;       // visiting order of one NMS pass
-  DevBuf list[2];                         // kept pixels of passes 1 / 2, visiting order
+  DevBuf list[3];                         // kept pixels of passes 1 / 2 / 3, visiting order
   DevBuf cand3, cls3;                     // pass 3 input: concatenation + class (1 = keypoint mask)
   DevBuf cell;                            // scene-sized rank/state image
-  DevBuf tile_und, round_cnt, flags32;    // NMS rounds
+  DevBuf tile_und, round_cnt;             // NMS rounds
   DevBuf ghist;                           // counting sort
-  int* h_pin = nullptr;                   // pinned host ints for small read-backs
+  void* h_pin = nullptr;                  // kPinBytes of pinned host memory for small read-backs
   // pair queries
   DevBuf pts32, t_cnt, t_off, members, nbr, tile_xy;
   std::vector<int> h_cnt, h_off;
@@ -85,6 +102,8 @@ struct samroad_graph_ctx {
   int nbr_stride = 16;                    // row length of nbr: 16 for max_nbr <= 16, else 32
   // aggregation
   DevBuf adj_deg, adj_off, adj_src, adj_tgt, adj_sum, adj_cnt, adj_first, eflags, tile_soff;
+
+  ~samroad_graph_ctx() { if (h_pin) cudaFreeHost(h_pin); }
 };
 
 namespace {
@@ -274,14 +293,6 @@ __global__ void __launch_bounds__(32) sort_scatter_kernel(const uint8_t* __restr
   }
 }
 
-// order of pass 3 without a host permutation: class-1 entries (first m0) in descending index, then
-// the class-0 entries in descending index  ==  np.argsort(scores, kind='stable')[::-1]
-__global__ void order3_stable_kernel(int m0, int m1, int32_t* __restrict__ order) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= m0 + m1) return;
-  order[i] = i < m0 ? (m0 - 1 - i) : (m0 + m1 - 1 - (i - m0));
-}
-
 // host permutation (ascending argsort, int64) -> visiting order (its reverse, int32)
 __global__ void order_from_host_kernel(const int64_t* __restrict__ asc, int n, int32_t* __restrict__ order,
                                        int* __restrict__ err) {
@@ -294,7 +305,8 @@ __global__ void order_from_host_kernel(const int64_t* __restrict__ asc, int n, i
 
 // sorted_points = points[order]; immune = score > 1.0 (never suppressed, graph_utils.py:573,585).
 // Also checks that the order really is non-increasing in score (a bad callback would silently change
-// the greedy result) and counts the entries that can be suppressed at all.
+// the greedy result) and counts the entries that can be suppressed at all.  In pass 3 `score` is the
+// class (1 or 0), so nothing is immune there.
 __global__ void gather_sorted_kernel(const int32_t* __restrict__ pix, const uint8_t* __restrict__ score,
                                      const int32_t* __restrict__ order, int n,
                                      int32_t* __restrict__ sorted_pix, uint8_t* __restrict__ immune,
@@ -307,20 +319,6 @@ __global__ void gather_sorted_kernel(const int32_t* __restrict__ pix, const uint
   immune[i] = s >= 2 ? 1 : 0;              // uint8 score > 1.0
   if (s < 2) atomicAdd(n_mortal, 1);
   if (i > 0 && score[order[i - 1]] < s) atomicOr(err, 2);
-}
-
-// pass 3 input: class from position (first m0 entries came from the keypoint mask: score 1.0, the
-// rest score 0.0, graph_extraction.py:136-137); nothing is immune.
-__global__ void gather_sorted3_kernel(const int32_t* __restrict__ cand3, const int32_t* __restrict__ order,
-                                      int m0, int n, int32_t* __restrict__ sorted_pix, int* __restrict__ err) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int o = order[i];
-  sorted_pix[i] = cand3[o];
-  if (i > 0) {
-    const int prev_cls = order[i - 1] < m0 ? 1 : 0, cls = o < m0 ? 1 : 0;
-    if (prev_cls < cls) atomicOr(err, 2);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -483,12 +481,13 @@ nms_round_generic_kernel(uint32_t* __restrict__ cell, const int32_t* __restrict_
   else atomicAdd(round_total, 1);
 }
 
-// pass 3 input = concat(kept0, kept1)
+// pass 3 input = concat(kept0, kept1) and its class: the keypoint-mask entries score 1.0, the rest 0.0
+// (graph_extraction.py:136-137)
 __global__ void concat_kernel(const int32_t* __restrict__ a, int na, const int32_t* __restrict__ b, int nb,
-                              int32_t* __restrict__ out) {
+                              int32_t* __restrict__ out, uint8_t* __restrict__ cls) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < na) out[i] = a[i];
-  else if (i < na + nb) out[i] = b[i - na];
+  if (i < na) { out[i] = a[i]; cls[i] = 1; }
+  else if (i < na + nb) { out[i] = b[i - na]; cls[i] = 0; }
 }
 
 __global__ void pix_to_xy_kernel(const int32_t* __restrict__ pix, int n, int W, int64_t* __restrict__ out) {
@@ -501,11 +500,13 @@ __global__ void pix_to_xy_kernel(const int32_t* __restrict__ pix, int n, int W, 
 
 inline int blocks_for(long n, int per = 256) { return static_cast<int>((n + per - 1) / per); }
 
-// read small device ints back (synchronises the stream)
-int read_ints(samroad_graph_ctx* g, const int* dev, int n, int* host, cudaStream_t st) {
-  SRB_CUDA_OK(cudaMemcpyAsync(g->h_pin, dev, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+// read a small device object back (synchronises the stream)
+template <typename T>
+int read_back(samroad_graph_ctx* g, const T* dev, T* host, cudaStream_t st) {
+  static_assert(sizeof(T) <= kPinBytes, "read-back larger than the pinned staging buffer");
+  SRB_CUDA_OK(cudaMemcpyAsync(g->h_pin, dev, sizeof(T), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
-  for (int i = 0; i < n; ++i) host[i] = g->h_pin[i];
+  std::memcpy(host, g->h_pin, sizeof(T));
   return 0;
 }
 
@@ -516,15 +517,94 @@ int thr_to_int(double thr) {
   return static_cast<int>(std::floor(thr)) + 1;
 }
 
-// One NMS pass over `n` entries already in visiting order.  Returns the survivors (visiting order)
-// in `out` and their number in *n_out.  Synchronises.
-int nms_pass(samroad_graph_ctx* g, const int32_t* sorted_pix, const uint8_t* immune, int n, int n_mortal,
-             int H, int W, double radius, int32_t* out, int* n_out, int* rounds_out, cudaStream_t st) {
-  *rounds_out = 0;
-  if (n == 0) { *n_out = 0; return 0; }
-  if (n_mortal == 0) {        // every score > 1: nothing can be suppressed, the pass only reorders
+using clk = std::chrono::steady_clock;
+int32_t us_since(clk::time_point t) {
+  return static_cast<int32_t>(std::chrono::duration_cast<std::chrono::microseconds>(clk::now() - t).count());
+}
+
+// Visiting order from the host: the reverse of the callback's ascending argsort of the `n` device keys,
+// which it sees as `key_dtype` (SAMROAD_U8, or SAMROAD_F64 holding the same values).  `pre_asc`, when
+// given, is that argsort already made.  An index out of range sets bit 1 of *err.  Synchronises.
+int host_order(samroad_graph_ctx* g, const uint8_t* key, int n, int key_dtype, samroad_argsort_fn cb, void* user,
+               const std::vector<int64_t>* pre_asc, int32_t* order, int* err, cudaStream_t st) {
+  std::vector<int64_t> own;
+  if (!pre_asc) {
+    std::vector<uint8_t> keys(n);
+    SRB_CUDA_OK(cudaMemcpyAsync(keys.data(), key, n, cudaMemcpyDeviceToHost, st));
+    SRB_CUDA_OK(cudaStreamSynchronize(st));
+    own.resize(n);
+    if (key_dtype == SAMROAD_F64) {
+      const std::vector<double> keys64(keys.begin(), keys.end());
+      SRB_REQUIRE(cb(keys64.data(), SAMROAD_F64, n, own.data(), user) == 0,
+                  "argsort callback failed (float64 priorities)");
+    } else {
+      SRB_REQUIRE(cb(keys.data(), SAMROAD_U8, n, own.data(), user) == 0, "argsort callback failed (uint8 scores)");
+    }
+  }
+  const std::vector<int64_t>& asc = pre_asc ? *pre_asc : own;
+  if (int rc = g->ghist.ensure(sizeof(int64_t) * n)) return rc;
+  SRB_CUDA_OK(cudaMemcpyAsync(g->ghist.p, asc.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
+  order_from_host_kernel<<<blocks_for(n), 256, 0, st>>>(g->ghist.as<int64_t>(), n, order, err);
+  note_launch();
+  SRB_CUDA_OK(cudaStreamSynchronize(st));   // `asc` is pageable host memory: keep it alive until copied
+  return 0;
+}
+
+// Visiting order on the device: np.argsort(key, kind='stable')[::-1] by the counting sort
+int stable_order(samroad_graph_ctx* g, const uint8_t* key, int n, int32_t* order, int* scan_total,
+                 cudaStream_t st) {
+  const int nchunks = (n + kSortChunk - 1) / kSortChunk;
+  if (int rc = g->ghist.ensure(sizeof(int) * 256 * static_cast<size_t>(nchunks) * 2 + 16)) return rc;
+  int* hist = g->ghist.as<int>();
+  int* off = hist + 256 * static_cast<size_t>(nchunks);
+  sort_hist_kernel<<<nchunks, 32, 0, st>>>(key, n, nchunks, hist);
+  scan_single_block_kernel<<<1, 1024, 0, st>>>(hist, 256 * nchunks, off, scan_total);
+  sort_scatter_kernel<<<nchunks, 32, 0, st>>>(key, n, nchunks, off, order);
+  SRB_CUDA_OK(cudaGetLastError());
+  note_launch(3);
+  return 0;
+}
+
+struct PassStats {
+  int kept = 0, rounds = 0;
+  int32_t us_order = 0, us_nms = 0;    // host wall clock of the two halves, each ending on a synchronisation
+};
+
+// One greedy NMS pass (graph_utils.py:572-591) from candidates to survivors: visiting order -> gather
+// and check -> fixed point -> compaction.  `key` holds one uint8 per candidate: the mask score in passes
+// 1 and 2, the class in pass 3.  With a callback the host decides the order of equal keys (see
+// host_order), without one the device sorts stably.  `what` names the pass in errors.  Returns the
+// survivors (visiting order) in `out`.  Synchronises.
+int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n, int key_dtype,
+             samroad_argsort_fn cb, void* user, const std::vector<int64_t>* pre_asc, const char* what, int H,
+             int W, double radius, int32_t* out, PassStats* ps, cudaStream_t st) {
+  *ps = PassStats{};
+  if (n == 0) return 0;
+  if (int rc = g->order.ensure(sizeof(int32_t) * static_cast<size_t>(n))) return rc;
+  if (int rc = g->sorted_pix.ensure(sizeof(int32_t) * static_cast<size_t>(n))) return rc;
+  if (int rc = g->immune.ensure(static_cast<size_t>(n))) return rc;
+  int32_t* order = g->order.as<int32_t>();
+  int32_t* sorted_pix = g->sorted_pix.as<int32_t>();
+  uint8_t* immune = g->immune.as<uint8_t>();
+  Counters* ctr = g->counters.as<Counters>();
+  clk::time_point t0 = clk::now();
+  if (int rc = cb ? host_order(g, key, n, key_dtype, cb, user, pre_asc, order, &ctr->order_err, st)
+                  : stable_order(g, key, n, order, &ctr->sort_total, st))
+    return rc;
+  SRB_CUDA_OK(cudaMemsetAsync(&ctr->n_mortal, 0, sizeof(int), st));
+  gather_sorted_kernel<<<blocks_for(n), 256, 0, st>>>(pix, key, order, n, sorted_pix, immune, &ctr->n_mortal,
+                                                      &ctr->order_err);
+  note_launch();
+  Counters c;
+  if (int rc = read_back(g, ctr, &c, st)) return rc;
+  SRB_REQUIRE(c.order_err == 0, "argsort callback returned an invalid permutation (code %d) for %s", c.order_err,
+              what);
+  ps->us_order = us_since(t0);
+  t0 = clk::now();
+  if (c.n_mortal == 0) {        // every score > 1: nothing can be suppressed, the pass only reorders
     SRB_CUDA_OK(cudaMemcpyAsync(out, sorted_pix, sizeof(int32_t) * n, cudaMemcpyDeviceToDevice, st));
-    *n_out = n;
+    ps->kept = n;
+    ps->us_nms = us_since(t0);
     return 0;
   }
   SRB_REQUIRE(radius >= 0.0 && radius < 4096.0, "nms radius %.3f unsupported", radius);
@@ -564,47 +644,15 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* sorted_pix, const uint8_t* imm
     }
     SRB_CUDA_OK(cudaGetLastError());
     int open = 0;
-    if (int rc = read_ints(g, round_cnt + round - 1, 1, &open, st)) return rc;
+    if (int rc = read_back(g, round_cnt + round - 1, &open, st)) return rc;
     if (open == 0) break;
     SRB_REQUIRE(round < kMaxRounds, "greedy NMS did not converge in %d rounds (%d pixels open)", round, open);
   }
-  *rounds_out = round;
+  ps->rounds = round;
   KeptByRank kb{cell, sorted_pix, out};
-  int* tot = g->totals.as<int>();
-  if (int rc = compact(g, kb, n, tot, st)) return rc;
-  return read_ints(g, tot, 1, n_out, st);
-}
-
-// visiting order of a uint8-scored candidate set: host permutation (NumPy) or device stable sort
-int make_order_u8(samroad_graph_ctx* g, const uint8_t* score_dev, int n, samroad_argsort_fn cb, void* user,
-                  const std::vector<int64_t>* pre_asc, int32_t* order, int* err_dev, cudaStream_t st) {
-  if (n == 0) return 0;
-  if (cb) {
-    std::vector<int64_t> own;
-    if (!pre_asc) {
-      std::vector<uint8_t> keys(n);
-      own.resize(n);
-      SRB_CUDA_OK(cudaMemcpyAsync(keys.data(), score_dev, n, cudaMemcpyDeviceToHost, st));
-      SRB_CUDA_OK(cudaStreamSynchronize(st));
-      SRB_REQUIRE(cb(keys.data(), SAMROAD_U8, n, own.data(), user) == 0, "argsort callback failed (uint8 scores)");
-    }
-    const std::vector<int64_t>& asc = pre_asc ? *pre_asc : own;
-    if (int rc = g->ghist.ensure(sizeof(int64_t) * n)) return rc;
-    SRB_CUDA_OK(cudaMemcpyAsync(g->ghist.p, asc.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
-    order_from_host_kernel<<<blocks_for(n), 256, 0, st>>>(g->ghist.as<int64_t>(), n, order, err_dev);
-    note_launch();
-    SRB_CUDA_OK(cudaStreamSynchronize(st));   // `asc` is pageable host memory: keep it alive until copied
-    return 0;
-  }
-  const int nchunks = (n + kSortChunk - 1) / kSortChunk;
-  if (int rc = g->ghist.ensure(sizeof(int) * 256 * static_cast<size_t>(nchunks) * 2 + 16)) return rc;
-  int* hist = g->ghist.as<int>();
-  int* off = hist + 256 * static_cast<size_t>(nchunks);
-  sort_hist_kernel<<<nchunks, 32, 0, st>>>(score_dev, n, nchunks, hist);
-  scan_single_block_kernel<<<1, 1024, 0, st>>>(hist, 256 * nchunks, off, g->totals.as<int>() + 3);
-  sort_scatter_kernel<<<nchunks, 32, 0, st>>>(score_dev, n, nchunks, off, order);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(3);
+  if (int rc = compact(g, kb, n, &ctr->survivors, st)) return rc;
+  if (int rc = read_back(g, &ctr->survivors, &ps->kept, st)) return rc;
+  ps->us_nms = us_since(t0);
   return 0;
 }
 
@@ -622,12 +670,12 @@ extern "C" int samroad_graph_create(int device, samroad_graph_t* out) {
   SRB_CUDA_OK(cudaSetDevice(device));
   samroad_graph_ctx* g = new samroad_graph_ctx();
   g->device = device;
-  if (cudaMallocHost(reinterpret_cast<void**>(&g->h_pin), 64 * sizeof(int)) != cudaSuccess) {
+  if (cudaMallocHost(&g->h_pin, kPinBytes) != cudaSuccess) {
     delete g;
     set_last_error("samroad_graph_create: cudaMallocHost failed");
     return 1;
   }
-  if (g->totals.ensure(64 * sizeof(int)) != 0) { cudaFreeHost(g->h_pin); delete g; return 1; }
+  if (g->counters.ensure(sizeof(Counters)) != 0) { delete g; return 1; }
   *out = g;
   return 0;
 }
@@ -636,14 +684,6 @@ extern "C" int samroad_graph_destroy(samroad_graph_t g) {
   if (!g) return 0;
   cudaSetDevice(g->device);
   cudaDeviceSynchronize();
-  DevBuf* bufs[] = {&g->blk_cnt, &g->blk_off, &g->totals, &g->cand_pix[0], &g->cand_pix[1], &g->cand_score[0],
-                    &g->cand_score[1], &g->order, &g->sorted_pix, &g->immune, &g->list[0], &g->list[1],
-                    &g->cand3, &g->cls3, &g->cell, &g->tile_und, &g->round_cnt, &g->flags32, &g->ghist,
-                    &g->pts32, &g->t_cnt, &g->t_off, &g->members, &g->nbr, &g->tile_xy, &g->adj_deg,
-                    &g->adj_off, &g->adj_src, &g->adj_tgt, &g->adj_sum, &g->adj_cnt, &g->adj_first,
-                    &g->eflags, &g->tile_soff};
-  for (DevBuf* b : bufs) b->release();
-  if (g->h_pin) cudaFreeHost(g->h_pin);
   delete g;
   return 0;
 }
@@ -662,28 +702,24 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
   SRB_CUDA_OK(cudaSetDevice(g->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int npx = H * W;
-  int* tot = g->totals.as<int>();          // [0],[1]: candidate counts, [2]: scratch, [4]: err, [5]: n_mortal
-  SRB_CUDA_OK(cudaMemsetAsync(tot, 0, 64 * sizeof(int), st));
+  Counters* ctr = g->counters.as<Counters>();
+  SRB_CUDA_OK(cudaMemsetAsync(ctr, 0, sizeof(Counters), st));
   const uint8_t* masks[2] = {keypoint_mask, road_mask};
   const double thr[2] = {itsc_thr255, road_thr255};
   const double radius[2] = {itsc_radius, road_radius};
-  int n_cand[2] = {0, 0}, n_kept[2] = {0, 0}, rounds[3] = {0, 0, 0};
-  using clk = std::chrono::steady_clock;
-  auto us_since = [](clk::time_point t) {
-    return static_cast<int32_t>(std::chrono::duration_cast<std::chrono::microseconds>(clk::now() - t).count());
-  };
   const clk::time_point t_begin = clk::now();
-  int32_t us_cand = 0, us_order[3] = {0, 0, 0}, us_nms[3] = {0, 0, 0};
 
   // candidates of both masks (np.where order).  Worst case every pixel qualifies.
   for (int m = 0; m < 2; ++m) {
     if (int rc = g->cand_pix[m].ensure(sizeof(int32_t) * static_cast<size_t>(npx))) return rc;
     if (int rc = g->cand_score[m].ensure(static_cast<size_t>(npx))) return rc;
     MaskCand mc{masks[m], thr_to_int(thr[m]), g->cand_pix[m].as<int32_t>(), g->cand_score[m].as<uint8_t>()};
-    if (int rc = compact(g, mc, npx, tot + m, st)) return rc;
+    if (int rc = compact(g, mc, npx, &ctr->cand[m], st)) return rc;
   }
-  if (int rc = read_ints(g, tot, 2, n_cand, st)) return rc;
-  us_cand = us_since(t_begin);
+  Counters c;
+  if (int rc = read_back(g, ctr, &c, st)) return rc;
+  const int n_cand[2] = {c.cand[0], c.cand[1]};
+  const int32_t us_cand = us_since(t_begin);
 
   // Host permutations (NumPy tie order): when every candidate score is > 1 the first two passes only reorder,
   // so the sizes of the third pass are known now and the three argsorts can run side by side (np.argsort
@@ -719,93 +755,48 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
   }
 
   // passes 1 and 2: per-mask NMS (graph_extraction.py:131-134)
+  PassStats ps[3];
   for (int m = 0; m < 2; ++m) {
     const int n = n_cand[m];
     if (int rc = g->list[m].ensure(sizeof(int32_t) * static_cast<size_t>(n > 0 ? n : 1))) return rc;
-    if (n == 0) continue;
-    if (int rc = g->order.ensure(sizeof(int32_t) * static_cast<size_t>(n))) return rc;
-    if (int rc = g->sorted_pix.ensure(sizeof(int32_t) * static_cast<size_t>(n))) return rc;
-    if (int rc = g->immune.ensure(static_cast<size_t>(n))) return rc;
-    clk::time_point t0 = clk::now();
-    if (int rc = make_order_u8(g, g->cand_score[m].as<uint8_t>(), n, argsort, user,
-                               have_pre ? &pre_asc[m] : nullptr, g->order.as<int32_t>(), tot + 4, st))
+    if (int rc = nms_pass(g, g->cand_pix[m].as<int32_t>(), g->cand_score[m].as<uint8_t>(), n, SAMROAD_U8, argsort,
+                          user, have_pre ? &pre_asc[m] : nullptr, m == 0 ? "mask 0" : "mask 1", H, W, radius[m],
+                          g->list[m].as<int32_t>(), &ps[m], st))
       return rc;
-    SRB_CUDA_OK(cudaMemsetAsync(tot + 5, 0, sizeof(int), st));
-    gather_sorted_kernel<<<blocks_for(n), 256, 0, st>>>(g->cand_pix[m].as<int32_t>(), g->cand_score[m].as<uint8_t>(),
-                                                        g->order.as<int32_t>(), n, g->sorted_pix.as<int32_t>(),
-                                                        g->immune.as<uint8_t>(), tot + 5, tot + 4);
-    note_launch();
-    int info[2];
-    if (int rc = read_ints(g, tot + 4, 2, info, st)) return rc;
-    SRB_REQUIRE(info[0] == 0, "argsort callback returned an invalid permutation (code %d) for mask %d", info[0], m);
-    us_order[m] = us_since(t0);
-    t0 = clk::now();
-    if (int rc = nms_pass(g, g->sorted_pix.as<int32_t>(), g->immune.as<uint8_t>(), n, info[1], H, W, radius[m],
-                          g->list[m].as<int32_t>(), &n_kept[m], &rounds[m], st))
-      return rc;
-    us_nms[m] = us_since(t0);
   }
 
-  // pass 3: intersections first (graph_extraction.py:135-138), radius = ROAD_NMS_RADIUS
-  const int m0 = n_kept[0], m1 = n_kept[1], n3 = m0 + m1;
-  int n_out = 0;
+  // pass 3: intersections first (graph_extraction.py:135-138), radius = ROAD_NMS_RADIUS.  The reference
+  // sorts float64 priorities here, whose ties NumPy orders differently from uint8 ones (DESIGN.md §9).
+  const int m0 = ps[0].kept, m1 = ps[1].kept, n3 = m0 + m1;
   if (n3 > 0) {
     if (int rc = g->cand3.ensure(sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
-    if (int rc = g->order.ensure(sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
-    if (int rc = g->sorted_pix.ensure(sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
-    if (int rc = g->flags32.ensure(sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
-    clk::time_point t0 = clk::now();
+    if (int rc = g->cls3.ensure(static_cast<size_t>(n3))) return rc;
+    if (int rc = g->list[2].ensure(sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
     concat_kernel<<<blocks_for(n3), 256, 0, st>>>(g->list[0].as<int32_t>(), m0, g->list[1].as<int32_t>(), m1,
-                                                  g->cand3.as<int32_t>());
+                                                  g->cand3.as<int32_t>(), g->cls3.as<uint8_t>());
     note_launch();
-    if (argsort) {
-      std::vector<int64_t> own3;
-      const bool pre3 = have_pre && m0 == n_cand[0] && m1 == n_cand[1];
-      if (!pre3) {
-        std::vector<double> keys(n3);
-        for (int i = 0; i < n3; ++i) keys[i] = i < m0 ? 1.0 : 0.0;
-        own3.resize(n3);
-        SRB_REQUIRE(argsort(keys.data(), SAMROAD_F64, n3, own3.data(), user) == 0,
-                    "argsort callback failed (float64 priorities)");
-      }
-      const std::vector<int64_t>& asc = pre3 ? pre_asc[2] : own3;
-      if (int rc = g->ghist.ensure(sizeof(int64_t) * static_cast<size_t>(n3))) return rc;
-      SRB_CUDA_OK(cudaMemcpyAsync(g->ghist.p, asc.data(), sizeof(int64_t) * n3, cudaMemcpyHostToDevice, st));
-      order_from_host_kernel<<<blocks_for(n3), 256, 0, st>>>(g->ghist.as<int64_t>(), n3, g->order.as<int32_t>(),
-                                                             tot + 4);
-      note_launch();
-      SRB_CUDA_OK(cudaStreamSynchronize(st));
-    } else {
-      order3_stable_kernel<<<blocks_for(n3), 256, 0, st>>>(m0, m1, g->order.as<int32_t>());
-      note_launch();
-    }
-    gather_sorted3_kernel<<<blocks_for(n3), 256, 0, st>>>(g->cand3.as<int32_t>(), g->order.as<int32_t>(), m0, n3,
-                                                          g->sorted_pix.as<int32_t>(), tot + 4);
-    note_launch();
-    int err = 0;
-    if (int rc = read_ints(g, tot + 4, 1, &err, st)) return rc;
-    SRB_REQUIRE(err == 0, "argsort callback returned an invalid permutation (code %d) for the merged pass", err);
-    us_order[2] = us_since(t0);
-    t0 = clk::now();
-    if (int rc = nms_pass(g, g->sorted_pix.as<int32_t>(), nullptr, n3, n3, H, W, road_radius,
-                          g->flags32.as<int32_t>(), &n_out, &rounds[2], st))
+    const bool pre3 = have_pre && m0 == n_cand[0] && m1 == n_cand[1];
+    if (int rc = nms_pass(g, g->cand3.as<int32_t>(), g->cls3.as<uint8_t>(), n3, SAMROAD_F64, argsort, user,
+                          pre3 ? &pre_asc[2] : nullptr, "the merged pass", H, W, road_radius, g->list[2].as<int32_t>(),
+                          &ps[2], st))
       return rc;
-    us_nms[2] = us_since(t0);
-    SRB_REQUIRE(points_xy != nullptr || n_out == 0, "samroad_extract_graph_points: null output");
-    SRB_REQUIRE(n_out <= cap, "samroad_extract_graph_points: %d keypoints exceed the output capacity %d", n_out, cap);
-    if (n_out > 0) {
-      pix_to_xy_kernel<<<blocks_for(n_out), 256, 0, st>>>(g->flags32.as<int32_t>(), n_out, W, points_xy);
-      note_launch();
-      SRB_CUDA_OK(cudaGetLastError());
-    }
+  }
+  const int n_out = ps[2].kept;
+  SRB_REQUIRE(points_xy != nullptr || n_out == 0, "samroad_extract_graph_points: null output");
+  SRB_REQUIRE(n_out <= cap, "samroad_extract_graph_points: %d keypoints exceed the output capacity %d", n_out, cap);
+  if (n_out > 0) {
+    pix_to_xy_kernel<<<blocks_for(n_out), 256, 0, st>>>(g->list[2].as<int32_t>(), n_out, W, points_xy);
+    note_launch();
+    SRB_CUDA_OK(cudaGetLastError());
   }
   *n_points = n_out;
   if (stats) {
     stats[0] = n_cand[0]; stats[1] = n_cand[1]; stats[2] = m0; stats[3] = m1;
-    stats[4] = rounds[0]; stats[5] = rounds[1]; stats[6] = rounds[2]; stats[7] = n_out;
+    stats[4] = ps[0].rounds; stats[5] = ps[1].rounds; stats[6] = ps[2].rounds; stats[7] = n_out;
     // host wall-clock split in microseconds (each stage ends on a stream synchronisation)
-    stats[8] = us_cand; stats[9] = us_order[0] + us_presort; stats[10] = us_order[1]; stats[11] = us_order[2];
-    stats[12] = us_nms[0]; stats[13] = us_nms[1]; stats[14] = us_nms[2]; stats[15] = us_since(t_begin);
+    stats[8] = us_cand; stats[9] = ps[0].us_order + us_presort; stats[10] = ps[1].us_order;
+    stats[11] = ps[2].us_order; stats[12] = ps[0].us_nms; stats[13] = ps[1].us_nms; stats[14] = ps[2].us_nms;
+    stats[15] = us_since(t_begin);
   }
   return 0;
 }
@@ -1087,6 +1078,24 @@ __device__ __forceinline__ int lower_bound_i32(const int32_t* a, int n, int v) {
   return lo;
 }
 
+// arguments of the two aggregation kernels
+struct AggArgs {
+  const int32_t* pts;              // [N,2] keypoints
+  int N;
+  const int32_t* txy;              // [n_tiles,2] tile origins
+  int n_tiles, P;
+  const int *cnt, *off;            // the pair-query plan: per-tile count, offset, members, neighbour rows
+  const int32_t *members, *nbr;
+  const float* scores;             // tile t's block starts at tile_soff[t] (< 0: batch skipped)
+  const int64_t* tile_soff;
+  int K;
+  const int* adj_off;              // adjacency slots of each source, targets ascending
+  const int32_t* adj_tgt;
+  float *sum, *num;                // per slot: score sum, count and first occurrence
+  int32_t* first;
+  int* bad;                        // set when a score lies outside [0, 1]
+};
+
 // One WARP per source point walks its tiles in tile-list order and its pair slots in order: for a fixed
 // (src, tgt) that is exactly the order in which the reference's triple loop adds the scores, so the
 // float32 sum is bit-identical.  The lanes own the source's adjacency slots (slot = lane + 32 d) and keep
@@ -1094,40 +1103,35 @@ __device__ __forceinline__ int lower_bound_i32(const int32_t* a, int n, int v) {
 // once and broadcast one by one.  first[] records the key's first occurrence in the loop (dict order).
 // nbr rows are NS long.
 template <int DPL, int NS>
-__global__ void __launch_bounds__(256)
-aggregate_warp_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restrict__ txy, int n_tiles, int P,
-                      const int* __restrict__ cnt, const int* __restrict__ off, const int32_t* __restrict__ members,
-                      const int32_t* __restrict__ nbr, const float* __restrict__ scores,
-                      const int64_t* __restrict__ tile_soff, int K, const int* __restrict__ adj_off,
-                      const int32_t* __restrict__ adj_tgt, float* __restrict__ sum, float* __restrict__ num,
-                      int32_t* __restrict__ first, int* __restrict__ bad) {
+__global__ void __launch_bounds__(256) aggregate_warp_kernel(const AggArgs a) {
   const int S = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (S >= N) return;
-  const int px = pts[2 * S], py = pts[2 * S + 1];
-  const int a0 = adj_off[S], deg = adj_off[S + 1] - a0;
+  if (S >= a.N) return;
+  const int px = a.pts[2 * S], py = a.pts[2 * S + 1];
+  const int a0 = a.adj_off[S], deg = a.adj_off[S + 1] - a0;
   int tg[DPL], fi[DPL];
   float sm[DPL], nm[DPL];
 #pragma unroll
   for (int d = 0; d < DPL; ++d) {
     const int sl = lane + 32 * d;
-    tg[d] = sl < deg ? adj_tgt[a0 + sl] : -2;
+    tg[d] = sl < deg ? a.adj_tgt[a0 + sl] : -2;
     fi[d] = -1; sm[d] = 0.f; nm[d] = 0.f;
   }
+  const int K = a.K;
   bool badv = false;
-  for (int t = 0; t < n_tiles; ++t) {
-    if (!in_tile(px, py, txy[2 * t], txy[2 * t + 1], P)) continue;
-    const int64_t so = tile_soff[t];
+  for (int t = 0; t < a.n_tiles; ++t) {
+    if (!in_tile(px, py, a.txy[2 * t], a.txy[2 * t + 1], a.P)) continue;
+    const int64_t so = a.tile_soff[t];
     if (so < 0) continue;                                   // batch skipped: no points (inferencer.py:188-189)
-    const int base = off[t];
-    const int j = lower_bound_i32(members + base, cnt[t], S);
+    const int base = a.off[t];
+    const int j = lower_bound_i32(a.members + base, a.cnt[t], S);
     int Tk = -1;
     float vk = 0.f;
     if (lane < K) {
-      const int nb = nbr[(static_cast<size_t>(base) + j) * NS + lane];
+      const int nb = a.nbr[(static_cast<size_t>(base) + j) * NS + lane];
       if (nb >= 0) {
-        Tk = members[base + nb];
-        vk = scores[so + static_cast<int64_t>(j) * K + lane];
+        Tk = a.members[base + nb];
+        vk = a.scores[so + static_cast<int64_t>(j) * K + lane];
       }
     }
     for (int k = 0; k < K; ++k) {
@@ -1149,57 +1153,52 @@ aggregate_warp_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __r
 #pragma unroll
   for (int d = 0; d < DPL; ++d) {
     const int sl = lane + 32 * d;
-    if (sl < deg) { sum[a0 + sl] = sm[d]; num[a0 + sl] = nm[d]; first[a0 + sl] = fi[d]; }
+    if (sl < deg) { a.sum[a0 + sl] = sm[d]; a.num[a0 + sl] = nm[d]; a.first[a0 + sl] = fi[d]; }
   }
-  if (badv && lane == 0) atomicOr(bad, 1);
+  if (badv && lane == 0) atomicOr(a.bad, 1);
 }
 
 // Fallback for sources with more than 128 points within the neighbour radius (tiny NMS radii): one thread per
 // source, slots in global memory.  Same order of additions.
 template <int NS>
-__global__ void __launch_bounds__(128)
-aggregate_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restrict__ txy, int n_tiles, int P,
-                 const int* __restrict__ cnt, const int* __restrict__ off, const int32_t* __restrict__ members,
-                 const int32_t* __restrict__ nbr, const float* __restrict__ scores,
-                 const int64_t* __restrict__ tile_soff, int K, const int* __restrict__ adj_off,
-                 const int32_t* __restrict__ adj_tgt, float* __restrict__ sum, float* __restrict__ num,
-                 int32_t* __restrict__ first, int* __restrict__ bad) {
+__global__ void __launch_bounds__(128) aggregate_kernel(const AggArgs a) {
   const int S = blockIdx.x * blockDim.x + threadIdx.x;
-  if (S >= N) return;
-  const int px = pts[2 * S], py = pts[2 * S + 1];
-  const int a0 = adj_off[S], deg = adj_off[S + 1] - a0;
-  for (int t = 0; t < n_tiles; ++t) {
-    if (!in_tile(px, py, txy[2 * t], txy[2 * t + 1], P)) continue;
-    const int64_t so = tile_soff[t];
+  if (S >= a.N) return;
+  const int px = a.pts[2 * S], py = a.pts[2 * S + 1];
+  const int a0 = a.adj_off[S], deg = a.adj_off[S + 1] - a0;
+  const int K = a.K;
+  for (int t = 0; t < a.n_tiles; ++t) {
+    if (!in_tile(px, py, a.txy[2 * t], a.txy[2 * t + 1], a.P)) continue;
+    const int64_t so = a.tile_soff[t];
     if (so < 0) continue;                                   // batch skipped: no points (inferencer.py:188-189)
-    const int base = off[t];
-    const int j = lower_bound_i32(members + base, cnt[t], S);
-    const float* sc = scores + so + static_cast<int64_t>(j) * K;
+    const int base = a.off[t];
+    const int j = lower_bound_i32(a.members + base, a.cnt[t], S);
+    const float* sc = a.scores + so + static_cast<int64_t>(j) * K;
     for (int k = 0; k < K; ++k) {
-      const int nb = nbr[(static_cast<size_t>(base) + j) * NS + k];
+      const int nb = a.nbr[(static_cast<size_t>(base) + j) * NS + k];
       if (nb < 0) break;                                     // prefix-valid
-      const int T = members[base + nb];
+      const int T = a.members[base + nb];
       float v = sc[k];
       if (v != v) v = -100.0f;                               // inferencer.py:206
-      if (!(v >= 0.0f && v <= 1.0f)) atomicOr(bad, 1);       // the reference asserts (inferencer.py:219)
-      const int slot = a0 + lower_bound_i32(adj_tgt + a0, deg, T);
-      sum[slot] = __fadd_rn(sum[slot], v);
-      num[slot] = __fadd_rn(num[slot], 1.0f);
-      if (first[slot] < 0) first[slot] = (base + j) * K + k;
+      if (!(v >= 0.0f && v <= 1.0f)) atomicOr(a.bad, 1);     // the reference asserts (inferencer.py:219)
+      const int slot = a0 + lower_bound_i32(a.adj_tgt + a0, deg, T);
+      a.sum[slot] = __fadd_rn(a.sum[slot], v);
+      a.num[slot] = __fadd_rn(a.num[slot], 1.0f);
+      if (a.first[slot] < 0) a.first[slot] = (base + j) * K + k;
     }
   }
 }
 
-template <int NS, typename... Args>
-void launch_aggregate(int max_deg, int N, cudaStream_t st, Args... args) {
+template <int NS>
+void launch_aggregate(int max_deg, const AggArgs& a, cudaStream_t st) {
   if (max_deg <= 32)
-    aggregate_warp_kernel<1, NS><<<blocks_for(32L * N, 256), 256, 0, st>>>(args...);
+    aggregate_warp_kernel<1, NS><<<blocks_for(32L * a.N, 256), 256, 0, st>>>(a);
   else if (max_deg <= 64)
-    aggregate_warp_kernel<2, NS><<<blocks_for(32L * N, 256), 256, 0, st>>>(args...);
+    aggregate_warp_kernel<2, NS><<<blocks_for(32L * a.N, 256), 256, 0, st>>>(a);
   else if (max_deg <= 128)
-    aggregate_warp_kernel<4, NS><<<blocks_for(32L * N, 256), 256, 0, st>>>(args...);
+    aggregate_warp_kernel<4, NS><<<blocks_for(32L * a.N, 256), 256, 0, st>>>(a);
   else
-    aggregate_kernel<NS><<<blocks_for(N, 128), 128, 0, st>>>(args...);
+    aggregate_kernel<NS><<<blocks_for(a.N, 128), 128, 0, st>>>(a);
 }
 
 __global__ void edge_select_kernel(const float* __restrict__ sum, const float* __restrict__ num,
@@ -1232,15 +1231,16 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
   if (int rc = g->tile_soff.ensure(sizeof(int64_t) * g->n_tiles)) return rc;
   SRB_CUDA_OK(cudaMemcpyAsync(g->tile_soff.p, tile_score_offset_host, sizeof(int64_t) * g->n_tiles,
                               cudaMemcpyHostToDevice, st));
-  int* tot = g->totals.as<int>();
-  SRB_CUDA_OK(cudaMemsetAsync(tot + 8, 0, 4 * sizeof(int), st));
-  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, nullptr, g->adj_deg.as<int>(), nullptr, nullptr, tot + 10);
-  scan_single_block_kernel<<<1, 1024, 0, st>>>(g->adj_deg.as<int>(), N, g->adj_off.as<int>(), tot + 11);
+  Counters* ctr = g->counters.as<Counters>();
+  SRB_CUDA_OK(cudaMemsetAsync(ctr, 0, sizeof(Counters), st));
+  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, nullptr, g->adj_deg.as<int>(), nullptr, nullptr,
+                                                 &ctr->max_deg);
+  scan_single_block_kernel<<<1, 1024, 0, st>>>(g->adj_deg.as<int>(), N, g->adj_off.as<int>(), &ctr->nnz);
   note_launch(2);
-  int degs[2];
-  if (int rc = read_ints(g, tot + 10, 2, degs, st)) return rc;
-  const int max_deg = degs[0], nnz = degs[1];
-  SRB_CUDA_OK(cudaMemcpyAsync(g->adj_off.as<int>() + N, tot + 11, sizeof(int), cudaMemcpyDeviceToDevice, st));
+  Counters c;
+  if (int rc = read_back(g, ctr, &c, st)) return rc;
+  const int max_deg = c.max_deg, nnz = c.nnz;
+  SRB_CUDA_OK(cudaMemcpyAsync(g->adj_off.as<int>() + N, &ctr->nnz, sizeof(int), cudaMemcpyDeviceToDevice, st));
   if (nnz == 0) return 0;
   const size_t nz = static_cast<size_t>(nnz);
   if (int rc = g->adj_src.ensure(4 * nz)) return rc;
@@ -1256,27 +1256,24 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
   SRB_CUDA_OK(cudaMemsetAsync(g->eflags.p, 0xFF, 4 * static_cast<size_t>(n_entries), st));
   adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, g->adj_off.as<int>(), nullptr,
                                                  g->adj_src.as<int32_t>(), g->adj_tgt.as<int32_t>(), nullptr);
-#define SRB_AGG_ARGS                                                                                         \
-  pts, N, g->tile_xy.as<int32_t>(), g->n_tiles, g->P, g->t_cnt.as<int>(), g->t_off.as<int>(),               \
-      g->members.as<int32_t>(), g->nbr.as<int32_t>(), topo_scores, g->tile_soff.as<int64_t>(), K,           \
-      g->adj_off.as<int>(), g->adj_tgt.as<int32_t>(), g->adj_sum.as<float>(), g->adj_cnt.as<float>(),       \
-      g->adj_first.as<int32_t>(), tot + 8
+  const AggArgs args{pts, N, g->tile_xy.as<int32_t>(), g->n_tiles, g->P, g->t_cnt.as<int>(), g->t_off.as<int>(),
+                     g->members.as<int32_t>(), g->nbr.as<int32_t>(), topo_scores, g->tile_soff.as<int64_t>(), K,
+                     g->adj_off.as<int>(), g->adj_tgt.as<int32_t>(), g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
+                     g->adj_first.as<int32_t>(), &ctr->bad_score};
   if (g->nbr_stride == 16)
-    launch_aggregate<16>(max_deg, N, st, SRB_AGG_ARGS);
+    launch_aggregate<16>(max_deg, args, st);
   else
-    launch_aggregate<32>(max_deg, N, st, SRB_AGG_ARGS);
-#undef SRB_AGG_ARGS
+    launch_aggregate<32>(max_deg, args, st);
   edge_select_kernel<<<blocks_for(nnz), 256, 0, st>>>(g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
                                                       g->adj_first.as<int32_t>(), nnz, threshold,
                                                       g->eflags.as<int32_t>());
   note_launch(3);
   EdgeFlag ef{g->eflags.as<int32_t>(), g->adj_src.as<int32_t>(), g->adj_tgt.as<int32_t>(), edges, edges ? cap : 0};
-  if (int rc = compact(g, ef, static_cast<int>(n_entries), tot + 9, st)) return rc;
-  int res[2];
-  if (int rc = read_ints(g, tot + 8, 2, res, st)) return rc;
-  if (bad_score) *bad_score = res[0];
-  *n_edges = res[1];
-  SRB_REQUIRE(res[1] <= cap || edges == nullptr, "samroad_aggregate_edges: %d edges exceed the output capacity %d",
-              res[1], cap);
+  if (int rc = compact(g, ef, static_cast<int>(n_entries), &ctr->n_edges, st)) return rc;
+  if (int rc = read_back(g, ctr, &c, st)) return rc;
+  if (bad_score) *bad_score = c.bad_score;
+  *n_edges = c.n_edges;
+  SRB_REQUIRE(c.n_edges <= cap || edges == nullptr, "samroad_aggregate_edges: %d edges exceed the output capacity %d",
+              c.n_edges, cap);
   return 0;
 }
