@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define SAMROAD_ABI_VERSION 4
+#define SAMROAD_ABI_VERSION 5
 
 typedef struct samroad_ctx* samroad_handle_t;
 
@@ -190,6 +190,48 @@ int samroad_infer_batch_host_async(samroad_handle_t h, int slot, const void* rgb
                                    int N, int Ns, int Np, float* mask_scores_host,
                                    float* image_embeddings_host, float* topo_scores_host);
 int samroad_infer_batch_host_wait(samroad_handle_t h, int slot);
+
+/* ---- threshold search: exact binary precision-recall curves ---------------------------------------- */
+
+/* One accumulator stands for one torchmetrics BinaryPrecisionRecallCurve(thresholds=None,
+ * ignore_index=-1) of SAMRoad (model.py:361-363), fed by test_step (model.py:602-617) and read by
+ * on_test_end (model.py:619-634).  Each kept entry is stored as one 32-bit key on the device (4 bytes);
+ * compute needs 4 more bytes per entry and 28 bytes per distinct score while it runs.  At most 2^31-1
+ * entries per accumulator.  Calls on one handle are ordered on the stream they are given. */
+typedef struct samroad_prc_ctx* samroad_prc_t;
+
+int samroad_prc_create(int device, samroad_prc_t* out);
+int samroad_prc_destroy(samroad_prc_t p);
+/* Drops every entry (torchmetrics' reset()).  Asynchronous. */
+int samroad_prc_reset(samroad_prc_t p, void* stream);
+/* Appends n entries; asynchronous, no host synchronisation.  preds: device fp32, element i at
+ * preds[i * pred_stride] (so mask_scores[..., c] of [B,P,P,2] is read in place with stride 2).
+ * target: n contiguous SAMROAD_F32 values (label = int32(target), truncating as .to(torch.int32) does)
+ * or SAMROAD_U8 bytes.  valid: NULL or n bytes, 0 = ignored (the reference's target -1).
+ * An update with a kept prediction that is NaN or outside [0, 1] (torchmetrics would apply a sigmoid to
+ * the whole batch instead) or a kept label other than 0 / 1 (torchmetrics raises) adds nothing; the next
+ * samroad_prc_compute or samroad_prc_export_keys fails with code 3 and reports every refused update since
+ * the last report (their number, the first in detail), and the handle stays usable. */
+int samroad_prc_update(samroad_prc_t p, const float* preds, int64_t pred_stride, const void* target,
+                       int target_dtype, const uint8_t* valid, int64_t n, void* stream);
+/* Distributed evaluation (one accumulator per rank; the curve of the whole split needs every rank's
+ * entries, as torchmetrics' sync on compute gathers them): export_keys synchronises, reports refused
+ * updates like compute, writes the number of accepted entries to *n_keys and, when keys != NULL, copies
+ * their packed 32-bit keys (any order) into keys (device or host, room for cap).  append_keys adds keys
+ * exported by other accumulators (device memory, asynchronous); a key whose score is outside [0, 1]
+ * refuses the call like a bad update. */
+int samroad_prc_export_keys(samroad_prc_t p, uint32_t* keys, int64_t cap, int64_t* n_keys, void* stream);
+int samroad_prc_append_keys(samroad_prc_t p, const uint32_t* keys, int64_t n, void* stream);
+/* Sorts the entries and builds the curve (synchronises).  counts (host, 4): entries, positives,
+ * distinct thresholds T, index of the best point.  best (host, 4): threshold, precision, recall and F1 at
+ * the first maximum of F1 = 2*(P*R)/(P+R), a NaN F1 counting as larger than any number (torch.argmax).
+ * Counts are exact integers; P, R and F1 are the float32 operations of the reference in its order. */
+int samroad_prc_compute(samroad_prc_t p, int64_t* counts, float* best, void* stream);
+/* The curve of the last successful compute in torchmetrics' layout, each pointer may be NULL (device or
+ * host memory): thresholds [T] ascending, precision / recall [T+1] ending with the point (1, 0), and
+ * the int64 true / false positive counts [T] at each threshold (score >= threshold).  Asynchronous. */
+int samroad_prc_read_curve(samroad_prc_t p, float* thresholds, float* precision, float* recall,
+                           int64_t* tps, int64_t* fps, void* stream);
 
 /* Stream memory operations on a 32-bit flag word in device (or peer-mapped) memory, executed by the stream
  * front end without a kernel: an ordered write of `value`, and a wait until *addr >= value.  The exchange step

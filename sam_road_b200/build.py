@@ -18,7 +18,7 @@ CSRC = PKG_DIR / "csrc"
 OBJ_DIR = PKG_DIR / "_build"
 LIB_PATH = PKG_DIR / "libsamroad_b200.so"
 
-SOURCES = ["common.cu", "gemm_ops.cu", "kernels.cu", "attention.cu", "toponet.cu", "sam_decoder.cu", "graph.cu", "model.cu"]
+SOURCES = ["common.cu", "gemm_ops.cu", "kernels.cu", "attention.cu", "toponet.cu", "sam_decoder.cu", "graph.cu", "metrics.cu", "model.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",

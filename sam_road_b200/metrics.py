@@ -1,0 +1,169 @@
+"""Exact binary precision-recall curves on the device (the threshold search of the reference's test.py).
+
+`PrecisionRecallCurve` stands for one torchmetrics `BinaryPrecisionRecallCurve(ignore_index=-1)` of
+SAMRoad (reference model.py:361-363): `update` appends scores and labels on the device without a host
+synchronisation, `compute` returns the exact curve in torchmetrics' layout.  Under torch.distributed
+(world size > 1) `compute` is the curve of every rank's entries, as torchmetrics' sync on compute gives:
+the ranks all-gather their packed keys, and since the curve depends only on the multiset of keys the
+result is exact and the same on every rank.  The work runs in the
+`samroad_prc_*` kernels of libsamroad_b200.so (include/samroad_b200.h); DESIGN.md §10 states where the
+result differs from torchmetrics' (integer counts, no sigmoid of out-of-range scores).
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Optional, Tuple
+
+import torch
+
+from . import _lib
+
+
+class PrecisionRecallCurve:
+    """Accumulates (score, label) pairs on one CUDA device; state persists until `reset()`."""
+
+    def __init__(self, device):
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError(f"PrecisionRecallCurve runs on CUDA only; got '{device}'. There is no CPU path.")
+        self.device = torch.device("cuda", device.index if device.index is not None else torch.cuda.current_device())
+        h = C.c_void_p()
+        _lib.check(_lib.load().samroad_prc_create(self.device.index, C.byref(h)), "samroad_prc_create")
+        self._h = h.value
+        self._curve_h = self._h     # the handle the last compute ran on (a gathered one under distributed)
+        self._best = None
+
+    def __del__(self):
+        try:
+            self._drop_gathered()
+            if self.__dict__.get("_h"):
+                _lib.load().samroad_prc_destroy(self._h)
+        except Exception:
+            pass
+
+    def _drop_gathered(self):
+        h = self.__dict__.get("_curve_h")
+        if h and h != self.__dict__.get("_h"):
+            _lib.load().samroad_prc_destroy(h)
+        self._curve_h = self.__dict__.get("_h")
+
+    def __getstate__(self):
+        raise TypeError("PrecisionRecallCurve holds device state and cannot be copied or pickled")
+
+    def reset(self) -> None:
+        with torch.cuda.device(self.device):
+            self._drop_gathered()
+            _lib.check(_lib.load().samroad_prc_reset(self._h, _lib.current_stream_ptr()), "samroad_prc_reset")
+        self._best = None
+
+    def update(self, preds: torch.Tensor, target: torch.Tensor, valid: Optional[torch.Tensor] = None) -> None:
+        """preds: float32 scores in [0, 1], any view whose elements sit at one common stride (such as
+        mask_scores[..., c]) is read in place.  target: float (label = int32(target)) or bool / uint8
+        labels of the same number of elements.  valid: optional bool / uint8 mask, False = ignored.
+        Asynchronous: an update with a NaN or out-of-range score or a label other than 0 / 1 adds nothing
+        and is reported by the next `compute()`."""
+        n = preds.numel()
+        if target.numel() != n or (valid is not None and valid.numel() != n):
+            raise ValueError(f"preds, target and valid must have the same number of elements; got {n}, "
+                             f"{target.numel()}, {None if valid is None else valid.numel()}")
+        for name, t in (("preds", preds), ("target", target), ("valid", valid)):
+            if t is not None and t.device != self.device:
+                raise RuntimeError(f"{name} is on {t.device}, the accumulator on {self.device}")
+        if preds.dtype != torch.float32:
+            raise TypeError(f"preds must be float32, got {preds.dtype}")
+        flat = preds.reshape(-1)            # a view whenever the elements share one stride
+        stride = flat.stride(0) if n > 1 else 1
+        if target.dtype in (torch.bool, torch.uint8):
+            tgt, tdt = target.reshape(-1).contiguous().view(torch.uint8), _lib.U8
+        elif target.dtype == torch.float32:
+            tgt, tdt = target.reshape(-1).contiguous(), _lib.F32
+        else:
+            raise TypeError(f"target must be float32, bool or uint8, got {target.dtype}")
+        val = None
+        if valid is not None:
+            if valid.dtype not in (torch.bool, torch.uint8):
+                raise TypeError(f"valid must be bool or uint8, got {valid.dtype}")
+            val = valid.reshape(-1).contiguous().view(torch.uint8)
+        self._best = None
+        if n == 0:
+            return
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().samroad_prc_update(
+                self._h, flat.data_ptr(), stride, tgt.data_ptr(), tdt, _lib.ptr(val), n,
+                _lib.current_stream_ptr()), "samroad_prc_update")
+
+    def _gathered_handle(self, dist) -> int:
+        """A new accumulator holding the accepted keys of every rank.  Every rank takes part in the same
+        collectives even when one of them fails, so a refusal on one rank raises on all of them instead of
+        leaving the others waiting."""
+        lib, stream = _lib.load(), _lib.current_stream_ptr()
+        world = dist.get_world_size()
+        comm_dev = self.device if dist.get_backend() == "nccl" else torch.device("cpu")
+        n = C.c_int64(0)
+        rc = lib.samroad_prc_export_keys(self._h, None, 0, C.byref(n), stream)
+        err = _lib.last_error() if rc else ""
+        mine = torch.tensor([n.value if rc == 0 else -1], dtype=torch.int64, device=comm_dev)
+        counts = [torch.empty_like(mine) for _ in range(world)]
+        dist.all_gather(counts, mine)
+        counts = [int(c) for c in counts]
+        if rc:
+            raise RuntimeError(f"samroad_prc_export_keys failed (code {rc}): {err}")
+        if min(counts) < 0:
+            raise RuntimeError(f"rank {counts.index(-1)} could not contribute its entries to the curve "
+                               "(its own error names the cause)")
+        m = max(max(counts), 1)
+        local = torch.zeros(m, dtype=torch.int32, device=self.device)    # packed uint32 keys, as int32
+        _lib.check(lib.samroad_prc_export_keys(self._h, local.data_ptr(), m, C.byref(n), stream),
+                   "samroad_prc_export_keys")
+        send = local.to(comm_dev)
+        parts = [torch.empty(m, dtype=torch.int32, device=comm_dev) for _ in range(world)]
+        dist.all_gather(parts, send)
+        h = C.c_void_p()
+        _lib.check(lib.samroad_prc_create(self.device.index, C.byref(h)), "samroad_prc_create")
+        try:
+            for part, c in zip(parts, counts):
+                part = part[:c].to(self.device)
+                _lib.check(lib.samroad_prc_append_keys(h.value, part.data_ptr(), c, stream), "samroad_prc_append_keys")
+            torch.cuda.current_stream().synchronize()    # `parts` are freed on return
+        except Exception:
+            lib.samroad_prc_destroy(h.value)
+            raise
+        return h.value
+
+    def _compute(self):
+        counts = (C.c_int64 * 4)()
+        best = (C.c_float * 4)()
+        with torch.cuda.device(self.device):
+            self._drop_gathered()
+            dist = torch.distributed
+            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+                self._curve_h = self._gathered_handle(dist)
+            _lib.check(_lib.load().samroad_prc_compute(self._curve_h, counts, best, _lib.current_stream_ptr()),
+                       "samroad_prc_compute")
+        self._best = (tuple(counts), tuple(best))
+        return self._best
+
+    def compute(self, with_counts: bool = False):
+        """(precision [T+1], recall [T+1], thresholds [T]) as device float32 tensors, thresholds ascending
+        and the curve ending with the point (1, 0) like torchmetrics'.  With `with_counts` the int64
+        true / false positive counts [T] at each threshold follow."""
+        (n, n_pos, T, _), _ = self._compute()
+        dev = self.device
+        thr = torch.empty(T, dtype=torch.float32, device=dev)
+        prec = torch.empty(T + 1, dtype=torch.float32, device=dev)
+        rec = torch.empty(T + 1, dtype=torch.float32, device=dev)
+        tps = torch.empty(T, dtype=torch.int64, device=dev) if with_counts else None
+        fps = torch.empty(T, dtype=torch.int64, device=dev) if with_counts else None
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().samroad_prc_read_curve(
+                self._curve_h, thr.data_ptr(), prec.data_ptr(), rec.data_ptr(), _lib.ptr(tps), _lib.ptr(fps),
+                _lib.current_stream_ptr()), "samroad_prc_read_curve")
+        return (prec, rec, thr, tps, fps) if with_counts else (prec, rec, thr)
+
+    def best(self) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+        """0-dim float32 device tensors (threshold, precision, recall, F1) at torch.argmax of
+        F1 = 2*(P*R)/(P+R) over the curve: the first maximum, a NaN counting as the largest value."""
+        if self._best is None:
+            self._compute()
+        _, vals = self._best
+        return tuple(torch.tensor(v, dtype=torch.float32, device=self.device) for v in vals)

@@ -211,6 +211,8 @@ class SAMRoad(_Base):
         self._handles: Dict[int, int] = {}     # cuda device index -> samroad_handle_t
         self._weights_version = 0
         self._synced_version: Dict[int, int] = {}
+        self._test_curves = None               # (keypoint, road, topo) PrecisionRecallCurve, see test_step
+        self.best_thresholds = None
         self.matched_param_names = set()
         ckpt_path = _cfg_get(config, "SAM_CKPT_PATH", None)
         if ckpt_path and os.path.isfile(str(ckpt_path)):
@@ -303,6 +305,7 @@ class SAMRoad(_Base):
         state = dict(self.__dict__)
         state["_handles"] = {}
         state["_synced_version"] = {}
+        state["_test_curves"] = None
         return state
 
     def __deepcopy__(self, memo):
@@ -313,6 +316,8 @@ class SAMRoad(_Base):
         for k, v in self.__dict__.items():
             if k in ("_handles", "_synced_version"):
                 new.__dict__[k] = {}
+            elif k == "_test_curves":
+                new.__dict__[k] = None
             else:
                 new.__dict__[k] = copy.deepcopy(v, memo)
         return new
@@ -450,3 +455,56 @@ class SAMRoad(_Base):
 
     def training_step(self, *a, **k):
         raise NotImplementedError("sam_road_b200.SAMRoad is inference-only (SURVEY.md §8b)")
+
+    # ---- threshold search (test.py) ----------------------------------------------------------------
+    _CURVE_NAMES = ("keypoint", "road", "topo")
+
+    @torch.no_grad()
+    def test_step(self, batch, batch_idx):
+        """model.py:602-617: mask and topology scores of one evaluation batch go into three exact
+        precision-recall curves (sam_road_b200.metrics).  batch is the reference's collated dict: rgb
+        [B,P,P,3], keypoint_mask / road_mask [B,P,P] (float, label = int32(mask)), graph_points [B,N,2],
+        pairs [B,Ns,Np,2], valid / connected [B,Ns,Np] bool.  Autocast is ignored, as by the inference
+        calls: the scores are the engine's own."""
+        from .metrics import PrecisionRecallCurve
+        rgb, valid = batch["rgb"], batch["valid"]
+        scores, _, emb = self._encode(rgb, False)
+        _, topo_scores = self._topo(emb, batch["graph_points"], batch["pairs"], valid, False)
+        if self._test_curves is None:
+            self._test_curves = tuple(PrecisionRecallCurve(rgb.device) for _ in self._CURVE_NAMES)
+        kp, road, topo = self._test_curves
+        if kp.device != scores.device:
+            raise RuntimeError(f"test batches arrive on {scores.device}, the curves were started on {kp.device}; "
+                               "call reset_test_metrics() first")
+        kp.update(scores[..., 0], batch["keypoint_mask"])
+        road.update(scores[..., 1], batch["road_mask"])
+        topo.update(topo_scores, batch["connected"], valid)   # valid == False is the reference's label -1
+
+    def on_test_end(self):
+        """model.py:619-634: prints the best-F1 threshold, precision, recall and F1 of each curve as
+        Python floats (the form the configs record) and returns / stores them in `best_thresholds`:
+        {"keypoint" | "road" | "topo": (threshold, P, R, F1)}.  Under torch.distributed (Lightning's DDP
+        test loop) every rank reports the curves of the whole split: the ranks gather their entries
+        (sam_road_b200.metrics), as torchmetrics' sync on compute does in the reference."""
+        if self._test_curves is None:
+            dist = torch.distributed
+            if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+                raise RuntimeError("on_test_end: no test_step ran since the last reset_test_metrics()")
+            from .metrics import PrecisionRecallCurve   # a rank without batches still joins the gathers
+            dev = torch.device("cuda", torch.cuda.current_device())
+            self._test_curves = tuple(PrecisionRecallCurve(dev) for _ in self._CURVE_NAMES)
+        print("======= Finding best thresholds ======")
+        best = {}
+        for name, curve in zip(self._CURVE_NAMES, self._test_curves):
+            print(f"======= {name} ======")
+            thr, p, r, f1 = (t.item() for t in curve.best())
+            print(f"Best threshold {thr}, P={p} R={r} F1={f1}")
+            best[name] = (thr, p, r, f1)
+        self.best_thresholds = best
+        return best
+
+    def reset_test_metrics(self) -> None:
+        """Drops every entry of the three curves (they persist across test runs, like torchmetrics
+        state, until this is called)."""
+        self._test_curves = None      # the accumulators free their device memory
+        self.best_thresholds = None
