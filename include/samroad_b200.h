@@ -233,6 +233,46 @@ int samroad_prc_compute(samroad_prc_t p, int64_t* counts, float* best, void* str
 int samroad_prc_read_curve(samroad_prc_t p, float* thresholds, float* precision, float* recall,
                            int64_t* tps, int64_t* fps, void* stream);
 
+/* ---- validation: losses, IoUs and F1 of validation_step / on_validation_epoch_end --------------------- */
+
+/* One accumulator stands for the criteria and metrics of SAMRoad (model.py:349-359) as validation_step
+ * (model.py:547-588) feeds them and on_validation_epoch_end (model.py:591-600) reads them: the epoch's
+ * batch-size-weighted mean of the three step losses, and exact int64 confusion counts of the keypoint mask,
+ * the road mask and the valid pair slots (prediction positive when score > 0.5).  O(1) device state.  Calls
+ * on one handle are ordered on the stream they are given. */
+typedef struct samroad_val_ctx* samroad_val_t;
+
+#define SAMROAD_LOSS_BCE 0   /* BCEWithLogitsLoss() */
+#define SAMROAD_LOSS_FOCAL 1 /* torchvision sigmoid_focal_loss(alpha=0.25, gamma=2, reduction='mean') */
+
+int samroad_val_create(int device, samroad_val_t* out);
+int samroad_val_destroy(samroad_val_t v);
+/* Clears the epoch state (counts, loss sums) and any unreported refusal.  Asynchronous. */
+int samroad_val_reset(samroad_val_t v, void* stream);
+/* One validation step; asynchronous, no host synchronisation.  Device pointers:
+ *   mask_logits, mask_scores  [B,P,P,2] float32 as samroad_encode_masks writes them (8-byte aligned);
+ *   keypoint_mask, road_mask  [B,P,P] float32 targets, each exactly 0.0 or 1.0;
+ *   topo_logits, topo_scores  [B*Ns*Np] float32; connected, valid [B*Ns*Np] bytes, 0 or 1;
+ *   out                       [3] float32: the step's (mask_loss, topo_loss, loss).
+ * mask_loss is the mean of the per-element loss (loss_kind) over both channels, topo_loss the mean of the
+ * BCE over the valid slots (NaN without one), loss = mask_loss + topo_loss; the element terms are the
+ * reference's float32 expressions, their sums fp64, each mean rounded to float32 once.  A step with a mask
+ * target other than 0.0 / 1.0, a counted score that is NaN or outside [0, 1], or a connected / valid byte
+ * other than 0 / 1 is refused as a whole: it adds nothing and writes NaN to out; the next samroad_val_read
+ * fails with code 3 and reports every refused step since the last report (their number, the first in
+ * detail: element index e < 2*B*P*P is mask entry e of [B,P,P,2], above it pair slot e - 2*B*P*P), and the
+ * handle stays usable. */
+int samroad_val_update(samroad_val_t v, const float* mask_logits, const float* mask_scores,
+                       const float* keypoint_mask, const float* road_mask, const float* topo_logits,
+                       const float* topo_scores, const uint8_t* connected, const uint8_t* valid, int B, int P,
+                       int Ns, int Np, int loss_kind, float* out, void* stream);
+/* Synchronises and reports refused steps (see update).  Host outputs:
+ *   counts [11] int64: keypoint tp, fp, fn, tn; road tp, fp, fn, tn; topology tp, fp, fn (valid slots);
+ *   means  [3] float32: epoch (mask_loss, topo_loss, loss) = f32(sum(step value * B) / sum(B)), NaN
+ *          before the first accepted step;
+ *   totals [2] int64: accepted steps, sum of their B. */
+int samroad_val_read(samroad_val_t v, int64_t* counts, float* means, int64_t* totals, void* stream);
+
 /* Stream memory operations on a 32-bit flag word in device (or peer-mapped) memory, executed by the stream
  * front end without a kernel: an ordered write of `value`, and a wait until *addr >= value.  The exchange step
  * between ranks (sam_road_b200/exchange.py; no reference counterpart, the reference is single-GPU) builds its

@@ -15,6 +15,7 @@ LIB_PATH = _PKG / "libsamroad_b200.so"
 F32, I64, I32, U8, F64 = 0, 1, 2, 3, 4
 ABI_VERSION = 5
 TOPO_NORMAL, TOPO_NO_OFFSET, TOPO_NO_TRANSFORMER = 0, 1, 2
+LOSS_BCE, LOSS_FOCAL = 0, 1
 ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
 
 
@@ -69,6 +70,11 @@ SIGNATURES = {
     "samroad_prc_read_curve": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "samroad_prc_export_keys": (_i, [_vp, _vp, C.c_int64, C.POINTER(C.c_int64), _vp]),
     "samroad_prc_append_keys": (_i, [_vp, _vp, C.c_int64, _vp]),
+    "samroad_val_create": (_i, [_i, C.POINTER(_vp)]),
+    "samroad_val_destroy": (_i, [_vp]),
+    "samroad_val_reset": (_i, [_vp, _vp]),
+    "samroad_val_update": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "samroad_val_read": (_i, [_vp, C.POINTER(C.c_int64), C.POINTER(C.c_float), C.POINTER(C.c_int64), _vp]),
     "samroad_stream_write_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_stream_wait_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_timing_enable": (_i, [_vp, _i]),

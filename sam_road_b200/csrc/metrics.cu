@@ -1,4 +1,5 @@
-// sam_road_b200 :: metrics.cu -- exact binary precision-recall curves for threshold search.
+// sam_road_b200 :: metrics.cu -- exact binary precision-recall curves for threshold search, and the
+// losses and metrics of the validation loop (second half of the file, DESIGN.md §11).
 //
 // Replaces the three torchmetrics BinaryPrecisionRecallCurve(ignore_index=-1) of SAMRoad (reference
 // model.py:361-363) that test_step feeds (model.py:602-617) and on_test_end reads (model.py:619-634).
@@ -16,7 +17,9 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
+#include <cstdint>
 #include <cstdio>
 #include <cstring>
 
@@ -27,21 +30,29 @@ using namespace srb;
 
 namespace {
 
-// Device-side state of one accumulator.  `staged` runs ahead of `committed` while an update appends;
-// the commit kernel keeps or drops the update's entries as a whole.
-struct PrcState {
-  unsigned long long committed;   // entries accepted so far
-  unsigned long long staged;      // committed + entries of the update in flight
+// Refusal bookkeeping shared by the accumulators: an update in flight raises flag bits; its commit either
+// accepts it or counts it as refused (the first one in detail) until a synchronising call reports it.
+struct Refusals {
   unsigned int flags;             // kBad* bits of the update in flight
   unsigned long long first_bad;   // smallest offending element index of the update in flight
   unsigned int sticky_count;      // refused updates not yet reported
   unsigned int sticky_flags;      // union of their kBad* bits
   unsigned long long sticky_bad;  // offending element of the first of them
   long long sticky_update;        // serial number of the first of them (counted from the last reset)
+};
+
+// Device-side state of one precision-recall accumulator.  `staged` runs ahead of `committed` while an
+// update appends; the commit kernel keeps or drops the update's entries as a whole.
+struct PrcState {
+  unsigned long long committed;   // entries accepted so far
+  unsigned long long staged;      // committed + entries of the update in flight
+  Refusals ref;
   unsigned long long best;        // compute: argmax key, see best_key()
 };
 
 constexpr unsigned kBadPred = 1u, kBadTarget = 2u;
+const char* const kPrcBadText[] = {" a prediction is NaN or outside [0, 1]",
+                                   " a target is not 0 or 1 after truncation to int32"};
 
 // Tile sizes.  The radix sort gives one warp a chunk of kSortChunk keys (stable within the warp by
 // __match_any_sync ranks); scans and the curve kernel give a 256-thread block kTile elements.
@@ -106,6 +117,28 @@ int ensure(T*& p, size_t& cap, size_t n) {
   return 0;
 }
 
+__device__ __forceinline__ void refusal_note(Refusals* r, unsigned flag, unsigned long long i) {
+  atomicOr(&r->flags, flag);
+  atomicMin(&r->first_bad, i);
+}
+
+__device__ __forceinline__ void refusal_begin(Refusals* r) {
+  r->flags = 0;
+  r->first_bad = ~0ull;
+}
+
+// true: the update in flight is accepted.  Otherwise it is counted as refused.  Single thread.
+__device__ __forceinline__ bool refusal_commit(Refusals* r, long long serial) {
+  if (r->flags == 0) return true;
+  if (r->sticky_count == 0) {
+    r->sticky_bad = r->first_bad;
+    r->sticky_update = serial;
+  }
+  ++r->sticky_count;
+  r->sticky_flags |= r->flags;
+  return false;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // update
 // ---------------------------------------------------------------------------------------------------
@@ -148,8 +181,8 @@ __global__ void __launch_bounds__(256) prc_append_kernel(const float* __restrict
     }
     const bool pred_ok = s >= 0.0f && s <= 1.0f;   // false for NaN
     if (!pred_ok || !tgt_ok) {
-      atomicOr(&st->flags, (pred_ok ? 0u : kBadPred) | (tgt_ok ? 0u : kBadTarget));
-      atomicMin(&st->first_bad, static_cast<unsigned long long>(i));
+      refusal_note(&st->ref, (pred_ok ? 0u : kBadPred) | (tgt_ok ? 0u : kBadTarget),
+                   static_cast<unsigned long long>(i));
     } else {
       keep = true;
       key = (__float_as_uint(s == 0.0f ? 0.0f : s) << 1) | static_cast<uint32_t>(label);
@@ -169,33 +202,20 @@ __global__ void __launch_bounds__(256) prc_append_keys_kernel(const uint32_t* __
   if (i < n) {
     key = in[i];
     keep = (key >> 1) <= 0x3F800000u;          // float bits of a score in [0, 1]
-    if (!keep) {
-      atomicOr(&st->flags, kBadPred);
-      atomicMin(&st->first_bad, static_cast<unsigned long long>(i));
-    }
+    if (!keep) refusal_note(&st->ref, kBadPred, static_cast<unsigned long long>(i));
   }
   append_key(keep, key, keys, st);
 }
 
 __global__ void prc_begin_kernel(PrcState* st) {
   st->staged = st->committed;
-  st->flags = 0;
-  st->first_bad = ~0ull;
+  refusal_begin(&st->ref);
 }
 
 // Keeps the update's entries, or drops all of them and counts the refusal (the first one in detail) until a
 // synchronising call reports it.
 __global__ void prc_commit_kernel(PrcState* st, long long serial) {
-  if (st->flags == 0) {
-    st->committed = st->staged;
-  } else {
-    if (st->sticky_count == 0) {
-      st->sticky_bad = st->first_bad;
-      st->sticky_update = serial;
-    }
-    ++st->sticky_count;
-    st->sticky_flags |= st->flags;
-  }
+  if (refusal_commit(&st->ref, serial)) st->committed = st->staged;
   st->staged = st->committed;
 }
 
@@ -424,24 +444,32 @@ int read_state(samroad_prc_ctx* p, cudaStream_t st) {
   return 0;
 }
 
-// Synchronises, and fails with code 3 while refused updates are unreported: it reports them all (their
-// number, the first in detail) and clears the count, so no later call can succeed past an unreported
-// refusal.  On success *committed holds the number of accepted entries.
+// `s` is a synchronised host copy of the device bookkeeping `dev`.  Fails with code 3 while refused
+// updates are unreported: it reports them all (their number, the first in detail, the text of every
+// flag bit raised) and clears the count, so no later call can succeed past an unreported refusal.
+int report_refusals(const Refusals& s, Refusals* dev, const char* what, const char* const* bad_text, int n_bad,
+                    cudaStream_t st) {
+  if (s.sticky_count == 0) return 0;
+  SRB_CUDA_OK(cudaMemsetAsync(&dev->sticky_count, 0, sizeof(unsigned int), st));
+  SRB_CUDA_OK(cudaMemsetAsync(&dev->sticky_flags, 0, sizeof(unsigned int), st));
+  SRB_CUDA_OK(cudaStreamSynchronize(st));
+  char why[512] = "";
+  for (int b = 0; b < n_bad; ++b)
+    if (s.sticky_flags & (1u << b)) strncat(why, bad_text[b], sizeof(why) - strlen(why) - 1);
+  set_last_error("%s: %u update(s) since the last report were refused and added nothing; the first, "
+                 "update #%lld since the last reset, at element %llu:%s",
+                 what, s.sticky_count, s.sticky_update, s.sticky_bad, why);
+  return 3;
+}
+
+// Synchronises and reports refused updates (report_refusals).  On success *committed holds the number of
+// accepted entries.
 int take_refusals(samroad_prc_ctx* p, const char* what, long long* committed, cudaStream_t st) {
   if (int rc = read_state(p, st)) return rc;
   const PrcState s = *p->h_state;
   p->reserved = s.committed;
   *committed = static_cast<long long>(s.committed);
-  if (s.sticky_count == 0) return 0;
-  SRB_CUDA_OK(cudaMemsetAsync(&p->state->sticky_count, 0, sizeof(unsigned int), st));
-  SRB_CUDA_OK(cudaMemsetAsync(&p->state->sticky_flags, 0, sizeof(unsigned int), st));
-  SRB_CUDA_OK(cudaStreamSynchronize(st));
-  set_last_error("%s: %u update(s) since the last report were refused and added nothing; the first, "
-                 "update #%lld since the last reset, at element %llu:%s%s",
-                 what, s.sticky_count, s.sticky_update, s.sticky_bad,
-                 (s.sticky_flags & kBadPred) ? " a prediction is NaN or outside [0, 1]" : "",
-                 (s.sticky_flags & kBadTarget) ? " a target is not 0 or 1 after truncation to int32" : "");
-  return 3;
+  return report_refusals(s.ref, &p->state->ref, what, kPrcBadText, 2, st);
 }
 
 void free_curve(samroad_prc_ctx* p) {
@@ -689,5 +717,352 @@ extern "C" int samroad_prc_read_curve(samroad_prc_t p, float* thresholds, float*
   if (recall) SRB_CUDA_OK(cudaMemcpyAsync(recall, p->rec, sizeof(float) * (T + 1), k, st));
   if (tps) SRB_CUDA_OK(cudaMemcpyAsync(tps, p->tps, sizeof(int64_t) * T, k, st));
   if (fps) SRB_CUDA_OK(cudaMemcpyAsync(fps, p->fps, sizeof(int64_t) * T, k, st));
+  return 0;
+}
+
+// =================================================================================================
+// Validation: the losses, IoUs and F1 of SAMRoad.validation_step / on_validation_epoch_end (reference
+// model.py:349-359, 547-600).  One update is one validation step: a grid-stride pass over the pixels (both
+// mask channels), a pass over the pair slots, then one block that reduces the per-block partials in a fixed
+// order, writes the step's (mask_loss, topo_loss, loss) and commits the step to the epoch state.  Sums of
+// the float32 loss terms are fp64, counts are integers, so the result does not depend on scheduling.
+// =================================================================================================
+namespace {
+
+constexpr unsigned kBadMaskTarget = 1u, kBadScore = 2u, kBadPairByte = 4u;
+const char* const kValBadText[] = {" a mask target is not exactly 0.0 or 1.0",
+                                   " a counted score is NaN or outside [0, 1]",
+                                   " a connected or valid byte is not 0 or 1"};
+constexpr int kValCounts = 11;      // keypoint tp fp fn tn, road tp fp fn tn, topology tp fp fn
+constexpr int kValBlocksPerSm = 4;  // blocks per SM of each pass (grid-stride beyond that)
+
+struct ValState {
+  double loss_wsum[3];              // Σ f64(step value) · B over the accepted steps
+  long long steps, samples;         // accepted steps, Σ B
+  long long counts[kValCounts];
+  Refusals ref;
+};
+
+// One block's share of a step.  Mask pass: Σ terms of both channels; tp, fp, fn of keypoint then road.
+// Pair pass: Σ terms over valid slots; n_valid, tp, fp, fn.
+struct ValPartial {
+  double sum;
+  unsigned long long c[6];
+};
+
+// torch's CUDA log_sigmoid: min(0, x) - log1p(exp(-|x|))
+__device__ __forceinline__ float log_sigmoid_f32(float x) {
+  return __fsub_rn(fminf(0.0f, x), log1pf(expf(-fabsf(x))));
+}
+
+// F.binary_cross_entropy_with_logits(x, y, reduction='none') = (1 - y) * x - log_sigmoid(x), one rounding
+// per torch op
+__device__ __forceinline__ float bce_term(float x, float y) {
+  return __fsub_rn(__fmul_rn(__fsub_rn(1.0f, y), x), log_sigmoid_f32(x));
+}
+
+// torchvision.ops.sigmoid_focal_loss(x, y, alpha=0.25, gamma=2, reduction='none') in its order
+__device__ __forceinline__ float focal_term(float x, float y) {
+  const float p = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x)));
+  const float one_y = __fsub_rn(1.0f, y);
+  const float p_t = __fadd_rn(__fmul_rn(p, y), __fmul_rn(__fsub_rn(1.0f, p), one_y));
+  const float m = __fsub_rn(1.0f, p_t);
+  const float loss = __fmul_rn(bce_term(x, y), __fmul_rn(m, m));
+  const float alpha_t = __fadd_rn(__fmul_rn(0.25f, y), __fmul_rn(0.75f, one_y));
+  return __fmul_rn(alpha_t, loss);
+}
+
+// Block-wide sum of a partial in a fixed order; the result is valid in thread 0.
+template <int kN>
+__device__ __forceinline__ void block_sum_partial(double& sum, unsigned long long (&c)[kN], ValPartial* sh /*[8]*/) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    sum += __shfl_down_sync(0xffffffffu, sum, o);
+#pragma unroll
+    for (int k = 0; k < kN; ++k) c[k] += __shfl_down_sync(0xffffffffu, c[k], o);
+  }
+  if (lane == 0) {
+    sh[wid].sum = sum;
+#pragma unroll
+    for (int k = 0; k < kN; ++k) sh[wid].c[k] = c[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < static_cast<int>(blockDim.x >> 5); ++w) {
+      sum += sh[w].sum;
+#pragma unroll
+      for (int k = 0; k < kN; ++k) c[k] += sh[w].c[k];
+    }
+  }
+}
+
+__device__ __forceinline__ void note_bad(unsigned& bad, unsigned long long& first, unsigned flag,
+                                         unsigned long long i) {
+  bad |= flag;
+  first = i < first ? i : first;
+}
+
+// Pixels: logits / scores are [npix] float2 (the two channels of [B,P,P,2]), kp / road [npix] float.
+// Element index of a refusal: pixel * 2 + channel.
+template <bool kFocal>
+__global__ void __launch_bounds__(256) val_mask_kernel(const float2* __restrict__ logits,
+                                                       const float2* __restrict__ scores,
+                                                       const float* __restrict__ kp, const float* __restrict__ road,
+                                                       long long npix, ValPartial* __restrict__ part,
+                                                       Refusals* __restrict__ ref) {
+  __shared__ ValPartial sh[8];
+  double sum = 0.0;
+  unsigned c[6] = {0, 0, 0, 0, 0, 0};
+  unsigned bad = 0;
+  unsigned long long first = ~0ull;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < npix; i += stride) {
+    const float2 x = logits[i], s = scores[i];
+    const float y[2] = {kp[i], road[i]};
+    const float xs[2] = {x.x, x.y}, ss[2] = {s.x, s.y};
+#pragma unroll
+    for (int ch = 0; ch < 2; ++ch) {
+      const unsigned long long e = static_cast<unsigned long long>(i) * 2 + ch;
+      if (!(y[ch] == 0.0f || y[ch] == 1.0f)) note_bad(bad, first, kBadMaskTarget, e);
+      if (!(ss[ch] >= 0.0f && ss[ch] <= 1.0f)) note_bad(bad, first, kBadScore, e);
+      sum += static_cast<double>(kFocal ? focal_term(xs[ch], y[ch]) : bce_term(xs[ch], y[ch]));
+      const bool pred = ss[ch] > 0.5f, lab = y[ch] == 1.0f;
+      c[3 * ch + 0] += pred && lab;
+      c[3 * ch + 1] += pred && !lab;
+      c[3 * ch + 2] += !pred && lab;
+    }
+  }
+  if (bad) refusal_note(ref, bad, first);
+  unsigned long long cc[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) cc[k] = c[k];
+  block_sum_partial<6>(sum, cc, sh);
+  if (threadIdx.x == 0) {
+    part[blockIdx.x].sum = sum;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) part[blockIdx.x].c[k] = cc[k];
+  }
+}
+
+// Pair slots [n]: topology BCE over the valid ones (label = connected), counts of the valid ones.  An
+// invalid slot is skipped, which equals the reference's `* valid` because its logit is finite.  Element
+// index of a refusal: elem_base + slot.
+__global__ void __launch_bounds__(256) val_pair_kernel(const float* __restrict__ logits,
+                                                       const float* __restrict__ scores,
+                                                       const uint8_t* __restrict__ connected,
+                                                       const uint8_t* __restrict__ valid, long long n,
+                                                       unsigned long long elem_base, ValPartial* __restrict__ part,
+                                                       Refusals* __restrict__ ref) {
+  __shared__ ValPartial sh[8];
+  double sum = 0.0;
+  unsigned c[4] = {0, 0, 0, 0};   // n_valid, tp, fp, fn
+  unsigned bad = 0;
+  unsigned long long first = ~0ull;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const unsigned v = valid[i], lab = connected[i];
+    const unsigned long long e = elem_base + static_cast<unsigned long long>(i);
+    if (v > 1u || lab > 1u) note_bad(bad, first, kBadPairByte, e);
+    if (v == 1u) {
+      const float s = scores[i];
+      if (!(s >= 0.0f && s <= 1.0f)) note_bad(bad, first, kBadScore, e);
+      sum += static_cast<double>(bce_term(logits[i], lab == 1u ? 1.0f : 0.0f));
+      const bool pred = s > 0.5f, pos = lab == 1u;
+      c[0] += 1;
+      c[1] += pred && pos;
+      c[2] += pred && !pos;
+      c[3] += !pred && pos;
+    }
+  }
+  if (bad) refusal_note(ref, bad, first);
+  unsigned long long cc[4] = {c[0], c[1], c[2], c[3]};
+  block_sum_partial<4>(sum, cc, sh);
+  if (threadIdx.x == 0) {
+    part[blockIdx.x].sum = sum;
+    part[blockIdx.x].c[0] = cc[0];
+    part[blockIdx.x].c[1] = cc[1];
+    part[blockIdx.x].c[2] = cc[2];
+    part[blockIdx.x].c[3] = cc[3];
+    part[blockIdx.x].c[4] = part[blockIdx.x].c[5] = 0;
+  }
+}
+
+// Fixed-order sum of g partials by the whole block (result in thread 0).
+__device__ void reduce_partials(const ValPartial* __restrict__ part, int g, ValPartial* sh, double& sum,
+                                unsigned long long (&c)[6]) {
+  sum = 0.0;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) c[k] = 0;
+  for (int b = threadIdx.x; b < g; b += blockDim.x) {
+    sum += part[b].sum;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) c[k] += part[b].c[k];
+  }
+  block_sum_partial<6>(sum, c, sh);
+  __syncthreads();   // sh is reused by the next call
+}
+
+// One 256-thread block: the step's three values into out, then the step is committed to the epoch state or
+// refused as a whole.  Leaves the refusal flags cleared for the next step.
+__global__ void __launch_bounds__(256) val_finish_kernel(const ValPartial* __restrict__ mask_part, int g_mask,
+                                                         const ValPartial* __restrict__ pair_part, int g_pair,
+                                                         long long npix, int B, float* __restrict__ out,
+                                                         ValState* __restrict__ st, long long serial) {
+  __shared__ ValPartial sh[8];
+  double msum, psum;
+  unsigned long long mc[6], pc[6];
+  reduce_partials(mask_part, g_mask, sh, msum, mc);
+  reduce_partials(pair_part, g_pair, sh, psum, pc);
+  if (threadIdx.x != 0) return;
+  if (!refusal_commit(&st->ref, serial)) {
+    out[0] = out[1] = out[2] = __int_as_float(0x7fc00000);
+  } else {
+    const float mask_loss = __double2float_rn(msum / static_cast<double>(2 * npix));
+    const float topo_loss = pc[0] ? __double2float_rn(psum / static_cast<double>(pc[0])) : __int_as_float(0x7fc00000);
+    const float loss = __fadd_rn(mask_loss, topo_loss);
+    const float v[3] = {mask_loss, topo_loss, loss};
+    for (int k = 0; k < 3; ++k) {
+      out[k] = v[k];
+      st->loss_wsum[k] = __dadd_rn(st->loss_wsum[k], __dmul_rn(static_cast<double>(v[k]), static_cast<double>(B)));
+    }
+    st->steps += 1;
+    st->samples += B;
+    for (int ch = 0; ch < 2; ++ch) {
+      const long long tp = mc[3 * ch], fp = mc[3 * ch + 1], fn = mc[3 * ch + 2];
+      st->counts[4 * ch + 0] += tp;
+      st->counts[4 * ch + 1] += fp;
+      st->counts[4 * ch + 2] += fn;
+      st->counts[4 * ch + 3] += npix - tp - fp - fn;
+    }
+    st->counts[8] += pc[1];
+    st->counts[9] += pc[2];
+    st->counts[10] += pc[3];
+  }
+  refusal_begin(&st->ref);
+}
+
+__global__ void val_reset_kernel(ValState* st) {
+  ValState z = {};
+  z.ref.first_bad = ~0ull;
+  *st = z;
+}
+
+}  // namespace
+
+struct samroad_val_ctx {
+  int device = 0;
+  int max_blocks = 0;              // per pass
+  ValState* state = nullptr;       // device
+  ValPartial* part = nullptr;      // device, 2 * max_blocks: mask pass, then pair pass
+  ValState* h_state = nullptr;     // pinned read-back
+  long long n_updates = 0;         // updates since the last reset
+
+  ~samroad_val_ctx() {
+    if (state) cudaFree(state);
+    if (part) cudaFree(part);
+    if (h_state) cudaFreeHost(h_state);
+  }
+};
+
+extern "C" int samroad_val_create(int device, samroad_val_t* out) {
+  SRB_REQUIRE(out != nullptr, "samroad_val_create: null argument");
+  int ndev = 0;
+  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
+  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
+  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
+  SRB_CUDA_OK(cudaSetDevice(device));
+  samroad_val_ctx* v = new samroad_val_ctx();
+  v->device = device;
+  v->max_blocks = kValBlocksPerSm * device_sm_count();
+  if (cudaMalloc(&v->state, sizeof(ValState)) != cudaSuccess ||
+      cudaMalloc(&v->part, sizeof(ValPartial) * 2 * v->max_blocks) != cudaSuccess ||
+      cudaMallocHost(&v->h_state, sizeof(ValState)) != cudaSuccess) {
+    cudaGetLastError();
+    delete v;
+    set_last_error("samroad_val_create: device or pinned allocation failed");
+    return 1;
+  }
+  val_reset_kernel<<<1, 1>>>(v->state);
+  if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
+    delete v;
+    set_last_error("samroad_val_create: initialising the state failed");
+    return 1;
+  }
+  note_launch(1);
+  *out = v;
+  return 0;
+}
+
+extern "C" int samroad_val_destroy(samroad_val_t v) {
+  if (!v) return 0;
+  cudaSetDevice(v->device);
+  cudaDeviceSynchronize();
+  delete v;
+  return 0;
+}
+
+extern "C" int samroad_val_reset(samroad_val_t v, void* stream) {
+  SRB_REQUIRE(v != nullptr, "samroad_val_reset: null handle");
+  SRB_CUDA_OK(cudaSetDevice(v->device));
+  val_reset_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(v->state);
+  SRB_CUDA_OK(cudaGetLastError());
+  note_launch(1);
+  v->n_updates = 0;
+  return 0;
+}
+
+extern "C" int samroad_val_update(samroad_val_t v, const float* mask_logits, const float* mask_scores,
+                                  const float* keypoint_mask, const float* road_mask, const float* topo_logits,
+                                  const float* topo_scores, const uint8_t* connected, const uint8_t* valid, int B,
+                                  int P, int Ns, int Np, int loss_kind, float* out, void* stream) {
+  SRB_REQUIRE(v != nullptr, "samroad_val_update: null handle");
+  SRB_REQUIRE(B >= 1 && P >= 1 && Ns >= 0 && Np >= 0, "samroad_val_update: B=%d, P=%d, Ns=%d, Np=%d", B, P, Ns,
+              Np);
+  SRB_REQUIRE(loss_kind == SAMROAD_LOSS_BCE || loss_kind == SAMROAD_LOSS_FOCAL,
+              "samroad_val_update: loss kind %d (SAMROAD_LOSS_BCE or SAMROAD_LOSS_FOCAL)", loss_kind);
+  const long long n_pairs = static_cast<long long>(B) * Ns * Np;
+  SRB_REQUIRE(mask_logits && mask_scores && keypoint_mask && road_mask && out, "samroad_val_update: null argument");
+  SRB_REQUIRE(n_pairs == 0 || (topo_logits && topo_scores && connected && valid),
+              "samroad_val_update: null topology argument");
+  SRB_REQUIRE(reinterpret_cast<uintptr_t>(mask_logits) % 8 == 0 && reinterpret_cast<uintptr_t>(mask_scores) % 8 == 0,
+              "samroad_val_update: mask logits and scores must be 8-byte aligned ([B,P,P,2] float32)");
+  SRB_CUDA_OK(cudaSetDevice(v->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long npix = static_cast<long long>(B) * P * P;
+  const int g_mask = static_cast<int>(std::min<long long>(grid_for(npix, 256), v->max_blocks));
+  const int g_pair = static_cast<int>(std::min<long long>(grid_for(n_pairs, 256), v->max_blocks));
+  ValPartial* pair_part = v->part + v->max_blocks;
+  if (loss_kind == SAMROAD_LOSS_FOCAL)
+    val_mask_kernel<true><<<g_mask, 256, 0, st>>>(reinterpret_cast<const float2*>(mask_logits),
+                                                  reinterpret_cast<const float2*>(mask_scores), keypoint_mask,
+                                                  road_mask, npix, v->part, &v->state->ref);
+  else
+    val_mask_kernel<false><<<g_mask, 256, 0, st>>>(reinterpret_cast<const float2*>(mask_logits),
+                                                   reinterpret_cast<const float2*>(mask_scores), keypoint_mask,
+                                                   road_mask, npix, v->part, &v->state->ref);
+  if (g_pair > 0)
+    val_pair_kernel<<<g_pair, 256, 0, st>>>(topo_logits, topo_scores, connected, valid, n_pairs,
+                                            static_cast<unsigned long long>(2 * npix), pair_part, &v->state->ref);
+  val_finish_kernel<<<1, 256, 0, st>>>(v->part, g_mask, pair_part, g_pair, npix, B, out, v->state, v->n_updates);
+  SRB_CUDA_OK(cudaGetLastError());
+  note_launch(g_pair > 0 ? 3 : 2);
+  ++v->n_updates;
+  return 0;
+}
+
+extern "C" int samroad_val_read(samroad_val_t v, int64_t* counts, float* means, int64_t* totals, void* stream) {
+  SRB_REQUIRE(v != nullptr && counts && means && totals, "samroad_val_read: null argument");
+  SRB_CUDA_OK(cudaSetDevice(v->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SRB_CUDA_OK(cudaMemcpyAsync(v->h_state, v->state, sizeof(ValState), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaStreamSynchronize(st));
+  const ValState s = *v->h_state;
+  if (int rc = report_refusals(s.ref, &v->state->ref, "samroad_val_read", kValBadText, 3, st)) return rc;
+  for (int k = 0; k < kValCounts; ++k) counts[k] = s.counts[k];
+  for (int k = 0; k < 3; ++k)
+    means[k] = s.samples ? static_cast<float>(s.loss_wsum[k] / static_cast<double>(s.samples)) : NAN;
+  totals[0] = s.steps;
+  totals[1] = s.samples;
   return 0;
 }

@@ -213,6 +213,9 @@ class SAMRoad(_Base):
         self._synced_version: Dict[int, int] = {}
         self._test_curves = None               # (keypoint, road, topo) PrecisionRecallCurve, see test_step
         self.best_thresholds = None
+        self.focal_loss = bool(_cfg_get(config, "FOCAL_LOSS", False))   # mask criterion, model.py:350-353
+        self._val_metrics = None               # ValidationMetrics, see validation_step
+        self.val_metrics = None
         self.matched_param_names = set()
         ckpt_path = _cfg_get(config, "SAM_CKPT_PATH", None)
         if ckpt_path and os.path.isfile(str(ckpt_path)):
@@ -306,6 +309,7 @@ class SAMRoad(_Base):
         state["_handles"] = {}
         state["_synced_version"] = {}
         state["_test_curves"] = None
+        state["_val_metrics"] = None
         return state
 
     def __deepcopy__(self, memo):
@@ -316,7 +320,7 @@ class SAMRoad(_Base):
         for k, v in self.__dict__.items():
             if k in ("_handles", "_synced_version"):
                 new.__dict__[k] = {}
-            elif k == "_test_curves":
+            elif k in ("_test_curves", "_val_metrics"):
                 new.__dict__[k] = None
             else:
                 new.__dict__[k] = copy.deepcopy(v, memo)
@@ -455,6 +459,73 @@ class SAMRoad(_Base):
 
     def training_step(self, *a, **k):
         raise NotImplementedError("sam_road_b200.SAMRoad is inference-only (SURVEY.md §8b)")
+
+    # ---- validation (train.py's per-epoch loop, trainer.validate) -----------------------------------
+    _VAL_LOG = dict(on_step=False, on_epoch=True, prog_bar=True)    # model.py:566-568
+
+    def _attached(self) -> bool:
+        """True when a Lightning trainer drives this module (then self.log is Lightning's)."""
+        return self.__dict__.get("_trainer") is not None
+
+    @torch.no_grad()
+    def validation_step(self, batch, batch_idx):
+        """model.py:547-588 without autograd: the forward pass, the mask loss (BCEWithLogitsLoss, or
+        sigmoid_focal_loss with FOCAL_LOSS) and the valid-slot topology BCE, and the updates of keypoint_iou,
+        road_iou and topo_f1, all on the device (sam_road_b200.metrics.ValidationMetrics, DESIGN.md §11).
+        batch is the reference's collated dict (masks float 0.0 / 1.0, valid / connected bool).  Returns
+        {"val_mask_loss", "val_topo_loss", "val_loss"} as 0-dim float32 device tensors and, under a Lightning
+        trainer, logs them with the reference's names and flags.  A step with a target other than 0 / 1
+        adds nothing and makes on_validation_epoch_end raise.  Autocast is ignored, as by the inference
+        calls.  The wandb image table the reference logs at batch_idx == 0 is visualisation and not served
+        (DESIGN.md §7)."""
+        from .metrics import VAL_LOSS_NAMES, ValidationMetrics
+        rgb, valid = batch["rgb"], batch["valid"]
+        scores, logits, emb = self._encode(rgb, True)
+        t_logits, t_scores = self._topo(emb, batch["graph_points"], batch["pairs"], valid, True)
+        if self._val_metrics is None:
+            self._val_metrics = ValidationMetrics(rgb.device, focal=self.focal_loss)
+        vm = self._val_metrics
+        if vm.device != scores.device:
+            raise RuntimeError(f"validation batches arrive on {scores.device}, the metrics were started on "
+                               f"{vm.device}; call reset_validation_metrics() first")
+        out = vm.update(logits, scores, batch["keypoint_mask"], batch["road_mask"], t_logits, t_scores,
+                        batch["connected"], valid)
+        res = dict(zip(VAL_LOSS_NAMES, out.unbind(0)))
+        if self._attached():
+            for name, v in res.items():
+                self.log(name, v, **self._VAL_LOG)
+        return res
+
+    def on_validation_epoch_end(self):
+        """model.py:591-600: keypoint_iou, road_iou and topo_f1 of the epoch (logged under a Lightning
+        trainer), then the accumulator is reset.  Returns and stores in `val_metrics` a dict of the six
+        numbers as Python floats: those three and the epoch means of val_mask_loss, val_topo_loss and val_loss
+        (Lightning's batch-size-weighted on_epoch mean, taken exactly).  Under torch.distributed the counts of
+        every rank are summed first, as torchmetrics' sync on compute does; the losses stay per rank.  Raises
+        when a validation step was refused since the last report."""
+        from .metrics import ValidationMetrics
+        if self._val_metrics is None:
+            dist = torch.distributed
+            if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+                raise RuntimeError("on_validation_epoch_end: no validation_step ran since the last reset")
+            # a rank without batches still joins the all-reduce of the counts
+            self._val_metrics = ValidationMetrics(torch.device("cuda", torch.cuda.current_device()),
+                                                  focal=self.focal_loss)
+        vm = self._val_metrics
+        try:
+            res = vm.compute()
+        finally:
+            vm.reset()
+        if self._attached():
+            for name in ("keypoint_iou", "road_iou", "topo_f1"):
+                self.log(name, torch.tensor(res[name], dtype=torch.float32, device=vm.device))
+        self.val_metrics = res
+        return res
+
+    def reset_validation_metrics(self) -> None:
+        """Drops the validation accumulator (its counts and loss sums) and `val_metrics`."""
+        self._val_metrics = None
+        self.val_metrics = None
 
     # ---- threshold search (test.py) ----------------------------------------------------------------
     _CURVE_NAMES = ("keypoint", "road", "topo")
