@@ -273,6 +273,50 @@ int samroad_val_update(samroad_val_t v, const float* mask_logits, const float* m
  *   totals [2] int64: accepted steps, sum of their B. */
 int samroad_val_read(samroad_val_t v, int64_t* counts, float* means, int64_t* totals, void* stream);
 
+/* ---- training of the heads with a frozen encoder: SAMRoad.training_step (model.py:511-544) ---------------- */
+
+/* One step of FREEZE_ENCODER training (naive map decoder + TopoNet; USE_SAM_DECODER is refused).  The
+ * encoder runs as in samroad_encode_masks; the heads run in fp32 from the caller's parameters, given as a
+ * table of (state_dict key, device fp32 pointer in the reference layout): every map_decoder.* and topo_net.*
+ * parameter of the configuration.  Backward regenerates the dropout masks from (seed, layer, site, element). */
+typedef struct SamRoadTrainArgs {
+  int32_t B, N, Ns, Np;   /* tiles, points per tile, samples per tile, pairs per sample (1..32)          */
+  int32_t loss_kind;      /* SAMROAD_LOSS_BCE or SAMROAD_LOSS_FOCAL (mask criterion)                      */
+  float dropout_p;        /* TopoNet dropout: 0.1 in training mode, 0 in eval mode                        */
+  uint64_t seed;          /* dropout seed                                                                 */
+} SamRoadTrainArgs;
+
+/* Bytes of the workspace one step needs: forward activations kept for backward plus backward scratch. */
+int samroad_train_workspace_bytes(samroad_handle_t h, const SamRoadTrainArgs* args, size_t* bytes);
+/* Forward of one step; asynchronous.  Device inputs as samroad_encode_masks / samroad_toponet take them, plus
+ * connected [B,Ns,Np] bytes and keypoint_mask / road_mask [B,P,P] fp32 targets (any finite value).  Writes
+ * losses[2] = (mask_loss, topo_loss) (device fp32; topo_loss is NaN without a valid slot, as in the
+ * reference), keeps what backward needs in ws, and copies the image embeddings [B,256,P/16,P/16] when
+ * image_embeddings != NULL. */
+int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                          const float* const* params, int n_params, const void* rgb, int rgb_dtype,
+                          const void* points, int pts_dtype, const void* pairs, int pairs_dtype,
+                          const uint8_t* valid, const uint8_t* connected, const float* keypoint_mask,
+                          const float* road_mask, void* ws, size_t ws_bytes, float* losses,
+                          float* image_embeddings, void* stream);
+/* Backward of the step whose forward filled ws (ws is not modified where forward wrote it, so backward may
+ * run more than once); asynchronous.  g: device fp32 [2] = incoming gradients of (mask_loss, topo_loss).
+ * Writes (overwrites) the gradient of every parameter of the table into grads[i] (device fp32, reference
+ * layout).  Deterministic: no float atomics. */
+int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                           const float* const* params, float* const* grads, int n_params, void* ws,
+                           size_t ws_bytes, const float* g, void* stream);
+/* Repacks one head tensor (map_decoder.* / topo_net.*) of finalized weights from DEVICE fp32 memory,
+ * stream-ordered; the packed result equals what samroad_finalize_weights makes from the same values, bit for
+ * bit.  Encoder tensors and the SAM mask decoder are refused. */
+int samroad_update_tensor_device(samroad_handle_t h, const char* key, const float* dev_data,
+                                 const int64_t* shape, int ndim, void* stream);
+/* Test hook: keep[i] = 1 when element i of dropout site `site` (0 attention probabilities [rows,4,Np,Np],
+ * 1 dropout1, 2 the dropout between ReLU and linear2, 3 dropout2, each [tokens,128]) of TopoNet layer `layer`
+ * survives at rate 1 - p under `seed`, else 0. */
+int samroad_debug_train_dropout_keep(float p, uint64_t seed, int layer, int site, int64_t n, uint8_t* keep,
+                                     void* stream);
+
 /* Stream memory operations on a 32-bit flag word in device (or peer-mapped) memory, executed by the stream
  * front end without a kernel: an ordered write of `value`, and a wait until *addr >= value.  The exchange step
  * between ranks (sam_road_b200/exchange.py; no reference counterpart, the reference is single-GPU) builds its

@@ -33,8 +33,21 @@ class SamRoadCfg(C.Structure):
     ]
 
 
+class SamRoadTrainArgs(C.Structure):
+    _fields_ = [
+        ("B", C.c_int32),
+        ("N", C.c_int32),
+        ("Ns", C.c_int32),
+        ("Np", C.c_int32),
+        ("loss_kind", C.c_int32),
+        ("dropout_p", C.c_float),
+        ("seed", C.c_uint64),
+    ]
+
+
 _vp, _i, _f, _d = C.c_void_p, C.c_int, C.c_float, C.c_double
 _ip = C.POINTER(C.c_int)
+_targs = C.POINTER(SamRoadTrainArgs)
 
 # samroad_argsort_fn: int (*)(const void* keys, int key_dtype, int64_t n, int64_t* order_out, void* user)
 ARGSORT_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_int64), C.c_void_p)
@@ -75,6 +88,12 @@ SIGNATURES = {
     "samroad_val_reset": (_i, [_vp, _vp]),
     "samroad_val_update": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "samroad_val_read": (_i, [_vp, C.POINTER(C.c_int64), C.POINTER(C.c_float), C.POINTER(C.c_int64), _vp]),
+    "samroad_train_workspace_bytes": (_i, [_vp, _targs, C.POINTER(C.c_size_t)]),
+    "samroad_train_forward": (_i, [_vp, _targs, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp,
+                                   C.c_size_t, _vp, _vp, _vp]),
+    "samroad_train_backward": (_i, [_vp, _targs, _vp, _vp, _vp, _i, _vp, C.c_size_t, _vp, _vp]),
+    "samroad_update_tensor_device": (_i, [_vp, C.c_char_p, _vp, C.POINTER(C.c_int64), _i, _vp]),
+    "samroad_debug_train_dropout_keep": (_i, [_f, C.c_uint64, _i, _i, C.c_int64, _vp, _vp]),
     "samroad_stream_write_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_stream_wait_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_timing_enable": (_i, [_vp, _i]),

@@ -24,6 +24,7 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "loss_terms.cuh"
 #include "ops.h"
 
 using namespace srb;
@@ -749,28 +750,6 @@ struct ValPartial {
   double sum;
   unsigned long long c[6];
 };
-
-// torch's CUDA log_sigmoid: min(0, x) - log1p(exp(-|x|))
-__device__ __forceinline__ float log_sigmoid_f32(float x) {
-  return __fsub_rn(fminf(0.0f, x), log1pf(expf(-fabsf(x))));
-}
-
-// F.binary_cross_entropy_with_logits(x, y, reduction='none') = (1 - y) * x - log_sigmoid(x), one rounding
-// per torch op
-__device__ __forceinline__ float bce_term(float x, float y) {
-  return __fsub_rn(__fmul_rn(__fsub_rn(1.0f, y), x), log_sigmoid_f32(x));
-}
-
-// torchvision.ops.sigmoid_focal_loss(x, y, alpha=0.25, gamma=2, reduction='none') in its order
-__device__ __forceinline__ float focal_term(float x, float y) {
-  const float p = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x)));
-  const float one_y = __fsub_rn(1.0f, y);
-  const float p_t = __fadd_rn(__fmul_rn(p, y), __fmul_rn(__fsub_rn(1.0f, p), one_y));
-  const float m = __fsub_rn(1.0f, p_t);
-  const float loss = __fmul_rn(bce_term(x, y), __fmul_rn(m, m));
-  const float alpha_t = __fadd_rn(__fmul_rn(0.25f, y), __fmul_rn(0.75f, one_y));
-  return __fmul_rn(alpha_t, loss);
-}
 
 // Block-wide sum of a partial in a fixed order; the result is valid in thread 0.
 template <int kN>

@@ -680,6 +680,120 @@ extern "C" int samroad_finalize_weights(samroad_handle_t h) {
   return 0;
 }
 
+// Used by train.cu: the tile size and head variants of a handle.
+int samroad_handle_head_config(samroad_handle_t h, int* patch_size, int* toponet_version, int* use_sam_decoder) {
+  SRB_TRY(check_handle(h, true));
+  *patch_size = h->cfg.patch_size;
+  *toponet_version = h->cfg.toponet_version;
+  *use_sam_decoder = h->cfg.use_sam_decoder;
+  return 0;
+}
+
+// ---- device repack of one head tensor (samroad_update_tensor_device) ------------------------------------------
+namespace {
+
+enum RepackMode { RP_COPY, RP_CONVT, RP_TILE4, RP_DEC4, RP_PAIR_ST, RP_PAIR_OFF };
+
+// dst[i] = src[index(i)] for the packings of samroad_finalize_weights, fp16 (round to nearest even, as the host
+// pack) or fp32
+__global__ void repack_kernel(const float* __restrict__ src, int mode, int cin, int cout, long long n, float* d32,
+                              __half* d16) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  long long j = i;
+  switch (mode) {
+    case RP_CONVT: {   // o[(d*cout + co)*cin + ci] = w[(ci*cout + co)*4 + d]
+      const long long ci = i % cin, dc = i / cin, co = dc % cout, d = dc / cout;
+      j = (ci * cout + co) * 4 + d;
+      break;
+    }
+    case RP_TILE4: j = i % cout; break;
+    case RP_DEC4: {    // o[ci*8 + d*2 + co] = w[(ci*2 + co)*4 + d]
+      const long long ci = i / 8, d = (i % 8) / 2, co = i % 2;
+      j = (ci * 2 + co) * 4 + d;
+      break;
+    }
+    case RP_PAIR_ST: {   // rows 0..127: Ws, 128..255: Wt of pair_proj.weight [128, 258]
+      const long long r = i / 128, k = i % 128;
+      j = (r % 128) * 258 + (r / 128) * 128 + k;
+      break;
+    }
+    case RP_PAIR_OFF: j = (i / 2) * 258 + 256 + i % 2; break;
+    default: break;
+  }
+  const float v = src[j];
+  if (d16) d16[i] = __float2half_rn(v);
+  else d32[i] = v;
+}
+
+}  // namespace
+
+extern "C" int samroad_update_tensor_device(samroad_handle_t h, const char* key, const float* dev_data,
+                                            const int64_t* shape, int ndim, void* stream) {
+  SRB_TRY(check_handle(h, true));
+  SRB_REQUIRE(key && dev_data && (shape || ndim == 0) && ndim >= 0 && ndim <= 8,
+              "samroad_update_tensor_device: bad arguments");
+  SRB_REQUIRE(!h->cfg.use_sam_decoder, "samroad_update_tensor_device: the SAM mask decoder is repacked on the host only");
+  const std::string k = key;
+  struct Target { int mode; int cin, cout; long long n; float* d32; __half* d16; };
+  std::vector<Target> tg;
+  std::vector<int64_t> want;
+  auto f32 = [&](const float* p, long long n) { tg.push_back({RP_COPY, 0, 0, n, const_cast<float*>(p), nullptr}); };
+  auto f16 = [&](const __half* p, long long n) { tg.push_back({RP_COPY, 0, 0, n, nullptr, const_cast<__half*>(p)}); };
+  if (k == "map_decoder.0.weight") { want = {256, 128, 2, 2}; tg.push_back({RP_CONVT, 256, 128, 4LL * 128 * 256, nullptr, h->dec1_w}); }
+  else if (k == "map_decoder.0.bias") { want = {128}; tg.push_back({RP_TILE4, 0, 128, 512, h->dec1_b, nullptr}); }
+  else if (k == "map_decoder.1.weight") { want = {128}; f32(h->dec_ln_g, 128); }
+  else if (k == "map_decoder.1.bias") { want = {128}; f32(h->dec_ln_b, 128); }
+  else if (k == "map_decoder.3.weight") { want = {128, 64, 2, 2}; tg.push_back({RP_CONVT, 128, 64, 4LL * 64 * 128, nullptr, h->dec2_w}); }
+  else if (k == "map_decoder.3.bias") { want = {64}; tg.push_back({RP_TILE4, 0, 64, 256, h->dec2_b, nullptr}); }
+  else if (k == "map_decoder.5.weight") { want = {64, 32, 2, 2}; tg.push_back({RP_CONVT, 64, 32, 4LL * 32 * 64, nullptr, h->dec3_w}); }
+  else if (k == "map_decoder.5.bias") { want = {32}; f32(h->dec3_b, 32); }
+  else if (k == "map_decoder.7.weight") { want = {32, 2, 2, 2}; tg.push_back({RP_DEC4, 0, 0, 256, h->dec4_w, nullptr}); }
+  else if (k == "map_decoder.7.bias") { want = {2}; f32(h->dec4_b, 2); }
+  else if (k == "topo_net.feature_proj.weight") { want = {128, 256}; f16(h->tp_feat_w, 128 * 256); }
+  else if (k == "topo_net.feature_proj.bias") { want = {128}; f32(h->tp_feat_b, 128); }
+  else if (k == "topo_net.pair_proj.weight") {
+    want = {128, 258};
+    tg.push_back({RP_PAIR_ST, 0, 0, 256 * 128, nullptr, h->tp_st_w});
+    tg.push_back({RP_PAIR_OFF, 0, 0, 256, h->tp_off_w, nullptr});
+  }
+  else if (k == "topo_net.pair_proj.bias") { want = {128}; f32(h->tp_pair_b, 128); }
+  else if (k == "topo_net.output_proj.weight") { want = {1, 128}; f32(h->tp_out_w, 128); }
+  else if (k == "topo_net.output_proj.bias") { want = {1}; f32(h->tp_out_b, 1); }
+  else if (h->cfg.toponet_version != SAMROAD_TOPO_NO_TRANSFORMER &&
+           k.rfind("topo_net.transformer_encoder.layers.", 0) == 0 && k.size() > 38 && k[37] == '.' &&
+           k[36] >= '0' && k[36] <= '2') {
+    const int l = k[36] - '0';
+    const std::string s = k.substr(38);
+    const TopoLayerParams& t = h->tp_layers[l];
+    const __half* chunk = h->tp_chunks + static_cast<size_t>(l) * 6 * 128 * 128;
+    if (s == "self_attn.in_proj_weight") { want = {384, 128}; f16(chunk, 384 * 128); }
+    else if (s == "self_attn.out_proj.weight") { want = {128, 128}; f16(chunk + 3 * 128 * 128, 128 * 128); }
+    else if (s == "linear1.weight") { want = {128, 128}; f16(chunk + 4 * 128 * 128, 128 * 128); }
+    else if (s == "linear2.weight") { want = {128, 128}; f16(chunk + 5 * 128 * 128, 128 * 128); }
+    else if (s == "self_attn.in_proj_bias") { want = {384}; f32(t.in_b, 384); }
+    else if (s == "self_attn.out_proj.bias") { want = {128}; f32(t.out_b, 128); }
+    else if (s == "linear1.bias") { want = {128}; f32(t.l1_b, 128); }
+    else if (s == "linear2.bias") { want = {128}; f32(t.l2_b, 128); }
+    else if (s == "norm1.weight") { want = {128}; f32(t.n1_g, 128); }
+    else if (s == "norm1.bias") { want = {128}; f32(t.n1_b, 128); }
+    else if (s == "norm2.weight") { want = {128}; f32(t.n2_g, 128); }
+    else if (s == "norm2.bias") { want = {128}; f32(t.n2_b, 128); }
+  }
+  SRB_REQUIRE(!tg.empty(), "samroad_update_tensor_device: '%s' is not a head tensor of this configuration", key);
+  bool same = static_cast<size_t>(ndim) == want.size();
+  for (int i = 0; same && i < ndim; ++i) same = shape[i] == want[i];
+  SRB_REQUIRE(same, "samroad_update_tensor_device: '%s' has the wrong shape", key);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (const Target& t : tg) {
+    repack_kernel<<<static_cast<unsigned>((t.n + 255) / 256), 256, 0, st>>>(dev_data, t.mode, t.cin, t.cout, t.n,
+                                                                            t.d32, t.d16);
+    SRB_CUDA_OK(cudaGetLastError());
+    note_launch();
+  }
+  return 0;
+}
+
 // =================================================================================================
 // encoder + mask head
 // =================================================================================================

@@ -67,6 +67,8 @@ void attention_force_simt(int mode);   // bit 0: SIMT kernel
 // points dtype: 0 = float32, 1 = int64, 2 = int32 ; pairs dtype: 1 = int64, 2 = int32
 int topo_sample_features(const float* feat_nchw, int B, int C, int s, int P, const void* points,
                          int pts_dtype, int N, __half* out, cudaStream_t st);
+int topo_sample_features_f32(const float* feat_nchw, int B, int C, int s, int P, const void* points,
+                             int pts_dtype, int N, float* out, cudaStream_t st);
 // pair features (model.py:96-120): x = relu(Ws f[src] + Wt f[tgt] + Wo (pt[tgt] - pt[src]) + bias)
 struct TopoPairInputs {
   const float* pst;          // [B*N, 256] per-point projections (Ws f | Wt f)

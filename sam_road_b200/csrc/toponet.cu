@@ -19,11 +19,15 @@ namespace srb {
 // Bilinear sampling of image_embeddings [B,C,s,s] fp32 at pixel-space points (x,y):
 //   g = pt / P * 2 - 1 (model.py:47) ; grid_sample unnormalise: u = ((g + 1) * s - 1) / 2 ;
 //   4 taps, out-of-range taps contribute zero (SURVEY.md §8a P8).  One block per point, one thread
-//   per channel.  Output fp16 [B*N, C] = A operand of feature_proj.
+//   per channel.  Output [B*N, C] = A operand of feature_proj: fp16 for inference, fp32 for training.
 // ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void store_feature(__half* p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void store_feature(float* p, float v) { *p = v; }
+
+template <typename T>
 __global__ void __launch_bounds__(256)
 topo_sample_kernel(const float* __restrict__ feat, int C, int s, float P, const void* points,
-                   int pts_dtype, int N, __half* __restrict__ out) {
+                   int pts_dtype, int N, T* __restrict__ out) {
   const int pt = blockIdx.x;           // b*N + n
   const int b = pt / N;
   const float px = load_coord(points, pts_dtype, static_cast<size_t>(pt) * 2 + 0);
@@ -46,19 +50,30 @@ topo_sample_kernel(const float* __restrict__ feat, int C, int s, float P, const 
     if (vy0 && vx1) acc += f[y0 * s + x0 + 1] * w01;
     if (vy1 && vx0) acc += f[(y0 + 1) * s + x0] * w10;
     if (vy1 && vx1) acc += f[(y0 + 1) * s + x0 + 1] * w11;
-    out[static_cast<size_t>(pt) * C + c] = __float2half_rn(acc);
+    store_feature(out + static_cast<size_t>(pt) * C + c, acc);
   }
+}
+
+template <typename T>
+int topo_sample_launch(const float* feat_nchw, int B, int C, int s, int P, const void* points,
+                       int pts_dtype, int N, T* out, cudaStream_t st) {
+  SRB_REQUIRE(pts_dtype >= 0 && pts_dtype <= 2, "topo_sample: points dtype %d", pts_dtype);
+  if (B * N <= 0) return 0;
+  topo_sample_kernel<T><<<B * N, 256, 0, st>>>(feat_nchw, C, s, static_cast<float>(P), points,
+                                               pts_dtype, N, out);
+  SRB_CUDA_OK(cudaGetLastError());
+  note_launch();
+  return 0;
 }
 
 int topo_sample_features(const float* feat_nchw, int B, int C, int s, int P, const void* points,
                          int pts_dtype, int N, __half* out, cudaStream_t st) {
-  SRB_REQUIRE(pts_dtype >= 0 && pts_dtype <= 2, "topo_sample: points dtype %d", pts_dtype);
-  if (B * N <= 0) return 0;
-  topo_sample_kernel<<<B * N, 256, 0, st>>>(feat_nchw, C, s, static_cast<float>(P), points,
-                                            pts_dtype, N, out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
-  return 0;
+  return topo_sample_launch(feat_nchw, B, C, s, P, points, pts_dtype, N, out, st);
+}
+
+int topo_sample_features_f32(const float* feat_nchw, int B, int C, int s, int P, const void* points,
+                             int pts_dtype, int N, float* out, cudaStream_t st) {
+  return topo_sample_launch(feat_nchw, B, C, s, P, points, pts_dtype, N, out, st);
 }
 
 // ------------------------------------------------------------------------------------------------

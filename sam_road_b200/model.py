@@ -176,7 +176,7 @@ except Exception:  # lightning is absent in this image; inference needs nothing 
 
 
 class SAMRoad(_Base):
-    """H100-native SAMRoad (inference only)."""
+    """H100-native SAMRoad: inference, test, validation, and training of the heads with a frozen encoder."""
 
     def __init__(self, config):
         super().__init__()
@@ -211,6 +211,7 @@ class SAMRoad(_Base):
         self._handles: Dict[int, int] = {}     # cuda device index -> samroad_handle_t
         self._weights_version = 0
         self._synced_version: Dict[int, int] = {}
+        self._packed_versions: Dict[int, Dict[str, int]] = {}   # device -> key -> _version at the last pack
         self._test_curves = None               # (keypoint, road, topo) PrecisionRecallCurve, see test_step
         self.best_thresholds = None
         self.focal_loss = bool(_cfg_get(config, "FOCAL_LOSS", False))   # mask criterion, model.py:350-353
@@ -252,6 +253,7 @@ class SAMRoad(_Base):
 
     def _apply(self, fn, *a, **k):
         out = super()._apply(fn, *a, **k)
+        self.__dict__.pop("_heads_cache", None)   # conversions may swap the parameter objects
         self._weights_version += 1
         return out
 
@@ -281,6 +283,14 @@ class SAMRoad(_Base):
             h = C.c_void_p()
             _lib.check(lib.samroad_create(C.byref(cfg), idx, C.byref(h)), "samroad_create")
             self._handles[idx] = h.value
+        # parameters that require grad (the trained heads) are watched through their autograd version
+        # counter: an optimizer step changes them in place, and only those are repacked, on the device
+        watched = [(k, p) for k, p in self._head_params() if p.requires_grad]
+        seen = self._packed_versions.setdefault(idx, {})
+        stale = [(k, p) for k, p in watched if seen.get(k) != p._version]
+        if stale and self._synced_version.get(idx) == self._weights_version and any(
+                p.device != device or p.dtype != torch.float32 or not p.is_contiguous() for _, p in stale):
+            self._weights_version += 1     # not device-resident fp32: repack on the host
         if self._synced_version.get(idx) != self._weights_version:
             h = self._handles[idx]
             tensors = list(self.named_parameters()) + [(k, b) for k, b in self.named_buffers()
@@ -292,6 +302,16 @@ class SAMRoad(_Base):
                            f"samroad_load_tensor({key})")
             _lib.check(lib.samroad_finalize_weights(h), "samroad_finalize_weights")
             self._synced_version[idx] = self._weights_version
+        elif stale:
+            h = self._handles[idx]
+            with torch.cuda.device(device):
+                for key, p in stale:
+                    shape = (C.c_int64 * p.dim())(*p.shape)
+                    _lib.check(lib.samroad_update_tensor_device(h, key.encode(), p.data_ptr(), shape, p.dim(),
+                                                                _lib.current_stream_ptr()),
+                               f"samroad_update_tensor_device({key})")
+        for k, p in watched:
+            seen[k] = p._version
         return self._handles[idx]
 
     def __del__(self):
@@ -308,6 +328,7 @@ class SAMRoad(_Base):
         state = dict(self.__dict__)
         state["_handles"] = {}
         state["_synced_version"] = {}
+        state["_packed_versions"] = {}
         state["_test_curves"] = None
         state["_val_metrics"] = None
         return state
@@ -318,7 +339,7 @@ class SAMRoad(_Base):
         new = cls.__new__(cls)
         memo[id(self)] = new
         for k, v in self.__dict__.items():
-            if k in ("_handles", "_synced_version"):
+            if k in ("_handles", "_synced_version", "_packed_versions"):
                 new.__dict__[k] = {}
             elif k in ("_test_curves", "_val_metrics"):
                 new.__dict__[k] = None
@@ -457,8 +478,67 @@ class SAMRoad(_Base):
         of B*Ns*Np elements the scores are written into."""
         return self._topo(image_embeddings, graph_points, pairs, valid, False, out_scores=out)[1]
 
-    def training_step(self, *a, **k):
-        raise NotImplementedError("sam_road_b200.SAMRoad is inference-only (SURVEY.md §8b)")
+    # ---- training of the heads with a frozen encoder (train.py, FREEZE_ENCODER: True) ---------------------------
+    _TRAIN_LOG = dict(on_step=True, on_epoch=False, prog_bar=True)    # model.py:541-543
+
+    def _head_params(self):
+        """(key, parameter) of map_decoder.* and topo_net.*, in registration order (cached: the inference calls
+        look at them on every call)."""
+        heads = self.__dict__.get("_heads_cache")
+        if heads is None:
+            heads = [(k, p) for k, p in self.named_parameters() if k.startswith(("map_decoder.", "topo_net."))]
+            self.__dict__["_heads_cache"] = heads
+        return heads
+
+    def _enable_training(self) -> None:
+        """Head parameters require grad from here on (the encoder's stay frozen), so that autograd fills their
+        .grad and an optimizer step is repacked on the device before the next call."""
+        from .train import check_trainable
+        check_trainable(self.config, _cfg_get)
+        if not self.__dict__.get("_training_enabled", False):   # once: a head frozen later by the user stays so
+            for _, p in self._head_params():
+                p.requires_grad_(True)
+            self._training_enabled = True
+
+    def training_step(self, batch, batch_idx):
+        """model.py:511-544 for FREEZE_ENCODER: True with the naive decoder: the encoder as the inference calls run
+        it, then the map decoder and TopoNet (dropout 0.1 at torch's four sites when self.training) on the device,
+        mask loss (BCEWithLogitsLoss, or sigmoid_focal_loss with FOCAL_LOSS) + the valid-slot topology BCE.  Returns
+        the 0-dim fp32 loss, differentiable with respect to the map_decoder.* and topo_net.* parameters; its
+        backward writes their .grad on the device (DESIGN.md §12).  Other configurations raise NotImplementedError
+        before the batch is read.  The dropout seed is drawn from torch's default generator."""
+        from . import train as T
+        self._enable_training()
+        heads = self._head_params()
+        dev = heads[0][1].device
+        if dev.type != "cuda":
+            raise RuntimeError(f"training runs on CUDA (sm_90a) only; the head parameters are on '{dev}'")
+        b = T.validate_batch(batch, self.image_size, dev)
+        h = self._handle(dev)
+        dropout_p = 0.1 if self.training else 0.0
+        seed = int(torch.randint(0, 2 ** 62, (), dtype=torch.int64).item()) if dropout_p > 0 else 0
+        args = T.make_args(b, self.focal_loss, dropout_p, seed)
+        mask_loss, topo_loss = T.head_losses(h, b, args, [k for k, _ in heads], [p for _, p in heads])
+        loss = mask_loss + topo_loss
+        if self._attached():
+            self.log("train_mask_loss", mask_loss, **self._TRAIN_LOG)
+            self.log("train_topo_loss", topo_loss, **self._TRAIN_LOG)
+            self.log("train_loss", loss, **self._TRAIN_LOG)
+        return loss
+
+    def configure_optimizers(self):
+        """model.py:637-685 for FREEZE_ENCODER: True with the naive decoder: Adam over map_decoder then topo_net,
+        both at BASE_LR, and MultiStepLR(milestones=[9], gamma=0.1).  Prints the parameter count of each group as
+        the reference does."""
+        self._enable_training()
+        lr = _cfg_get(self.config, "BASE_LR")
+        groups = [{"params": [p for k, p in self._head_params() if k.startswith(prefix)], "lr": lr}
+                  for prefix in ("map_decoder.", "topo_net.")]
+        for i, g in enumerate(groups):
+            print(f"optim param dict {i} params num: {sum(int(p.numel()) for p in g['params'])}")
+        optimizer = torch.optim.Adam(groups, lr=lr)
+        step_lr = torch.optim.lr_scheduler.MultiStepLR(optimizer, milestones=[9, ], gamma=0.1)
+        return {"optimizer": optimizer, "lr_scheduler": step_lr}
 
     # ---- validation (train.py's per-epoch loop, trainer.validate) -----------------------------------
     _VAL_LOG = dict(on_step=False, on_epoch=True, prog_bar=True)    # model.py:566-568

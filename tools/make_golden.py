@@ -196,8 +196,81 @@ def shape_fixtures():
     toponet_npairs_fixture(TOPO_NPAIRS_WIDE, "toponet_npairs_wide")
 
 
+TRAIN_SAMPLES = 64     # gradient entries kept per parameter (seeded positions)
+
+
+def train_heads_batch(P=256, B=2, n_points=24, Ns=20, Np=16, seed=31):
+    """The batch of train_heads_vitb_256.npz, regenerated from seeds (float tiles, k/255 keypoint targets,
+    binary road targets, one all-invalid sample row)."""
+    g = torch.Generator().manual_seed(seed)
+    pts, prs, val = synth.make_topo_inputs(B, P, n_points, seed=seed, max_nbr=Np)
+    prs, val = prs[:, :Ns].contiguous(), val[:, :Ns].contiguous()
+    val[0, 0] = False
+    return {"rgb": synth.make_tiles(B, P, seed=seed, dtype=torch.float32), "graph_points": pts, "pairs": prs,
+            "valid": val, "connected": torch.rand(val.shape, generator=g) < 0.4,
+            "keypoint_mask": torch.randint(0, 256, (B, P, P), generator=g).float() / 255.0,
+            "road_mask": (torch.rand((B, P, P), generator=g) < 0.5).float()}
+
+
+def train_heads_fixture():
+    """Reference training_step + loss.backward() (ViT-B @256, B=2, FREEZE_ENCODER: True, eval mode so no
+    dropout, grad enabled so torch's slow path), BCE and focal; the oracle must agree on the same embeddings."""
+    import contextlib
+    import io
+
+    from oracle import train_oracle as TO
+    out = {}
+    for focal in (False, True):
+        cfg = dict(_cfg(256), FREEZE_ENCODER=True, FOCAL_LOSS=focal, BASE_LR=1e-3)
+        torch.manual_seed(0)
+        net = ref_loader.load_reference_model(cfg)
+        net.load_state_dict(synth.make_state_dict(cfg, seed=12, logit_gain=4.0), strict=True)
+        b = train_heads_batch()
+        tag = "focal" if focal else "bce"
+        heads = [(k, p) for k, p in net.named_parameters() if k.startswith(("map_decoder.", "topo_net."))]
+        net.zero_grad(set_to_none=True)
+        losses = {}
+        net.log = lambda name, v, **k: losses.__setitem__(name, v.detach().clone())
+        loss = net.training_step(b, 0)
+        loss.backward()
+        with torch.no_grad():
+            emb = net.infer_masks_and_img_features(b["rgb"])[1]
+        params = {k: p.detach().clone().requires_grad_(True) for k, p in heads}
+        oml, otl = TO.heads_losses(params, emb, b, 256, focal, "normal", None, 0.0)
+        (oml + otl).backward()
+        for name, o in (("train_mask_loss", oml), ("train_topo_loss", otl)):
+            r = losses[name]
+            assert abs(o.item() - r.item()) <= 1e-6 * abs(r.item()), (tag, name, o.item(), r.item())
+        gen = torch.Generator().manual_seed(99)
+        worst = 0.0
+        for k, p in heads:
+            g, og = p.grad, params[k].grad
+            rel = ((g - og).abs().max() / g.abs().max()).item()
+            worst = max(worst, rel)
+            assert rel <= 2e-6, (tag, k, rel)   # fp32 against fp32, summation orders differ
+            idx = torch.randint(0, g.numel(), (TRAIN_SAMPLES,), generator=gen)
+            out[f"{tag}/{k}/idx"] = idx.numpy().astype(np.int32)
+            out[f"{tag}/{k}/val"] = g.reshape(-1)[idx].numpy()
+            out[f"{tag}/{k}/norm_maxabs"] = np.array([g.double().norm().item(), g.abs().max().item()])
+        out[f"{tag}/losses"] = np.array([losses["train_mask_loss"].item(), losses["train_topo_loss"].item(),
+                                         losses["train_loss"].item()], np.float32)
+        buf = io.StringIO()
+        with contextlib.redirect_stdout(buf):
+            net.configure_optimizers()
+        out[f"{tag}/param_counts"] = np.array([int(line.rsplit(":", 1)[1]) for line in buf.getvalue().splitlines()
+                                               if line.startswith("optim param dict")])
+        out[f"{tag}/emb_stats"] = _stats(emb)
+        print(f"train_heads[{tag}]: losses {out[f'{tag}/losses']}, oracle-vs-reference max relative gradient "
+              f"error {worst:.2e}, param counts {out[f'{tag}/param_counts']}")
+    np.savez_compressed(os.path.join(OUT, "train_heads_vitb_256.npz"), **out)
+
+
 def main():
     assert ref_loader.available(), "needs /root/reference"
+    if "--train-heads" in sys.argv:   # training_step / backward of the heads with a frozen encoder
+        os.makedirs(OUT, exist_ok=True)
+        train_heads_fixture()
+        return
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
     if "--only-new" in sys.argv:      # fixtures added in round 2 (the round-1 files stay byte-identical)
