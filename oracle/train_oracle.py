@@ -1,11 +1,13 @@
-"""fp32 torch restatement of the heads' training loss (reference model.py:286-295, 61-148, 511-544).
+"""Torch restatement of the heads' training loss (reference model.py:286-295, 61-148, 511-544).
 
 The naive map decoder and TopoNet in the semantics of torch's slow path of TransformerEncoderLayer (the
 path a grad-enabled call takes): post-norm, key-padding mask, all-invalid rows flipped to all-valid, padded
 query rows computed like the others, dropout at four sites per layer.  Dropout is injected: `keep` maps
 (layer, site) to a bool keep mask (site 0 attention probabilities [rows,4,Np,Np]; 1 dropout1, 2 the dropout
 between ReLU and linear2, 3 dropout2, each [tokens,128]), survivors scaled by 1 / (1 - p).  Gradients come
-from torch.autograd on the parameters passed in.
+from torch.autograd on the parameters passed in.  The arithmetic runs in the dtype of the embeddings and
+parameters: fp32 is the reference's own, float64 gives the rounding-free yardstick the device gradients are
+measured against (the dropout scale stays the fp32 value of 1 / (1 - p), which is what the reference multiplies by).
 """
 from __future__ import annotations
 
@@ -33,7 +35,7 @@ def mask_logits(p: Dict[str, torch.Tensor], emb: torch.Tensor) -> torch.Tensor:
 
 
 def mask_loss(logits, kp, road, focal: bool):
-    gt = torch.stack([kp, road], dim=3)
+    gt = torch.stack([kp, road], dim=3).to(logits.dtype)
     if focal:
         from torchvision.ops import sigmoid_focal_loss
         return sigmoid_focal_loss(logits, gt, alpha=0.25, gamma=2, reduction="mean")
@@ -44,7 +46,7 @@ def topo_logits(p, emb, points, pairs, valid, P: int, version: str = "normal",
                 keep: Optional[Dict[Tuple[int, int], torch.Tensor]] = None, dropout_p: float = 0.1):
     """TopoNet logits [B,Ns,Np] from the sampled embeddings, slow-path semantics."""
     B, Ns, Np, _ = pairs.shape
-    pts = points.to(torch.float32)
+    pts = points.to(emb.dtype)
     g = (pts / P * 2.0 - 1.0).unsqueeze(2)
     feats = F.grid_sample(emb, g, mode="bilinear", align_corners=False).squeeze(-1).permute(0, 2, 1)
     pf = F.relu(F.linear(feats, p["topo_net.feature_proj.weight"], p["topo_net.feature_proj.bias"]))
@@ -85,8 +87,8 @@ def topo_logits(p, emb, points, pairs, valid, P: int, version: str = "normal",
 
 
 def topo_loss(logits, connected, valid):
-    m = valid.to(torch.float32)
-    t = F.binary_cross_entropy_with_logits(logits, connected.to(torch.float32), reduction="none") * m
+    m = valid.to(logits.dtype)
+    t = F.binary_cross_entropy_with_logits(logits, connected.to(logits.dtype), reduction="none") * m
     return t.sum() / m.sum()
 
 

@@ -218,73 +218,80 @@ __global__ void __launch_bounds__(256) gemm_mma_kernel(LA A, LB Bm, OUT out, lon
                                                        long long kchunk) {
   __shared__ __align__(16) __half As[2][kTile][kLdh];   // hi / lo, [m][k]
   __shared__ __align__(16) __half Bs[2][kTile][kLdh];   // hi / lo, [n][k]
-  const long long m0 = static_cast<long long>(blockIdx.y) * kTile, n0 = static_cast<long long>(blockIdx.x) * kTile;
+  const long long n0 = static_cast<long long>(blockIdx.x) * kTile;
   const int z = blockIdx.z;
   const long long kb = z * kchunk, ke = kb + kchunk < K ? kb + kchunk : K;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const int wm = (warp >> 1) * 16, wn = (warp & 1) * 32;
   const bool a_kfast = A.second_unit(), b_kfast = Bm.first_unit();
-  float acc[4][4];
+  // one row tile per block unless M has more row tiles than grid.y holds
+  for (long long m0 = static_cast<long long>(blockIdx.y) * kTile; m0 < M; m0 += static_cast<long long>(gridDim.y) * kTile) {
+    float acc[4][4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j)
+    for (int j = 0; j < 4; ++j)
 #pragma unroll
-    for (int r = 0; r < 4; ++r) acc[j][r] = 0.f;
-  for (long long k0 = kb; k0 < ke; k0 += kTk) {
-    for (int i = threadIdx.x; i < kTk * kTile; i += 256) {
-      int mm = a_kfast ? i / kTk : i % kTile, kk = a_kfast ? i % kTk : i / kTile;
-      long long r = m0 + mm, k = k0 + kk;
-      float v = (r < M && k < ke) ? A(r, k) : 0.f;
-      __half h = __float2half_rn(v);
-      As[0][mm][kk] = h;
-      As[1][mm][kk] = __float2half_rn(v - __half2float(h));
-      mm = b_kfast ? i / kTk : i % kTile;
-      kk = b_kfast ? i % kTk : i / kTile;
-      r = n0 + mm;
-      k = k0 + kk;
-      v = (r < N && k < ke) ? Bm(k, r) : 0.f;
-      h = __float2half_rn(v);
-      Bs[0][mm][kk] = h;
-      Bs[1][mm][kk] = __float2half_rn(v - __half2float(h));
-    }
-    __syncthreads();
-#pragma unroll
-    for (int ks = 0; ks < kTk; ks += 16) {
-      uint32_t a[2][4];
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        a[u][0] = ld_h2(&As[u][wm + g][ks + 2 * t]);
-        a[u][1] = ld_h2(&As[u][wm + g + 8][ks + 2 * t]);
-        a[u][2] = ld_h2(&As[u][wm + g][ks + 2 * t + 8]);
-        a[u][3] = ld_h2(&As[u][wm + g + 8][ks + 2 * t + 8]);
+      for (int r = 0; r < 4; ++r) acc[j][r] = 0.f;
+    for (long long k0 = kb; k0 < ke; k0 += kTk) {
+      for (int i = threadIdx.x; i < kTk * kTile; i += 256) {
+        int mm = a_kfast ? i / kTk : i % kTile, kk = a_kfast ? i % kTk : i / kTile;
+        long long r = m0 + mm, k = k0 + kk;
+        float v = (r < M && k < ke) ? A(r, k) : 0.f;
+        __half h = __float2half_rn(v);
+        As[0][mm][kk] = h;
+        As[1][mm][kk] = __float2half_rn(v - __half2float(h));
+        mm = b_kfast ? i / kTk : i % kTile;
+        kk = b_kfast ? i % kTk : i / kTile;
+        r = n0 + mm;
+        k = k0 + kk;
+        v = (r < N && k < ke) ? Bm(k, r) : 0.f;
+        h = __float2half_rn(v);
+        Bs[0][mm][kk] = h;
+        Bs[1][mm][kk] = __float2half_rn(v - __half2float(h));
       }
+      __syncthreads();
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint32_t bh0 = ld_h2(&Bs[0][wn + 8 * j + g][ks + 2 * t]), bh1 = ld_h2(&Bs[0][wn + 8 * j + g][ks + 2 * t + 8]);
-        const uint32_t bl0 = ld_h2(&Bs[1][wn + 8 * j + g][ks + 2 * t]), bl1 = ld_h2(&Bs[1][wn + 8 * j + g][ks + 2 * t + 8]);
-        mma16816(acc[j], a[1][0], a[1][1], a[1][2], a[1][3], bh0, bh1);   // small terms first
-        mma16816(acc[j], a[0][0], a[0][1], a[0][2], a[0][3], bl0, bl1);
-        mma16816(acc[j], a[0][0], a[0][1], a[0][2], a[0][3], bh0, bh1);
+      for (int ks = 0; ks < kTk; ks += 16) {
+        uint32_t a[2][4];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          a[u][0] = ld_h2(&As[u][wm + g][ks + 2 * t]);
+          a[u][1] = ld_h2(&As[u][wm + g + 8][ks + 2 * t]);
+          a[u][2] = ld_h2(&As[u][wm + g][ks + 2 * t + 8]);
+          a[u][3] = ld_h2(&As[u][wm + g + 8][ks + 2 * t + 8]);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const uint32_t bh0 = ld_h2(&Bs[0][wn + 8 * j + g][ks + 2 * t]), bh1 = ld_h2(&Bs[0][wn + 8 * j + g][ks + 2 * t + 8]);
+          const uint32_t bl0 = ld_h2(&Bs[1][wn + 8 * j + g][ks + 2 * t]), bl1 = ld_h2(&Bs[1][wn + 8 * j + g][ks + 2 * t + 8]);
+          mma16816(acc[j], a[1][0], a[1][1], a[1][2], a[1][3], bh0, bh1);   // small terms first
+          mma16816(acc[j], a[0][0], a[0][1], a[0][2], a[0][3], bl0, bl1);
+          mma16816(acc[j], a[0][0], a[0][1], a[0][2], a[0][3], bh0, bh1);
+        }
       }
+      __syncthreads();
     }
-    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const long long m = m0 + wm + g + (r >> 1) * 8, n = n0 + wn + 8 * j + 2 * t + (r & 1);
+        if (m < M && n < N) out(z, m, n, acc[j][r]);
+      }
   }
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      const long long m = m0 + wm + g + (r >> 1) * 8, n = n0 + wn + 8 * j + 2 * t + (r & 1);
-      if (m < M && n < N) out(z, m, n, acc[j][r]);
-    }
 }
 
+// Column tiles on grid.x, row tiles on grid.y, k chunks on grid.z.  A GEMM with more than 65535 row tiles (the
+// decoder's stage-3 GEMMs have 64 B (P/16)^2 rows: from B = 16 @1024) launches 65535 of them and each block walks
+// its row tiles with that stride; smaller GEMMs run one tile per block.
 template <class LA, class LB, class OUT>
 int tc_gemm(LA A, LB Bm, OUT out, long long M, long long N, long long K, int chunks, cudaStream_t st) {
   if (M <= 0 || N <= 0) return 0;
   const long long kchunk = chunks > 1 ? ((K + chunks - 1) / chunks + kTk - 1) / kTk * kTk : (K > 0 ? K : 1);
   const long long z = K > 0 ? (K + kchunk - 1) / kchunk : 1;
-  SRB_REQUIRE((M + kTile - 1) / kTile < 65536 && z < 65536, "train: GEMM of %lld rows is too large", M);
-  const dim3 grid(static_cast<unsigned>((N + kTile - 1) / kTile), static_cast<unsigned>((M + kTile - 1) / kTile),
-                  static_cast<unsigned>(z));
+  const long long mt = (M + kTile - 1) / kTile, nt = (N + kTile - 1) / kTile;
+  // make_dims bounds every GEMM of a step far below these limits
+  SRB_REQUIRE(nt < 65536 && z < 65536, "train: GEMM of %lld x %lld (%lld chunks) is too large", M, N, z);
+  const dim3 grid(static_cast<unsigned>(nt), static_cast<unsigned>(mt < 65535 ? mt : 65535), static_cast<unsigned>(z));
   gemm_mma_kernel<<<grid, 256, 0, st>>>(A, Bm, out, M, N, K, kchunk);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch();

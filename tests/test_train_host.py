@@ -162,11 +162,7 @@ def test_train_symbols_reject_bad_arguments_without_gpu():
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "train_heads_vitb_256.npz")
 
 
-@pytest.mark.parametrize("focal", [False, True])
-def test_oracle_reproduces_reference_training_step(focal):
-    """tests/golden/train_heads_vitb_256.npz holds the unmodified reference's training_step + loss.backward()
-    (tools/make_golden.py --train-heads).  The embeddings are recomputed here by the fp32 encoder oracle, which
-    agrees with the reference's within 2e-5 (tests/test_oracle_golden.py); that difference bounds the match."""
+def _check_reference_training_step(focal, dtype):
     from oracle import samroad_oracle as O
     from tools.make_golden import train_heads_batch
     z = np.load(GOLDEN)
@@ -179,8 +175,9 @@ def test_oracle_reproduces_reference_training_step(focal):
     d = emb.double()
     np.testing.assert_allclose([d.sum().item(), d.abs().sum().item(), (d * d).sum().item()], z[f"{tag}/emb_stats"],
                                rtol=1e-5)
-    params = {k: v.clone().requires_grad_(True) for k, v in sd.items() if k.startswith(("map_decoder.", "topo_net."))}
-    ml, tl = TO.heads_losses(params, emb, b, 256, focal, "normal", None, 0.0)
+    params = {k: v.to(dtype).requires_grad_(True) for k, v in sd.items() if k.startswith(("map_decoder.", "topo_net."))}
+    ml, tl = TO.heads_losses(params, emb.to(dtype), b, 256, focal, "normal", None, 0.0)
+    assert ml.dtype == tl.dtype == dtype
     (ml + tl).backward()
     np.testing.assert_allclose([ml.item(), tl.item(), (ml + tl).item()], z[f"{tag}/losses"], rtol=1e-5)
     for k, p in params.items():
@@ -191,6 +188,21 @@ def test_oracle_reproduces_reference_training_step(focal):
         idx = torch.from_numpy(z[f"{tag}/{k}/idx"].astype(np.int64))
         assert np.abs(g[idx].numpy() - z[f"{tag}/{k}/val"]).max() <= 1e-4 * mx + 1e-30, k
     assert list(z[f"{tag}/param_counts"]) == [172770, 364929]     # the reference's printed group sizes
+
+
+@pytest.mark.parametrize("focal", [False, True])
+def test_oracle_reproduces_reference_training_step(focal):
+    """tests/golden/train_heads_vitb_256.npz holds the unmodified reference's training_step + loss.backward()
+    (tools/make_golden.py --train-heads).  The embeddings are recomputed here by the fp32 encoder oracle, which
+    agrees with the reference's within 2e-5 (tests/test_oracle_golden.py); that difference bounds the match."""
+    _check_reference_training_step(focal, torch.float32)
+
+
+@pytest.mark.parametrize("focal", [False, True])
+def test_float64_oracle_reproduces_reference_training_step(focal):
+    """The same step with the embeddings and the head parameters cast to float64: the float64 oracle, which the
+    GPU tests measure the device gradients against, computes the reference's training step."""
+    _check_reference_training_step(focal, torch.float64)
 
 
 def test_enable_training_once():
