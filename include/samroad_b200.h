@@ -317,6 +317,51 @@ int samroad_update_tensor_device(samroad_handle_t h, const char* key, const floa
 int samroad_debug_train_dropout_keep(float p, uint64_t seed, int layer, int site, int64_t n, uint8_t* keep,
                                      void* stream);
 
+/* ---- training / evaluation batches on the device (sam_road_b200/dataset.py, DESIGN.md §13) ----
+ * A labels object holds the scenes of one dataset: each scene's subdivided ground-truth graph as
+ * GraphLabelGenerator.__init__ (dataset.py:71-125) builds it, precomputed on the host, and its uint8 RGB and
+ * masks.  A batch runs GraphLabelGenerator.sample_patch (dataset.py:127-231) for B patches and collates them as
+ * graph_collate_fn (dataset.py:287-302).  Not thread-safe; one batch at a time. */
+typedef struct samroad_labels_ctx* samroad_labels_t;
+typedef struct SamRoadLabelCfg {
+  int32_t patch_size;            /* P                                                                      */
+  int32_t image_size;            /* side of the (square) scenes                                            */
+  int32_t sample_margin;         /* patch origins lie in [margin, image_size - P - margin]                 */
+  int32_t topo_sample_num;       /* sources per patch (TOPO_SAMPLE_NUM) >= 1                               */
+  int32_t max_neighbor_queries;  /* pairs per source (MAX_NEIGHBOR_QUERIES), 1..32                         */
+  int32_t max_patch_points;      /* most non-excluded graph points any admissible P x P window holds       */
+  double road_nms_radius;        /* ROAD_NMS_RADIUS > 0 (inclusive)                                        */
+  double neighbor_radius;        /* NEIGHBOR_RADIUS > 0 (kNN strictly inside; BFS depth radius // 4)       */
+} SamRoadLabelCfg;
+
+int samroad_labels_create(int device, const SamRoadLabelCfg* cfg, samroad_labels_t* out);
+int samroad_labels_destroy(samroad_labels_t L);
+/* Copies one scene (host memory) to the device; *scene_index gets its index (upload order).  points [n,2]
+ * float64 (x, y) of the subdivided graph; flags [n] bit 0 = excluded (near a crossover), bit 1 = never
+ * suppressed by NMS (degree != 2); weights [n] sampling weights; adj_start [n+1] / adj CSR adjacency;
+ * rgb [S,S,3], keypoint_mask / road_mask [S,S] uint8 with S = image_size. */
+int samroad_labels_upload(samroad_labels_t L, const uint8_t* rgb, const uint8_t* keypoint_mask,
+                          const uint8_t* road_mask, int32_t n_points, const double* points, const uint8_t* flags,
+                          const float* weights, const int32_t* adj_start, const int32_t* adj,
+                          int32_t* scene_index);
+/* One batch of B patches on `stream`.  patches: device int32 [B,4] (scene, x0, y0, rot) or NULL to draw them
+ * (training: uniform scene, origins in the margin range, rot 0..3).  Every other draw is Philox keyed by `seed`.
+ * Outputs (device): rgb [B,P,P,3] float32 0..255, keypoint_mask / road_mask [B,P,P] float32 /255,
+ * points [B,N,2] float32 (capacity B * max_patch_points * 2), pairs [B,S,Np,2] int32, connected / valid
+ * [B,S,Np] bytes 0/1; *n_points = N (host), the largest point count of the batch.  Synchronises the stream once
+ * to read the point counts. */
+int samroad_labels_batch(samroad_labels_t L, int B, uint64_t seed, const int32_t* patches, float* rgb,
+                         float* keypoint_mask, float* road_mask, float* points, int32_t* pairs,
+                         uint8_t* connected, uint8_t* valid, int32_t* n_points, void* stream);
+/* Test hook on the draw arrays of a batch (device or host memory): patches [B,4]; score_u [B,max_patch_points]
+ * U[0,1) of the j-th candidate in ascending id; source_u [B,S] U[0,1); noise [B,max_patch_points,2] added to the
+ * i-th point.  mode 0: the batch takes the caller-filled arrays instead of drawing them (seed unused).
+ * mode 1: the batch draws as samroad_labels_batch(patches = NULL, seed) does and copies its draws out. */
+int samroad_debug_labels_batch_draws(samroad_labels_t L, int B, int mode, uint64_t seed, int32_t* patches,
+                                     double* score_u, double* source_u, double* noise, float* rgb,
+                                     float* keypoint_mask, float* road_mask, float* points, int32_t* pairs,
+                                     uint8_t* connected, uint8_t* valid, int32_t* n_points, void* stream);
+
 /* Stream memory operations on a 32-bit flag word in device (or peer-mapped) memory, executed by the stream
  * front end without a kernel: an ordered write of `value`, and a wait until *addr >= value.  The exchange step
  * between ranks (sam_road_b200/exchange.py; no reference counterpart, the reference is single-GPU) builds its

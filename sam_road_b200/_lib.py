@@ -45,6 +45,19 @@ class SamRoadTrainArgs(C.Structure):
     ]
 
 
+class SamRoadLabelCfg(C.Structure):
+    _fields_ = [
+        ("patch_size", C.c_int32),
+        ("image_size", C.c_int32),
+        ("sample_margin", C.c_int32),
+        ("topo_sample_num", C.c_int32),
+        ("max_neighbor_queries", C.c_int32),
+        ("max_patch_points", C.c_int32),
+        ("road_nms_radius", C.c_double),
+        ("neighbor_radius", C.c_double),
+    ]
+
+
 _vp, _i, _f, _d = C.c_void_p, C.c_int, C.c_float, C.c_double
 _ip = C.POINTER(C.c_int)
 _targs = C.POINTER(SamRoadTrainArgs)
@@ -94,6 +107,14 @@ SIGNATURES = {
     "samroad_train_backward": (_i, [_vp, _targs, _vp, _vp, _vp, _i, _vp, C.c_size_t, _vp, _vp]),
     "samroad_update_tensor_device": (_i, [_vp, C.c_char_p, _vp, C.POINTER(C.c_int64), _i, _vp]),
     "samroad_debug_train_dropout_keep": (_i, [_f, C.c_uint64, _i, _i, C.c_int64, _vp, _vp]),
+    "samroad_labels_create": (_i, [_i, C.POINTER(SamRoadLabelCfg), C.POINTER(_vp)]),
+    "samroad_labels_destroy": (_i, [_vp]),
+    "samroad_labels_upload": (_i, [_vp, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp, _vp, _vp,
+                                   C.POINTER(C.c_int32)]),
+    "samroad_labels_batch": (_i, [_vp, _i, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                  C.POINTER(C.c_int32), _vp]),
+    "samroad_debug_labels_batch_draws": (_i, [_vp, _i, _i, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                              _vp, _vp, C.POINTER(C.c_int32), _vp]),
     "samroad_stream_write_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_stream_wait_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_timing_enable": (_i, [_vp, _i]),

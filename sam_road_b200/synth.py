@@ -108,3 +108,77 @@ def make_topo_inputs(batch: int, patch_size: int, n_points: int, seed: int = 0, 
     return (torch.tensor(np.stack([pad(p) for p in pts_l])),
             torch.tensor(np.stack([pad(p) for p in pairs_l])),
             torch.tensor(np.stack([pad(v) for v in valid_l])))
+
+
+def make_road_graph(extent: int, seed: int = 0, spacing: int = 48, lo: int = 16):
+    """Sat2graph adjacency dict {(row, col): [(row, col), ...]} of a synthetic road network inside
+    [lo, extent]^2: an axis-aligned street grid with nodes every `spacing` pixels and intermediate nodes (equal
+    distances along axis-aligned runs), a few missing grid edges (degree-3 intersections), dead-end spurs, and two
+    diagonal overpasses that cross grid edges without sharing a node (crossovers)."""
+    rng = np.random.RandomState(3000 + seed)
+    adj: Dict = {}
+
+    def link(a, b):
+        adj.setdefault(a, [])
+        adj.setdefault(b, [])
+        if b not in adj[a]:
+            adj[a].append(b)
+            adj[b].append(a)
+
+    lines = list(range(lo, extent + 1, spacing))
+    for r in lines:
+        for i, c in enumerate(lines[:-1]):
+            c2 = lines[i + 1]
+            if rng.rand() < 0.12:
+                continue
+            mid = (r, c + (c2 - c) // 2)
+            link((r, c), mid)
+            link(mid, (r, c2))
+    for c in lines:
+        for i, r in enumerate(lines[:-1]):
+            r2 = lines[i + 1]
+            if rng.rand() < 0.12:
+                continue
+            link((r, c), (r2, c))
+    for _ in range(max(2, len(lines))):       # dead ends
+        r, c = lines[rng.randint(len(lines))], lines[rng.randint(len(lines))]
+        link((r, c), (r + int(rng.randint(9, spacing // 2)), c + int(rng.randint(5, spacing // 2))))
+    for k in range(2):                          # overpasses: off-grid nodes only
+        a = (lo + 7 + 11 * k, lo + 5 + 3 * k)
+        m = (lo + (extent - lo) // 2 + 5 + 2 * k, lo + (extent - lo) // 2 + 9 - 4 * k)
+        b = (extent - 3 - 7 * k, extent - 13 + 5 * k)
+        if k:
+            a, b = (a[0], b[1]), (b[0], a[1])
+            m = (m[0] + 3, m[1] - 6)
+        link(a, m)
+        link(m, b)
+    return adj
+
+
+def write_label_scenes(root: str, dataset: str, tiles, size: int, seed: int = 0, extent: int = None,
+                       empty=()) -> None:
+    """Scene files of `tiles` in the reference's cityscale / spacenet layout under root (dataset.py:311-340):
+    a seeded RGB PNG, binary keypoint / road mask PNGs (0 / 255) and the pickled ground-truth graph (an empty
+    dict for the tiles in `empty`).  Graph coordinates are (row, col) for cityscale and the spacenet convention
+    (x = col, y = 400 - row) is applied by the dataset."""
+    import os
+    import pickle
+
+    import cv2
+    pat = {"cityscale": ("cityscale/20cities/region_{}_sat.png", "cityscale/processed/keypoint_mask_{}.png",
+                         "cityscale/processed/road_mask_{}.png", "cityscale/20cities/region_{}_refine_gt_graph.p"),
+           "spacenet": ("spacenet/RGB_1.0_meter/{}__rgb.png", "spacenet/processed/keypoint_mask_{}.png",
+                        "spacenet/processed/road_mask_{}.png", "spacenet/RGB_1.0_meter/{}__gt_graph.p")}[dataset]
+    for p in pat:
+        os.makedirs(os.path.join(root, os.path.dirname(p)), exist_ok=True)
+    for k, t in enumerate(tiles):
+        rng = np.random.RandomState(4000 + 97 * seed + k)
+        rgb = rng.randint(0, 256, (size, size, 3)).astype(np.uint8)
+        kp = ((rng.rand(size, size) < 0.1) * 255).astype(np.uint8)
+        road = ((rng.rand(size, size) < 0.3) * 255).astype(np.uint8)
+        cv2.imwrite(os.path.join(root, pat[0].format(t)), rgb[:, :, ::-1])
+        cv2.imwrite(os.path.join(root, pat[1].format(t)), kp)
+        cv2.imwrite(os.path.join(root, pat[2].format(t)), road)
+        adj = {} if t in empty else make_road_graph(extent or size - 16, seed=seed + k)
+        with open(os.path.join(root, pat[3].format(t)), "wb") as f:
+            pickle.dump(adj, f)

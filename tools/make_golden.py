@@ -265,8 +265,121 @@ def train_heads_fixture():
     np.savez_compressed(os.path.join(OUT, "train_heads_vitb_256.npz"), **out)
 
 
+LABEL_CFG = dict(PATCH_SIZE=256, TOPO_SAMPLE_NUM=24, MAX_NEIGHBOR_QUERIES=16, NEIGHBOR_RADIUS=64,
+                 ROAD_NMS_RADIUS=16)
+LABEL_EXTENT = 360                 # the synthetic graph lies in [16, 360]^2: windows past it are empty
+# (x0, y0, rot): rot 0..3, the empty window, and windows holding the overpass crossings
+LABEL_PATCHES = ((40, 20, 0), (96, 64, 1), (10, 100, 2), (60, 30, 3), (384, 384, 1), (0, 0, 0), (100, 100, 2))
+
+
+def label_scene():
+    """The synthetic ground-truth graph of labels_synth.npz and its coordinate transform (cityscale's)."""
+    from sam_road_b200 import dataset as D
+    return synth.make_road_graph(LABEL_EXTENT, seed=0), D.cityscale_transform
+
+
+class _IndexLog(np.ndarray):
+    """An ndarray that records the row indices it is fancy-indexed with (`pts[idx, :]`)."""
+
+    def __getitem__(self, key):
+        if isinstance(key, tuple) and len(key) == 2 and isinstance(key[0], np.ndarray):
+            self.log.append(np.array(key[0]))
+        return np.asarray(self).__getitem__(key)
+
+
+def labels_fixture():
+    """GraphLabelGenerator.__init__ / sample_patch (dataset.py:71-231) of the unmodified reference on a synthetic
+    graph.  The draws are recorded by wrapping np.random.uniform / choice / normal and graph_utils.nms_points from
+    outside; the candidate and source ids by indexing a logging view of subdivide_points."""
+    from oracle import label_oracle as LO
+    from sam_road_b200 import dataset as D
+    ref = ref_loader.load_reference_dataset()
+    gu = sys.modules["graph_utils"]
+    adj, transform = label_scene()
+    cfg = ref_loader.AttrDict(LABEL_CFG)
+    gen = ref.GraphLabelGenerator(cfg, adj, transform)
+    mine = D.precompute_scene(adj, transform)
+    ref_cross = np.array(gen.crossover_points, dtype=np.float64).reshape(-1, 2)
+    assert np.array_equal(gen.subdivide_points, mine.points), "subdivision differs"
+    assert np.array_equal(np.unique(ref_cross, axis=0), np.unique(mine.crossovers, axis=0)), "crossovers differ"
+    assert set(np.nonzero(mine.excluded)[0].tolist()) == set(gen.exclude_indices), "excluded set differs"
+    assert np.array_equal(gen.nms_score_override, mine.nms_override) and np.array_equal(gen.sample_weights,
+                                                                                          mine.weights)
+    out = dict(cfg=np.array([LABEL_CFG[k] for k in sorted(LABEL_CFG)]), cfg_keys=np.array(sorted(LABEL_CFG)),
+               extent=LABEL_EXTENT, subdivide_points=gen.subdivide_points, crossovers=ref_cross,
+               excluded=np.array(sorted(gen.exclude_indices), dtype=np.int32),
+               nms_override=gen.nms_score_override, sample_weights=gen.sample_weights,
+               patches=np.array(LABEL_PATCHES, dtype=np.int32))
+    log = gen.subdivide_points.view(_IndexLog)
+    log.log = []
+    gen.subdivide_points = log
+    drawn = {}
+    real = {k: getattr(np.random, k) for k in ("uniform", "choice", "normal")}
+    real_nms = gu.nms_points
+
+    def wrap(name):
+        def f(*a, **k):
+            r = real[name](*a, **k)
+            drawn[name] = np.array(r)
+            return r
+        return f
+
+    def nms_rec(*a, **k):
+        r = real_nms(*a, **k)
+        drawn["kept"] = np.array(r[1])
+        return r
+
+    P = LABEL_CFG["PATCH_SIZE"]
+    lc = dict(P=P, S=LABEL_CFG["TOPO_SAMPLE_NUM"], Np=LABEL_CFG["MAX_NEIGHBOR_QUERIES"],
+              r_nms=LABEL_CFG["ROAD_NMS_RADIUS"], r_nbr=LABEL_CFG["NEIGHBOR_RADIUS"])
+    np.random.seed(1234)
+    try:
+        for name in real:
+            setattr(np.random, name, wrap(name))
+        gu.nms_points = nms_rec
+        for k, (x0, y0, rot) in enumerate(LABEL_PATCHES):
+            drawn.clear()
+            log.log.clear()
+            pts, samples = gen.sample_patch(((x0, y0), (x0 + P, y0 + P)), rot)
+            pairs, conn, valid = (np.array(v) for v in zip(*samples))
+            rec = dict(points=np.asarray(pts, dtype=np.float64), pairs=pairs.astype(np.int32),
+                       connected=conn.astype(bool), valid=valid.astype(bool))
+            if log.log:
+                cand, src_ids = log.log[0], log.log[1]
+                rec.update(candidates=cand.astype(np.int64), score=drawn["uniform"],
+                           survivors=cand[drawn["kept"]].astype(np.int64),
+                           source_index=drawn["choice"].astype(np.int64), noise=drawn["normal"])
+                assert np.array_equal(rec["survivors"][rec["source_index"]], src_ids)
+                o = LO.sample_patch(mine, x0, y0, rot, lc, dict(score=rec["score"], source_index=rec["source_index"],
+                                                               noise=rec["noise"]), ties="scipy")
+                assert np.array_equal(o["candidates"], rec["candidates"]), f"patch {k}: candidate order"
+                assert np.array_equal(o["survivors"], rec["survivors"]), f"patch {k}: NMS"
+                assert np.array_equal(o["points"], rec["points"].astype(np.float32)), f"patch {k}: points"
+            else:
+                o = LO.sample_patch(mine, x0, y0, rot, lc, {}, ties="scipy")
+            for key in ("pairs", "connected", "valid"):
+                assert np.array_equal(o[key], rec[key]), f"patch {k}: {key}"
+            for key, v in rec.items():
+                out[f"p{k}/{key}"] = v
+            print(f"labels patch {k} (x0={x0}, y0={y0}, rot={rot}): {len(rec.get('candidates', []))} candidates, "
+                  f"{len(rec.get('survivors', []))} survivors, {int(rec['valid'].sum())} valid pairs, "
+                  f"{int(rec['connected'].sum())} connected; oracle (ties='scipy') identical")
+    finally:
+        for name, fn in real.items():
+            setattr(np.random, name, fn)
+        gu.nms_points = real_nms
+    path = os.path.join(OUT, "labels_synth.npz")
+    np.savez_compressed(path, **out)
+    print(f"{path}: {os.path.getsize(path)} bytes, {len(ref_cross)} crossover points "
+          f"({len(np.unique(ref_cross, axis=0))} distinct), {len(gen.exclude_indices)} excluded")
+
+
 def main():
     assert ref_loader.available(), "needs /root/reference"
+    if "--labels" in sys.argv:        # GraphLabelGenerator / sample_patch on a synthetic graph
+        os.makedirs(OUT, exist_ok=True)
+        labels_fixture()
+        return
     if "--train-heads" in sys.argv:   # training_step / backward of the heads with a frozen encoder
         os.makedirs(OUT, exist_ok=True)
         train_heads_fixture()
