@@ -331,14 +331,15 @@ typedef struct SamRoadLabelCfg {
   int32_t max_neighbor_queries;  /* pairs per source (MAX_NEIGHBOR_QUERIES), 1..32                         */
   int32_t max_patch_points;      /* most non-excluded graph points any admissible P x P window holds       */
   double road_nms_radius;        /* ROAD_NMS_RADIUS > 0 (inclusive)                                        */
-  double neighbor_radius;        /* NEIGHBOR_RADIUS > 0 (kNN strictly inside; BFS depth radius // 4)       */
+  double neighbor_radius;        /* NEIGHBOR_RADIUS > 0 (kNN strictly inside; BFS depth radius // 4 <= INT_MAX) */
 } SamRoadLabelCfg;
 
 int samroad_labels_create(int device, const SamRoadLabelCfg* cfg, samroad_labels_t* out);
 int samroad_labels_destroy(samroad_labels_t L);
 /* Copies one scene (host memory) to the device; *scene_index gets its index (upload order).  points [n,2]
  * float64 (x, y) of the subdivided graph; flags [n] bit 0 = excluded (near a crossover), bit 1 = never
- * suppressed by NMS (degree != 2); weights [n] sampling weights; adj_start [n+1] / adj CSR adjacency;
+ * suppressed by NMS (degree != 2); weights [n] sampling weights, each positive and finite; adj_start [n+1] /
+ * adj CSR adjacency;
  * rgb [S,S,3], keypoint_mask / road_mask [S,S] uint8 with S = image_size. */
 int samroad_labels_upload(samroad_labels_t L, const uint8_t* rgb, const uint8_t* keypoint_mask,
                           const uint8_t* road_mask, int32_t n_points, const double* points, const uint8_t* flags,

@@ -73,8 +73,8 @@ struct Work {          // per-batch device arrays, [B, ...]
   double* sxy;         // [B, cap, 2] survivor coordinates
   double* cdf;         // [B, cap] running sum of the survivors' weights
   int32_t* src;        // [B, S] source, index into the survivors
-  int32_t* nsurv;      // [B] survivors (0: empty patch)
   int32_t* status;     // [1] kBadPatch | kBfsOverflow | kOverCap
+  int32_t* nsurv;      // [B] survivors (0: empty patch), right after the status word
 };
 
 // ---- Philox4x32-10 keyed by the 64-bit seed, counter (ctr, element, stream, 0) ---------------------------------
@@ -488,6 +488,15 @@ __global__ void __launch_bounds__(32 * kPairWarps, 4) pairs_kernel(Params p, Wor
     ++hits;
   }
   const int nt = hits > 0 ? hits - 1 : 0;   // targets held by lanes 0 .. nt-1
+  if (nt == 0) {   // no target in range: every slot is padding and the walk decides nothing
+    for (int k = lane; k < p.Np; k += 32) {
+      pairs[2 * (slot + k)] = si;
+      pairs[2 * (slot + k) + 1] = si;
+      valid[slot + k] = 0;
+      connected[slot + k] = 0;
+    }
+    return;
+  }
 
   // BFS (graph_utils.py:594-630): reached = visited set
   for (int h = lane; h < kBfsHash; h += 32) sm.hash[h] = -1;
@@ -573,7 +582,7 @@ struct samroad_labels_ctx {
   int B_alloc = 0;
   void* work_mem = nullptr;
   Work work{};
-  int32_t* h_read = nullptr;   // pinned [B + 1]
+  int32_t* h_read = nullptr;   // pinned [1 + B]: status word, then the survivor counts
   size_t smem_patch = 0;
 };
 
@@ -592,6 +601,9 @@ int cfg_check(const SamRoadLabelCfg* c) {
               "labels: ROAD_NMS_RADIUS must be a positive number (got %g)", c->road_nms_radius);
   SRB_REQUIRE(std::isfinite(c->neighbor_radius) && c->neighbor_radius > 0.0,
               "labels: NEIGHBOR_RADIUS must be a positive number (got %g)", c->neighbor_radius);
+  SRB_REQUIRE(std::floor(c->neighbor_radius / 4.0) <= static_cast<double>(INT_MAX),
+              "labels: NEIGHBOR_RADIUS %g gives a BFS depth NEIGHBOR_RADIUS // 4 beyond %d", c->neighbor_radius,
+              INT_MAX);
   SRB_REQUIRE(c->max_patch_points >= 1, "labels: max_patch_points must be >= 1 (got %d)", c->max_patch_points);
   return 0;
 }
@@ -632,7 +644,8 @@ int ensure_work(samroad_labels_ctx* L, int B) {
   L->h_read = nullptr;
   L->B_alloc = 0;
   const size_t cap = L->cfg.max_patch_points, S = L->cfg.topo_sample_num, nb = B;
-  // the last region is nsurv [B] followed by the status word, so that one copy reads both
+  // the last region is the status word followed by nsurv [B], so that one copy of 1 + B words reads both for
+  // any batch up to B_alloc (a status word after nsurv [B_alloc] would be missed by smaller batches)
   const size_t bytes[] = {16 * nb, 8 * cap * nb, 8 * S * nb, 16 * cap * nb, 4 * cap * nb, 4 * cap * nb,
                           16 * cap * nb, 8 * cap * nb, 4 * S * nb, 4 * (nb + 1)};
   size_t total = 0;
@@ -655,8 +668,8 @@ int ensure_work(samroad_labels_ctx* L, int B) {
   w.sxy = static_cast<double*>(ptrs[6]);
   w.cdf = static_cast<double*>(ptrs[7]);
   w.src = static_cast<int32_t*>(ptrs[8]);
-  w.nsurv = static_cast<int32_t*>(ptrs[9]);
-  w.status = w.nsurv + B;
+  w.status = static_cast<int32_t*>(ptrs[9]);
+  w.nsurv = w.status + 1;
   L->B_alloc = B;
   return 0;
 }
@@ -693,16 +706,16 @@ int run_batch(samroad_labels_ctx* L, int B, unsigned long long seed, const int32
       p, w, pairs, connected, valid);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(3);
-  SRB_CUDA_OK(cudaMemcpyAsync(L->h_read, w.nsurv, sizeof(int32_t) * (B + 1), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(L->h_read, w.status, sizeof(int32_t) * (B + 1), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
-  const int status = L->h_read[B];
+  const int status = L->h_read[0];
   SRB_REQUIRE(!(status & kBadPatch), "%s: a patch names a missing scene, an origin outside [%d, %d] or a "
               "rotation outside 0..3", what, p.lo, p.hi);
   SRB_REQUIRE(!(status & kOverCap), "%s: a patch holds more than max_patch_points=%d candidates", what, p.cap);
   SRB_REQUIRE(!(status & kBfsOverflow), "%s: a BFS reached more than %d nodes within NEIGHBOR_RADIUS // 4 = %d "
               "steps", what, kBfsList, p.depth);
   int N = 1;
-  for (int b = 0; b < B; ++b) N = std::max(N, L->h_read[b]);
+  for (int b = 0; b < B; ++b) N = std::max(N, L->h_read[1 + b]);
   points_kernel<<<dim3(grid_of(N, 128), B), 128, 0, st>>>(p, w, N, points);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(1);
@@ -768,8 +781,11 @@ extern "C" int samroad_labels_upload(samroad_labels_t L, const uint8_t* rgb, con
     SRB_REQUIRE(adj_start[i + 1] >= adj_start[i], "samroad_labels_upload: adjacency offsets decrease at %d", i);
     SRB_REQUIRE(std::isfinite(points[2 * i]) && std::isfinite(points[2 * i + 1]),
                 "samroad_labels_upload: point %d is not finite", i);
-    SRB_REQUIRE(std::isfinite(weights[i]) && weights[i] >= 0.0f,
-                "samroad_labels_upload: weight %d is negative or not finite", i);
+    // np.random.choice(p=w / w.sum()) refuses a window whose weights are all zero; the running sum would
+    // silently pick its last survivor, so every weight must be positive
+    SRB_REQUIRE(std::isfinite(weights[i]) && weights[i] > 0.0f,
+                "samroad_labels_upload: weight %d is not a positive finite number (got %g)", i,
+                static_cast<double>(weights[i]));
   }
   const int32_t m = adj_start[n_points];
   SRB_REQUIRE(m == 0 || adj != nullptr, "samroad_labels_upload: null adjacency");

@@ -266,10 +266,14 @@ def _positive_float(config, key) -> float:
 
 def label_config(config, image_size: int, margin: int) -> Dict:
     """The configuration keys the batches use, checked: PATCH_SIZE, TOPO_SAMPLE_NUM, MAX_NEIGHBOR_QUERIES
-    (1..32), ROAD_NMS_RADIUS, NEIGHBOR_RADIUS.  Raises ValueError without touching a GPU."""
+    (1..32), ROAD_NMS_RADIUS, NEIGHBOR_RADIUS (its BFS depth NEIGHBOR_RADIUS // 4 must fit an int32).  Raises
+    ValueError without touching a GPU."""
     c = dict(P=_positive_int(config, "PATCH_SIZE"), S=_positive_int(config, "TOPO_SAMPLE_NUM"),
              Np=_positive_int(config, "MAX_NEIGHBOR_QUERIES", 1, 32),
              r_nms=_positive_float(config, "ROAD_NMS_RADIUS"), r_nbr=_positive_float(config, "NEIGHBOR_RADIUS"))
+    if c["r_nbr"] // SUBDIVIDE_RESOLUTION > 2 ** 31 - 1:
+        raise ValueError(f"NEIGHBOR_RADIUS {c['r_nbr']!r} gives a BFS depth NEIGHBOR_RADIUS // "
+                         f"{SUBDIVIDE_RESOLUTION} beyond 2**31 - 1")
     if c["P"] + 2 * margin > image_size:
         raise ValueError(f"PATCH_SIZE {c['P']} with margin {margin} does not fit a {image_size}-pixel scene")
     return c

@@ -156,11 +156,11 @@ def make_road_graph(extent: int, seed: int = 0, spacing: int = 48, lo: int = 16)
 
 
 def write_label_scenes(root: str, dataset: str, tiles, size: int, seed: int = 0, extent: int = None,
-                       empty=()) -> None:
+                       empty=(), spacing: int = 48) -> None:
     """Scene files of `tiles` in the reference's cityscale / spacenet layout under root (dataset.py:311-340):
     a seeded RGB PNG, binary keypoint / road mask PNGs (0 / 255) and the pickled ground-truth graph (an empty
     dict for the tiles in `empty`).  Graph coordinates are (row, col) for cityscale and the spacenet convention
-    (x = col, y = 400 - row) is applied by the dataset."""
+    (x = col, y = 400 - row) is applied by the dataset.  `spacing` is the street grid's (make_road_graph)."""
     import os
     import pickle
 
@@ -179,6 +179,6 @@ def write_label_scenes(root: str, dataset: str, tiles, size: int, seed: int = 0,
         cv2.imwrite(os.path.join(root, pat[0].format(t)), rgb[:, :, ::-1])
         cv2.imwrite(os.path.join(root, pat[1].format(t)), kp)
         cv2.imwrite(os.path.join(root, pat[2].format(t)), road)
-        adj = {} if t in empty else make_road_graph(extent or size - 16, seed=seed + k)
+        adj = {} if t in empty else make_road_graph(extent or size - 16, seed=seed + k, spacing=spacing)
         with open(os.path.join(root, pat[3].format(t)), "wb") as f:
             pickle.dump(adj, f)

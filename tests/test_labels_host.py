@@ -14,6 +14,7 @@ from sam_road_b200 import dataset as D
 from sam_road_b200 import synth
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "labels_synth.npz")
+GOLDEN_EDGES = os.path.join(os.path.dirname(__file__), "golden", "labels_edges.npz")
 
 
 @pytest.fixture(scope="module")
@@ -150,7 +151,8 @@ def test_max_window_points_is_exact():
 
 @pytest.mark.parametrize("key,value", [("MAX_NEIGHBOR_QUERIES", 0), ("MAX_NEIGHBOR_QUERIES", 33),
                                        ("TOPO_SAMPLE_NUM", 0), ("ROAD_NMS_RADIUS", -1.0),
-                                       ("NEIGHBOR_RADIUS", float("nan")), ("PATCH_SIZE", 4096),
+                                       ("NEIGHBOR_RADIUS", float("nan")), ("NEIGHBOR_RADIUS", 2.0 ** 33),
+                                       ("PATCH_SIZE", 4096),
                                        ("PATCH_SIZE", 2.5)])
 def test_bad_config_is_refused(key, value):
     cfg = dict(PATCH_SIZE=512, TOPO_SAMPLE_NUM=512, MAX_NEIGHBOR_QUERIES=16, ROAD_NMS_RADIUS=16, NEIGHBOR_RADIUS=64)
@@ -178,10 +180,81 @@ def test_c_abi_refuses_bad_label_config_before_any_device_call():
                 max_patch_points=100, road_nms_radius=16.0, neighbor_radius=64.0)
     for key, value, msg in (("max_neighbor_queries", 33, "MAX_NEIGHBOR_QUERIES"),
                             ("patch_size", 2000, "does not fit"), ("road_nms_radius", 0.0, "ROAD_NMS_RADIUS"),
-                            ("max_patch_points", 0, "max_patch_points"), ("topo_sample_num", 0, "TOPO_SAMPLE_NUM")):
+                            ("max_patch_points", 0, "max_patch_points"), ("topo_sample_num", 0, "TOPO_SAMPLE_NUM"),
+                            ("neighbor_radius", 2.0 ** 33, "BFS depth")):
         cfg = _lib.SamRoadLabelCfg(**dict(good, **{key: value}))
         h = C.c_void_p()
         assert lib.samroad_labels_create(0, C.byref(cfg), C.byref(h)) == 2
         assert msg in _lib.last_error() and not h.value
     assert lib.samroad_labels_batch(None, 1, 0, None, *([None] * 7), None, None) != 0
     assert "null labels object" in _lib.last_error()
+
+
+def test_oracle_reproduces_reference_at_edge_settings(scene):
+    """labels_edges.npz (tools/make_golden.py --labels-edges): the unmodified reference at NMS / neighbour radii
+    10 / 30 (depth 7) with Np 4 and S 5, at NEIGHBOR_RADIUS 3 (depth 3 // 4 = 0) with S 3, and one PATCH_SIZE 1024
+    window.  The oracle's depth rule (r // 4 on a float) and its inclusive NMS / exclusive kNN radius tests must
+    reproduce scipy's samples there, not only at 16 / 64."""
+    fx = dict(np.load(GOLDEN_EDGES))
+    assert int(fx["extent"]) == 360
+    seen = set()
+    for g in (str(v) for v in fx["groups"]):
+        c = dict(zip([str(k) for k in fx[f"{g}/cfg_keys"]], fx[f"{g}/cfg"].tolist()))
+        lc = dict(P=int(c["PATCH_SIZE"]), S=int(c["TOPO_SAMPLE_NUM"]), Np=int(c["MAX_NEIGHBOR_QUERIES"]),
+                  r_nms=c["ROAD_NMS_RADIUS"], r_nbr=c["NEIGHBOR_RADIUS"])
+        for k, (x0, y0, rot) in enumerate(fx[f"{g}/patches"].tolist()):
+            rec = {key.split("/", 2)[2]: v for key, v in fx.items() if key.startswith(f"{g}/p{k}/")}
+            o = LO.sample_patch(scene, x0, y0, rot, lc, dict(score=rec["score"], source_index=rec["source_index"],
+                                                             noise=rec["noise"]), ties="scipy")
+            assert np.array_equal(o["candidates"], rec["candidates"]), (g, k)
+            assert np.array_equal(o["survivors"], rec["survivors"]), (g, k)
+            assert np.array_equal(o["points"], rec["points"].astype(np.float32)), (g, k)
+            for key in ("pairs", "connected", "valid"):
+                assert o[key].shape == (lc["S"], lc["Np"]) + (() if key != "pairs" else (2,))
+                assert np.array_equal(o[key], rec[key]), (g, k, key)
+            seen.add((g, int(rec["valid"].sum()) > 0, int(rec["connected"].sum()) > 0))
+    # radii 10 / 30 and P 1024 have connected and unconnected targets; radius 3 has none in range
+    assert {("r10_30", True, True), ("p1024", True, True), ("r3", False, False)} <= seen
+    r = dict(zip([str(k) for k in fx["r10_30/cfg_keys"]], fx["r10_30/cfg"].tolist()))
+    assert r["NEIGHBOR_RADIUS"] // 4 == 7 and r["ROAD_NMS_RADIUS"] == 10
+
+
+# P with an inexact float32 np.linalg.inv of the reference's centring matrix (DESIGN.md §13): there the reference's
+# point transform may differ from the device's float64 one by one float64 ulp before the float32 rounding
+INEXACT_TRANSFORM_P = (1488, 1584, 1680, 1872)
+
+
+def _transform_like_device(pts, x0, y0, P, rot, noise):
+    c = 0.5 * P
+    x, y = (pts[:, 0] - x0) - c, (pts[:, 1] - y0) - c
+    for _ in range(rot):
+        x, y = y, -x
+    return np.stack([(x + c) + noise[:, 0], (y + c) + noise[:, 1]], 1)
+
+
+def test_point_transform_is_exact_except_listed_patch_sizes():
+    """The float64 transform of labels.cu (subtract, rotate, add) equals the reference's matrix product with the
+    float32 inverse of the centring matrix for every multiple of 16 up to 1920 except INEXACT_TRANSFORM_P."""
+    inexact = []
+    rng = np.random.RandomState(3)
+    for P in range(16, 1921, 16):
+        t = np.array([[1, 0, -0.5 * P], [0, 1, -0.5 * P], [0, 0, 1]], dtype=np.float32)
+        exact_inv = np.array([[1, 0, 0], [0, 1, 0], [0.5 * P, 0.5 * P, 1]], dtype=np.float32)
+        if not np.array_equal(np.linalg.inv(t.T), exact_inv):
+            inexact.append(P)
+            continue
+        x0, y0 = 64, 37
+        pts = np.concatenate([rng.rand(64, 2) * P, rng.randint(0, P + 1, (16, 2))]) + [x0, y0]
+        noise = rng.randn(pts.shape[0], 2)
+        for rot in range(4):
+            want = LO.transform_points(pts, x0, y0, P, rot, noise)
+            assert np.array_equal(_transform_like_device(pts, x0, y0, P, rot, noise), want), (P, rot)
+    assert tuple(inexact) == INEXACT_TRANSFORM_P
+    assert not {256, 512, 1024} & set(inexact)
+    P = INEXACT_TRANSFORM_P[0]   # the documented bound where the inverse is inexact: one float32 ulp
+    pts = rng.rand(4096, 2) * P
+    noise = rng.randn(4096, 2)
+    for rot in range(4):
+        a = _transform_like_device(pts, 0, 0, P, rot, noise).astype(np.float32)
+        b = LO.transform_points(pts, 0, 0, P, rot, noise).astype(np.float32)
+        assert (np.abs(a - b) <= np.spacing(np.maximum(np.abs(a), np.abs(b)))).all(), rot

@@ -287,16 +287,18 @@ class _IndexLog(np.ndarray):
         return np.asarray(self).__getitem__(key)
 
 
-def labels_fixture():
-    """GraphLabelGenerator.__init__ / sample_patch (dataset.py:71-231) of the unmodified reference on a synthetic
-    graph.  The draws are recorded by wrapping np.random.uniform / choice / normal and graph_utils.nms_points from
-    outside; the candidate and source ids by indexing a logging view of subdivide_points."""
+def _reference_samples(cfg_dict, patches, seed):
+    """sample_patch of the unmodified reference GraphLabelGenerator (dataset.py:71-231) on the synthetic graph of
+    label_scene() with the configuration cfg_dict, at patches [(x0, y0, rot)], after np.random.seed(seed).  The draws
+    are recorded by wrapping np.random.uniform / choice / normal and graph_utils.nms_points from outside; the
+    candidate and source ids by indexing a logging view of subdivide_points.  Every sample is checked against the
+    oracle (ties="scipy") before it is returned.  Returns (generator, precompute, {"p<k>/<key>": array})."""
     from oracle import label_oracle as LO
     from sam_road_b200 import dataset as D
     ref = ref_loader.load_reference_dataset()
     gu = sys.modules["graph_utils"]
     adj, transform = label_scene()
-    cfg = ref_loader.AttrDict(LABEL_CFG)
+    cfg = ref_loader.AttrDict(cfg_dict)
     gen = ref.GraphLabelGenerator(cfg, adj, transform)
     mine = D.precompute_scene(adj, transform)
     ref_cross = np.array(gen.crossover_points, dtype=np.float64).reshape(-1, 2)
@@ -305,14 +307,11 @@ def labels_fixture():
     assert set(np.nonzero(mine.excluded)[0].tolist()) == set(gen.exclude_indices), "excluded set differs"
     assert np.array_equal(gen.nms_score_override, mine.nms_override) and np.array_equal(gen.sample_weights,
                                                                                           mine.weights)
-    out = dict(cfg=np.array([LABEL_CFG[k] for k in sorted(LABEL_CFG)]), cfg_keys=np.array(sorted(LABEL_CFG)),
-               extent=LABEL_EXTENT, subdivide_points=gen.subdivide_points, crossovers=ref_cross,
-               excluded=np.array(sorted(gen.exclude_indices), dtype=np.int32),
-               nms_override=gen.nms_score_override, sample_weights=gen.sample_weights,
-               patches=np.array(LABEL_PATCHES, dtype=np.int32))
-    log = gen.subdivide_points.view(_IndexLog)
+    points = gen.subdivide_points
+    log = points.view(_IndexLog)
     log.log = []
     gen.subdivide_points = log
+    out = {}
     drawn = {}
     real = {k: getattr(np.random, k) for k in ("uniform", "choice", "normal")}
     real_nms = gu.nms_points
@@ -329,15 +328,15 @@ def labels_fixture():
         drawn["kept"] = np.array(r[1])
         return r
 
-    P = LABEL_CFG["PATCH_SIZE"]
-    lc = dict(P=P, S=LABEL_CFG["TOPO_SAMPLE_NUM"], Np=LABEL_CFG["MAX_NEIGHBOR_QUERIES"],
-              r_nms=LABEL_CFG["ROAD_NMS_RADIUS"], r_nbr=LABEL_CFG["NEIGHBOR_RADIUS"])
-    np.random.seed(1234)
+    P = cfg_dict["PATCH_SIZE"]
+    lc = dict(P=P, S=cfg_dict["TOPO_SAMPLE_NUM"], Np=cfg_dict["MAX_NEIGHBOR_QUERIES"],
+              r_nms=cfg_dict["ROAD_NMS_RADIUS"], r_nbr=cfg_dict["NEIGHBOR_RADIUS"])
+    np.random.seed(seed)
     try:
         for name in real:
             setattr(np.random, name, wrap(name))
         gu.nms_points = nms_rec
-        for k, (x0, y0, rot) in enumerate(LABEL_PATCHES):
+        for k, (x0, y0, rot) in enumerate(patches):
             drawn.clear()
             log.log.clear()
             pts, samples = gen.sample_patch(((x0, y0), (x0 + P, y0 + P)), rot)
@@ -361,21 +360,69 @@ def labels_fixture():
                 assert np.array_equal(o[key], rec[key]), f"patch {k}: {key}"
             for key, v in rec.items():
                 out[f"p{k}/{key}"] = v
-            print(f"labels patch {k} (x0={x0}, y0={y0}, rot={rot}): {len(rec.get('candidates', []))} candidates, "
-                  f"{len(rec.get('survivors', []))} survivors, {int(rec['valid'].sum())} valid pairs, "
+            print(f"labels patch {k} (x0={x0}, y0={y0}, rot={rot}, P={P}): {len(rec.get('candidates', []))} "
+                  f"candidates, {len(rec.get('survivors', []))} survivors, {int(rec['valid'].sum())} valid pairs, "
                   f"{int(rec['connected'].sum())} connected; oracle (ties='scipy') identical")
     finally:
         for name, fn in real.items():
             setattr(np.random, name, fn)
         gu.nms_points = real_nms
+        gen.subdivide_points = points
+    return gen, mine, out
+
+
+def labels_fixture():
+    """labels_synth.npz: the reference's precompute and samples on the synthetic graph at LABEL_CFG."""
+    gen, _, samples = _reference_samples(LABEL_CFG, LABEL_PATCHES, 1234)
+    ref_cross = np.array(gen.crossover_points, dtype=np.float64).reshape(-1, 2)
+    out = dict(cfg=np.array([LABEL_CFG[k] for k in sorted(LABEL_CFG)]), cfg_keys=np.array(sorted(LABEL_CFG)),
+               extent=LABEL_EXTENT, subdivide_points=gen.subdivide_points, crossovers=ref_cross,
+               excluded=np.array(sorted(gen.exclude_indices), dtype=np.int32),
+               nms_override=gen.nms_score_override, sample_weights=gen.sample_weights,
+               patches=np.array(LABEL_PATCHES, dtype=np.int32))
+    out.update(samples)
     path = os.path.join(OUT, "labels_synth.npz")
     np.savez_compressed(path, **out)
     print(f"{path}: {os.path.getsize(path)} bytes, {len(ref_cross)} crossover points "
           f"({len(np.unique(ref_cross, axis=0))} distinct), {len(gen.exclude_indices)} excluded")
 
 
+# labels_edges.npz: the same synthetic graph at settings the benched configurations never use.  Each group is
+# (configuration, patches (x0, y0, rot), np.random seed).
+LABEL_EDGE_GROUPS = {
+    # ROAD_NMS_RADIUS 10 (cell = radius, inexact division), NEIGHBOR_RADIUS 30 (depth 7, not a multiple of 4),
+    # Np 4 and S 5 (not a multiple of the pair kernel's 4 warps)
+    "r10_30": (dict(PATCH_SIZE=256, TOPO_SAMPLE_NUM=5, MAX_NEIGHBOR_QUERIES=4, NEIGHBOR_RADIUS=30,
+                    ROAD_NMS_RADIUS=10), ((40, 20, 0), (96, 64, 1), (100, 100, 2), (60, 30, 3)), 4321),
+    # NEIGHBOR_RADIUS 3: depth 3 // 4 = 0, nothing is expanded; the kNN radius is below the NMS radius
+    "r3": (dict(PATCH_SIZE=256, TOPO_SAMPLE_NUM=3, MAX_NEIGHBOR_QUERIES=4, NEIGHBOR_RADIUS=3,
+                ROAD_NMS_RADIUS=2), ((40, 20, 0), (96, 64, 3)), 4322),
+    # PATCH_SIZE 1024 at toponet_vitb_1024's radii and pair count; one window over the whole graph
+    "p1024": (dict(PATCH_SIZE=1024, TOPO_SAMPLE_NUM=64, MAX_NEIGHBOR_QUERIES=16, NEIGHBOR_RADIUS=64,
+                   ROAD_NMS_RADIUS=16), ((0, 0, 1),), 4323),
+}
+
+
+def labels_edges_fixture():
+    out = dict(extent=LABEL_EXTENT, groups=np.array(sorted(LABEL_EDGE_GROUPS)))
+    for name in sorted(LABEL_EDGE_GROUPS):
+        cfg, patches, seed = LABEL_EDGE_GROUPS[name]
+        _, _, samples = _reference_samples(cfg, patches, seed)
+        out[f"{name}/cfg"] = np.array([cfg[k] for k in sorted(cfg)], dtype=np.float64)
+        out[f"{name}/cfg_keys"] = np.array(sorted(cfg))
+        out[f"{name}/patches"] = np.array(patches, dtype=np.int32)
+        out.update({f"{name}/{k}": v for k, v in samples.items()})
+    path = os.path.join(OUT, "labels_edges.npz")
+    np.savez_compressed(path, **out)
+    print(f"{path}: {os.path.getsize(path)} bytes")
+
+
 def main():
     assert ref_loader.available(), "needs /root/reference"
+    if "--labels-edges" in sys.argv:  # the same at non-default radii, odd pair counts and PATCH_SIZE 1024
+        os.makedirs(OUT, exist_ok=True)
+        labels_edges_fixture()
+        return
     if "--labels" in sys.argv:        # GraphLabelGenerator / sample_patch on a synthetic graph
         os.makedirs(OUT, exist_ok=True)
         labels_fixture()
