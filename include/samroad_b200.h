@@ -363,6 +363,38 @@ int samroad_debug_labels_batch_draws(samroad_labels_t L, int B, int mode, uint64
                                      float* keypoint_mask, float* road_mask, float* points, int32_t* pairs,
                                      uint8_t* connected, uint8_t* valid, int32_t* n_points, void* stream);
 
+/* ---- the TOPO graph metric (sam_road_b200/topo_metric.py, DESIGN.md §14) ----
+ * A topo object holds one tile's two road graphs (0 ground truth, 1 proposal) as RoadGraph builds them
+ * (cityscale_metrics/topo/graph.py) and scores (GT, proposal) pairs as TOPOWithPairs does: per pair the three
+ * TOPOWalks, the candidate marble-hole edges and the two maximum matchings.  Capacities bound the device
+ * workspaces; a run that exceeds one is refused with an error naming the pair, never truncated.  Not
+ * thread-safe; one run at a time.  Synchronous (default stream). */
+typedef struct samroad_topo_ctx* samroad_topo_t;
+typedef struct SamRoadTopoCaps {
+  int32_t max_marbles;      /* marbles (or holes) one walk may place                            */
+  int32_t max_queue;        /* entries the FIFO of one walk may hold at once                     */
+  int32_t max_covered;      /* directed edges one walk may sample (its edge_covered entries)     */
+  int32_t max_candidates;   /* candidate marble-hole edges of one pair, per matching             */
+  int32_t slots;            /* pairs in flight on the device at once                             */
+} SamRoadTopoCaps;
+
+int samroad_topo_create(int device, const SamRoadTopoCaps* caps, samroad_topo_t* out);
+int samroad_topo_destroy(samroad_topo_t T);
+/* Copies one graph (host memory) to the device, replacing the previous graph of that kind.  latlon [n,2] float64
+ * (lat, lon) by node id; cos_lat [n] = math.cos(math.radians(lat)); link_start [n+1] / link: nodeLink, and
+ * rlink_start [n+1] / rlink: nodeLinkReverse, each node's list in the reference's order.  Refuses a coordinate
+ * that is not finite and an edge of length zero (naming it). */
+int samroad_topo_upload_graph(samroad_topo_t T, int which, int32_t n_nodes, const double* latlon,
+                              const double* cos_lat, const int32_t* link_start, const int32_t* link,
+                              const int32_t* rlink_start, const int32_t* rlink);
+/* Scores n_pairs pairs (host memory in and out).  pair_nodes [n,4] int32 (gpsn1, gpsn2, osmn1, osmn2): the
+ * proposal edge and the GT edge of each pair; pair_dists [n,4] float64 (gpsd1, gpsd2, osmd1, osmd2).  r, step and
+ * threshold as TOPOWithPairs takes them; cos40 = math.cos(math.radians(40)).  counts [n,6] int32 out: marbles,
+ * holes, bidirectional holes, the maximum matching of marbles to bidirectional holes (precision), that of holes
+ * to marbles (recall), and a status word that is 0 for every pair of a successful run. */
+int samroad_topo_run(samroad_topo_t T, int32_t n_pairs, const int32_t* pair_nodes, const double* pair_dists,
+                     double r, double step, double threshold, double cos40, int32_t* counts);
+
 /* Stream memory operations on a 32-bit flag word in device (or peer-mapped) memory, executed by the stream
  * front end without a kernel: an ordered write of `value`, and a wait until *addr >= value.  The exchange step
  * between ranks (sam_road_b200/exchange.py; no reference counterpart, the reference is single-GPU) builds its

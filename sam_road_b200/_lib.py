@@ -58,6 +58,16 @@ class SamRoadLabelCfg(C.Structure):
     ]
 
 
+class SamRoadTopoCaps(C.Structure):
+    _fields_ = [
+        ("max_marbles", C.c_int32),
+        ("max_queue", C.c_int32),
+        ("max_covered", C.c_int32),
+        ("max_candidates", C.c_int32),
+        ("slots", C.c_int32),
+    ]
+
+
 _vp, _i, _f, _d = C.c_void_p, C.c_int, C.c_float, C.c_double
 _ip = C.POINTER(C.c_int)
 _targs = C.POINTER(SamRoadTrainArgs)
@@ -115,6 +125,10 @@ SIGNATURES = {
                                   C.POINTER(C.c_int32), _vp]),
     "samroad_debug_labels_batch_draws": (_i, [_vp, _i, _i, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                               _vp, _vp, C.POINTER(C.c_int32), _vp]),
+    "samroad_topo_create": (_i, [_i, C.POINTER(SamRoadTopoCaps), C.POINTER(_vp)]),
+    "samroad_topo_destroy": (_i, [_vp]),
+    "samroad_topo_upload_graph": (_i, [_vp, _i, C.c_int32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "samroad_topo_run": (_i, [_vp, C.c_int32, _vp, _vp, _d, _d, _d, _d, _vp]),
     "samroad_stream_write_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_stream_wait_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_timing_enable": (_i, [_vp, _i]),

@@ -12,6 +12,7 @@ oracle against these files on any machine (no reference needed).
 from __future__ import annotations
 
 import ast
+import math
 import os
 import sys
 
@@ -417,8 +418,352 @@ def labels_edges_fixture():
     print(f"{path}: {os.path.getsize(path)} bytes")
 
 
+# ---- TOPO metric (cityscale_metrics/topo/*.py) ----------------------------------------------------------------------
+
+
+def topo_synth_tiles():
+    """Three synthetic (GT, proposal) adjacency dicts in the graph pickle format, in tile order.  Tile 0 stays within
+    1000 px of the top edge (r = 0.0015); tile 1 reaches x = 1250, so from it on the carried min_lat switches the
+    cityscale driver to r = 0.003; tile 2 is small again and still scored at r = 0.003."""
+    rng = np.random.default_rng(7)
+
+    def add(adj, a, b, two_way=True):
+        adj.setdefault(a, [])
+        adj.setdefault(b, [])
+        if b not in adj[a]:
+            adj[a].append(b)
+        if two_way and a not in adj[b]:
+            adj[b].append(a)
+
+    def street(adj, p, q, seg, two_way=True):
+        n = max(1, int(round(math.hypot(q[0] - p[0], q[1] - p[1]) / seg)))
+        pts = [(float(p[0] + (q[0] - p[0]) * k / n), float(p[1] + (q[1] - p[1]) * k / n)) for k in range(n + 1)]
+        for a, b in zip(pts, pts[1:]):
+            add(adj, a, b, two_way)
+
+    def grid(adj, x0, y0, nx, ny, sp, seg):
+        for i in range(nx):
+            street(adj, (x0 + i * sp, y0), (x0 + i * sp, y0 + (ny - 1) * sp), seg)
+        for j in range(ny):
+            street(adj, (x0, y0 + j * sp), (x0 + (nx - 1) * sp, y0 + j * sp), seg)
+
+    def proposal(gt, drop, shift, extra, oneway):
+        prop = {}
+        keys = list(gt)
+        moved = {k: (k[0] + float(rng.integers(-shift, shift + 1)), k[1] + float(rng.integers(-shift, shift + 1)))
+                 for k in keys}
+        edges = [(a, b) for a in keys for b in gt[a]]
+        for (a, b) in edges:
+            if rng.random() < drop:
+                continue
+            add(prop, moved[a], moved[b], two_way=False)
+        for (a, b) in extra:
+            add(prop, a, b, two_way=rng.random() >= oneway)
+        return prop
+
+    tiles = []
+    # tile 0: a 4 x 4 grid of 90 px blocks, nodes every 30 px, an overpass (a diagonal with no shared node), two dead
+    # ends and a one-way street
+    gt = {}
+    grid(gt, 100.0, 100.0, 4, 4, 90.0, 30.0)
+    street(gt, (80.0, 95.0), (395.0, 410.0), 25.0)               # overpass: crosses the grid without a node
+    street(gt, (370.0, 190.0), (450.0, 190.0), 20.0)             # dead end
+    street(gt, (190.0, 370.0), (190.0, 440.0), 35.0)             # dead end
+    street(gt, (145.0, 100.0), (145.0, 370.0), 45.0, two_way=False)   # one-way
+    prop = proposal(gt, 0.15, 7, [((300.0, 300.0), (330.0, 360.0)), ((120.0, 400.0), (160.0, 430.0)),
+                              ((250.0, 120.0), (250.0, 260.0)), ((160.0, 200.0), (240.0, 215.0))], 0.5)
+    tiles.append((gt, prop))
+    # tile 1: a long arterial to x = 1250 and a small grid
+    gt = {}
+    street(gt, (100.0, 150.0), (1250.0, 150.0), 50.0)
+    grid(gt, 200.0, 200.0, 3, 3, 100.0, 25.0)
+    street(gt, (200.0, 150.0), (200.0, 200.0), 25.0)
+    prop = proposal(gt, 0.1, 9, [((400.0, 400.0), (460.0, 400.0)), ((260.0, 230.0), (330.0, 260.0))], 0.0)
+    tiles.append((gt, prop))
+    # tile 2: a 3 x 3 grid, the proposal equal to the GT
+    gt = {}
+    grid(gt, 120.0, 120.0, 3, 3, 80.0, 40.0)
+    prop = proposal(gt, 0.0, 0, [], 0.0)
+    tiles.append((gt, prop))
+    # tile 3: two parallel streets 12 px apart joined at both ends, with two spurs; the proposal draws one street between them with
+    # spurious side branches, so nearby starting points compete for the same proposal edges with precisions below
+    # 0.9 and TOPO121 drops some of them
+    gt = {}
+    street(gt, (200.0, 100.0), (200.0, 420.0), 20.0)
+    street(gt, (212.0, 100.0), (212.0, 420.0), 20.0)
+    street(gt, (200.0, 100.0), (212.0, 100.0), 12.0)
+    street(gt, (200.0, 420.0), (212.0, 420.0), 12.0)
+    street(gt, (212.0, 260.0), (270.0, 260.0), 29.0)             # dead-end spurs: degree-3 nodes start the chains
+    street(gt, (200.0, 200.0), (160.0, 200.0), 20.0)
+    prop = {}
+    street(prop, (206.0, 100.0), (206.0, 420.0), 20.0)
+    for y in (160.0, 260.0, 360.0):
+        street(prop, (206.0, y), (150.0, y + 30.0), 20.0)
+        street(prop, (206.0, y + 20.0), (280.0, y + 50.0), 20.0)
+    tiles.append((gt, prop))
+    # tile 4 (spacenet only): a GT with no starting point (one 3 px edge), where spacenet's topo.py writes its
+    # zeros line; cityscale's divides by the start count first and raises
+    tiles.append(({(300.0, 300.0): [(300.0, 303.0)]}, {(300.0, 300.0): [(300.0, 340.0)]}))
+    return tiles
+
+
+def adj_to_arrays(adj):
+    keys = np.array([k for k in adj], dtype=np.float64).reshape(-1, 2)
+    cnt = np.array([len(v) for v in adj.values()], dtype=np.int32)
+    nb = np.array([n for v in adj.values() for n in v], dtype=np.float64).reshape(-1, 2)
+    return keys, cnt, nb
+
+
+def _load_reference_topo():
+    import types
+    ref_loader._install_graph_shims()
+    if "svgwrite" not in sys.modules and not ref_loader._has("svgwrite"):
+        # showTOPO's import: spacenet's topo.py renders coverage SVGs; here every drawing call does nothing
+        svg = types.ModuleType("svgwrite")
+
+        class Drawing:
+            def __init__(self, *a, **k):
+                pass
+
+            def __getattr__(self, name):
+                return lambda *a, **k: None
+
+        svg.Drawing = Drawing
+        sys.modules["svgwrite"] = svg
+    if "hopcroftkarp" not in sys.modules and not ref_loader._has("hopcroftkarp"):
+        import networkx as nx
+        hk = types.ModuleType("hopcroftkarp")
+
+        class HopcroftKarp:
+            """hopcroftkarp.HopcroftKarp(graph).maximum_matching(): a maximum matching as a dict holding both
+            directions (left -> right and right -> left), as the library documents."""
+
+            def __init__(self, graph):
+                self.graph = graph
+
+            def maximum_matching(self):
+                g = nx.Graph()
+                left = [("L", k) for k in self.graph]
+                g.add_nodes_from(left, bipartite=0)
+                for k, vs in self.graph.items():
+                    for v in vs:
+                        g.add_edge(("L", k), ("R", v))
+                m = nx.bipartite.hopcroft_karp_matching(g, top_nodes=left)
+                out = {a[1]: b[1] for a, b in m.items()}
+                HopcroftKarp.sizes.append(len(out) // 2)
+                return out
+
+        HopcroftKarp.sizes = []
+        hk.HopcroftKarp = HopcroftKarp
+        sys.modules["hopcroftkarp"] = hk
+    tdir = os.path.join(ref_loader.REF_ROOT, "cityscale_metrics", "topo")
+    if tdir not in sys.path:
+        sys.path.insert(0, tdir)
+    import graph as ref_graph  # noqa: the reference's cityscale_metrics/topo/graph.py
+    import topo as ref_topo    # noqa: the reference's cityscale_metrics/topo/topo.py
+    # spacenet_metrics/topo/topo.py under its own name; its graph.py and showTOPO.py are the same files as
+    # cityscale's, so its `import graph` / `import showTOPO` resolve to the modules above
+    if "spacenet_topo" not in sys.modules:
+        import importlib.util
+        spec = importlib.util.spec_from_file_location(
+            "spacenet_topo", os.path.join(ref_loader.REF_ROOT, "spacenet_metrics", "topo", "topo.py"))
+        mod = importlib.util.module_from_spec(spec)
+        sys.modules["spacenet_topo"] = mod
+        spec.loader.exec_module(mod)
+    topos = {"cityscale": ref_topo, "spacenet": sys.modules["spacenet_topo"]}
+    return ref_graph, topos, sys.modules["hopcroftkarp"].HopcroftKarp
+
+
+def _reference_topo_run(tiles, dataset, workdir):
+    """main.py's loop (cityscale or spacenet) over `tiles`, restated around the reference's own graph.RoadGraph and
+    topo.py functions; returns per-tile records."""
+    import contextlib
+    import io
+    import pickle
+    splfy, topos, HK = _load_reference_topo()
+    topo = topos[dataset]
+    lat_top_left, lon_top_left = 41.0, -71.0
+    g = dict(min_lat=41.0, max_lon=-71.0)
+    walk_lens = []
+    orig_walk = splfy.RoadGraph.TOPOWalk
+
+    def walk(self, *a, **k):
+        out = orig_walk(self, *a, **k)
+        walk_lens.append(len(out))
+        return out
+
+    seen_results = []
+    orig_121 = topo.TOPO121
+
+    def t121(res, rg):
+        seen_results.append(list(res))
+        return orig_121(res, rg)
+
+    splfy.RoadGraph.TOPOWalk = walk
+    topo.TOPO121 = t121
+    records = []
+    try:
+        for t, (map1, map2) in enumerate(tiles):
+            def xy2latlon(x, y):
+                lat = lat_top_left - x * 1.0 / 111111.0
+                lon = lon_top_left + (y * 1.0 / 111111.0) / math.cos(math.radians(lat_top_left))
+                return lat, lon
+
+            def create_graph(m):
+                graph = splfy.RoadGraph()
+                nid = 0
+                idmap = {}
+                for k, v in m.items():
+                    n1 = k
+                    lat1, lon1 = xy2latlon(n1[0], n1[1])
+                    if lat1 < g["min_lat"]:
+                        g["min_lat"] = lat1
+                    if lon1 > g["max_lon"]:
+                        g["max_lon"] = lon1
+                    for n2 in v:
+                        lat2, lon2 = xy2latlon(n2[0], n2[1])
+                        if n1 in idmap:
+                            id1 = idmap[n1]
+                        else:
+                            id1 = nid
+                            idmap[n1] = nid
+                            nid = nid + 1
+                        if n2 in idmap:
+                            id2 = idmap[n2]
+                        else:
+                            id2 = nid
+                            idmap[n2] = nid
+                            nid = nid + 1
+                        graph.addEdge(id1, lat1, lon1, id2, lat2, lon2)
+                graph.ReverseDirectionLink()
+                for node in graph.nodes.keys():
+                    graph.nodeScore[node] = 100
+                for edge in graph.edges.keys():
+                    graph.edgeScore[edge] = 100
+                return graph
+
+            output = os.path.join(workdir, "results", "topo", "%d.txt" % t)
+            os.makedirs(os.path.dirname(output), exist_ok=True)
+            with contextlib.redirect_stdout(io.StringIO()):
+                graph_gt = create_graph(map1)
+                graph_prop = create_graph(map2)
+                region = [g["min_lat"] - 300 * 1.0 / 111111.0, lon_top_left - 500 * 1.0 / 111111.0,
+                          lat_top_left + 300 * 1.0 / 111111.0, g["max_lon"] + 500 * 1.0 / 111111.0]
+                graph_gt.region = region
+                graph_prop.region = region
+                losm = topo.TOPOGenerateStartingPoints(graph_gt, region=region, image="NULL", check=False,
+                                                       direction=False, metaData=None)
+                lmap = topo.TOPOGeneratePairs(graph_prop, graph_gt, losm, threshold=0.00010, region=region)
+                if dataset == "cityscale":
+                    r = 0.00300
+                    if lat_top_left - g["min_lat"] < 0.01000:
+                        r = 0.00150
+                else:
+                    r = 0.00150
+                del walk_lens[:], seen_results[:], HK.sizes[:]
+                kept = topo.TOPOWithPairs(graph_prop, graph_gt, lmap, losm, r=r, step=0.00005, threshold=0.00010,
+                                          outputfile=output, one2oneMatching=True, metaData=None)
+            pickle.dump([losm, kept, region], open(output.replace('txt', 'topo.p'), 'wb'))
+            # per pair: 3 walks and the precision matching, then the recall matching unless the pair was skipped
+            counts, sizes, w = [], list(HK.sizes), list(walk_lens)
+            for _ in lmap:
+                nm, nh, nhb = w[:3]
+                del w[:3]
+                mp = sizes.pop(0)
+                mr = sizes.pop(0) if nm and nh else -1
+                counts.append([nm, nh, nhb, mp, mr])
+            with open(output) as f:
+                text = f.read()
+            records.append(dict(r=r, region=region, losm=losm, lmap=lmap, kept=kept, results=seen_results[0],
+                                counts=counts, text=text))
+    finally:
+        splfy.RoadGraph.TOPOWalk = orig_walk
+        topo.TOPO121 = orig_121
+    return records
+
+
+def _reference_aggregate(workdir, dataset, order):
+    """The dataset's topo.py, run as it lies with os.listdir pinned to `order` (its own order is the file system's)."""
+    import contextlib
+    import io
+    import runpy
+    script = os.path.join(ref_loader.REF_ROOT, f"{dataset}_metrics", "topo.py")
+    run_dir = os.path.join(workdir, "cwd")
+    os.makedirs(run_dir, exist_ok=True)
+    saved = (sys.argv, os.getcwd(), os.listdir)
+    rel = os.path.relpath(workdir, os.path.dirname(run_dir))
+    sys.argv = [script, "-savedir", rel]
+    os.chdir(run_dir)
+    os.listdir = lambda p: list(order)
+    try:
+        with contextlib.redirect_stdout(io.StringIO()):
+            runpy.run_path(script, run_name="__main__")
+    finally:
+        sys.argv, _, os.listdir = saved
+        os.chdir(saved[1])
+    path = os.path.join(workdir, "score", "topo.json") if dataset == "cityscale" else os.path.join(workdir, "topo.json")
+    with open(path) as f:
+        return f.read()
+
+
+def topo_fixture():
+    import tempfile
+    from oracle import topo_oracle
+    from sam_road_b200 import topo_metric as TM
+    tiles = topo_synth_tiles()
+    out = {}
+    for t, (gt, prop) in enumerate(tiles):
+        for name, adj in (("gt", gt), ("prop", prop)):
+            k, c, n = adj_to_arrays(adj)
+            out[f"tile{t}/{name}_keys"], out[f"tile{t}/{name}_cnt"], out[f"tile{t}/{name}_nbrs"] = k, c, n
+    for dataset in ("cityscale", "spacenet"):
+        with tempfile.TemporaryDirectory() as wd:
+            dtiles = tiles if dataset == "spacenet" else tiles[:4]
+            recs = _reference_topo_run(dtiles, dataset, wd)
+            order = ["%d.txt" % t for t in range(len(dtiles))] + ["%d.topo.p" % t for t in range(len(dtiles))]
+            js = _reference_aggregate(wd, dataset, order)
+        state = TM.TopoState()
+        for t, rec in enumerate(recs):
+            p, rr, d = TM.topo_tile(tiles[t][0], tiles[t][1], state, dataset, scorer=topo_oracle.scorer)
+            mine = [tuple(x) for x in d.results]
+            assert d.r == rec["r"] and d.region == rec["region"], (dataset, t)
+            assert d.starts == rec["losm"] and d.pairs == rec["lmap"], (dataset, t)
+            ref_counts = np.array(rec["counts"], dtype=np.int64).reshape(-1, 5)
+            mc = np.asarray(d.counts, dtype=np.int64).reshape(-1, 6)[:, :5]
+            defined = ref_counts[:, 4] >= 0
+            assert np.array_equal(ref_counts[:, :4], mc[:, :4]) and np.array_equal(ref_counts[defined, 4],
+                                                                                   mc[defined, 4]), (dataset, t)
+            assert mine == [tuple(x) for x in rec["results"]], (dataset, t)
+            assert [tuple(x) for x in d.kept] == [tuple(x) for x in rec["kept"]], (dataset, t)
+            assert "".join(d.lines) == rec["text"], (dataset, t)
+            if t == 3:   # the TOPO121 tile: the reference drops some scored starting points
+                assert len(rec["kept"]) < len(rec["results"]), (dataset, len(rec["kept"]), len(rec["results"]))
+            if t == 4:   # spacenet's no-starting-point tile: the zeros line
+                assert rec["text"] == "0 0 0 0\n", rec["text"]
+            pre = f"{dataset}/tile{t}/"
+            out[pre + "r"] = np.float64(rec["r"])
+            out[pre + "region"] = np.array(rec["region"], dtype=np.float64)
+            out[pre + "starts"] = np.array(rec["losm"], dtype=np.float64).reshape(-1, 6)
+            out[pre + "pair_keys"] = np.array(list(rec["lmap"]), dtype=np.int64)
+            out[pre + "pairs"] = np.array(list(rec["lmap"].values()), dtype=np.float64).reshape(-1, 7)
+            out[pre + "counts"] = ref_counts
+            out[pre + "results"] = np.array(rec["results"], dtype=np.float64).reshape(-1, 8)
+            out[pre + "kept"] = np.array(rec["kept"], dtype=np.float64).reshape(-1, 8)
+            out[pre + "text"] = np.array(rec["text"])
+            print(f"{dataset} tile {t}: r={rec['r']} starts={len(rec['losm'])} pairs={len(rec['lmap'])} "
+                  f"scored={len(rec['results'])} kept={len(rec['kept'])} last={rec['text'].splitlines()[-1]!r}")
+        out[f"{dataset}/topo_json"] = np.array(js)
+    path = os.path.join(OUT, "topo_synth.npz")
+    np.savez_compressed(path, **out)
+    print(f"{path}: {os.path.getsize(path)} bytes")
+
+
 def main():
     assert ref_loader.available(), "needs /root/reference"
+    if "--topo" in sys.argv:          # the TOPO metric on three synthetic tiles, both drivers and aggregators
+        os.makedirs(OUT, exist_ok=True)
+        topo_fixture()
+        return
     if "--labels-edges" in sys.argv:  # the same at non-default radii, odd pair counts and PATCH_SIZE 1024
         os.makedirs(OUT, exist_ok=True)
         labels_edges_fixture()
