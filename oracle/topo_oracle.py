@@ -18,8 +18,13 @@ def _dist(p1, p2):
     return math.sqrt(a * a + b * b)
 
 
-def topo_walk(g, nid1, nid2, dist1, dist2, r, step, bidirection=False):
-    """RoadGraph.TOPOWalk(1, step, r, direction=False, newstyle=True, nid1, nid2, dist1, dist2, bidirection)."""
+def topo_walk(g, nid1, nid2, dist1, dist2, r, step, bidirection=False, stats=None):
+    """RoadGraph.TOPOWalk(1, step, r, direction=False, newstyle=True, nid1, nid2, dist1, dist2, bidirection).
+
+    `stats`, when a dict, receives what the device's capacities are measured in: `marbles` (twins included),
+    `queue` (the most entries waiting at once, counted as an entry is pushed), `pushes` (all entries ever queued),
+    `covered` (distinct directed edges in the covered map) and `lowered` (times a node that already had a distance
+    was expanded again at a smaller one)."""
     mables, seen = [], set()
 
     def add(t, twin):
@@ -51,6 +56,7 @@ def topo_walk(g, nid1, nid2, dist1, dist2, r, step, bidirection=False):
     dmap, covered = {}, {}
     queue = [(nid1, -1, dist1), (nid2, -1, dist2)]
     head = 0
+    high, lowered = 2, 0
     while head < len(queue):
         cur, prev, dist = queue[head]
         head += 1
@@ -61,6 +67,7 @@ def topo_walk(g, nid1, nid2, dist1, dist2, r, step, bidirection=False):
                 continue
         if dist > r:
             continue
+        lowered += cur in dmap
         dmap[cur] = dist
         done = []
         lat1, lon1 = g.nodes[cur]
@@ -73,6 +80,7 @@ def topo_walk(g, nid1, nid2, dist1, dist2, r, step, bidirection=False):
             c = step * math.ceil(dist / step) - dist
             if old + l < r:
                 queue.append((nx, cur, dist + l))
+                high = max(high, len(queue) - head)
                 continue
             start_lim = covered.get((cur, nx), 0)
             end_lim = l - covered[(nx, cur)] if (nx, cur) in covered else l
@@ -91,6 +99,9 @@ def topo_walk(g, nid1, nid2, dist1, dist2, r, step, bidirection=False):
                 c += step
             covered[(cur, nx)] = c - step
             queue.append((nx, cur, dist + l))
+            high = max(high, len(queue) - head)
+    if stats is not None:
+        stats.update(marbles=len(mables), queue=high, pushes=len(queue), covered=len(covered), lowered=lowered)
     return mables
 
 
@@ -127,32 +138,77 @@ def candidate_graph(left, right, left_is_marble, threshold):
     return out
 
 
+def candidate_graph_boxed(left, right, left_is_marble, threshold):
+    """candidate_graph with the box test of a whole right list at once.  The box test is float64 adds and
+    comparisons, which numpy rounds as Python does; the distance and angle tests of the few survivors stay scalar
+    (math.cos), so the result is candidate_graph's."""
+    out = {}
+    if not left or not right:
+        return out
+    rr = threshold * 1.8
+    ra = np.array([(b[0], b[1]) for b in right], dtype=np.float64)
+    # the left item is the query in both loops (a marble for precision, a hole for recall): its box is +-rr, the
+    # indexed right point's +-0.00001
+    for a in left:
+        hit = (ra[:, 0] - 0.00001 <= a[0] + rr) & (ra[:, 0] + 0.00001 >= a[0] - rr) & \
+              (ra[:, 1] - 0.00001 <= a[1] + rr) & (ra[:, 1] + 0.00001 >= a[1] - rr)
+        for j in np.nonzero(hit)[0].tolist():
+            b = right[j]
+            ok = is_candidate(a, b, True, threshold) if left_is_marble else is_candidate(b, a, False, threshold)
+            if ok:
+                out.setdefault(a, set()).add(j)
+    return out
+
+
 def matching_size(adj: dict) -> int:
-    """Size of a maximum matching of a bipartite graph {left: iterable of right} (Kuhn's augmenting paths)."""
+    """Size of a maximum matching of a bipartite graph {left: iterable of right}: Kuhn's augmenting paths, one
+    depth-first search per left vertex on an explicit stack (a path may be thousands of vertices long)."""
     match_r = {}
-    keys = list(adj)
+    nbrs = {u: sorted(vs) for u, vs in adj.items()}
+    size = 0
+    for root in nbrs:
+        seen = set()
+        stack = [(root, iter(nbrs[root]))]      # frames: a left vertex and its untried neighbours
+        taken = []                              # the right vertex each frame below the top went through
+        while stack:
+            u, it = stack[-1]
+            for v in it:
+                if v in seen:
+                    continue
+                seen.add(v)
+                if v in match_r:
+                    taken.append(v)
+                    stack.append((match_r[v], iter(nbrs[match_r[v]])))
+                else:
+                    taken.append(v)
+                    for (x, _), w in zip(stack, taken):
+                        match_r[w] = x
+                    size += 1
+                    stack = []
+                break
+            else:
+                stack.pop()
+                if taken:
+                    taken.pop()
+    return size
 
-    def augment(u, seen):
-        for v in sorted(adj[u]):
-            if v in seen:
-                continue
-            seen.add(v)
-            if v not in match_r or augment(match_r[v], seen):
-                match_r[v] = u
-                return True
-        return False
 
-    return sum(1 for u in keys if augment(u, set()))
+def pair_counts(gt, prop, n, d, r, step, threshold, stats=None):
+    """[6] counts of one pair: marbles, holes, bidirectional holes, matched (precision), matched (recall), 0.
 
-
-def pair_counts(gt, prop, n, d, r, step, threshold):
-    """[6] counts of one pair: marbles, holes, bidirectional holes, matched (precision), matched (recall), 0."""
-    marbles = topo_walk(prop, n[0], n[1], d[0], d[1], r, step)
-    holes = topo_walk(gt, n[2], n[3], d[2], d[3], r, step)
-    holes_b = topo_walk(gt, n[2], n[3], d[2], d[3], r, step, bidirection=True)
-    mp = matching_size(candidate_graph(marbles, holes_b, True, threshold))
-    mr = matching_size(candidate_graph(holes, marbles, False, threshold))
-    return [len(marbles), len(holes), len(holes_b), mp, mr, 0]
+    `stats`, when a dict, receives per walk (marbles, holes, bidirectional holes) the lists `marbles`, `queue`,
+    `pushes`, `covered` and `lowered` of topo_walk, and `candidates`: the candidate edges of the precision and of the recall
+    graph."""
+    w = [{}, {}, {}]
+    marbles = topo_walk(prop, n[0], n[1], d[0], d[1], r, step, stats=w[0])
+    holes = topo_walk(gt, n[2], n[3], d[2], d[3], r, step, stats=w[1])
+    holes_b = topo_walk(gt, n[2], n[3], d[2], d[3], r, step, bidirection=True, stats=w[2])
+    gp = candidate_graph_boxed(marbles, holes_b, True, threshold)
+    gr = candidate_graph_boxed(holes, marbles, False, threshold)
+    if stats is not None:
+        stats.update({k: [x[k] for x in w] for k in w[0]})
+        stats["candidates"] = [sum(len(v) for v in gp.values()), sum(len(v) for v in gr.values())]
+    return [len(marbles), len(holes), len(holes_b), matching_size(gp), matching_size(gr), 0]
 
 
 def scorer(gt, prop):

@@ -14,50 +14,11 @@ import sys
 import tempfile
 import time
 
-import numpy as np
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from sam_road_b200 import topo_metric as TM  # noqa: E402
-
-
-def city_tile(size=2048, block=128, seg=16, seed=0):
-    """A grid of two-way streets every `block` px with nodes every `seg` px, some diagonals, and a proposal with
-    displaced nodes (up to 6 px), 8 % of the directed edges dropped and a few spurious streets."""
-    rng = np.random.default_rng(seed)
-    gt = {}
-
-    def add(adj, a, b, two_way=True):
-        adj.setdefault(a, [])
-        adj.setdefault(b, [])
-        if b not in adj[a]:
-            adj[a].append(b)
-        if two_way and a not in adj[b]:
-            adj[b].append(a)
-
-    def street(adj, p, q):
-        n = max(1, int(round(np.hypot(q[0] - p[0], q[1] - p[1]) / seg)))
-        pts = [(float(p[0] + (q[0] - p[0]) * k / n), float(p[1] + (q[1] - p[1]) * k / n)) for k in range(n + 1)]
-        for a, b in zip(pts, pts[1:]):
-            add(adj, a, b)
-
-    lo, hi = 64, size - 64
-    for v in range(lo, hi + 1, block):
-        street(gt, (v, lo), (v, hi))
-        street(gt, (lo, v), (hi, v))
-    for k in range(4):
-        street(gt, (lo + 37 + k * 400, lo + 11), (lo + 37 + k * 400 + 300, lo + 311))
-    prop = {}
-    moved = {k: (k[0] + float(rng.integers(-6, 7)), k[1] + float(rng.integers(-6, 7))) for k in gt}
-    for a, vs in gt.items():
-        for b in vs:
-            if rng.random() >= 0.08:
-                add(prop, moved[a], moved[b], two_way=False)
-    for k in range(6):
-        x = float(rng.integers(lo, hi - 200))
-        street(prop, (x, x + 40), (x + 150, x + 190))
-    return gt, prop
+from sam_road_b200.synth import city_tile  # noqa: E402
 
 
 def gpu_info():
