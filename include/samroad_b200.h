@@ -395,6 +395,57 @@ int samroad_topo_upload_graph(samroad_topo_t T, int which, int32_t n_nodes, cons
 int samroad_topo_run(samroad_topo_t T, int32_t n_pairs, const int32_t* pair_nodes, const double* pair_dists,
                      double r, double step, double threshold, double cos40, int32_t* counts);
 
+/* ---- the APLS graph metric (sam_road_b200/apls_metric.py, DESIGN.md §15) ----
+ * An apls object holds one tile's two densified road graphs (0 ground truth, 1 proposal) as main.go's
+ * GraphDensify builds them, with the directed integer arc weights int(GPSDistance(u, v) * 100.0) from the host.
+ * It finds the snapping candidates of the control points and, per direction, the shortest paths between the
+ * matched control points on both graphs and the pair score.  Capacities are per handle; a call past one is refused
+ * with an error naming it, never truncated, and the handle stays usable.  Not thread-safe; one call at a time.
+ * Synchronous (the handle's own non-blocking stream). */
+#define SAMROAD_APLS_CANDIDATES 10
+typedef struct samroad_apls_ctx* samroad_apls_t;
+typedef struct SamRoadAplsCaps {
+  int32_t max_nodes;            /* nodes of one graph                                            */
+  int32_t max_arcs;             /* directed arcs of one graph (adjacency entries)                */
+  int32_t max_control_points;   /* control points of one direction (also candidate queries)      */
+} SamRoadAplsCaps;
+typedef struct SamRoadAplsResult {
+  int64_t pairs;                /* unordered pairs of control points                             */
+  int64_t cc;                   /* penalty + scored                                              */
+  int64_t penalty;              /* pairs with an unmatched control point: each adds 1            */
+  int64_t skipped;              /* both matched, d1 <= min_distance_filter or unreachable        */
+  int64_t scored;               /* both matched, d1 > min_distance_filter: adds min(|d1-d2|/d1, 1) */
+  uint64_t sum_fixed[3];        /* the exact sum of all terms, a 192-bit integer with LSB 2^-128 */
+  double sum;                   /* sum_fixed rounded once to the nearest double, ties to even    */
+  int32_t n_sources_gt;         /* matched control points (rows of dist_gt)                      */
+  int32_t n_sources_prop;       /* their distinct matches (rows of dist_prop)                    */
+  int32_t terminals_gt;         /* nodes of the contracted graphs the shortest paths ran on      */
+  int32_t terminals_prop;
+} SamRoadAplsResult;
+
+int samroad_apls_create(int device, const SamRoadAplsCaps* caps, samroad_apls_t* out);
+int samroad_apls_destroy(samroad_apls_t A);
+/* Copies one graph (host memory) to the handle, replacing the previous graph of that kind.  latlon [n,2] float64
+ * (lat, lon) by node id; row_start [n+1] / col / weight: the directed arcs of each node with their weights in cm.
+ * Any digraph is accepted: arcs need no reverse arc, and self-loops and repeated arcs are allowed (a repeated arc
+ * counts with its lightest weight).  Refuses a coordinate that is not finite, a negative weight, and
+ * weights that sum to 2^31 - 1 or more (a distance could then exceed int32). */
+int samroad_apls_upload_graph(samroad_apls_t A, int which, int32_t n_nodes, const double* latlon,
+                              const int32_t* row_start, const int32_t* col, const int32_t* weight);
+/* For each query point (lat, lon), the SAMROAD_APLS_CANDIDATES nodes of graph `which` nearest to it by squared
+ * distance to the node's [x - 1e-6, x + 1e-6] box in degree space, ties by ascending node id, nearest first;
+ * -1 pads when the graph has fewer nodes.  out [n_queries, SAMROAD_APLS_CANDIDATES] int32. */
+int samroad_apls_candidates(samroad_apls_t A, int which, int32_t n_queries, const double* query_latlon,
+                            int32_t* out);
+/* One direction of main.go's apls_one_way after the snapping: graph gt_role plays the ground truth.  cp_gt [n_cp]:
+ * the control points, ascending node ids of graph gt_role; cp_match [n_cp]: the node of the other graph each is
+ * matched to, or -1.  Shortest paths run from every matched control point to the others on graph gt_role, and
+ * between their matches on the other graph; the pair score runs over every unordered pair.  dist_gt
+ * [n_sources_gt, n_sources_gt] (matched control points in cp order) and dist_prop [n_sources_prop, n_sources_prop]
+ * (distinct matches in order of first appearance) receive the distances in cm (-1: unreachable) when not NULL. */
+int samroad_apls_one_way(samroad_apls_t A, int gt_role, int32_t n_cp, const int32_t* cp_gt, const int32_t* cp_match,
+                         double min_distance_filter, SamRoadAplsResult* out, int32_t* dist_gt, int32_t* dist_prop);
+
 /* Stream memory operations on a 32-bit flag word in device (or peer-mapped) memory, executed by the stream
  * front end without a kernel: an ordered write of `value`, and a wait until *addr >= value.  The exchange step
  * between ranks (sam_road_b200/exchange.py; no reference counterpart, the reference is single-GPU) builds its

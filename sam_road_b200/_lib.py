@@ -68,6 +68,32 @@ class SamRoadTopoCaps(C.Structure):
     ]
 
 
+class SamRoadAplsCaps(C.Structure):
+    _fields_ = [
+        ("max_nodes", C.c_int32),
+        ("max_arcs", C.c_int32),
+        ("max_control_points", C.c_int32),
+    ]
+
+
+class SamRoadAplsResult(C.Structure):
+    _fields_ = [
+        ("pairs", C.c_int64),
+        ("cc", C.c_int64),
+        ("penalty", C.c_int64),
+        ("skipped", C.c_int64),
+        ("scored", C.c_int64),
+        ("sum_fixed", C.c_uint64 * 3),
+        ("sum", C.c_double),
+        ("n_sources_gt", C.c_int32),
+        ("n_sources_prop", C.c_int32),
+        ("terminals_gt", C.c_int32),
+        ("terminals_prop", C.c_int32),
+    ]
+
+
+APLS_CANDIDATES = 10
+
 _vp, _i, _f, _d = C.c_void_p, C.c_int, C.c_float, C.c_double
 _ip = C.POINTER(C.c_int)
 _targs = C.POINTER(SamRoadTrainArgs)
@@ -129,6 +155,11 @@ SIGNATURES = {
     "samroad_topo_destroy": (_i, [_vp]),
     "samroad_topo_upload_graph": (_i, [_vp, _i, C.c_int32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "samroad_topo_run": (_i, [_vp, C.c_int32, _vp, _vp, _d, _d, _d, _d, _vp]),
+    "samroad_apls_create": (_i, [_i, C.POINTER(SamRoadAplsCaps), C.POINTER(_vp)]),
+    "samroad_apls_destroy": (_i, [_vp]),
+    "samroad_apls_upload_graph": (_i, [_vp, _i, C.c_int32, _vp, _vp, _vp, _vp]),
+    "samroad_apls_candidates": (_i, [_vp, _i, C.c_int32, _vp, _vp]),
+    "samroad_apls_one_way": (_i, [_vp, _i, C.c_int32, _vp, _vp, _d, C.POINTER(SamRoadAplsResult), _vp, _vp]),
     "samroad_stream_write_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_stream_wait_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_timing_enable": (_i, [_vp, _i]),

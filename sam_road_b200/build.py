@@ -18,16 +18,16 @@ CSRC = PKG_DIR / "csrc"
 OBJ_DIR = PKG_DIR / "_build"
 LIB_PATH = PKG_DIR / "libsamroad_b200.so"
 
-SOURCES = ["common.cu", "gemm_ops.cu", "kernels.cu", "attention.cu", "toponet.cu", "sam_decoder.cu", "graph.cu", "metrics.cu", "model.cu", "train.cu", "labels.cu", "topo_metric.cu"]
+SOURCES = ["common.cu", "gemm_ops.cu", "kernels.cu", "attention.cu", "toponet.cu", "sam_decoder.cu", "graph.cu", "metrics.cu", "model.cu", "train.cu", "labels.cu", "topo_metric.cu", "apls_metric.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
 ]
-# per-source additions: the TOPO metric repeats the reference's float64 arithmetic operation by operation, so
-# no multiply-add may be contracted into an FMA there
-EXTRA_FLAGS = {"topo_metric.cu": ["-fmad=false"]}
+# per-source additions: the TOPO and APLS metrics repeat the reference's float64 arithmetic operation by
+# operation, so no multiply-add may be contracted into an FMA there
+EXTRA_FLAGS = {"topo_metric.cu": ["-fmad=false"], "apls_metric.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:
