@@ -6,8 +6,10 @@
 
 namespace srb {
 
-// 128x256 tiles (3-stage ring) when N allows and the grid still fills the GPU, otherwise 128x128
-// tiles (5-stage ring).
+// Streaming epilogues (EpiF16, EpiF32) run on the ping-pong kernel (128x128 tiles, one per consumer
+// warpgroup).  The row-statistics epilogues (EpiLN, EpiDecFinal) need whole rows of a tile staged in
+// shared memory and stay on gemm_tc_kernel: 128x256 tiles (3-stage ring) when N allows and the grid
+// still fills the GPU, otherwise 128x128 tiles (5-stage ring).
 
 static inline bool use_bn256(int M, int N) {
   if (N % 256 != 0) return false;
@@ -21,8 +23,7 @@ int gemm_f16out(const __half* A, int lda, const __half* W, int ldw, int M, int N
               "gemm_f16out: act=%d must be 0 (none), 1 (GELU) or 2 (ReLU)", act);
   EpiF16::Params p{out, bias, ldo, act};
   SRB_REQUIRE(ldo % 8 == 0, "gemm_f16out: ldo=%d must be a multiple of 8", ldo);
-  if (use_bn256(M, N)) return launch_gemm_tc<256, 3, EpiF16>(A, lda, W, ldw, M, N, K, p, st);
-  return launch_gemm_tc<128, 5, EpiF16>(A, lda, W, ldw, M, N, K, p, st);
+  return launch_gemm_pp<EpiF16>(A, lda, W, ldw, M, N, K, p, st);
 }
 
 int gemm_f32out(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
@@ -30,8 +31,7 @@ int gemm_f32out(const __half* A, int lda, const __half* W, int ldw, int M, int N
                 int ldo, cudaStream_t st) {
   EpiF32::Params p{out, bias, resid, pos, ldo, pos_rows > 0 ? pos_rows : 1, N};
   SRB_REQUIRE(ldo % 4 == 0, "gemm_f32out: ldo=%d must be a multiple of 4", ldo);
-  if (use_bn256(M, N)) return launch_gemm_tc<256, 3, EpiF32>(A, lda, W, ldw, M, N, K, p, st);
-  return launch_gemm_tc<128, 5, EpiF32>(A, lda, W, ldw, M, N, K, p, st);
+  return launch_gemm_pp<EpiF32>(A, lda, W, ldw, M, N, K, p, st);
 }
 
 int gemm_ln(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,

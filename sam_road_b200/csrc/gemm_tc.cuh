@@ -1,17 +1,16 @@
 // sam_road_b200 :: wgmma GEMM  C[M,N] = A[M,K] * W[N,K]^T  (+ fused epilogue)
 //
-// One kernel template covers every dense contraction of the hot path (SURVEY.md §2.4 K2, K5, K9,
-// K10, K11, K12, K16): fp16 operands (both K-major), fp32 accumulation in registers.
+// Two kernel templates cover every dense contraction of the hot path (SURVEY.md §2.4 K2, K5, K9,
+// K10, K11, K12, K16): fp16 operands (both K-major), fp32 accumulation in registers.  The streaming
+// epilogues (EpiF16, EpiF32) run on gemm_pp_kernel (below, at the end of the file); the
+// row-statistics epilogues (EpiLN, EpiDecFinal) on gemm_tc_kernel:
 //
 //   warpgroup 0     : TMA producer (one thread; cp.async.bulk.tensor, 128B-swizzled 128x64 / BNx64
 //                     boxes), registers handed to the consumers with setmaxnreg
 //   warpgroups 1, 2 : consumers.  Each issues wgmma m64 x BN x 16 for its 64 rows of the 128-row
 //                     tile, then stages its fp32 accumulators in shared memory and runs the fused
 //                     epilogue over them: warp w of consumer g reads rows 32*(2g + (w&1)) .. +31 (one
-//                     row per lane) and columns half (w>>1) of the tile.  Streaming epilogues (EpiF16)
-//                     transpose each 32x32 fp32 block through a per-warp smem scratch so that global
-//                     stores are row-contiguous (8 lanes x 16 B per row); row-statistics epilogues
-//                     (EpiLN, EpiDecFinal) keep one row per thread.
+//                     row per lane) and columns half (w>>1) of the tile.
 //
 // Persistent CTAs (grid = min(#tiles, #SMs)) and a STAGES-deep smem ring between TMA and the MMAs.
 // The accumulator staging area reuses the ring (an m128 x n256 fp32 tile needs 130 KB, and a second
@@ -56,33 +55,30 @@ struct AccRow {
 };
 
 // ------------------------------------------------------------------------------------------------
-// Streaming epilogues.  A warp owns 32 tile rows (a row quarter of the tile) x n_cols columns.  Per
-// 32-column chunk: lane r holds row r's 32 accumulators -> scratch[r][0..31] (row pitch 36 floats,
-// float4 accesses, conflict-free) -> re-read as "lane l holds columns 4*(l&7).. of row 4*j + (l>>3)", j = 0..7 ->
-// bias / activation / residual in that layout -> 8 lanes cover 128 (fp32) or 64 (fp16) contiguous
-// bytes of a row per store instruction.
+// Streaming epilogues of the ping-pong kernel, straight from the wgmma accumulator fragments of one
+// consumer warpgroup's 128x128 tile: d[h] is the m64n128 fragment of tile rows 64h .. 64h+63, so a
+// thread (warp w of the warpgroup, lane l) holds, per n8 block j, the two adjacent columns
+// 8j + 2(l&3) .. +1 of rows 16w + l/4 and 16w + l/4 + 8 of each half.  The four lanes of a quad
+// cover 32 contiguous bytes of an fp32 row (one sector) and 16 of an fp16 row; every output element
+// is read (residual) and written by the one thread that holds its accumulator, which keeps `out`
+// aliasing `resid` legal.
 // ------------------------------------------------------------------------------------------------
-template <class F>
-__device__ __forceinline__ void epi_stream_chunks(int n_cols, const AccRow& row, float* scratch,
-                                                  int lane, F&& body) {
-  const int nchunks = n_cols >> 5;
-  const int cc = (lane & 7) * 4, rsub = lane >> 3;
-  for (int c = 0; c < nchunks; ++c) {
-    float v[32];
-    row.load(c, v);
-    // 16-byte accesses with a 36-float row pitch are bank-conflict free in both directions
-    float4* wp = reinterpret_cast<float4*>(scratch + lane * 36);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) wp[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int rr = 4 * j + rsub;
-      body(c, rr, cc, *reinterpret_cast<const float4*>(scratch + rr * 36 + cc));
-    }
-    __syncwarp();
-  }
-}
+struct FragPos {
+  int r0;       // first of this thread's four rows r0, r0 + 8, r0 + 64, r0 + 72
+  int n_tile;   // first column of the tile
+  int c0;       // this thread's column pair in n8 block j: c0 + 8j, c0 + 8j + 1
+  __device__ __forceinline__ FragPos(int m_tile, int n_tile_, int w, int lane)
+      : r0(m_tile + 16 * w + (lane >> 2)), n_tile(n_tile_), c0(n_tile_ + 2 * (lane & 3)) {}
+  // row of fragment element pair q = 2h + hr (half h, lower/upper 8-row group hr)
+  __device__ __forceinline__ int row(int q) const { return r0 + 64 * (q >> 1) + 8 * (q & 1); }
+  // N is a multiple of 32, so a 16- or 32-column chunk is wholly inside or wholly outside the matrix
+  __device__ __forceinline__ bool cols_in(int col, int N) const { return n_tile + col < N; }
+};
+
+// Both epilogues load every operand of a chunk before they store an earlier one: the compiler may not
+// move a load above a store to `out`, which it must assume aliases the operand, and a load issued
+// after the stores costs one L2 round trip each (at K = 768 the epilogue then outlasts the other
+// consumer's mainloop).
 
 // Epilogue 1: out16[m,n] = act(acc + bias[n])                       (qkv, MLP lin1, TopoNet lin)
 struct EpiF16 {
@@ -92,35 +88,41 @@ struct EpiF16 {
     int ldo;
     int act;
   };
-  static __device__ __forceinline__ void run(const Params& p, int m0, int M, int n_base, int n_cols,
-                                             const AccRow& row, float* scratch, int lane) {
-    epi_stream_chunks(n_cols, row, scratch, lane, [&](int c, int rr, int cc, float4 x) {
-      const int n = n_base + c * 32 + cc;
-      if (p.bias) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-        x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
+  static __device__ __forceinline__ void run(const Params& p, int M, int N, const FragPos& f,
+                                             float (&d)[2][64]) {
+    float2 b[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      b[j] = make_float2(0.f, 0.f);
+      if (p.bias && f.cols_in(32 * (j >> 2), N)) b[j] = __ldg(reinterpret_cast<const float2*>(p.bias + f.c0 + 8 * j));
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      if (!f.cols_in(32 * c, N)) continue;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * c + jj;
+        const int n = f.c0 + 8 * j;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          float2 x = make_float2(d[q >> 1][4 * j + 2 * (q & 1)], d[q >> 1][4 * j + 2 * (q & 1) + 1]);
+          if (p.bias) { x.x += b[j].x; x.y += b[j].y; }
+          if (p.act == ACT_GELU) x = gelu_erf_fast2(x);
+          else if (p.act == ACT_RELU) x = make_float2(fmaxf(x.x, 0.0f), fmaxf(x.y, 0.0f));
+          const int m = f.row(q);
+          if (m < M) *reinterpret_cast<uint32_t*>(p.out + static_cast<size_t>(m) * p.ldo + n) = pack_half2(x.x, x.y);
+        }
       }
-      if (p.act == ACT_GELU) {
-        const float2 g0 = gelu_erf_fast2(make_float2(x.x, x.y));
-        const float2 g1 = gelu_erf_fast2(make_float2(x.z, x.w));
-        x = make_float4(g0.x, g0.y, g1.x, g1.y);
-      } else if (p.act == ACT_RELU) {
-        x = make_float4(fmaxf(x.x, 0.0f), fmaxf(x.y, 0.0f), fmaxf(x.z, 0.0f), fmaxf(x.w, 0.0f));
-      }
-      const int m = m0 + rr;
-      if (m < M) {
-        uint2 u;
-        u.x = pack_half2(x.x, x.y);
-        u.y = pack_half2(x.z, x.w);
-        *reinterpret_cast<uint2*>(p.out + static_cast<size_t>(m) * p.ldo + n) = u;
-      }
-    });
+    }
   }
-  static __device__ __forceinline__ void drain(int /*lane*/) {}
 };
 
-// Epilogue 2: out32[m,n] = acc + bias[n] + resid[m,n] + pos[m % pos_rows, n]
+// Epilogue 2: out32[m,n] = acc + resid[m,n] + bias[n] + pos[m % pos_rows, n]
 //             (patch-embed + pos_embed, attention proj + shortcut, MLP lin2 + shortcut; plain f32)
+// fp32 in/out makes this epilogue HBM-bound for short K (attention proj): the residual of 16-column
+// chunk c+1 is loaded into registers before chunk c is stored (it never touches an element chunk c
+// stores).  Bias and pos-embed (L1- / L2-resident) are loaded when their chunk starts, all before its
+// first store.  (Double-buffering pos-embed too spills next to the 128 accumulators.)
 struct EpiF32 {
   struct Params {
     float* out;           // [M, ldo]
@@ -131,54 +133,59 @@ struct EpiF32 {
     int pos_rows;
     int n_total;
   };
-  // fp32 in/out makes this epilogue HBM-bound for short K (attention proj): one row per lane with
-  // 128 B contiguous per lane and chunk, and the residual of chunk c+1 prefetched into registers
-  // while chunk c is processed, keeps more bytes in flight than the transposed scheme.
-  static __device__ __forceinline__ void run(const Params& p, int m0, int M, int n_base, int n_cols,
-                                             const AccRow& row, float* /*scratch*/, int lane) {
-    const int nchunks = n_cols >> 5;
-    const int m = m0 + lane;
-    const bool valid = m < M;
-    const float* rrow = (p.resid && valid) ? p.resid + static_cast<size_t>(m) * p.ldo + n_base : nullptr;
-    const float* prow = (p.pos && valid)
-                            ? p.pos + static_cast<size_t>(m % p.pos_rows) * p.n_total + n_base
-                            : nullptr;
-    float* orow = p.out + static_cast<size_t>(valid ? m : 0) * p.ldo + n_base;
-    float4 nxt[8];
+  // residuals of n8 blocks 2c + jj, jj = 0, 1: r[4 * jj + q] for row pair q
+  static __device__ __forceinline__ void load_resid(const Params& p, int M, int N, const FragPos& f, int c,
+                                                    float2 (&r)[8]) {
+    const bool in_n = f.cols_in(16 * c, N);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) nxt[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (rrow && nchunks > 0) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) nxt[i] = reinterpret_cast<const float4*>(rrow)[i];
+    for (int i = 0; i < 8; ++i) {
+      const int m = f.row(i & 3);
+      r[i] = make_float2(0.f, 0.f);
+      if (p.resid && in_n && m < M)
+        r[i] = *reinterpret_cast<const float2*>(p.resid + static_cast<size_t>(m) * p.ldo + f.c0 + 8 * (2 * c + (i >> 2)));
     }
-    for (int c = 0; c < nchunks; ++c) {
-      float4 cur[8];
+  }
+  static __device__ __forceinline__ void run(const Params& p, int M, int N, const FragPos& f,
+                                             float (&d)[2][64]) {
+    int pos_row[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) pos_row[q] = p.pos ? f.row(q) % p.pos_rows : 0;
+    float2 nxt[8];
+    load_resid(p, M, N, f, 0, nxt);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      float2 cur[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) cur[i] = nxt[i];
-      if (rrow && c + 1 < nchunks) {
+      if (c + 1 < 8) load_resid(p, M, N, f, c + 1, nxt);
+      if (!f.cols_in(16 * c, N)) continue;
+      float2 b[2], e[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) nxt[i] = reinterpret_cast<const float4*>(rrow + (c + 1) * 32)[i];
+      for (int jj = 0; jj < 2; ++jj) {
+        const int n = f.c0 + 8 * (2 * c + jj);
+        b[jj] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          e[4 * jj + q] = p.pos && f.row(q) < M
+                              ? __ldg(reinterpret_cast<const float2*>(p.pos + static_cast<size_t>(pos_row[q]) * p.n_total + n))
+                              : make_float2(0.f, 0.f);
       }
-      float v[32];
-      row.load(c, v);
-      const int n0 = c * 32;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float4 x = make_float4(v[4 * i] + cur[i].x, v[4 * i + 1] + cur[i].y, v[4 * i + 2] + cur[i].z,
-                               v[4 * i + 3] + cur[i].w);
-        if (p.bias) {
-          const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n_base + n0) + i);
-          x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
+      for (int jj = 0; jj < 2; ++jj) {
+        const int n = f.c0 + 8 * (2 * c + jj);
+        const int j = 2 * c + jj;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int m = f.row(q);
+          const float2 r = cur[4 * jj + q];
+          float2 x = make_float2(d[q >> 1][4 * j + 2 * (q & 1)] + r.x, d[q >> 1][4 * j + 2 * (q & 1) + 1] + r.y);
+          if (p.bias) { x.x += b[jj].x; x.y += b[jj].y; }
+          if (p.pos) { x.x += e[4 * jj + q].x; x.y += e[4 * jj + q].y; }
+          if (m < M) *reinterpret_cast<float2*>(p.out + static_cast<size_t>(m) * p.ldo + n) = x;
         }
-        if (prow) {
-          const float4 b = __ldg(reinterpret_cast<const float4*>(prow + n0) + i);
-          x.x += b.x; x.y += b.y; x.z += b.z; x.w += b.w;
-        }
-        if (valid) reinterpret_cast<float4*>(orow + n0)[i] = x;
       }
     }
   }
-  static __device__ __forceinline__ void drain(int /*lane*/) {}
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -627,6 +634,166 @@ int launch_gemm_tc(const __half* A, int lda, const __half* W, int ldw, int M, in
   const int num_tiles = ((M + kGemmBM - 1) / kGemmBM) * ((N + BN - 1) / BN);
   const int grid = num_tiles < device_sm_count() ? num_tiles : device_sm_count();
   kern<<<grid, kGemmThreads, SM::kTotal, stream>>>(tmA, tmB, M, N, K, ep, conv_s);
+  SRB_CUDA_OK(cudaGetLastError());
+  note_launch(1);
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Ping-pong kernel for the streaming epilogues (EpiF16, EpiF32).  Same block as gemm_tc_kernel
+// (warpgroup 0 = TMA producer, warpgroups 1 and 2 = consumers), but each consumer owns whole 128x128
+// tiles: two wgmma m64n128k16 per k16 step, 2 x 64 fp32 accumulators per thread.  The CTA's tiles
+// t0, t1, t2, ... alternate between the consumers (t0, t2, ... and t1, t3, ...), and an ordering
+// mbarrier pair starts a consumer's mainloop when the other's has issued its last MMAs, so one
+// warpgroup is on the tensor cores while the other runs its epilogue from registers.  The ring
+// holds operands only; the producer never waits for an epilogue.
+//
+// Ring bookkeeping.  The producer fills ring positions p = 0, 1, 2, ... in CTA tile order: local
+// tile i (the CTA's i-th tile) owns positions i*num_k .. i*num_k + num_k - 1, slot p % STAGES,
+// fill number n = p / STAGES of that slot.  The consumer of tile i waits on full_bar[slot] with
+// parity n & 1 and, once its MMAs have read the slot, releases it with one arrive per warp
+// (empty_bar count 4); the other consumer never touches the slot for that fill.  Invariant: when a
+// consumer waits on position p, every position before p has already been seen full by its own
+// consumer (its own earlier k-blocks, and through the ordering barrier every k-block of the tiles
+// before), so fill n - 1 of the slot is complete and fill n + 1 cannot start before this consumer
+// releases fill n: the slot's full barrier is exactly one phase from the waited parity, never two.
+// ------------------------------------------------------------------------------------------------
+template <int STAGES>
+struct GemmPPSmem {
+  static constexpr int kABytes = kGemmBM * kGemmBK * 2;
+  static constexpr int kBBytes = 128 * kGemmBK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kBarOffset = STAGES * kStageBytes;
+  static constexpr int kTotal = kBarOffset + 256 + 1024;
+};
+
+template <int STAGES, class Epi>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               int M, int N, int K, const __grid_constant__ typename Epi::Params ep) {
+  using SM = GemmPPSmem<STAGES>;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOffset);
+  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* order_bar = empty_bar + STAGES;       // [g]: the other consumer has issued its mainloop
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
+
+  const int num_n = (N + 127) / 128;
+  const int num_tiles = ((M + kGemmBM - 1) / kGemmBM) * num_n;
+  const int num_k = (K + kGemmBK - 1) / kGemmBK;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);
+    }
+    mbar_init(&order_bar[0], 4);
+    mbar_init(&order_bar[1], 4);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_blk = tile / num_n, n_blk = tile % num_n;
+        for (int kb = 0; kb < num_k; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          uint8_t* sa = smem + stage * SM::kStageBytes;
+          mbar_arrive_expect_tx(&full_bar[stage], SM::kStageBytes);
+          tma_load_2d(sa, &tmA, &full_bar[stage], kb * kGemmBK, m_blk * kGemmBM);
+          tma_load_2d(sa + SM::kABytes, &tmB, &full_bar[stage], kb * kGemmBK, n_blk * 128);
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: MMA + epilogue, alternating tiles =====================
+    setmaxnreg_inc<232>();
+    const int g = wg - 1;
+    const int w = warp & 3;
+    uint32_t order_phase = 0;
+    int i = g;                                 // local tile index
+    for (int tile = blockIdx.x + g * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, i += 2) {
+      const int m_blk = tile / num_n, n_blk = tile % num_n;
+      if (i > 0) {                             // the other consumer has issued tile i - 1
+        mbar_wait(&order_bar[g], order_phase);
+        order_phase ^= 1u;
+      }
+      const int pos = i * num_k;
+      int stage = pos % STAGES;
+      uint32_t phase = static_cast<uint32_t>(pos / STAGES) & 1u;
+      float d[2][64];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 64; ++r) d[h][r] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_k; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * SM::kStageBytes);
+        const uint64_t adesc0 = wgmma_desc_k128(a_addr);
+        const uint64_t adesc1 = wgmma_desc_k128(a_addr + 64 * kGemmBK * 2);
+        const uint64_t bdesc = wgmma_desc_k128(a_addr + SM::kABytes);
+        wgmma_fence_operand(d[0]);
+        wgmma_fence_operand(d[1]);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kGemmBK / 16; ++k) {
+          const uint32_t acc = (kb | k) != 0 ? 1u : 0u;
+          wgmma_m64n128k16(d[0], adesc0 + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), acc);
+          wgmma_m64n128k16(d[1], adesc1 + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), acc);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                       // the previous k-block's MMAs have read their stage
+        wgmma_fence_operand(d[0]);
+        wgmma_fence_operand(d[1]);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      if (lane == 0) mbar_arrive(&order_bar[g ^ 1]);   // the other consumer may start its mainloop
+      wgmma_wait<0>();
+      wgmma_fence_operand(d[0]);
+      wgmma_fence_operand(d[1]);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      Epi::run(ep, M, N, FragPos(m_blk * kGemmBM, n_blk * 128, w, lane), d);
+    }
+  }
+}
+
+template <class Epi>
+int launch_gemm_pp(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
+                   const typename Epi::Params& ep, cudaStream_t stream) {
+  constexpr int kStages = 5;
+  using SM = GemmPPSmem<kStages>;
+  SRB_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
+  SRB_REQUIRE(N % 32 == 0, "gemm: N=%d must be a multiple of 32", N);
+  SRB_REQUIRE(K % 8 == 0 && lda % 8 == 0 && ldw % 8 == 0,
+              "gemm: K/lda/ldw (%d/%d/%d) must be multiples of 8", K, lda, ldw);
+  CUtensorMap tmA, tmB;
+  if (int rc = make_tmap_f16_2d(&tmA, A, M, K, lda, kGemmBM)) return rc;
+  if (int rc = make_tmap_f16_2d(&tmB, W, N, K, ldw, 128)) return rc;
+  auto kern = gemm_pp_kernel<kStages, Epi>;
+  static uint64_t attr_devs = 0;          // one bit per CUDA device: function attributes are per device
+  if (first_use_on_device(&attr_devs)) {
+    SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
+  }
+  const int num_tiles = ((M + kGemmBM - 1) / kGemmBM) * ((N + 127) / 128);
+  const int grid = num_tiles < device_sm_count() ? num_tiles : device_sm_count();
+  kern<<<grid, kGemmThreads, SM::kTotal, stream>>>(tmA, tmB, M, N, K, ep);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(1);
   return 0;

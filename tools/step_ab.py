@@ -3,7 +3,7 @@ copy of another commit (its library built beforehand) and from this tree.
 
     python tools/step_ab.py --parent parent_tree [--runs 3] [--workload c2] [--out DIR] [-- extra bench.py args]
 
-Per run it prints `value` (tiles/s), `ms_per_step`, the attention entries of `kernels` and `clocks`; at the end the
+Per run it prints `value` (tiles/s), `ms_per_step`, the attention and GEMM entries of `kernels` and `clocks`; at the end the
 fastest and slowest run of each tree.  With --out the first run of each tree also dumps its outputs
 (bench.py --dump-outputs) and the max-abs differences of mask_scores, img_features and topo_scores are printed.
 The card name, power limit and max SM clock are read in the same run."""
@@ -48,7 +48,8 @@ def main():
                 extra += ["--dump-outputs", os.path.join(os.path.abspath(args.out), f"dump_{args.workload}_{key}")]
             line = bench(tree, args.workload, extra)
             row = {"value": line["value"], "ms_per_step": line["ms_per_step"], "clocks": line["clocks"],
-                   "attention": {k: round(v["ms_per_step"], 3) for k, v in line["kernels"].items() if "attention" in k}}
+                   "attention": {k: round(v["ms_per_step"], 3) for k, v in line["kernels"].items() if "attention" in k},
+                   "gemm": {k: round(v["ms_per_step"], 3) for k, v in line["kernels"].items() if k.startswith("gemm_")}}
             rows[key].append(row)
             print(args.workload, key, i, json.dumps(row), flush=True)
     summary = {"workload": args.workload, "card": q.stdout.strip(), "runs": rows}
