@@ -7,6 +7,7 @@ or a call fails, a RuntimeError carrying `samroad_last_error()` is raised.
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from pathlib import Path
 
 _PKG = Path(__file__).resolve().parent
@@ -207,6 +208,31 @@ def last_error() -> str:
 def check(rc: int, what: str) -> None:
     if rc != 0:
         raise RuntimeError(f"{what} failed (code {rc}): {last_error()}")
+
+
+def refuse_copy(self):
+    """__getstate__ of every native handle owner: device state cannot be copied or pickled."""
+    raise TypeError(f"{type(self).__name__} owns a native handle and cannot be copied or pickled")
+
+
+class Handle:
+    """Owner of one native handle.  `Handle(create, destroy, *args)` calls the library's `create(*args, &out)`
+    (RuntimeError with samroad_last_error() when it fails) and releases the handle with `destroy` on the
+    first `close()` or, at the latest, when the object is collected.  It passes straight into ctypes calls;
+    once closed it passes as NULL, which every entry point refuses with an error."""
+
+    __getstate__ = refuse_copy
+
+    def __init__(self, create: str, destroy: str, *args):
+        lib = load()
+        h = C.c_void_p()
+        check(getattr(lib, create)(*args, C.byref(h)), create)
+        self._as_parameter_ = h.value
+        self._finalizer = weakref.finalize(self, getattr(lib, destroy), h.value)
+
+    def close(self) -> None:
+        self._as_parameter_ = None
+        self._finalizer()     # destroys the handle the first time only
 
 
 def ptr(t) -> int | None:

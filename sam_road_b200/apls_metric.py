@@ -250,20 +250,12 @@ class AplsDevice:
     def __init__(self, device: int = 0, **caps):
         self._lib = _lib.load()
         self.caps = _lib.SamRoadAplsCaps(**dict(DEFAULT_CAPS, **caps))
-        h = C.c_void_p()
-        _lib.check(self._lib.samroad_apls_create(device, C.byref(self.caps), C.byref(h)), "samroad_apls_create")
-        self._h = h
+        self._h = _lib.Handle("samroad_apls_create", "samroad_apls_destroy", device, C.byref(self.caps))
+
+    __getstate__ = _lib.refuse_copy
 
     def close(self):
-        if self._h:
-            self._lib.samroad_apls_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._h.close()
 
     def upload_csr(self, which: int, latlon, start, col, w):
         ll = np.ascontiguousarray(np.asarray(latlon, dtype=np.float64).reshape(-1, 2))

@@ -41,8 +41,6 @@ constexpr int kPairThreads = 256;
 constexpr int kKnnWarps = 8;
 enum : uint32_t { kBadTerm = 1 };
 
-__host__ __device__ inline size_t align_up(size_t x) { return (x + 255) & ~size_t(255); }
-
 // Squared distance from q to the box [x - tol, x + tol] in raw degree space (longitude not scaled)
 __device__ __forceinline__ double box_d2(double q0, double q1, double x0, double x1) {
   const double lo0 = x0 - kBoxTol, hi0 = x0 + kBoxTol, lo1 = x1 - kBoxTol, hi1 = x1 + kBoxTol;
@@ -123,6 +121,20 @@ struct SsspGraph {
   int32_t nt, nsrc;
 };
 
+// A CTA's shortest-path scratch for nt terminals: distances and two frontier flag arrays
+struct SsspScratch {
+  int32_t* dist;
+  uint8_t* fa;
+  uint8_t* fb;
+};
+__host__ __device__ inline SsspScratch sssp_scratch(Layout& L, int32_t nt) {
+  SsspScratch s;
+  s.dist = L.take<int32_t>(nt);
+  s.fa = L.take<uint8_t>(nt);
+  s.fb = L.take<uint8_t>(nt);
+  return s;
+}
+
 // One CTA per (graph, source), grid-stride.  dist / two frontier flag arrays live in dynamic shared memory when
 // `scratch` is null, else in the CTA's slice of it.
 __global__ void __launch_bounds__(kSsspThreads) sssp_kernel(SsspGraph g0, SsspGraph g1, char* scratch,
@@ -133,9 +145,11 @@ __global__ void __launch_bounds__(kSsspThreads) sssp_kernel(SsspGraph g0, SsspGr
   for (int job = blockIdx.x; job < njobs; job += gridDim.x) {
     const SsspGraph& g = job < g0.nsrc ? g0 : g1;
     const int s = job < g0.nsrc ? job : job - g0.nsrc;
-    int32_t* dist = reinterpret_cast<int32_t*>(base);
-    uint8_t* fa = reinterpret_cast<uint8_t*>(base + align_up(4ull * g.nt));
-    uint8_t* fb = fa + align_up(g.nt);
+    Layout L(base);
+    const SsspScratch sc = sssp_scratch(L, g.nt);
+    int32_t* dist = sc.dist;
+    uint8_t* fa = sc.fa;
+    uint8_t* fb = sc.fb;
     for (int i = threadIdx.x; i < g.nt; i += blockDim.x) {
       dist[i] = kInf;
       fa[i] = 0;
@@ -350,31 +364,11 @@ struct samroad_apls_ctx {
   SamRoadAplsCaps caps{};
   cudaStream_t stream = nullptr;   // the handle's own non-blocking stream: a call waits for its own work only
   HostGraph host[2];
-  double* ll[2] = {nullptr, nullptr};   // node lat/lon on the device, for the candidate search
-  size_t llcap[2] = {0, 0};
-  void* work = nullptr;                 // per call: contracted graphs, matrices, partials; grown on demand
-  size_t work_bytes = 0;
+  DeviceBuffer ll[2];                   // node lat/lon on the device, for the candidate search
+  DeviceBuffer work;                    // per call: contracted graphs, matrices, partials; grown on demand
   std::vector<char> staging;            // host copy of the per-call inputs, sent in one transfer
   int smem_optin = 0;
 };
-
-namespace {
-
-int ensure_work(samroad_apls_ctx* A, size_t need, const char* what) {
-  if (need <= A->work_bytes) return 0;
-  if (A->work) cudaFree(A->work);   // calls are synchronous: nothing of this handle still reads the old buffer
-  A->work = nullptr;
-  A->work_bytes = 0;
-  if (cudaMalloc(&A->work, need) != cudaSuccess) {
-    cudaGetLastError();
-    set_last_error("%s: out of device memory (%zu bytes)", what, need);
-    return 1;
-  }
-  A->work_bytes = need;
-  return 0;
-}
-
-}  // namespace
 
 extern "C" int samroad_apls_create(int device, const SamRoadAplsCaps* caps, samroad_apls_t* out) {
   SRB_REQUIRE(out != nullptr && caps != nullptr, "samroad_apls_create: null argument");
@@ -382,11 +376,7 @@ extern "C" int samroad_apls_create(int device, const SamRoadAplsCaps* caps, samr
               "samroad_apls_create: capacities must be positive");
   SRB_REQUIRE(caps->max_nodes <= (1 << 26) && caps->max_arcs <= (1 << 28) && caps->max_control_points <= (1 << 16),
               "samroad_apls_create: a capacity is larger than this build supports");
-  int ndev = 0;
-  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
-  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
-  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
-  SRB_CUDA_OK(cudaSetDevice(device));
+  if (int rc = open_device(device)) return rc;
   int optin = 0;
   SRB_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
   SRB_CUDA_OK(cudaFuncSetAttribute(sssp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
@@ -405,9 +395,6 @@ extern "C" int samroad_apls_destroy(samroad_apls_t A) {
   if (!A) return 0;
   cudaSetDevice(A->device);
   cudaStreamSynchronize(A->stream);
-  for (int k = 0; k < 2; ++k)
-    if (A->ll[k]) cudaFree(A->ll[k]);
-  if (A->work) cudaFree(A->work);
   cudaStreamDestroy(A->stream);
   delete A;
   return 0;
@@ -423,16 +410,12 @@ extern "C" int samroad_apls_upload_graph(samroad_apls_t A, int which, int32_t n_
               A->caps.max_nodes);
   SRB_REQUIRE(n_nodes == 0 || (latlon && row_start), "%s: null argument", what);
   const int32_t m = n_nodes ? row_start[n_nodes] : 0;
-  if (n_nodes) {
-    SRB_REQUIRE(row_start[0] == 0, "%s: adjacency offsets must start at 0", what);
-    for (int32_t i = 0; i < n_nodes; ++i)
-      SRB_REQUIRE(row_start[i + 1] >= row_start[i], "%s: adjacency offsets decrease at %d", what, i);
-  }
+  if (n_nodes)
+    if (int rc = check_csr(what, n_nodes, row_start, col)) return rc;
   SRB_REQUIRE(m <= A->caps.max_arcs, "%s: a graph of %d arcs exceeds max_arcs = %d", what, m, A->caps.max_arcs);
-  SRB_REQUIRE(m == 0 || (col && weight), "%s: null adjacency", what);
+  SRB_REQUIRE(m == 0 || weight, "%s: null adjacency", what);
   int64_t total = 0;
   for (int32_t e = 0; e < m; ++e) {
-    SRB_REQUIRE(col[e] >= 0 && col[e] < n_nodes, "%s: neighbour %d out of range", what, col[e]);
     SRB_REQUIRE(weight[e] >= 0, "%s: arc %d has a negative weight", what, e);
     total += weight[e];
   }
@@ -443,19 +426,9 @@ extern "C" int samroad_apls_upload_graph(samroad_apls_t A, int which, int32_t n_
   SRB_CUDA_OK(cudaSetDevice(A->device));
   HostGraph& g = A->host[which];
   g.n = 0;
-  if (n_nodes > 0 && 16ull * n_nodes > A->llcap[which]) {
-    if (A->ll[which]) cudaFree(A->ll[which]);
-    A->ll[which] = nullptr;
-    A->llcap[which] = 0;
-    if (cudaMalloc(&A->ll[which], 16ull * n_nodes) != cudaSuccess) {
-      cudaGetLastError();
-      set_last_error("%s: out of device memory for a graph of %d nodes", what, n_nodes);
-      return 1;
-    }
-    A->llcap[which] = 16ull * n_nodes;
-  }
-  if (n_nodes > 0) {
-    SRB_CUDA_OK(cudaMemcpyAsync(A->ll[which], latlon, 16ull * n_nodes, cudaMemcpyHostToDevice, A->stream));
+  if (n_nodes > 0) {   // calls are synchronous: nothing of this handle still reads the old buffer
+    if (A->ll[which].reserve(16ull * n_nodes, what)) return 1;
+    SRB_CUDA_OK(cudaMemcpyAsync(A->ll[which].get(), latlon, 16ull * n_nodes, cudaMemcpyHostToDevice, A->stream));
     SRB_CUDA_OK(cudaStreamSynchronize(A->stream));
   }
   g.off.assign(row_start, row_start + (n_nodes ? n_nodes + 1 : 0));
@@ -527,15 +500,20 @@ extern "C" int samroad_apls_candidates(samroad_apls_t A, int which, int32_t n_qu
     return 0;
   }
   SRB_CUDA_OK(cudaSetDevice(A->device));
-  const size_t qb = align_up(16ull * n_queries), ob = align_up(4ull * kK * n_queries);
-  if (ensure_work(A, qb + ob, what)) return 1;
-  char* base = static_cast<char*>(A->work);
-  double* dq = reinterpret_cast<double*>(base);
-  int32_t* dout = reinterpret_cast<int32_t*>(base + qb);
+  double* dq = nullptr;
+  int32_t* dout = nullptr;
+  auto carve = [&](void* base) {
+    Layout L(base);
+    dq = L.take<double>(2ull * n_queries);
+    dout = L.take<int32_t>(1ull * kK * n_queries);
+    return L.bytes();
+  };
+  if (A->work.reserve(carve(nullptr), what)) return 1;
+  carve(A->work.get());
   cudaStream_t st = A->stream;
   SRB_CUDA_OK(cudaMemcpyAsync(dq, query_latlon, 16ull * n_queries, cudaMemcpyHostToDevice, st));
-  knn_kernel<<<(n_queries + kKnnWarps - 1) / kKnnWarps, 32 * kKnnWarps, 0, st>>>(A->ll[which], n, dq, n_queries,
-                                                                                  dout);
+  knn_kernel<<<(n_queries + kKnnWarps - 1) / kKnnWarps, 32 * kKnnWarps, 0, st>>>(A->ll[which].as<double>(), n, dq,
+                                                                                  n_queries, dout);
   note_launch(1);
   SRB_CUDA_OK(cudaGetLastError());
   SRB_CUDA_OK(cudaMemcpyAsync(out, dout, 4ull * kK * n_queries, cudaMemcpyDeviceToHost, st));
@@ -587,7 +565,9 @@ extern "C" int samroad_apls_one_way(samroad_apls_t A, int gt_role, int32_t n_cp,
   int sms = 0;
   SRB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, A->device));
   const int32_t ntmax = std::max(ntg, ntp);
-  const size_t per_cta = align_up(4ull * ntmax) + 2 * align_up(static_cast<size_t>(ntmax));
+  Layout cta(nullptr);
+  sssp_scratch(cta, ntmax);
+  const size_t per_cta = cta.bytes();
   const bool in_smem = per_cta <= static_cast<size_t>(A->smem_optin);
   const int njobs = ng + np_;
   int sssp_grid = std::max(1, std::min(njobs, 4 * sms));
@@ -595,29 +575,34 @@ extern "C" int samroad_apls_one_way(samroad_apls_t A, int gt_role, int32_t n_cp,
   // device layout: contracted graphs, sources, per-cp indices, matrices, partials, and (global path) scratch
   const std::vector<int32_t>* arrs[] = {&cg.off, &cg.dst, &cg.w, &cg.src, &cpr.off, &cpr.dst, &cpr.w, &cpr.src, &gi,
                                         &pi};
-  size_t need = 0;
-  for (auto* a : arrs) need += align_up(std::max<size_t>(4 * a->size(), 4));
-  const size_t mg = align_up(std::max<size_t>(4ull * ng * ng, 4)), mp = align_up(std::max<size_t>(4ull * np_ * np_, 4));
-  const size_t pb = align_up(sizeof(PairPartial) * pair_grid);
-  const size_t scratch = in_smem ? 0 : per_cta * sssp_grid;
-  need += mg + mp + pb + scratch;
-  if (ensure_work(A, need, what)) return 1;
-  char* base = static_cast<char*>(A->work);
+  // device layout: contracted graphs, sources and per-cp indices (each at least one element, sent in one copy),
+  // then the matrices, the partials and (global path) the scratch
+  int32_t* dptr[10];
+  int32_t *dmg = nullptr, *dmp = nullptr;
+  PairPartial* dpart = nullptr;
+  char* dscratch = nullptr;
+  size_t staged = 0;
+  auto carve = [&](void* base) {
+    Layout L(base);
+    for (int k = 0; k < 10; ++k) dptr[k] = L.take<int32_t>(std::max<size_t>(arrs[k]->size(), 1));
+    staged = L.bytes();
+    dmg = L.take<int32_t>(std::max<size_t>(1ull * ng * ng, 1));
+    dmp = L.take<int32_t>(std::max<size_t>(1ull * np_ * np_, 1));
+    dpart = L.take<PairPartial>(pair_grid);
+    dscratch = L.take<char>(in_smem ? 0 : per_cta * sssp_grid);
+    return L.bytes();
+  };
+  if (A->work.reserve(carve(nullptr), what)) return 1;
+  char* base = A->work.as<char>();
+  carve(base);
+  if (in_smem) dscratch = nullptr;
   cudaStream_t st = A->stream;
   // one staging buffer, one copy
-  A->staging.assign(need - mg - mp - pb - scratch, 0);
-  const int32_t* dptr[10];
-  size_t o = 0;
-  for (int k = 0; k < 10; ++k) {
-    if (!arrs[k]->empty()) std::memcpy(A->staging.data() + o, arrs[k]->data(), 4 * arrs[k]->size());
-    dptr[k] = reinterpret_cast<const int32_t*>(base + o);
-    o += align_up(std::max<size_t>(4 * arrs[k]->size(), 4));
-  }
-  SRB_CUDA_OK(cudaMemcpyAsync(base, A->staging.data(), o, cudaMemcpyHostToDevice, st));
-  int32_t* dmg = reinterpret_cast<int32_t*>(base + o);
-  int32_t* dmp = reinterpret_cast<int32_t*>(base + o + mg);
-  PairPartial* dpart = reinterpret_cast<PairPartial*>(base + o + mg + mp);
-  char* dscratch = in_smem ? nullptr : base + o + mg + mp + pb;
+  A->staging.assign(staged, 0);
+  for (int k = 0; k < 10; ++k)
+    if (!arrs[k]->empty())
+      std::memcpy(A->staging.data() + (reinterpret_cast<char*>(dptr[k]) - base), arrs[k]->data(), 4 * arrs[k]->size());
+  SRB_CUDA_OK(cudaMemcpyAsync(base, A->staging.data(), staged, cudaMemcpyHostToDevice, st));
   SsspGraph s0{dptr[0], dptr[1], dptr[2], dptr[3], dmg, ntg, ng};
   SsspGraph s1{dptr[4], dptr[5], dptr[6], dptr[7], dmp, ntp, np_};
   if (njobs > 0) {

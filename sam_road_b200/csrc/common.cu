@@ -25,6 +25,50 @@ uint64_t launch_count(bool reset) {
   return reset ? g_launches.exchange(0) : g_launches.load();
 }
 
+template <bool kPinned>
+void Buffer<kPinned>::release() {
+  if (p_) kPinned ? cudaFreeHost(p_) : cudaFree(p_);
+  p_ = nullptr;
+  cap_ = 0;
+}
+
+template <bool kPinned>
+int Buffer<kPinned>::reserve(size_t bytes, const char* what) {
+  if (bytes <= cap_) return 0;
+  release();
+  if ((kPinned ? cudaMallocHost(&p_, bytes) : cudaMalloc(&p_, bytes)) != cudaSuccess) {
+    cudaGetLastError();   // a failed allocation must not fail the next call's launch check
+    p_ = nullptr;
+    set_last_error("%s: out of %s memory (%zu bytes)", what, kPinned ? "pinned host" : "device", bytes);
+    return 1;
+  }
+  cap_ = bytes;
+  return 0;
+}
+
+template class Buffer<false>;
+template class Buffer<true>;
+
+int open_device(int device) {
+  int ndev = 0;
+  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
+  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
+  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
+  SRB_CUDA_OK(cudaSetDevice(device));
+  return 0;
+}
+
+int check_csr(const char* what, int32_t n, const int32_t* start, const int32_t* list) {
+  SRB_REQUIRE(start[0] == 0, "%s: adjacency offsets must start at 0", what);
+  for (int32_t i = 0; i < n; ++i)
+    SRB_REQUIRE(start[i + 1] >= start[i], "%s: adjacency offsets decrease at %d", what, i);
+  const int32_t m = start[n];
+  SRB_REQUIRE(m == 0 || list != nullptr, "%s: null adjacency", what);
+  for (int32_t e = 0; e < m; ++e)
+    SRB_REQUIRE(list[e] >= 0 && list[e] < n, "%s: neighbour %d out of range", what, list[e]);
+  return 0;
+}
+
 int device_sm_count() {
   static int cached[64] = {0};     // per device: a process may drive several GPUs
   int dev = 0;

@@ -39,6 +39,76 @@ void note_launch(int n);
   } while (0)
 
 // ----------------------------------------------------------------------------------------------
+// resources: every handle owns its memory through these, so destructors free it
+// ----------------------------------------------------------------------------------------------
+// Move-only owner of one cudaMalloc (kPinned: cudaMallocHost) block.  reserve() replaces the block only
+// when `bytes` exceeds the capacity and allocates exactly `bytes`; on failure it clears the runtime's last
+// error, sets "<what>: out of device memory (<n> bytes)", leaves the buffer empty and returns 1.  It never
+// synchronises: a caller whose queued work may still use the old block synchronises before calling it.
+template <bool kPinned>
+class Buffer {
+ public:
+  Buffer() = default;
+  Buffer(Buffer&& o) noexcept : p_(o.p_), cap_(o.cap_) { o.p_ = nullptr; o.cap_ = 0; }
+  Buffer& operator=(Buffer&& o) noexcept {
+    if (this != &o) {
+      release();
+      p_ = o.p_;
+      cap_ = o.cap_;
+      o.p_ = nullptr;
+      o.cap_ = 0;
+    }
+    return *this;
+  }
+  Buffer(const Buffer&) = delete;
+  Buffer& operator=(const Buffer&) = delete;
+  ~Buffer() { release(); }
+
+  int reserve(size_t bytes, const char* what);
+  void release();
+  void* get() const { return p_; }
+  template <typename T> T* as() const { return static_cast<T*>(p_); }
+  size_t capacity() const { return cap_; }
+
+ private:
+  void* p_ = nullptr;
+  size_t cap_ = 0;
+};
+using DeviceBuffer = Buffer<false>;
+using PinnedBuffer = Buffer<true>;
+
+__host__ __device__ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Bump allocator over a workspace.  Each workspace has one function that takes its regions in order; called
+// with a null base it only counts (bytes() is then the size to allocate, and what take() returns is an
+// offset, not a pointer), called with the allocation it carves the same regions.  Every region starts at a
+// multiple of `align` from the base.
+class Layout {
+ public:
+  __host__ __device__ explicit Layout(void* base, size_t align = 256)
+      : base_(reinterpret_cast<uintptr_t>(base)), align_(align) {}
+  template <typename T>
+  __host__ __device__ T* take(size_t count) {
+    T* p = reinterpret_cast<T*>(base_ + off_);
+    off_ += align_up(sizeof(T) * count, align_);
+    return p;
+  }
+  __host__ __device__ size_t bytes() const { return off_; }
+
+ private:
+  uintptr_t base_;
+  size_t align_;
+  size_t off_ = 0;
+};
+
+// The shared start of every *_create: a device exists, `device` names one, and it becomes current.
+int open_device(int device);
+
+// CSR adjacency from outside: offsets start at 0 and never decrease, every neighbour is in [0, n), and the
+// neighbour list is present when it is not empty.  Messages start with `what`.
+int check_csr(const char* what, int32_t n, const int32_t* start, const int32_t* list);
+
+// ----------------------------------------------------------------------------------------------
 // small device helpers
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

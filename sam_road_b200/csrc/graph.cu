@@ -28,6 +28,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <thread>
 #include <vector>
 
@@ -38,28 +39,13 @@ using namespace srb;
 
 namespace {
 
-struct DevBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  DevBuf() = default;
-  DevBuf(const DevBuf&) = delete;
-  DevBuf& operator=(const DevBuf&) = delete;
-  ~DevBuf() { if (p) cudaFree(p); }
-  int ensure(size_t bytes) {
-    if (bytes <= cap) return 0;
-    if (p) {
-      SRB_CUDA_OK(cudaDeviceSynchronize());
-      SRB_CUDA_OK(cudaFree(p));
-      p = nullptr;
-      cap = 0;
-    }
-    const size_t want = bytes + bytes / 4 + 256;
-    SRB_CUDA_OK(cudaMalloc(&p, want));
-    cap = want;
-    return 0;
-  }
-  template <typename T> T* as() const { return static_cast<T*>(p); }
-};
+// Grows a scratch buffer to at least `bytes`, with 25 % + 256 B of slack.  Work queued on the caller's
+// stream may still read the old block, so the device is synchronised before it is replaced.
+int grow(DeviceBuffer& b, size_t bytes) {
+  if (bytes <= b.capacity()) return 0;
+  if (b.get()) SRB_CUDA_OK(cudaDeviceSynchronize());
+  return b.reserve(bytes + bytes / 4 + 256, "samroad_graph");
+}
 
 // Every count written on the device and read back by the host, one field each.  The entry points that
 // use them clear them all on entry.
@@ -81,19 +67,19 @@ constexpr size_t kPinBytes = 256;
 
 struct samroad_graph_ctx {
   int device = 0;
-  DevBuf counters;                        // one Counters
+  DeviceBuffer counters;                  // one Counters
   // keypoint extraction
-  DevBuf blk_cnt, blk_off;                // compaction scratch
-  DevBuf cand_pix[2], cand_score[2];      // candidates of the two masks, np.where order
-  DevBuf order, sorted_pix, immune;       // visiting order of one NMS pass
-  DevBuf list[3];                         // kept pixels of passes 1 / 2 / 3, visiting order
-  DevBuf cand3, cls3;                     // pass 3 input: concatenation + class (1 = keypoint mask)
-  DevBuf cell;                            // scene-sized rank/state image
-  DevBuf tile_und, round_cnt;             // NMS rounds
-  DevBuf ghist;                           // counting sort
-  void* h_pin = nullptr;                  // kPinBytes of pinned host memory for small read-backs
+  DeviceBuffer blk_cnt, blk_off;          // compaction scratch
+  DeviceBuffer cand_pix[2], cand_score[2]; // candidates of the two masks, np.where order
+  DeviceBuffer order, sorted_pix, immune; // visiting order of one NMS pass
+  DeviceBuffer list[3];                   // kept pixels of passes 1 / 2 / 3, visiting order
+  DeviceBuffer cand3, cls3;               // pass 3 input: concatenation + class (1 = keypoint mask)
+  DeviceBuffer cell;                      // scene-sized rank/state image
+  DeviceBuffer tile_und, round_cnt;       // NMS rounds
+  DeviceBuffer ghist;                     // counting sort
+  PinnedBuffer h_pin;                     // kPinBytes of pinned host memory for small read-backs
   // pair queries
-  DevBuf pts32, t_cnt, t_off, members, nbr, tile_xy;
+  DeviceBuffer pts32, t_cnt, t_off, members, nbr, tile_xy;
   std::vector<int> h_cnt, h_off;
   int N = 0, n_tiles = 0, P = 0;
   long total = 0;
@@ -101,9 +87,7 @@ struct samroad_graph_ctx {
   int max_nbr = 0;                        // K the plan was made for (fill / aggregate take K <= max_nbr)
   int nbr_stride = 16;                    // row length of nbr: 16 for max_nbr <= 16, else 32
   // aggregation
-  DevBuf adj_deg, adj_off, adj_src, adj_tgt, adj_sum, adj_cnt, adj_first, eflags, tile_soff;
-
-  ~samroad_graph_ctx() { if (h_pin) cudaFreeHost(h_pin); }
+  DeviceBuffer adj_deg, adj_off, adj_src, adj_tgt, adj_sum, adj_cnt, adj_first, eflags, tile_soff;
 };
 
 namespace {
@@ -205,8 +189,8 @@ int compact(samroad_graph_ctx* g, const F& f, int n, int* n_out_dev, cudaStream_
     SRB_CUDA_OK(cudaMemsetAsync(n_out_dev, 0, sizeof(int), st));
     return 0;
   }
-  if (int rc = g->blk_cnt.ensure(sizeof(int) * nblk)) return rc;
-  if (int rc = g->blk_off.ensure(sizeof(int) * nblk)) return rc;
+  if (int rc = grow(g->blk_cnt, sizeof(int) * nblk)) return rc;
+  if (int rc = grow(g->blk_off, sizeof(int) * nblk)) return rc;
   compact_count_kernel<F><<<nblk, 256, 0, st>>>(f, n, g->blk_cnt.as<int>());
   scan_single_block_kernel<<<1, 1024, 0, st>>>(g->blk_cnt.as<int>(), nblk, g->blk_off.as<int>(), n_out_dev);
   compact_fill_kernel<F><<<nblk, 256, 0, st>>>(f, n, g->blk_off.as<int>());
@@ -504,9 +488,9 @@ inline int blocks_for(long n, int per = 256) { return static_cast<int>((n + per 
 template <typename T>
 int read_back(samroad_graph_ctx* g, const T* dev, T* host, cudaStream_t st) {
   static_assert(sizeof(T) <= kPinBytes, "read-back larger than the pinned staging buffer");
-  SRB_CUDA_OK(cudaMemcpyAsync(g->h_pin, dev, sizeof(T), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(g->h_pin.get(), dev, sizeof(T), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
-  std::memcpy(host, g->h_pin, sizeof(T));
+  std::memcpy(host, g->h_pin.get(), sizeof(T));
   return 0;
 }
 
@@ -542,8 +526,8 @@ int host_order(samroad_graph_ctx* g, const uint8_t* key, int n, int key_dtype, s
     }
   }
   const std::vector<int64_t>& asc = pre_asc ? *pre_asc : own;
-  if (int rc = g->ghist.ensure(sizeof(int64_t) * n)) return rc;
-  SRB_CUDA_OK(cudaMemcpyAsync(g->ghist.p, asc.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
+  if (int rc = grow(g->ghist, sizeof(int64_t) * n)) return rc;
+  SRB_CUDA_OK(cudaMemcpyAsync(g->ghist.get(), asc.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
   order_from_host_kernel<<<blocks_for(n), 256, 0, st>>>(g->ghist.as<int64_t>(), n, order, err);
   note_launch();
   SRB_CUDA_OK(cudaStreamSynchronize(st));   // `asc` is pageable host memory: keep it alive until copied
@@ -554,7 +538,7 @@ int host_order(samroad_graph_ctx* g, const uint8_t* key, int n, int key_dtype, s
 int stable_order(samroad_graph_ctx* g, const uint8_t* key, int n, int32_t* order, int* scan_total,
                  cudaStream_t st) {
   const int nchunks = (n + kSortChunk - 1) / kSortChunk;
-  if (int rc = g->ghist.ensure(sizeof(int) * 256 * static_cast<size_t>(nchunks) * 2 + 16)) return rc;
+  if (int rc = grow(g->ghist, sizeof(int) * 256 * static_cast<size_t>(nchunks) * 2 + 16)) return rc;
   int* hist = g->ghist.as<int>();
   int* off = hist + 256 * static_cast<size_t>(nchunks);
   sort_hist_kernel<<<nchunks, 32, 0, st>>>(key, n, nchunks, hist);
@@ -580,9 +564,9 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
              int W, double radius, int32_t* out, PassStats* ps, cudaStream_t st) {
   *ps = PassStats{};
   if (n == 0) return 0;
-  if (int rc = g->order.ensure(sizeof(int32_t) * static_cast<size_t>(n))) return rc;
-  if (int rc = g->sorted_pix.ensure(sizeof(int32_t) * static_cast<size_t>(n))) return rc;
-  if (int rc = g->immune.ensure(static_cast<size_t>(n))) return rc;
+  if (int rc = grow(g->order, sizeof(int32_t) * static_cast<size_t>(n))) return rc;
+  if (int rc = grow(g->sorted_pix, sizeof(int32_t) * static_cast<size_t>(n))) return rc;
+  if (int rc = grow(g->immune, static_cast<size_t>(n))) return rc;
   int32_t* order = g->order.as<int32_t>();
   int32_t* sorted_pix = g->sorted_pix.as<int32_t>();
   uint8_t* immune = g->immune.as<uint8_t>();
@@ -612,18 +596,18 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
   const int d2max = static_cast<int>(std::floor(r2));   // d^2 <= r^2 on integer d^2
   const int halo = static_cast<int>(std::floor(radius));
   const size_t npx = static_cast<size_t>(H) * W;
-  if (int rc = g->cell.ensure(npx * 4)) return rc;
+  if (int rc = grow(g->cell, npx * 4)) return rc;
   uint32_t* cell = g->cell.as<uint32_t>();
   SRB_CUDA_OK(cudaMemsetAsync(cell, 0xFF, npx * 4, st));
   cell_build_kernel<<<blocks_for(n), 256, 0, st>>>(sorted_pix, immune, n, cell);
   note_launch();
   const int tx = (W + kNmsTile - 1) / kNmsTile, ty = (H + kNmsTile - 1) / kNmsTile;
   constexpr int kMaxRounds = 4096;
-  if (int rc = g->round_cnt.ensure(sizeof(int) * kMaxRounds)) return rc;
-  if (int rc = g->tile_und.ensure(sizeof(int) * tx * ty)) return rc;
+  if (int rc = grow(g->round_cnt, sizeof(int) * kMaxRounds)) return rc;
+  if (int rc = grow(g->tile_und, sizeof(int) * tx * ty)) return rc;
   int* round_cnt = g->round_cnt.as<int>();
   SRB_CUDA_OK(cudaMemsetAsync(round_cnt, 0, sizeof(int) * kMaxRounds, st));
-  SRB_CUDA_OK(cudaMemsetAsync(g->tile_und.p, 0x01, sizeof(int) * tx * ty, st));
+  SRB_CUDA_OK(cudaMemsetAsync(g->tile_und.get(), 0x01, sizeof(int) * tx * ty, st));
   const bool tiled = halo <= kNmsMaxHalo;
   const int SH = kNmsTile + 2 * halo;
   const size_t smem = tiled ? (static_cast<size_t>(SH) * (SH + 1) + 2 * halo + 1) * 4 + kNmsTile * kNmsTile * 2 : 0;
@@ -663,20 +647,12 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
 // =================================================================================================
 extern "C" int samroad_graph_create(int device, samroad_graph_t* out) {
   SRB_REQUIRE(out != nullptr, "samroad_graph_create: null argument");
-  int ndev = 0;
-  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
-  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
-  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
-  SRB_CUDA_OK(cudaSetDevice(device));
-  samroad_graph_ctx* g = new samroad_graph_ctx();
+  if (int rc = open_device(device)) return rc;
+  std::unique_ptr<samroad_graph_ctx> g(new samroad_graph_ctx());
   g->device = device;
-  if (cudaMallocHost(&g->h_pin, kPinBytes) != cudaSuccess) {
-    delete g;
-    set_last_error("samroad_graph_create: cudaMallocHost failed");
-    return 1;
-  }
-  if (g->counters.ensure(sizeof(Counters)) != 0) { delete g; return 1; }
-  *out = g;
+  if (g->h_pin.reserve(kPinBytes, "samroad_graph_create")) return 1;
+  if (int rc = grow(g->counters, sizeof(Counters))) return rc;
+  *out = g.release();
   return 0;
 }
 
@@ -711,8 +687,8 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
 
   // candidates of both masks (np.where order).  Worst case every pixel qualifies.
   for (int m = 0; m < 2; ++m) {
-    if (int rc = g->cand_pix[m].ensure(sizeof(int32_t) * static_cast<size_t>(npx))) return rc;
-    if (int rc = g->cand_score[m].ensure(static_cast<size_t>(npx))) return rc;
+    if (int rc = grow(g->cand_pix[m], sizeof(int32_t) * static_cast<size_t>(npx))) return rc;
+    if (int rc = grow(g->cand_score[m], static_cast<size_t>(npx))) return rc;
     MaskCand mc{masks[m], thr_to_int(thr[m]), g->cand_pix[m].as<int32_t>(), g->cand_score[m].as<uint8_t>()};
     if (int rc = compact(g, mc, npx, &ctr->cand[m], st)) return rc;
   }
@@ -733,7 +709,7 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
     for (int m = 0; m < 2; ++m) {
       keys[m].resize(n_cand[m]);
       if (n_cand[m])
-        SRB_CUDA_OK(cudaMemcpyAsync(keys[m].data(), g->cand_score[m].p, n_cand[m], cudaMemcpyDeviceToHost, st));
+        SRB_CUDA_OK(cudaMemcpyAsync(keys[m].data(), g->cand_score[m].get(), n_cand[m], cudaMemcpyDeviceToHost, st));
     }
     SRB_CUDA_OK(cudaStreamSynchronize(st));
     const int n3p = n_cand[0] + n_cand[1];
@@ -758,7 +734,7 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
   PassStats ps[3];
   for (int m = 0; m < 2; ++m) {
     const int n = n_cand[m];
-    if (int rc = g->list[m].ensure(sizeof(int32_t) * static_cast<size_t>(n > 0 ? n : 1))) return rc;
+    if (int rc = grow(g->list[m], sizeof(int32_t) * static_cast<size_t>(n > 0 ? n : 1))) return rc;
     if (int rc = nms_pass(g, g->cand_pix[m].as<int32_t>(), g->cand_score[m].as<uint8_t>(), n, SAMROAD_U8, argsort,
                           user, have_pre ? &pre_asc[m] : nullptr, m == 0 ? "mask 0" : "mask 1", H, W, radius[m],
                           g->list[m].as<int32_t>(), &ps[m], st))
@@ -769,9 +745,9 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
   // sorts float64 priorities here, whose ties NumPy orders differently from uint8 ones (DESIGN.md §9).
   const int m0 = ps[0].kept, m1 = ps[1].kept, n3 = m0 + m1;
   if (n3 > 0) {
-    if (int rc = g->cand3.ensure(sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
-    if (int rc = g->cls3.ensure(static_cast<size_t>(n3))) return rc;
-    if (int rc = g->list[2].ensure(sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
+    if (int rc = grow(g->cand3, sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
+    if (int rc = grow(g->cls3, static_cast<size_t>(n3))) return rc;
+    if (int rc = grow(g->list[2], sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
     concat_kernel<<<blocks_for(n3), 256, 0, st>>>(g->list[0].as<int32_t>(), m0, g->list[1].as<int32_t>(), m1,
                                                   g->cand3.as<int32_t>(), g->cls3.as<uint8_t>());
     note_launch();
@@ -956,22 +932,22 @@ extern "C" int samroad_pair_queries_plan_k(samroad_graph_t g, const int64_t* poi
   g->h_cnt.assign(n_tiles, 0);
   g->h_off.assign(n_tiles + 1, 0);
   g->total = 0;
-  if (int rc = g->tile_xy.ensure(sizeof(int32_t) * 2 * n_tiles)) return rc;
-  if (int rc = g->t_cnt.ensure(sizeof(int) * n_tiles)) return rc;
-  if (int rc = g->t_off.ensure(sizeof(int) * (n_tiles + 1))) return rc;
-  SRB_CUDA_OK(cudaMemcpyAsync(g->tile_xy.p, tile_xy_host, sizeof(int32_t) * 2 * n_tiles, cudaMemcpyHostToDevice, st));
+  if (int rc = grow(g->tile_xy, sizeof(int32_t) * 2 * n_tiles)) return rc;
+  if (int rc = grow(g->t_cnt, sizeof(int) * n_tiles)) return rc;
+  if (int rc = grow(g->t_off, sizeof(int) * (n_tiles + 1))) return rc;
+  SRB_CUDA_OK(cudaMemcpyAsync(g->tile_xy.get(), tile_xy_host, sizeof(int32_t) * 2 * n_tiles, cudaMemcpyHostToDevice, st));
   if (N == 0) {
-    SRB_CUDA_OK(cudaMemsetAsync(g->t_cnt.p, 0, sizeof(int) * n_tiles, st));
-    SRB_CUDA_OK(cudaMemsetAsync(g->t_off.p, 0, sizeof(int) * (n_tiles + 1), st));
+    SRB_CUDA_OK(cudaMemsetAsync(g->t_cnt.get(), 0, sizeof(int) * n_tiles, st));
+    SRB_CUDA_OK(cudaMemsetAsync(g->t_off.get(), 0, sizeof(int) * (n_tiles + 1), st));
     SRB_CUDA_OK(cudaStreamSynchronize(st));
     for (int t = 0; t < n_tiles; ++t) tile_counts_host[t] = 0;
     return 0;
   }
-  if (int rc = g->pts32.ensure(sizeof(int32_t) * 2 * static_cast<size_t>(N))) return rc;
+  if (int rc = grow(g->pts32, sizeof(int32_t) * 2 * static_cast<size_t>(N))) return rc;
   points_to_i32_kernel<<<blocks_for(2L * N), 256, 0, st>>>(points_xy, 2 * N, g->pts32.as<int32_t>());
   tile_count_kernel<<<n_tiles, 256, 0, st>>>(g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P, g->t_cnt.as<int>());
   note_launch(2);
-  SRB_CUDA_OK(cudaMemcpyAsync(g->h_cnt.data(), g->t_cnt.p, sizeof(int) * n_tiles, cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(g->h_cnt.data(), g->t_cnt.get(), sizeof(int) * n_tiles, cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   int max_cnt = 0;
   for (int t = 0; t < n_tiles; ++t) {
@@ -981,10 +957,10 @@ extern "C" int samroad_pair_queries_plan_k(samroad_graph_t g, const int64_t* poi
   }
   g->total = g->h_off[n_tiles];
   SRB_REQUIRE(g->total * g->max_nbr < 2147483647L, "samroad_pair_queries_plan: %ld (tile, point) instances is too many", g->total);
-  SRB_CUDA_OK(cudaMemcpyAsync(g->t_off.p, g->h_off.data(), sizeof(int) * (n_tiles + 1), cudaMemcpyHostToDevice, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(g->t_off.get(), g->h_off.data(), sizeof(int) * (n_tiles + 1), cudaMemcpyHostToDevice, st));
   if (g->total == 0) { SRB_CUDA_OK(cudaStreamSynchronize(st)); return 0; }
-  if (int rc = g->members.ensure(sizeof(int32_t) * static_cast<size_t>(g->total))) return rc;
-  if (int rc = g->nbr.ensure(sizeof(int32_t) * g->nbr_stride * static_cast<size_t>(g->total))) return rc;
+  if (int rc = grow(g->members, sizeof(int32_t) * static_cast<size_t>(g->total))) return rc;
+  if (int rc = grow(g->nbr, sizeof(int32_t) * g->nbr_stride * static_cast<size_t>(g->total))) return rc;
   tile_fill_kernel<<<n_tiles, 256, 0, st>>>(g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P, g->t_off.as<int>(),
                                             g->members.as<int32_t>());
   const dim3 knn_grid(n_tiles, (max_cnt + 127) / 128);
@@ -1226,10 +1202,10 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
               "planned for %d", K, g->max_nbr);
   SRB_REQUIRE(topo_scores != nullptr, "samroad_aggregate_edges: null scores");
   const int32_t* pts = g->pts32.as<int32_t>();
-  if (int rc = g->adj_deg.ensure(sizeof(int) * static_cast<size_t>(N))) return rc;
-  if (int rc = g->adj_off.ensure(sizeof(int) * (static_cast<size_t>(N) + 1))) return rc;
-  if (int rc = g->tile_soff.ensure(sizeof(int64_t) * g->n_tiles)) return rc;
-  SRB_CUDA_OK(cudaMemcpyAsync(g->tile_soff.p, tile_score_offset_host, sizeof(int64_t) * g->n_tiles,
+  if (int rc = grow(g->adj_deg, sizeof(int) * static_cast<size_t>(N))) return rc;
+  if (int rc = grow(g->adj_off, sizeof(int) * (static_cast<size_t>(N) + 1))) return rc;
+  if (int rc = grow(g->tile_soff, sizeof(int64_t) * g->n_tiles)) return rc;
+  SRB_CUDA_OK(cudaMemcpyAsync(g->tile_soff.get(), tile_score_offset_host, sizeof(int64_t) * g->n_tiles,
                               cudaMemcpyHostToDevice, st));
   Counters* ctr = g->counters.as<Counters>();
   SRB_CUDA_OK(cudaMemsetAsync(ctr, 0, sizeof(Counters), st));
@@ -1243,17 +1219,17 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
   SRB_CUDA_OK(cudaMemcpyAsync(g->adj_off.as<int>() + N, &ctr->nnz, sizeof(int), cudaMemcpyDeviceToDevice, st));
   if (nnz == 0) return 0;
   const size_t nz = static_cast<size_t>(nnz);
-  if (int rc = g->adj_src.ensure(4 * nz)) return rc;
-  if (int rc = g->adj_tgt.ensure(4 * nz)) return rc;
-  if (int rc = g->adj_sum.ensure(4 * nz)) return rc;
-  if (int rc = g->adj_cnt.ensure(4 * nz)) return rc;
-  if (int rc = g->adj_first.ensure(4 * nz)) return rc;
+  if (int rc = grow(g->adj_src, 4 * nz)) return rc;
+  if (int rc = grow(g->adj_tgt, 4 * nz)) return rc;
+  if (int rc = grow(g->adj_sum, 4 * nz)) return rc;
+  if (int rc = grow(g->adj_cnt, 4 * nz)) return rc;
+  if (int rc = grow(g->adj_first, 4 * nz)) return rc;
   const long n_entries = g->total * K;
-  if (int rc = g->eflags.ensure(4 * static_cast<size_t>(n_entries))) return rc;
-  SRB_CUDA_OK(cudaMemsetAsync(g->adj_sum.p, 0, 4 * nz, st));
-  SRB_CUDA_OK(cudaMemsetAsync(g->adj_cnt.p, 0, 4 * nz, st));
-  SRB_CUDA_OK(cudaMemsetAsync(g->adj_first.p, 0xFF, 4 * nz, st));
-  SRB_CUDA_OK(cudaMemsetAsync(g->eflags.p, 0xFF, 4 * static_cast<size_t>(n_entries), st));
+  if (int rc = grow(g->eflags, 4 * static_cast<size_t>(n_entries))) return rc;
+  SRB_CUDA_OK(cudaMemsetAsync(g->adj_sum.get(), 0, 4 * nz, st));
+  SRB_CUDA_OK(cudaMemsetAsync(g->adj_cnt.get(), 0, 4 * nz, st));
+  SRB_CUDA_OK(cudaMemsetAsync(g->adj_first.get(), 0xFF, 4 * nz, st));
+  SRB_CUDA_OK(cudaMemsetAsync(g->eflags.get(), 0xFF, 4 * static_cast<size_t>(n_entries), st));
   adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, g->adj_off.as<int>(), nullptr,
                                                  g->adj_src.as<int32_t>(), g->adj_tgt.as<int32_t>(), nullptr);
   const AggArgs args{pts, N, g->tile_xy.as<int32_t>(), g->n_tiles, g->P, g->t_cnt.as<int>(), g->t_off.as<int>(),

@@ -576,13 +576,13 @@ struct samroad_labels_ctx {
   SamRoadLabelCfg cfg;
   int device = 0;
   std::vector<SceneDev> scenes;
-  std::vector<void*> allocs;
-  SceneDev* d_scenes = nullptr;
+  std::vector<DeviceBuffer> allocs;   // the uploaded scenes' arrays
+  DeviceBuffer d_scenes;              // SceneDev [d_scenes_n]
   int d_scenes_n = -1;
   int B_alloc = 0;
-  void* work_mem = nullptr;
+  DeviceBuffer work_mem;
   Work work{};
-  int32_t* h_read = nullptr;   // pinned [1 + B]: status word, then the survivor counts
+  PinnedBuffer h_read;         // int32 [1 + B]: status word, then the survivor counts
   size_t smem_patch = 0;
 };
 
@@ -611,7 +611,7 @@ int cfg_check(const SamRoadLabelCfg* c) {
 Params make_params(const samroad_labels_ctx* L) {
   const SamRoadLabelCfg& c = L->cfg;
   Params p;
-  p.scenes = L->d_scenes;
+  p.scenes = L->d_scenes.as<SceneDev>();
   p.n_scenes = static_cast<int>(L->scenes.size());
   p.P = c.patch_size;
   p.size = c.image_size;
@@ -628,50 +628,26 @@ Params make_params(const samroad_labels_ctx* L) {
   return p;
 }
 
-int ensure_work(samroad_labels_ctx* L, int B) {
-  if (L->d_scenes_n != static_cast<int>(L->scenes.size())) {
-    if (L->d_scenes) cudaFree(L->d_scenes);
-    L->d_scenes = nullptr;
-    SRB_CUDA_OK(cudaMalloc(&L->d_scenes, sizeof(SceneDev) * L->scenes.size()));
-    SRB_CUDA_OK(cudaMemcpy(L->d_scenes, L->scenes.data(), sizeof(SceneDev) * L->scenes.size(),
-                           cudaMemcpyHostToDevice));
-    L->d_scenes_n = static_cast<int>(L->scenes.size());
-  }
-  if (B <= L->B_alloc) return 0;
-  if (L->work_mem) cudaFree(L->work_mem);
-  if (L->h_read) cudaFreeHost(L->h_read);
-  L->work_mem = nullptr;
-  L->h_read = nullptr;
-  L->B_alloc = 0;
-  const size_t cap = L->cfg.max_patch_points, S = L->cfg.topo_sample_num, nb = B;
-  // the last region is the status word followed by nsurv [B], so that one copy of 1 + B words reads both for
-  // any batch up to B_alloc (a status word after nsurv [B_alloc] would be missed by smaller batches)
-  const size_t bytes[] = {16 * nb, 8 * cap * nb, 8 * S * nb, 16 * cap * nb, 4 * cap * nb, 4 * cap * nb,
-                          16 * cap * nb, 8 * cap * nb, 4 * S * nb, 4 * (nb + 1)};
-  size_t total = 0;
-  for (size_t x : bytes) total += (x + 255) & ~static_cast<size_t>(255);
-  SRB_CUDA_OK(cudaMalloc(&L->work_mem, total));
-  SRB_CUDA_OK(cudaMallocHost(&L->h_read, sizeof(int32_t) * (B + 1)));
-  char* q = static_cast<char*>(L->work_mem);
-  void* ptrs[10];
-  for (int i = 0; i < 10; ++i) {
-    ptrs[i] = q;
-    q += (bytes[i] + 255) & ~static_cast<size_t>(255);
-  }
-  Work& w = L->work;
-  w.patch = static_cast<int32_t*>(ptrs[0]);
-  w.score_u = static_cast<double*>(ptrs[1]);
-  w.src_u = static_cast<double*>(ptrs[2]);
-  w.noise = static_cast<double*>(ptrs[3]);
-  w.cand = static_cast<int32_t*>(ptrs[4]);
-  w.surv = static_cast<int32_t*>(ptrs[5]);
-  w.sxy = static_cast<double*>(ptrs[6]);
-  w.cdf = static_cast<double*>(ptrs[7]);
-  w.src = static_cast<int32_t*>(ptrs[8]);
-  w.status = static_cast<int32_t*>(ptrs[9]);
+// The work area of a batch of nb patches; *bytes is its size.  The last region is the status word followed by
+// nsurv [nb], so that one copy of 1 + B words reads both for any batch up to B_alloc (a status word after
+// nsurv [B_alloc] would be missed by smaller batches).
+Work layout_work(const SamRoadLabelCfg& c, size_t nb, void* base, size_t* bytes) {
+  const size_t cap = c.max_patch_points, S = c.topo_sample_num;
+  Layout L(base);
+  Work w;
+  w.patch = L.take<int32_t>(4 * nb);
+  w.score_u = L.take<double>(cap * nb);
+  w.src_u = L.take<double>(S * nb);
+  w.noise = L.take<double>(2 * cap * nb);
+  w.cand = L.take<int32_t>(cap * nb);
+  w.surv = L.take<int32_t>(cap * nb);
+  w.sxy = L.take<double>(2 * cap * nb);
+  w.cdf = L.take<double>(cap * nb);
+  w.src = L.take<int32_t>(S * nb);
+  w.status = L.take<int32_t>(nb + 1);
   w.nsurv = w.status + 1;
-  L->B_alloc = B;
-  return 0;
+  *bytes = L.bytes();
+  return w;
 }
 
 int run_batch(samroad_labels_ctx* L, int B, unsigned long long seed, const int32_t* patches, const double* score_u,
@@ -684,8 +660,23 @@ int run_batch(samroad_labels_ctx* L, int B, unsigned long long seed, const int32
   SRB_REQUIRE(rgb && kp && road && points && pairs && connected && valid && n_points, "%s: null output", what);
   SRB_CUDA_OK(cudaSetDevice(L->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = ensure_work(L, B)) return rc;
+  // calls are synchronous: no earlier call still uses a block that is replaced here
+  if (L->d_scenes_n != static_cast<int>(L->scenes.size())) {
+    const size_t bytes = sizeof(SceneDev) * L->scenes.size();
+    if (L->d_scenes.reserve(bytes, what)) return 1;
+    SRB_CUDA_OK(cudaMemcpy(L->d_scenes.get(), L->scenes.data(), bytes, cudaMemcpyHostToDevice));
+    L->d_scenes_n = static_cast<int>(L->scenes.size());
+  }
+  if (B > L->B_alloc) {
+    L->B_alloc = 0;
+    size_t bytes = 0;
+    layout_work(L->cfg, B, nullptr, &bytes);
+    if (L->work_mem.reserve(bytes, what) || L->h_read.reserve(sizeof(int32_t) * (B + 1), what)) return 1;
+    L->work = layout_work(L->cfg, B, L->work_mem.get(), &bytes);
+    L->B_alloc = B;
+  }
   Work w = L->work;
+  int32_t* h_read = L->h_read.as<int32_t>();
   const Params p = make_params(L);
   const size_t cap = p.cap, S = p.S;
   if (injected) {   // caller-filled draws: copied into the batch arrays, the stages below are unchanged
@@ -706,16 +697,16 @@ int run_batch(samroad_labels_ctx* L, int B, unsigned long long seed, const int32
       p, w, pairs, connected, valid);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(3);
-  SRB_CUDA_OK(cudaMemcpyAsync(L->h_read, w.status, sizeof(int32_t) * (B + 1), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(h_read, w.status, sizeof(int32_t) * (B + 1), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
-  const int status = L->h_read[0];
+  const int status = h_read[0];
   SRB_REQUIRE(!(status & kBadPatch), "%s: a patch names a missing scene, an origin outside [%d, %d] or a "
               "rotation outside 0..3", what, p.lo, p.hi);
   SRB_REQUIRE(!(status & kOverCap), "%s: a patch holds more than max_patch_points=%d candidates", what, p.cap);
   SRB_REQUIRE(!(status & kBfsOverflow), "%s: a BFS reached more than %d nodes within NEIGHBOR_RADIUS // 4 = %d "
               "steps", what, kBfsList, p.depth);
   int N = 1;
-  for (int b = 0; b < B; ++b) N = std::max(N, L->h_read[1 + b]);
+  for (int b = 0; b < B; ++b) N = std::max(N, h_read[1 + b]);
   points_kernel<<<dim3(grid_of(N, 128), B), 128, 0, st>>>(p, w, N, points);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(1);
@@ -735,11 +726,7 @@ extern "C" int samroad_labels_create(int device, const SamRoadLabelCfg* cfg, sam
   SRB_REQUIRE(out != nullptr, "samroad_labels_create: null argument");
   if (int rc = cfg_check(cfg)) return rc;
   const size_t smem = patch_smem_bytes(cfg->max_patch_points);
-  int ndev = 0;
-  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
-  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
-  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
-  SRB_CUDA_OK(cudaSetDevice(device));
+  if (int rc = open_device(device)) return rc;
   int optin = 0;
   SRB_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
   SRB_REQUIRE(smem + 32 * 4 + 64 <= static_cast<size_t>(optin),
@@ -760,10 +747,6 @@ extern "C" int samroad_labels_destroy(samroad_labels_t L) {
   if (!L) return 0;
   cudaSetDevice(L->device);
   cudaDeviceSynchronize();
-  for (void* a : L->allocs) cudaFree(a);
-  if (L->d_scenes) cudaFree(L->d_scenes);
-  if (L->work_mem) cudaFree(L->work_mem);
-  if (L->h_read) cudaFreeHost(L->h_read);
   delete L;
   return 0;
 }
@@ -776,9 +759,8 @@ extern "C" int samroad_labels_upload(samroad_labels_t L, const uint8_t* rgb, con
   SRB_REQUIRE(rgb && keypoint_mask && road_mask && points && flags && weights && adj_start && scene_index,
               "samroad_labels_upload: null argument");
   SRB_REQUIRE(n_points >= 1, "samroad_labels_upload: a scene needs at least one graph point (got %d)", n_points);
-  SRB_REQUIRE(adj_start[0] == 0, "samroad_labels_upload: adjacency offsets must start at 0");
+  if (int rc = check_csr("samroad_labels_upload", n_points, adj_start, adj)) return rc;
   for (int32_t i = 0; i < n_points; ++i) {
-    SRB_REQUIRE(adj_start[i + 1] >= adj_start[i], "samroad_labels_upload: adjacency offsets decrease at %d", i);
     SRB_REQUIRE(std::isfinite(points[2 * i]) && std::isfinite(points[2 * i + 1]),
                 "samroad_labels_upload: point %d is not finite", i);
     // np.random.choice(p=w / w.sum()) refuses a window whose weights are all zero; the running sum would
@@ -788,9 +770,6 @@ extern "C" int samroad_labels_upload(samroad_labels_t L, const uint8_t* rgb, con
                 static_cast<double>(weights[i]));
   }
   const int32_t m = adj_start[n_points];
-  SRB_REQUIRE(m == 0 || adj != nullptr, "samroad_labels_upload: null adjacency");
-  for (int32_t e = 0; e < m; ++e)
-    SRB_REQUIRE(adj[e] >= 0 && adj[e] < n_points, "samroad_labels_upload: neighbour %d out of range", adj[e]);
   SRB_CUDA_OK(cudaSetDevice(L->device));
   const size_t px = static_cast<size_t>(L->cfg.image_size) * L->cfg.image_size;
   const size_t sizes[] = {16 * static_cast<size_t>(n_points), static_cast<size_t>(n_points),
@@ -799,8 +778,10 @@ extern "C" int samroad_labels_upload(samroad_labels_t L, const uint8_t* rgb, con
   const void* src[] = {points, flags, weights, adj_start, adj, rgb, keypoint_mask, road_mask};
   void* dst[8];
   for (int i = 0; i < 8; ++i) {
-    SRB_CUDA_OK(cudaMalloc(&dst[i], sizes[i]));
-    L->allocs.push_back(dst[i]);
+    DeviceBuffer b;
+    if (b.reserve(sizes[i], "samroad_labels_upload")) return 1;
+    dst[i] = b.get();
+    L->allocs.push_back(std::move(b));
     if (src[i] && !(i == 4 && m == 0)) SRB_CUDA_OK(cudaMemcpy(dst[i], src[i], sizes[i], cudaMemcpyHostToDevice));
   }
   SceneDev s;

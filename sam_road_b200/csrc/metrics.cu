@@ -22,6 +22,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 
 #include "common.cuh"
 #include "loss_terms.cuh"
@@ -66,38 +67,27 @@ constexpr int kTileItems = kTile / 256;
 
 struct samroad_prc_ctx {
   int device = 0;
-  PrcState* state = nullptr;       // device
+  DeviceBuffer state;              // one PrcState
   uint32_t* keys = nullptr;        // device, cap entries
-  uint32_t* alt = nullptr;         // compute: radix ping-pong buffer
-  size_t cap = 0, alt_cap = 0;
+  DeviceBuffer alt;                // compute: radix ping-pong buffer
+  size_t cap = 0;
   size_t reserved = 0;             // host upper bound of state->committed
   long long n_updates = 0;         // updates since the last reset
   // scratch of compute
-  uint32_t* hist = nullptr;        // per (digit, chunk) counts, scanned in place
-  uint32_t* tile_sums = nullptr;
-  unsigned long long* tile_cnt = nullptr;   // curve: (starts << 32 | positives) per tile, then scanned
-  size_t hist_cap = 0, tile_sums_cap = 0, tile_cnt_cap = 0;
-  // the curve of the last successful compute
-  float* thr = nullptr;            // [T]
-  float* prec = nullptr;           // [T+1]
-  float* rec = nullptr;            // [T+1]
-  long long* tps = nullptr;        // [T]
-  long long* fps = nullptr;        // [T]
+  DeviceBuffer hist;               // per (digit, chunk) counts, scanned in place
+  DeviceBuffer tile_sums;
+  DeviceBuffer tile_cnt;           // curve: (starts << 32 | positives) per tile, then scanned
+  // the curve of the last successful compute: thr [T], prec [T+1], rec [T+1], tps [T], fps [T]
+  DeviceBuffer thr, prec, rec, tps, fps;
   size_t curve_cap = 0;
   long long T = -1;                // -1: no curve
-  PrcState* h_state = nullptr;     // pinned read-back
+  PinnedBuffer h_state;            // one PrcState, pinned read-back
 
   ~samroad_prc_ctx() {
     if (keys) {   // allocated stream-ordered by samroad_prc_update
       cudaFreeAsync(keys, 0);
       cudaStreamSynchronize(0);
     }
-    for (void* p : {static_cast<void*>(state), static_cast<void*>(alt),
-                    static_cast<void*>(hist), static_cast<void*>(tile_sums), static_cast<void*>(tile_cnt),
-                    static_cast<void*>(thr), static_cast<void*>(prec), static_cast<void*>(rec),
-                    static_cast<void*>(tps), static_cast<void*>(fps)})
-      if (p) cudaFree(p);
-    if (h_state) cudaFreeHost(h_state);
   }
 };
 
@@ -105,17 +95,12 @@ namespace {
 
 inline int grid_for(long long n, int per) { return static_cast<int>((n + per - 1) / per); }
 
-// Grows a synchronously owned scratch buffer (compute synchronises anyway).
+// Grows a scratch buffer of compute to n elements of T, with 25 % + 64 elements of slack.  No
+// synchronisation: compute synchronises before it returns, so no earlier work still reads the old block.
 template <typename T>
-int ensure(T*& p, size_t& cap, size_t n) {
-  if (n <= cap) return 0;
-  if (p) SRB_CUDA_OK(cudaFree(p));
-  p = nullptr;
-  cap = 0;
-  const size_t want = n + n / 4 + 64;
-  SRB_CUDA_OK(cudaMalloc(&p, sizeof(T) * want));
-  cap = want;
-  return 0;
+int grow(DeviceBuffer& b, size_t n) {
+  if (sizeof(T) * n <= b.capacity()) return 0;
+  return b.reserve(sizeof(T) * (n + n / 4 + 64), "samroad_prc_compute");
 }
 
 __device__ __forceinline__ void refusal_note(Refusals* r, unsigned flag, unsigned long long i) {
@@ -440,7 +425,7 @@ __global__ void __launch_bounds__(256) curve_fill_kernel(const uint32_t* __restr
 }
 
 int read_state(samroad_prc_ctx* p, cudaStream_t st) {
-  SRB_CUDA_OK(cudaMemcpyAsync(p->h_state, p->state, sizeof(PrcState), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(p->h_state.get(), p->state.get(), sizeof(PrcState), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   return 0;
 }
@@ -467,39 +452,10 @@ int report_refusals(const Refusals& s, Refusals* dev, const char* what, const ch
 // accepted entries.
 int take_refusals(samroad_prc_ctx* p, const char* what, long long* committed, cudaStream_t st) {
   if (int rc = read_state(p, st)) return rc;
-  const PrcState s = *p->h_state;
+  const PrcState s = *p->h_state.as<PrcState>();
   p->reserved = s.committed;
   *committed = static_cast<long long>(s.committed);
-  return report_refusals(s.ref, &p->state->ref, what, kPrcBadText, 2, st);
-}
-
-void free_curve(samroad_prc_ctx* p) {
-  for (void** a : {reinterpret_cast<void**>(&p->thr), reinterpret_cast<void**>(&p->prec),
-                   reinterpret_cast<void**>(&p->rec), reinterpret_cast<void**>(&p->tps),
-                   reinterpret_cast<void**>(&p->fps)}) {
-    if (*a) cudaFree(*a);
-    *a = nullptr;
-  }
-  p->curve_cap = 0;
-}
-
-// The five curve arrays for T thresholds; all of them or none (curve_cap 0) after a failure.
-int ensure_curve(samroad_prc_ctx* p, size_t T) {
-  const size_t need = T + 1;
-  if (need <= p->curve_cap) return 0;
-  free_curve(p);
-  const size_t c = need + need / 4 + 64;
-  if (cudaMalloc(&p->thr, sizeof(float) * c) != cudaSuccess || cudaMalloc(&p->prec, sizeof(float) * c) != cudaSuccess ||
-      cudaMalloc(&p->rec, sizeof(float) * c) != cudaSuccess ||
-      cudaMalloc(&p->tps, sizeof(long long) * c) != cudaSuccess ||
-      cudaMalloc(&p->fps, sizeof(long long) * c) != cudaSuccess) {
-    cudaGetLastError();
-    free_curve(p);
-    set_last_error("samroad_prc_compute: out of device memory for a curve of %zu thresholds", T);
-    return 1;
-  }
-  p->curve_cap = c;
-  return 0;
+  return report_refusals(s.ref, &p->state.as<PrcState>()->ref, what, kPrcBadText, 2, st);
 }
 
 // Room for n more keys after the `reserved` ones, grown stream-ordered (no host synchronisation).
@@ -525,29 +481,31 @@ int grow_keys(samroad_prc_ctx* p, long long n, const char* what, cudaStream_t st
 // exclusive scan of m uint32 in place (values and their total < 2^32)
 int scan_u32(samroad_prc_ctx* p, uint32_t* a, long long m, cudaStream_t st) {
   const int tiles = grid_for(m, kTile);
-  if (int rc = ensure(p->tile_sums, p->tile_sums_cap, static_cast<size_t>(tiles))) return rc;
-  tile_sum_kernel<<<tiles, 256, 0, st>>>(a, m, p->tile_sums);
-  scan_one_block_kernel<uint32_t><<<1, 256, 0, st>>>(p->tile_sums, tiles);
-  tile_scan_kernel<<<tiles, 256, 0, st>>>(a, m, p->tile_sums);
+  if (int rc = grow<uint32_t>(p->tile_sums, static_cast<size_t>(tiles))) return rc;
+  uint32_t* sums = p->tile_sums.as<uint32_t>();
+  tile_sum_kernel<<<tiles, 256, 0, st>>>(a, m, sums);
+  scan_one_block_kernel<uint32_t><<<1, 256, 0, st>>>(sums, tiles);
+  tile_scan_kernel<<<tiles, 256, 0, st>>>(a, m, sums);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(3);
   return 0;
 }
 
 int radix_sort(samroad_prc_ctx* p, long long n, cudaStream_t st) {
-  if (int rc = ensure(p->alt, p->alt_cap, static_cast<size_t>(n))) return rc;
+  if (int rc = grow<uint32_t>(p->alt, static_cast<size_t>(n))) return rc;
   const int nchunks = grid_for(n, kSortChunk);
   const long long m = 256LL * nchunks;
-  if (int rc = ensure(p->hist, p->hist_cap, static_cast<size_t>(m))) return rc;
+  if (int rc = grow<uint32_t>(p->hist, static_cast<size_t>(m))) return rc;
+  uint32_t* hist = p->hist.as<uint32_t>();
   const int blocks = grid_for(nchunks, kSortWarps);
   uint32_t* src = p->keys;
-  uint32_t* dst = p->alt;
+  uint32_t* dst = p->alt.as<uint32_t>();
   for (int shift = 0; shift < 32; shift += 8) {    // 4 passes: the sorted keys end up back in p->keys
-    radix_hist_kernel<<<blocks, 32 * kSortWarps, 0, st>>>(src, n, nchunks, shift, p->hist);
+    radix_hist_kernel<<<blocks, 32 * kSortWarps, 0, st>>>(src, n, nchunks, shift, hist);
     SRB_CUDA_OK(cudaGetLastError());
     note_launch(1);
-    if (int rc = scan_u32(p, p->hist, m, st)) return rc;
-    radix_scatter_kernel<<<blocks, 32 * kSortWarps, 0, st>>>(src, n, nchunks, shift, p->hist, dst);
+    if (int rc = scan_u32(p, hist, m, st)) return rc;
+    radix_scatter_kernel<<<blocks, 32 * kSortWarps, 0, st>>>(src, n, nchunks, shift, hist, dst);
     SRB_CUDA_OK(cudaGetLastError());
     note_launch(1);
     uint32_t* t = src;
@@ -564,21 +522,13 @@ int radix_sort(samroad_prc_ctx* p, long long n, cudaStream_t st) {
 // =================================================================================================
 extern "C" int samroad_prc_create(int device, samroad_prc_t* out) {
   SRB_REQUIRE(out != nullptr, "samroad_prc_create: null argument");
-  int ndev = 0;
-  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
-  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
-  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
-  SRB_CUDA_OK(cudaSetDevice(device));
-  samroad_prc_ctx* p = new samroad_prc_ctx();
+  if (int rc = open_device(device)) return rc;
+  std::unique_ptr<samroad_prc_ctx> p(new samroad_prc_ctx());
   p->device = device;
-  if (cudaMalloc(&p->state, sizeof(PrcState)) != cudaSuccess ||
-      cudaMemset(p->state, 0, sizeof(PrcState)) != cudaSuccess ||
-      cudaMallocHost(&p->h_state, sizeof(PrcState)) != cudaSuccess) {
-    delete p;
-    set_last_error("samroad_prc_create: device or pinned allocation failed");
-    return 1;
-  }
-  *out = p;
+  if (p->state.reserve(sizeof(PrcState), "samroad_prc_create")) return 1;
+  SRB_CUDA_OK(cudaMemset(p->state.get(), 0, sizeof(PrcState)));
+  if (p->h_state.reserve(sizeof(PrcState), "samroad_prc_create")) return 1;
+  *out = p.release();
   return 0;
 }
 
@@ -593,7 +543,7 @@ extern "C" int samroad_prc_destroy(samroad_prc_t p) {
 extern "C" int samroad_prc_reset(samroad_prc_t p, void* stream) {
   SRB_REQUIRE(p != nullptr, "samroad_prc_reset: null handle");
   SRB_CUDA_OK(cudaSetDevice(p->device));
-  SRB_CUDA_OK(cudaMemsetAsync(p->state, 0, sizeof(PrcState), static_cast<cudaStream_t>(stream)));
+  SRB_CUDA_OK(cudaMemsetAsync(p->state.get(), 0, sizeof(PrcState), static_cast<cudaStream_t>(stream)));
   p->reserved = 0;
   p->n_updates = 0;
   p->T = -1;
@@ -612,12 +562,13 @@ extern "C" int samroad_prc_update(samroad_prc_t p, const float* preds, int64_t p
   SRB_CUDA_OK(cudaSetDevice(p->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = grow_keys(p, n, "samroad_prc_update", st)) return rc;
-  prc_begin_kernel<<<1, 1, 0, st>>>(p->state);
+  PrcState* state = p->state.as<PrcState>();
+  prc_begin_kernel<<<1, 1, 0, st>>>(state);
   if (target_dtype == SAMROAD_U8)
-    prc_append_kernel<true><<<grid_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, p->state);
+    prc_append_kernel<true><<<grid_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
   else
-    prc_append_kernel<false><<<grid_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, p->state);
-  prc_commit_kernel<<<1, 1, 0, st>>>(p->state, p->n_updates);
+    prc_append_kernel<false><<<grid_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
+  prc_commit_kernel<<<1, 1, 0, st>>>(state, p->n_updates);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(3);
   p->reserved += static_cast<size_t>(n);
@@ -632,9 +583,10 @@ extern "C" int samroad_prc_append_keys(samroad_prc_t p, const uint32_t* keys, in
   SRB_CUDA_OK(cudaSetDevice(p->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = grow_keys(p, n, "samroad_prc_append_keys", st)) return rc;
-  prc_begin_kernel<<<1, 1, 0, st>>>(p->state);
-  prc_append_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(keys, n, p->keys, p->state);
-  prc_commit_kernel<<<1, 1, 0, st>>>(p->state, p->n_updates);
+  PrcState* state = p->state.as<PrcState>();
+  prc_begin_kernel<<<1, 1, 0, st>>>(state);
+  prc_append_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(keys, n, p->keys, state);
+  prc_commit_kernel<<<1, 1, 0, st>>>(state, p->n_updates);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(3);
   p->reserved += static_cast<size_t>(n);
@@ -665,30 +617,40 @@ extern "C" int samroad_prc_compute(samroad_prc_t p, int64_t* counts, float* best
   SRB_REQUIRE(n > 0, "samroad_prc_compute: no entries (nothing was updated since the last reset)");
   if (int rc = radix_sort(p, n, st)) return rc;
   const int tiles = grid_for(n, kTile);
-  if (int rc = ensure(p->tile_cnt, p->tile_cnt_cap, static_cast<size_t>(tiles) + 1)) return rc;
-  curve_count_kernel<<<tiles, 256, 0, st>>>(p->keys, n, p->tile_cnt);
-  SRB_CUDA_OK(cudaMemsetAsync(p->tile_cnt + tiles, 0, sizeof(unsigned long long), st));
-  scan_one_block_kernel<unsigned long long><<<1, 256, 0, st>>>(p->tile_cnt, tiles + 1);
+  if (int rc = grow<unsigned long long>(p->tile_cnt, static_cast<size_t>(tiles) + 1)) return rc;
+  unsigned long long* tile_cnt = p->tile_cnt.as<unsigned long long>();
+  curve_count_kernel<<<tiles, 256, 0, st>>>(p->keys, n, tile_cnt);
+  SRB_CUDA_OK(cudaMemsetAsync(tile_cnt + tiles, 0, sizeof(unsigned long long), st));
+  scan_one_block_kernel<unsigned long long><<<1, 256, 0, st>>>(tile_cnt, tiles + 1);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(2);
   unsigned long long tot = 0;
-  SRB_CUDA_OK(cudaMemcpyAsync(&tot, p->tile_cnt + tiles, sizeof(tot), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(&tot, tile_cnt + tiles, sizeof(tot), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   const long long T = static_cast<long long>(tot >> 32), n_pos = static_cast<long long>(tot & 0xFFFFFFFFull);
-  if (int rc = ensure_curve(p, static_cast<size_t>(T))) return rc;
-  SRB_CUDA_OK(cudaMemsetAsync(&p->state->best, 0, sizeof(unsigned long long), st));
-  curve_fill_kernel<<<tiles, 256, 0, st>>>(p->keys, n, p->tile_cnt, n_pos, T, p->thr, p->prec, p->rec, p->tps,
-                                           p->fps, p->state);
+  if (static_cast<size_t>(T) + 1 > p->curve_cap) {   // the five curve arrays, all grown together
+    const size_t c = T + 1 + (T + 1) / 4 + 64;
+    p->curve_cap = 0;
+    for (DeviceBuffer* b : {&p->thr, &p->prec, &p->rec})
+      if (b->reserve(sizeof(float) * c, "samroad_prc_compute")) return 1;
+    for (DeviceBuffer* b : {&p->tps, &p->fps})
+      if (b->reserve(sizeof(long long) * c, "samroad_prc_compute")) return 1;
+    p->curve_cap = c;
+  }
+  SRB_CUDA_OK(cudaMemsetAsync(&p->state.as<PrcState>()->best, 0, sizeof(unsigned long long), st));
+  curve_fill_kernel<<<tiles, 256, 0, st>>>(p->keys, n, tile_cnt, n_pos, T, p->thr.as<float>(), p->prec.as<float>(),
+                                           p->rec.as<float>(), p->tps.as<long long>(), p->fps.as<long long>(),
+                                           p->state.as<PrcState>());
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(1);
   if (int rc = read_state(p, st)) return rc;
-  const unsigned long long bk = p->h_state->best;
+  const unsigned long long bk = p->h_state.as<PrcState>()->best;
   const long long bi = static_cast<long long>(0xFFFFFFFFull - (bk & 0xFFFFFFFFull));
   SRB_REQUIRE(bk != 0 && bi >= 0 && bi < T, "samroad_prc_compute: internal error (no best point)");
   float v[3];
-  SRB_CUDA_OK(cudaMemcpyAsync(&v[0], p->thr + bi, sizeof(float), cudaMemcpyDeviceToHost, st));
-  SRB_CUDA_OK(cudaMemcpyAsync(&v[1], p->prec + bi, sizeof(float), cudaMemcpyDeviceToHost, st));
-  SRB_CUDA_OK(cudaMemcpyAsync(&v[2], p->rec + bi, sizeof(float), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(&v[0], p->thr.as<float>() + bi, sizeof(float), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(&v[1], p->prec.as<float>() + bi, sizeof(float), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(&v[2], p->rec.as<float>() + bi, sizeof(float), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   const uint32_t fbits = static_cast<uint32_t>(bk >> 32);
   float f1;
@@ -713,11 +675,11 @@ extern "C" int samroad_prc_read_curve(samroad_prc_t p, float* thresholds, float*
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t T = static_cast<size_t>(p->T);
   const cudaMemcpyKind k = cudaMemcpyDefault;
-  if (thresholds) SRB_CUDA_OK(cudaMemcpyAsync(thresholds, p->thr, sizeof(float) * T, k, st));
-  if (precision) SRB_CUDA_OK(cudaMemcpyAsync(precision, p->prec, sizeof(float) * (T + 1), k, st));
-  if (recall) SRB_CUDA_OK(cudaMemcpyAsync(recall, p->rec, sizeof(float) * (T + 1), k, st));
-  if (tps) SRB_CUDA_OK(cudaMemcpyAsync(tps, p->tps, sizeof(int64_t) * T, k, st));
-  if (fps) SRB_CUDA_OK(cudaMemcpyAsync(fps, p->fps, sizeof(int64_t) * T, k, st));
+  if (thresholds) SRB_CUDA_OK(cudaMemcpyAsync(thresholds, p->thr.as<float>(), sizeof(float) * T, k, st));
+  if (precision) SRB_CUDA_OK(cudaMemcpyAsync(precision, p->prec.as<float>(), sizeof(float) * (T + 1), k, st));
+  if (recall) SRB_CUDA_OK(cudaMemcpyAsync(recall, p->rec.as<float>(), sizeof(float) * (T + 1), k, st));
+  if (tps) SRB_CUDA_OK(cudaMemcpyAsync(tps, p->tps.as<long long>(), sizeof(int64_t) * T, k, st));
+  if (fps) SRB_CUDA_OK(cudaMemcpyAsync(fps, p->fps.as<long long>(), sizeof(int64_t) * T, k, st));
   return 0;
 }
 
@@ -932,44 +894,29 @@ __global__ void val_reset_kernel(ValState* st) {
 struct samroad_val_ctx {
   int device = 0;
   int max_blocks = 0;              // per pass
-  ValState* state = nullptr;       // device
-  ValPartial* part = nullptr;      // device, 2 * max_blocks: mask pass, then pair pass
-  ValState* h_state = nullptr;     // pinned read-back
+  DeviceBuffer state;              // one ValState
+  DeviceBuffer part;               // ValPartial [2 * max_blocks]: mask pass, then pair pass
+  PinnedBuffer h_state;            // one ValState, pinned read-back
   long long n_updates = 0;         // updates since the last reset
-
-  ~samroad_val_ctx() {
-    if (state) cudaFree(state);
-    if (part) cudaFree(part);
-    if (h_state) cudaFreeHost(h_state);
-  }
 };
 
 extern "C" int samroad_val_create(int device, samroad_val_t* out) {
   SRB_REQUIRE(out != nullptr, "samroad_val_create: null argument");
-  int ndev = 0;
-  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
-  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
-  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
-  SRB_CUDA_OK(cudaSetDevice(device));
-  samroad_val_ctx* v = new samroad_val_ctx();
+  if (int rc = open_device(device)) return rc;
+  std::unique_ptr<samroad_val_ctx> v(new samroad_val_ctx());
   v->device = device;
   v->max_blocks = kValBlocksPerSm * device_sm_count();
-  if (cudaMalloc(&v->state, sizeof(ValState)) != cudaSuccess ||
-      cudaMalloc(&v->part, sizeof(ValPartial) * 2 * v->max_blocks) != cudaSuccess ||
-      cudaMallocHost(&v->h_state, sizeof(ValState)) != cudaSuccess) {
-    cudaGetLastError();
-    delete v;
-    set_last_error("samroad_val_create: device or pinned allocation failed");
+  const char* what = "samroad_val_create";
+  if (v->state.reserve(sizeof(ValState), what) || v->part.reserve(sizeof(ValPartial) * 2 * v->max_blocks, what) ||
+      v->h_state.reserve(sizeof(ValState), what))
     return 1;
-  }
-  val_reset_kernel<<<1, 1>>>(v->state);
+  val_reset_kernel<<<1, 1>>>(v->state.as<ValState>());
   if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
-    delete v;
     set_last_error("samroad_val_create: initialising the state failed");
     return 1;
   }
   note_launch(1);
-  *out = v;
+  *out = v.release();
   return 0;
 }
 
@@ -984,7 +931,7 @@ extern "C" int samroad_val_destroy(samroad_val_t v) {
 extern "C" int samroad_val_reset(samroad_val_t v, void* stream) {
   SRB_REQUIRE(v != nullptr, "samroad_val_reset: null handle");
   SRB_CUDA_OK(cudaSetDevice(v->device));
-  val_reset_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(v->state);
+  val_reset_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(v->state.as<ValState>());
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(1);
   v->n_updates = 0;
@@ -1011,19 +958,21 @@ extern "C" int samroad_val_update(samroad_val_t v, const float* mask_logits, con
   const long long npix = static_cast<long long>(B) * P * P;
   const int g_mask = static_cast<int>(std::min<long long>(grid_for(npix, 256), v->max_blocks));
   const int g_pair = static_cast<int>(std::min<long long>(grid_for(n_pairs, 256), v->max_blocks));
-  ValPartial* pair_part = v->part + v->max_blocks;
+  ValState* state = v->state.as<ValState>();
+  ValPartial* mask_part = v->part.as<ValPartial>();
+  ValPartial* pair_part = mask_part + v->max_blocks;
   if (loss_kind == SAMROAD_LOSS_FOCAL)
     val_mask_kernel<true><<<g_mask, 256, 0, st>>>(reinterpret_cast<const float2*>(mask_logits),
                                                   reinterpret_cast<const float2*>(mask_scores), keypoint_mask,
-                                                  road_mask, npix, v->part, &v->state->ref);
+                                                  road_mask, npix, mask_part, &state->ref);
   else
     val_mask_kernel<false><<<g_mask, 256, 0, st>>>(reinterpret_cast<const float2*>(mask_logits),
                                                    reinterpret_cast<const float2*>(mask_scores), keypoint_mask,
-                                                   road_mask, npix, v->part, &v->state->ref);
+                                                   road_mask, npix, mask_part, &state->ref);
   if (g_pair > 0)
     val_pair_kernel<<<g_pair, 256, 0, st>>>(topo_logits, topo_scores, connected, valid, n_pairs,
-                                            static_cast<unsigned long long>(2 * npix), pair_part, &v->state->ref);
-  val_finish_kernel<<<1, 256, 0, st>>>(v->part, g_mask, pair_part, g_pair, npix, B, out, v->state, v->n_updates);
+                                            static_cast<unsigned long long>(2 * npix), pair_part, &state->ref);
+  val_finish_kernel<<<1, 256, 0, st>>>(mask_part, g_mask, pair_part, g_pair, npix, B, out, state, v->n_updates);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(g_pair > 0 ? 3 : 2);
   ++v->n_updates;
@@ -1034,10 +983,10 @@ extern "C" int samroad_val_read(samroad_val_t v, int64_t* counts, float* means, 
   SRB_REQUIRE(v != nullptr && counts && means && totals, "samroad_val_read: null argument");
   SRB_CUDA_OK(cudaSetDevice(v->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  SRB_CUDA_OK(cudaMemcpyAsync(v->h_state, v->state, sizeof(ValState), cudaMemcpyDeviceToHost, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(v->h_state.get(), v->state.get(), sizeof(ValState), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
-  const ValState s = *v->h_state;
-  if (int rc = report_refusals(s.ref, &v->state->ref, "samroad_val_read", kValBadText, 3, st)) return rc;
+  const ValState s = *v->h_state.as<ValState>();
+  if (int rc = report_refusals(s.ref, &v->state.as<ValState>()->ref, "samroad_val_read", kValBadText, 3, st)) return rc;
   for (int k = 0; k < kValCounts; ++k) counts[k] = s.counts[k];
   for (int k = 0; k < 3; ++k)
     means[k] = s.samples ? static_cast<float>(s.loss_wsum[k] / static_cast<double>(s.samples)) : NAN;

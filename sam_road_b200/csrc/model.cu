@@ -93,7 +93,7 @@ struct samroad_ctx {
   std::map<std::string, HostTensor> staged;
 
   // device weight arena
-  std::vector<void*> weight_allocs;
+  std::vector<DeviceBuffer> weight_allocs;
 
   // encoder
   __half* pe_w = nullptr; float* pe_b = nullptr; float* pos = nullptr;
@@ -107,7 +107,7 @@ struct samroad_ctx {
   float* dec4_w = nullptr; float* dec4_b = nullptr;
   // SAM mask-decoder path (USE_SAM_DECODER)
   SamDecoderWeights sam{};
-  void* sam_ws = nullptr; size_t sam_ws_bytes = 0;
+  DeviceBuffer sam_ws;
   // toponet
   __half* tp_feat_w = nullptr; float* tp_feat_b = nullptr;
   __half* tp_st_w = nullptr; float* tp_off_w = nullptr; float* tp_pair_b = nullptr;
@@ -119,16 +119,14 @@ struct samroad_ctx {
 
   // activation workspace (grown on demand); TopoNet has its own so that the encoder of the next scene
   // (another stream) can run while the TopoNet pass of the previous one is still in flight
-  void* ws = nullptr;
-  size_t ws_bytes = 0;
-  void* topo_ws = nullptr;
-  size_t topo_ws_bytes = 0;
+  DeviceBuffer ws;
+  DeviceBuffer topo_ws;
   // staging for the host-buffer entry points: two slots so that step i's downloads overlap step
   // i+1's upload and compute (samroad_infer_batch_host_async / _wait)
   struct HostSlot {
-    void* in = nullptr;  size_t in_bytes = 0;           // tiles + TopoNet inputs + topology scores
-    float* scores = nullptr; size_t scores_bytes = 0;
-    float* emb = nullptr; size_t emb_bytes = 0;
+    DeviceBuffer in;                                      // tiles + TopoNet inputs + topology scores
+    DeviceBuffer scores;
+    DeviceBuffer emb;
     cudaEvent_t ev_h2d = nullptr, ev_emb = nullptr, ev_scores = nullptr, ev_compute = nullptr, ev_done = nullptr;
   };
   HostSlot slots[2];
@@ -143,8 +141,6 @@ constexpr float kPixelStd[3] = {58.395f, 57.12f, 57.375f};      // model.py:230
 
 // test hook (bit 4 of samroad_debug_disable_2cta_gemm): every encoder LayerNorm walks its rows ascending
 bool g_ln_ascending = false;
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // ---- staged-tensor access -----------------------------------------------------------------------
 struct Packer {
@@ -186,17 +182,18 @@ struct Packer {
   template <typename T>
   T* upload(const std::vector<T>& v) {
     if (!ok) return nullptr;
-    void* d = nullptr;
-    if (cudaMalloc(&d, v.size() * sizeof(T) + 256) != cudaSuccess) {
+    DeviceBuffer d;
+    if (d.reserve(v.size() * sizeof(T) + 256, "samroad_finalize_weights")) {
       fail("cudaMalloc of %zu bytes for weights failed", v.size() * sizeof(T));
       return nullptr;
     }
-    h->weight_allocs.push_back(d);
-    if (cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) {
+    T* p = d.as<T>();
+    h->weight_allocs.push_back(std::move(d));
+    if (cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) {
       fail("cudaMemcpy of weights failed");
       return nullptr;
     }
-    return static_cast<T*>(d);
+    return p;
   }
   float* f32(const std::string& key, std::initializer_list<int64_t> shape) {
     const HostTensor* t = get(key, shape);
@@ -244,17 +241,12 @@ std::vector<float> tile4(const std::vector<float>& b) {
   return o;
 }
 
-int ensure_bytes(void** p, size_t* cur, size_t need) {
-  if (*cur >= need) return 0;
-  if (*p) {
-    SRB_CUDA_OK(cudaDeviceSynchronize());
-    SRB_CUDA_OK(cudaFree(*p));
-    *p = nullptr;
-    *cur = 0;
-  }
-  SRB_CUDA_OK(cudaMalloc(p, need));
-  *cur = need;
-  return 0;
+// Grows a workspace or staging buffer to `need` bytes.  The handle's three streams may still read the old
+// block, so the device is synchronised before it is replaced.
+int grow(DeviceBuffer& b, size_t need, const char* what) {
+  if (need <= b.capacity()) return 0;
+  if (b.get()) SRB_CUDA_OK(cudaDeviceSynchronize());
+  return b.reserve(need, what);
 }
 
 // ---- activation workspace layout for the encoder + decoder ------------------------------------------
@@ -273,25 +265,18 @@ struct EncWs {
 
 EncWs layout_enc(const samroad_ctx* h, int B, void* base) {
   const size_t M = static_cast<size_t>(B) * h->T, D = h->D;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += align_up(bytes, 1024);
-    return o;
-  };
+  Layout L(base, 1024);
   EncWs w;
-  char* b = static_cast<char*>(base);
-  w.X = reinterpret_cast<float*>(b + take(M * D * 4));
-  w.XN = reinterpret_cast<__half*>(b + take(M * (D > 768 ? D : 768) * 2));
-  w.QKV = reinterpret_cast<__half*>(b + take(M * 3 * D * 2));
-  w.ATT = reinterpret_cast<__half*>(b + take(M * D * 2));
-  const size_t hbytes = M * 4 * D * 2;   // >= M*2304*2 and >= 4M*256*2 for D >= 768
-  w.H = reinterpret_cast<__half*>(b + take(hbytes));
-  w.N1 = reinterpret_cast<__half*>(b + take(M * 256 * 2));
-  w.FEAT = reinterpret_cast<__half*>(b + take(M * 256 * 2));
-  w.D1 = reinterpret_cast<__half*>(b + take(M * 512 * 2));
-  w.RGB = reinterpret_cast<uint8_t*>(b + take(M * 768));      // B * P * P * 3 = M * 256 * 3
-  w.total = off;
+  w.X = L.take<float>(M * D);
+  w.XN = L.take<__half>(M * (D > 768 ? D : 768));
+  w.QKV = L.take<__half>(M * 3 * D);
+  w.ATT = L.take<__half>(M * D);
+  w.H = L.take<__half>(M * 4 * D);   // >= M*2304 and >= 4M*256 for D >= 768
+  w.N1 = L.take<__half>(M * 256);
+  w.FEAT = L.take<__half>(M * 256);
+  w.D1 = L.take<__half>(M * 512);
+  w.RGB = L.take<uint8_t>(M * 768);    // B * P * P * 3 = M * 256 * 3
+  w.total = L.bytes();
   return w;
 }
 
@@ -310,24 +295,18 @@ struct TopoWs {
 
 TopoWs layout_topo(int B, int N, int Ns, int Np, void* base) {
   const size_t pts = static_cast<size_t>(B) * N, tok = static_cast<size_t>(B) * Ns * Np;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += align_up(bytes, 1024);
-    return o;
-  };
+  Layout L(base, 1024);
   TopoWs w;
-  char* b = static_cast<char*>(base);
-  w.F16 = reinterpret_cast<__half*>(b + take(pts * 256 * 2));
-  w.PF16 = reinterpret_cast<__half*>(b + take(pts * 128 * 2));
-  w.PST = reinterpret_cast<float*>(b + take(pts * 256 * 4));
-  w.VF = reinterpret_cast<uint8_t*>(b + take(tok));
-  w.X32 = reinterpret_cast<float*>(b + take(tok * 128 * 4));
-  w.X16 = reinterpret_cast<__half*>(b + take(tok * 128 * 2));
-  w.QKV16 = reinterpret_cast<__half*>(b + take(tok * 384 * 2));
-  w.ATT16 = reinterpret_cast<__half*>(b + take(tok * 128 * 2));
-  w.H16 = reinterpret_cast<__half*>(b + take(tok * 128 * 2));
-  w.total = off;
+  w.F16 = L.take<__half>(pts * 256);
+  w.PF16 = L.take<__half>(pts * 128);
+  w.PST = L.take<float>(pts * 256);
+  w.VF = L.take<uint8_t>(tok);
+  w.X32 = L.take<float>(tok * 128);
+  w.X16 = L.take<__half>(tok * 128);
+  w.QKV16 = L.take<__half>(tok * 384);
+  w.ATT16 = L.take<__half>(tok * 128);
+  w.H16 = L.take<__half>(tok * 128);
+  w.total = L.bytes();
   return w;
 }
 
@@ -372,11 +351,7 @@ extern "C" int samroad_create(const SamRoadCfg* cfg, int device, samroad_handle_
   SRB_REQUIRE(hd == 64 || hd == 80, "head_dim=%d unsupported (64 or 80)", hd);
   SRB_REQUIRE(cfg->depth > 0 && cfg->depth <= 64, "depth=%d unsupported", cfg->depth);
   SRB_REQUIRE(cfg->window_size > 0, "window_size=%d must be positive", cfg->window_size);
-  int ndev = 0;
-  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
-  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
-  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
-  SRB_CUDA_OK(cudaSetDevice(device));
+  SRB_TRY(open_device(device));
   cudaDeviceProp prop;
   SRB_CUDA_OK(cudaGetDeviceProperties(&prop, device));
   SRB_REQUIRE(prop.major == 9 && prop.minor == 0, "device %d is sm_%d%d; this library is built for sm_90a only",
@@ -396,18 +371,10 @@ extern "C" int samroad_destroy(samroad_handle_t h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
-  for (void* p : h->weight_allocs) cudaFree(p);
-  if (h->ws) cudaFree(h->ws);
-  if (h->topo_ws) cudaFree(h->topo_ws);
-  if (h->sam_ws) cudaFree(h->sam_ws);
   if (h->s_compute) { cudaStreamDestroy(h->s_h2d); cudaStreamDestroy(h->s_compute); cudaStreamDestroy(h->s_copy); }
-  for (auto& sl : h->slots) {
-    if (sl.in) cudaFree(sl.in);
-    if (sl.scores) cudaFree(sl.scores);
-    if (sl.emb) cudaFree(sl.emb);
+  for (auto& sl : h->slots)
     for (cudaEvent_t e : {sl.ev_h2d, sl.ev_emb, sl.ev_scores, sl.ev_compute, sl.ev_done})
       if (e) cudaEventDestroy(e);
-  }
   delete h;
   return 0;
 }
@@ -430,7 +397,6 @@ extern "C" int samroad_finalize_weights(samroad_handle_t h) {
   SRB_TRY(check_handle(h, false));
   // drop previously packed weights (re-load after load_state_dict)
   SRB_CUDA_OK(cudaDeviceSynchronize());
-  for (void* p : h->weight_allocs) cudaFree(p);
   h->weight_allocs.clear();
   h->blocks.clear();
 
@@ -815,8 +781,8 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
   const long Ml = static_cast<long>(B) * T;
   SRB_REQUIRE(Ml * 16 < 2147483647L, "batch of %d tiles is too large for one call", B);
   const int M = static_cast<int>(Ml);
-  SRB_TRY(ensure_bytes(&h->ws, &h->ws_bytes, layout_enc(h, B, nullptr).total));
-  EncWs w = layout_enc(h, B, h->ws);
+  SRB_TRY(grow(h->ws, layout_enc(h, B, nullptr).total, "samroad_encode_masks"));
+  EncWs w = layout_enc(h, B, h->ws.get());
 
   // patch embed + pos embed  (image_encoder.py:107-109, 387-395; normalisation model.py:465-467)
   const float inv_std[3] = {1.0f / kPixelStd[0], 1.0f / kPixelStd[1], 1.0f / kPixelStd[2]};
@@ -884,9 +850,9 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
   if (h->ev_emb_hook) SRB_CUDA_OK(cudaEventRecord(h->ev_emb_hook, st));   // embeddings are final here
   if ((mask_scores || mask_logits) && h->cfg.use_sam_decoder) {
     // SAM mask decoder (model.py:471-488): null prompts, TwoWayTransformer, upscaler, x4 bilinear
-    SRB_TRY(ensure_bytes(&h->sam_ws, &h->sam_ws_bytes, sam_decoder_ws_bytes(B, T)));
+    SRB_TRY(grow(h->sam_ws, sam_decoder_ws_bytes(B, T), "samroad_encode_masks"));
     SRB_T(KT_DECODER, 0.91e9 * B, Md * 256 * 4 * 10,
-          sam_decoder_forward(h->sam, image_embeddings, B, s, P, h->sam_ws, mask_scores, mask_logits, st));
+          sam_decoder_forward(h->sam, image_embeddings, B, s, P, h->sam_ws.get(), mask_scores, mask_logits, st));
   } else if (mask_scores || mask_logits) {
     SRB_T(KT_DECODER, 2 * Md * 512 * 256, Md * 256 * 2 + Md * 512 * 2,
           gemm_ln(w.FEAT, 256, h->dec1_w, 256, M, 512, 256, h->dec1_b, nullptr, h->dec_ln_g,
@@ -913,8 +879,8 @@ extern "C" int samroad_encode_masks_scene(samroad_handle_t h, const uint8_t* sce
   const int P = h->cfg.patch_size;
   SRB_REQUIRE(H >= P && W >= P, "samroad_encode_masks_scene: scene %dx%d smaller than a %d tile", H, W, P);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  SRB_TRY(ensure_bytes(&h->ws, &h->ws_bytes, layout_enc(h, B, nullptr).total));
-  EncWs w = layout_enc(h, B, h->ws);
+  SRB_TRY(grow(h->ws, layout_enc(h, B, nullptr).total, "samroad_encode_masks_scene"));
+  EncWs w = layout_enc(h, B, h->ws.get());
   SRB_T(KT_PATCH_IM2COL, 0, 2.0 * B * P * P * 3, crop_tiles(scene, H, W, tile_xy, B, P, w.RGB, st));
   return samroad_encode_masks(h, w.RGB, SAMROAD_U8, B, mask_scores, mask_logits, image_embeddings, stream);
 }
@@ -947,8 +913,8 @@ extern "C" int samroad_toponet(samroad_handle_t h, const float* image_embeddings
   SRB_REQUIRE(tokl < 2147483647L / 4, "samroad_toponet: %ld pair tokens is too many for one call",
               tokl);
   const int tok = static_cast<int>(tokl), pts = B * N, rows = B * Ns;
-  SRB_TRY(ensure_bytes(&h->topo_ws, &h->topo_ws_bytes, layout_topo(B, N, Ns, Np, nullptr).total));
-  TopoWs w = layout_topo(B, N, Ns, Np, h->topo_ws);
+  SRB_TRY(grow(h->topo_ws, layout_topo(B, N, Ns, Np, nullptr).total, "samroad_toponet"));
+  TopoWs w = layout_topo(B, N, Ns, Np, h->topo_ws.get());
   const int zero_off = h->cfg.toponet_version == SAMROAD_TOPO_NO_OFFSET;
   const bool no_tf = h->cfg.toponet_version == SAMROAD_TOPO_NO_TRANSFORMER;
 
@@ -1075,8 +1041,19 @@ extern "C" int samroad_infer_batch_host_async(samroad_handle_t h, int slot, cons
   const size_t prs_bytes = topo ? static_cast<size_t>(B) * Ns * Np * 2 * pr_sz : 0;
   const size_t val_bytes = topo ? static_cast<size_t>(B) * Ns * Np : 0;
   const size_t ts_bytes = topo ? static_cast<size_t>(B) * Ns * Np * 4 : 0;
-  const size_t o_pts = align_up(in_bytes, 256), o_prs = o_pts + align_up(pts_bytes, 256);
-  const size_t o_val = o_prs + align_up(prs_bytes, 256), o_ts = o_val + align_up(val_bytes, 256);
+  // the slot's input staging: tiles, then TopoNet's points, pairs and valid flags, then the topology scores
+  struct Staging { char *rgb, *pts, *prs, *val, *ts; size_t bytes; };
+  auto staging = [&](void* at) {
+    Layout L(at);
+    Staging g;
+    g.rgb = L.take<char>(in_bytes);
+    g.pts = L.take<char>(pts_bytes);
+    g.prs = L.take<char>(prs_bytes);
+    g.val = L.take<char>(val_bytes);
+    g.ts = L.take<char>(ts_bytes);
+    g.bytes = L.bytes();
+    return g;
+  };
   samroad_ctx::HostSlot& sl = h->slots[slot];
   if (!h->s_compute) {
     SRB_CUDA_OK(cudaStreamCreateWithFlags(&h->s_h2d, cudaStreamNonBlocking));
@@ -1087,48 +1064,51 @@ extern "C" int samroad_infer_batch_host_async(samroad_handle_t h, int slot, cons
     for (cudaEvent_t* e : {&sl.ev_h2d, &sl.ev_emb, &sl.ev_scores, &sl.ev_compute, &sl.ev_done})
       SRB_CUDA_OK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
   }
-  SRB_TRY(ensure_bytes(&sl.in, &sl.in_bytes, o_ts + align_up(ts_bytes, 256)));
-  SRB_TRY(ensure_bytes(reinterpret_cast<void**>(&sl.scores), &sl.scores_bytes, sc_bytes));
-  SRB_TRY(ensure_bytes(reinterpret_cast<void**>(&sl.emb), &sl.emb_bytes, em_bytes));
+  const char* what = "samroad_infer_batch_host_async";
+  SRB_TRY(grow(sl.in, staging(nullptr).bytes, what));
+  SRB_TRY(grow(sl.scores, sc_bytes, what));
+  SRB_TRY(grow(sl.emb, em_bytes, what));
   // the activation workspace is shared by both slots: grow it before anything is in flight on it
-  SRB_TRY(ensure_bytes(&h->ws, &h->ws_bytes, layout_enc(h, B, nullptr).total));
-  if (topo) SRB_TRY(ensure_bytes(&h->topo_ws, &h->topo_ws_bytes, layout_topo(B, N, Ns, Np, nullptr).total));
-  char* base = static_cast<char*>(sl.in);
+  SRB_TRY(grow(h->ws, layout_enc(h, B, nullptr).total, what));
+  if (topo) SRB_TRY(grow(h->topo_ws, layout_topo(B, N, Ns, Np, nullptr).total, what));
+  const Staging io = staging(sl.in.get());
+  float* scores = sl.scores.as<float>();
+  float* emb = sl.emb.as<float>();
   cudaStream_t su = h->s_h2d, st = h->s_compute, sc = h->s_copy;
   // upload: the slot's input staging was last read by the slot's previous compute
   SRB_CUDA_OK(cudaStreamWaitEvent(su, sl.ev_compute, 0));
-  SRB_CUDA_OK(cudaMemcpyAsync(base, rgb_host, in_bytes, cudaMemcpyHostToDevice, su));
+  SRB_CUDA_OK(cudaMemcpyAsync(io.rgb, rgb_host, in_bytes, cudaMemcpyHostToDevice, su));
   if (topo) {
-    SRB_CUDA_OK(cudaMemcpyAsync(base + o_pts, points_host, pts_bytes, cudaMemcpyHostToDevice, su));
-    SRB_CUDA_OK(cudaMemcpyAsync(base + o_prs, pairs_host, prs_bytes, cudaMemcpyHostToDevice, su));
-    SRB_CUDA_OK(cudaMemcpyAsync(base + o_val, valid_host, val_bytes, cudaMemcpyHostToDevice, su));
+    SRB_CUDA_OK(cudaMemcpyAsync(io.pts, points_host, pts_bytes, cudaMemcpyHostToDevice, su));
+    SRB_CUDA_OK(cudaMemcpyAsync(io.prs, pairs_host, prs_bytes, cudaMemcpyHostToDevice, su));
+    SRB_CUDA_OK(cudaMemcpyAsync(io.val, valid_host, val_bytes, cudaMemcpyHostToDevice, su));
   }
   SRB_CUDA_OK(cudaEventRecord(sl.ev_h2d, su));
   // compute: after the upload, and after the slot's previous results have left its output staging
   SRB_CUDA_OK(cudaStreamWaitEvent(st, sl.ev_h2d, 0));
   SRB_CUDA_OK(cudaStreamWaitEvent(st, sl.ev_done, 0));
   h->ev_emb_hook = sl.ev_emb;
-  const int rc_enc = samroad_encode_masks(h, base, rgb_dtype, B, mask_scores_host ? sl.scores : nullptr,
-                                          nullptr, sl.emb, st);
+  const int rc_enc = samroad_encode_masks(h, io.rgb, rgb_dtype, B, mask_scores_host ? scores : nullptr,
+                                          nullptr, emb, st);
   h->ev_emb_hook = nullptr;
   if (rc_enc != 0) return rc_enc;
   if (image_embeddings_host) {      // the embeddings go back while the mask decoder runs
     SRB_CUDA_OK(cudaStreamWaitEvent(sc, sl.ev_emb, 0));
-    SRB_CUDA_OK(cudaMemcpyAsync(image_embeddings_host, sl.emb, em_bytes, cudaMemcpyDeviceToHost, sc));
+    SRB_CUDA_OK(cudaMemcpyAsync(image_embeddings_host, emb, em_bytes, cudaMemcpyDeviceToHost, sc));
   }
   if (mask_scores_host) {           // the mask scores while TopoNet runs
     SRB_CUDA_OK(cudaEventRecord(sl.ev_scores, st));
     SRB_CUDA_OK(cudaStreamWaitEvent(sc, sl.ev_scores, 0));
-    SRB_CUDA_OK(cudaMemcpyAsync(mask_scores_host, sl.scores, sc_bytes, cudaMemcpyDeviceToHost, sc));
+    SRB_CUDA_OK(cudaMemcpyAsync(mask_scores_host, scores, sc_bytes, cudaMemcpyDeviceToHost, sc));
   }
   if (topo)
-    SRB_TRY(samroad_toponet(h, sl.emb, base + o_pts, pts_dtype, base + o_prs, pairs_dtype,
-                            reinterpret_cast<const uint8_t*>(base + o_val), B, N, Ns, Np, nullptr,
-                            reinterpret_cast<float*>(base + o_ts), st));
+    SRB_TRY(samroad_toponet(h, emb, io.pts, pts_dtype, io.prs, pairs_dtype,
+                            reinterpret_cast<const uint8_t*>(io.val), B, N, Ns, Np, nullptr,
+                            reinterpret_cast<float*>(io.ts), st));
   SRB_CUDA_OK(cudaEventRecord(sl.ev_compute, st));
   SRB_CUDA_OK(cudaStreamWaitEvent(sc, sl.ev_compute, 0));
   if (topo && topo_scores_host)
-    SRB_CUDA_OK(cudaMemcpyAsync(topo_scores_host, base + o_ts, ts_bytes, cudaMemcpyDeviceToHost, sc));
+    SRB_CUDA_OK(cudaMemcpyAsync(topo_scores_host, io.ts, ts_bytes, cudaMemcpyDeviceToHost, sc));
   SRB_CUDA_OK(cudaEventRecord(sl.ev_done, sc));
   return 0;
 }

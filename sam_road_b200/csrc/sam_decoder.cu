@@ -461,15 +461,40 @@ struct SamDecoderWs {
   float* keys32; __half* ka16; __half* va16; float* K32; float* V32; float* Q32; __half* att16;
   float* X; float* T0; float* T1; float* T2; float* T3; float* Hd; float* Qc; float* A2;
   float* k4; float* v4; float* hyper; __half* u1; __half* u2; float* lr;
+  size_t total;
 };
 
-size_t sam_decoder_ws_bytes(int B, int T) {
+SamDecoderWs layout_sam_decoder(int B, int T, void* base) {
   const size_t M = static_cast<size_t>(B) * T;
-  const size_t Bt = static_cast<size_t>(B) * 4;
-  return M * 256 * 4 + M * 256 * 2 * 2 + M * 128 * 4 * 3 + M * 128 * 2 + Bt * 256 * 4 * 5 + Bt * 2048 * 4 +
-         Bt * 128 * 4 * 4 + static_cast<size_t>(B) * 64 * 4 + M * 256 * 2 + M * 4 * 128 * 2 + M * 16 * 2 * 4 +
-         64 * 1024;
+  const size_t Bts = static_cast<size_t>(B) * 4;
+  Layout L(base, 1024);
+  SamDecoderWs b;
+  b.keys32 = L.take<float>(M * 256);
+  b.ka16 = L.take<__half>(M * 256);
+  b.va16 = L.take<__half>(M * 256);
+  b.K32 = L.take<float>(M * 128);
+  b.V32 = L.take<float>(M * 128);
+  b.Q32 = L.take<float>(M * 128);
+  b.att16 = L.take<__half>(M * 128);
+  b.X = L.take<float>(Bts * 256);
+  b.T0 = L.take<float>(Bts * 256);
+  b.T1 = L.take<float>(Bts * 256);
+  b.T2 = L.take<float>(Bts * 256);
+  b.T3 = L.take<float>(Bts * 256);
+  b.Hd = L.take<float>(Bts * 2048);
+  b.Qc = L.take<float>(Bts * 128);
+  b.A2 = L.take<float>(Bts * 128);
+  b.k4 = L.take<float>(Bts * 128);
+  b.v4 = L.take<float>(Bts * 128);
+  b.hyper = L.take<float>(static_cast<size_t>(B) * 64);
+  b.u1 = L.take<__half>(M * 256);
+  b.u2 = L.take<__half>(M * 4 * 128);
+  b.lr = L.take<float>(M * 16 * 2);
+  b.total = L.bytes();
+  return b;
 }
+
+size_t sam_decoder_ws_bytes(int B, int T) { return layout_sam_decoder(B, T, nullptr).total; }
 
 int sam_decoder_forward(const SamDecoderWeights& W, const float* emb_nchw, int B, int s, int P, void* ws,
                         float* mask_scores, float* mask_logits, cudaStream_t st) {
@@ -501,32 +526,7 @@ int sam_decoder_forward(const SamDecoderWeights& W, const float* emb_nchw, int B
     for (int j = 0; j < 3; ++j) { w.fin.hw[mi][j] = W.hw[mi][j]; w.fin.hb[mi][j] = W.hb[mi][j]; }
   w.up1_w = W.up1_w; w.up2_w = W.up2_w; w.up1_b = W.up1_b; w.up1_g = W.up1_g; w.up1_beta = W.up1_beta;
   w.up2_b = W.up2_b;
-  char* base = static_cast<char*>(ws);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* p = base + off; off += (bytes + 1023) / 1024 * 1024; return p; };
-  SamDecoderWs b;
-  b.keys32 = reinterpret_cast<float*>(take(M * 256 * 4));
-  b.ka16 = reinterpret_cast<__half*>(take(M * 256 * 2));
-  b.va16 = reinterpret_cast<__half*>(take(M * 256 * 2));
-  b.K32 = reinterpret_cast<float*>(take(M * 128 * 4));
-  b.V32 = reinterpret_cast<float*>(take(M * 128 * 4));
-  b.Q32 = reinterpret_cast<float*>(take(M * 128 * 4));
-  b.att16 = reinterpret_cast<__half*>(take(M * 128 * 2));
-  const size_t Bts = static_cast<size_t>(B) * 4;
-  b.X = reinterpret_cast<float*>(take(Bts * 256 * 4));
-  b.T0 = reinterpret_cast<float*>(take(Bts * 256 * 4));
-  b.T1 = reinterpret_cast<float*>(take(Bts * 256 * 4));
-  b.T2 = reinterpret_cast<float*>(take(Bts * 256 * 4));
-  b.T3 = reinterpret_cast<float*>(take(Bts * 256 * 4));
-  b.Hd = reinterpret_cast<float*>(take(Bts * 2048 * 4));
-  b.Qc = reinterpret_cast<float*>(take(Bts * 128 * 4));
-  b.A2 = reinterpret_cast<float*>(take(Bts * 128 * 4));
-  b.k4 = reinterpret_cast<float*>(take(Bts * 128 * 4));
-  b.v4 = reinterpret_cast<float*>(take(Bts * 128 * 4));
-  b.hyper = reinterpret_cast<float*>(take(static_cast<size_t>(B) * 64 * 4));
-  b.u1 = reinterpret_cast<__half*>(take(M * 256 * 2));
-  b.u2 = reinterpret_cast<__half*>(take(M * 4 * 128 * 2));
-  b.lr = reinterpret_cast<float*>(take(M * 16 * 2 * 4));
+  const SamDecoderWs b = layout_sam_decoder(B, T, ws);
 
   SRB_REQUIRE(W.q0 != nullptr, "SAM decoder: weights not prepared (sam_decoder_prepare)");
   const int Mi = static_cast<int>(M);

@@ -85,29 +85,16 @@ struct Ws {              // slot workspaces
   size_t slot_match_bytes;
 };
 
-__host__ __device__ inline size_t align_up(size_t x) { return (x + 255) & ~size_t(255); }
-
-__host__ __device__ inline size_t walk_bytes(const Params& p, int32_t n) {
-  return align_up(sizeof(double4) * p.cap_marbles) + align_up(sizeof(QEntry) * p.cap_queue) +
-         align_up(8ull * p.hash_size) + align_up(8ull * p.hash_size) + align_up(4ull * p.hash_size) +
-         align_up(8ull * n) + align_up(4ull * n);
-}
-
-__device__ WalkWs walk_ws(char* base, const Params& p, int32_t n) {
+// The workspace of one walk over a graph of n nodes (host: sized with a null base; device: carved)
+__host__ __device__ inline WalkWs walk_ws(Layout& L, const Params& p, int32_t n) {
   WalkWs w;
-  w.marbles = reinterpret_cast<double4*>(base);
-  base += align_up(sizeof(double4) * p.cap_marbles);
-  w.queue = reinterpret_cast<QEntry*>(base);
-  base += align_up(sizeof(QEntry) * p.cap_queue);
-  w.ckey = reinterpret_cast<uint64_t*>(base);
-  base += align_up(8ull * p.hash_size);
-  w.cval = reinterpret_cast<double*>(base);
-  base += align_up(8ull * p.hash_size);
-  w.cstamp = reinterpret_cast<uint32_t*>(base);
-  base += align_up(4ull * p.hash_size);
-  w.dist = reinterpret_cast<double*>(base);
-  base += align_up(8ull * n);
-  w.dstamp = reinterpret_cast<uint32_t*>(base);
+  w.marbles = L.take<double4>(p.cap_marbles);
+  w.queue = L.take<QEntry>(p.cap_queue);
+  w.ckey = L.take<uint64_t>(p.hash_size);
+  w.cval = L.take<double>(p.hash_size);
+  w.cstamp = L.take<uint32_t>(p.hash_size);
+  w.dist = L.take<double>(n);
+  w.dstamp = L.take<uint32_t>(n);
   return w;
 }
 
@@ -286,7 +273,8 @@ __global__ void __launch_bounds__(32) walk_kernel(Params p, Ws ws) {
   const GraphDev& g = which == 0 ? p.prop : p.gt;
   char* base = ws.walk + ws.slot_walk_bytes * slot;
   if (which > 0) base += ws.walk_bytes_prop + (which - 1) * ws.walk_bytes_gt;
-  Walker wk(g, p, walk_ws(base, p, g.n), lane);
+  Layout L(base);
+  Walker wk(g, p, walk_ws(L, p, g.n), lane);
   const int32_t* n = p.pn + 4 * pair;
   const double* d = p.pd + 4 * pair;
   if (which == 0) wk.run(n[0], n[1], d[0], d[1], false);
@@ -335,24 +323,15 @@ struct MatchWs {
   int32_t* stack;    // [2 * cap_marbles]
 };
 
-__host__ __device__ inline size_t match_side_bytes(int cap_marbles, int cap_cand) {
-  return align_up(4ull * (cap_marbles + 1)) + align_up(4ull * cap_cand) + 3 * align_up(4ull * cap_marbles) +
-         align_up(8ull * cap_marbles);
-}
-
-__device__ MatchWs match_ws(char* base, const Params& p) {
+// The workspace of one matching (a slot has two: precision, then recall)
+__host__ __device__ inline MatchWs match_ws(Layout& L, const Params& p) {
   MatchWs m;
-  m.off = reinterpret_cast<int32_t*>(base);
-  base += align_up(4ull * (p.cap_marbles + 1));
-  m.adj = reinterpret_cast<int32_t*>(base);
-  base += align_up(4ull * p.cap_cand);
-  m.match_r = reinterpret_cast<int32_t*>(base);
-  base += align_up(4ull * p.cap_marbles);
-  m.match_l = reinterpret_cast<int32_t*>(base);
-  base += align_up(4ull * p.cap_marbles);
-  m.visit = reinterpret_cast<int32_t*>(base);
-  base += align_up(4ull * p.cap_marbles);
-  m.stack = reinterpret_cast<int32_t*>(base);
+  m.off = L.take<int32_t>(p.cap_marbles + 1);
+  m.adj = L.take<int32_t>(p.cap_cand);
+  m.match_r = L.take<int32_t>(p.cap_marbles);
+  m.match_l = L.take<int32_t>(p.cap_marbles);
+  m.visit = L.take<int32_t>(p.cap_marbles);
+  m.stack = L.take<int32_t>(2ull * p.cap_marbles);
   return m;
 }
 
@@ -465,9 +444,9 @@ __global__ void __launch_bounds__(kMatchThreads) match_kernel(Params p, Ws ws) {
     const double4* marbles = reinterpret_cast<const double4*>(wb);
     const double4* holes = reinterpret_cast<const double4*>(wb + ws.walk_bytes_prop);
     const double4* holes_b = reinterpret_cast<const double4*>(wb + ws.walk_bytes_prop + ws.walk_bytes_gt);
-    char* mb = ws.match + ws.slot_match_bytes * slot;
-    const size_t side = match_side_bytes(p.cap_marbles, p.cap_cand);
-    MatchWs mprec = match_ws(mb, p), mrec = match_ws(mb + side, p);
+    Layout L(ws.match + ws.slot_match_bytes * slot);
+    const MatchWs mprec = match_ws(L, p);
+    const MatchWs mrec = match_ws(L, p);
     // precision: marbles -> holes_bidirection; recall: holes -> marbles
     const bool ok1 = build_csr(marbles, nm, holes_b, nhb, true, p, mprec, s_tot);
     const bool ok2 = build_csr(holes, nh, marbles, nm, false, p, mrec, s_tot);
@@ -498,24 +477,11 @@ struct samroad_topo_ctx {
   SamRoadTopoCaps caps{};
   cudaStream_t stream = nullptr;  // the handle's own non-blocking stream: a run waits for its own work only
   GraphDev g[2];                  // 0 GT, 1 proposal
-  void* gbuf[2] = {nullptr, nullptr};   // one allocation per graph, grown on demand and reused across tiles
-  size_t gcap[2] = {0, 0};
-  void* work = nullptr;
-  size_t work_bytes = 0;
+  DeviceBuffer gbuf[2];           // one allocation per graph, grown on demand and reused across tiles
+  DeviceBuffer work;
   size_t layout[3] = {0, 0, 0};   // the walk workspace layout the stamps were cleared for
   uint32_t serial = 0;
 };
-
-namespace {
-
-void free_graph(samroad_topo_ctx* T, int which) {
-  if (T->gbuf[which]) cudaFree(T->gbuf[which]);
-  T->gbuf[which] = nullptr;
-  T->gcap[which] = 0;
-  T->g[which] = GraphDev{};
-}
-
-}  // namespace
 
 extern "C" int samroad_topo_create(int device, const SamRoadTopoCaps* caps, samroad_topo_t* out) {
   SRB_REQUIRE(out != nullptr && caps != nullptr, "samroad_topo_create: null argument");
@@ -525,11 +491,7 @@ extern "C" int samroad_topo_create(int device, const SamRoadTopoCaps* caps, samr
   SRB_REQUIRE(caps->max_marbles <= (1 << 24) && caps->max_queue <= (1 << 26) && caps->max_covered <= (1 << 24) &&
                   caps->max_candidates <= (1 << 28) && caps->slots <= 65535,
               "samroad_topo_create: a capacity is larger than this build supports");
-  int ndev = 0;
-  SRB_CUDA_OK(cudaGetDeviceCount(&ndev));
-  SRB_REQUIRE(ndev > 0, "no CUDA device: libsamroad_b200 has no CPU fallback");
-  SRB_REQUIRE(device >= 0 && device < ndev, "device %d out of range (0..%d)", device, ndev - 1);
-  SRB_CUDA_OK(cudaSetDevice(device));
+  if (int rc = open_device(device)) return rc;
   cudaStream_t st = nullptr;
   SRB_CUDA_OK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   samroad_topo_ctx* T = new samroad_topo_ctx();
@@ -544,9 +506,6 @@ extern "C" int samroad_topo_destroy(samroad_topo_t T) {
   if (!T) return 0;
   cudaSetDevice(T->device);
   cudaStreamSynchronize(T->stream);
-  free_graph(T, 0);
-  free_graph(T, 1);
-  if (T->work) cudaFree(T->work);
   cudaStreamDestroy(T->stream);
   delete T;
   return 0;
@@ -560,17 +519,9 @@ extern "C" int samroad_topo_upload_graph(samroad_topo_t T, int which, int32_t n_
   SRB_REQUIRE(n_nodes >= 0, "samroad_topo_upload_graph: negative node count");
   SRB_REQUIRE(n_nodes == 0 || (latlon && cos_lat && link_start && rlink_start),
               "samroad_topo_upload_graph: null argument");
-  const int32_t* starts[2] = {link_start, rlink_start};
-  const int32_t* lists[2] = {link, rlink};
-  for (int s = 0; s < 2 && n_nodes > 0; ++s) {
-    SRB_REQUIRE(starts[s][0] == 0, "samroad_topo_upload_graph: adjacency offsets must start at 0");
-    for (int32_t i = 0; i < n_nodes; ++i)
-      SRB_REQUIRE(starts[s][i + 1] >= starts[s][i], "samroad_topo_upload_graph: adjacency offsets decrease at %d", i);
-    const int32_t m = starts[s][n_nodes];
-    SRB_REQUIRE(m == 0 || lists[s] != nullptr, "samroad_topo_upload_graph: null adjacency");
-    for (int32_t e = 0; e < m; ++e)
-      SRB_REQUIRE(lists[s][e] >= 0 && lists[s][e] < n_nodes, "samroad_topo_upload_graph: neighbour %d out of range",
-                  lists[s][e]);
+  if (n_nodes > 0) {
+    if (int rc = check_csr("samroad_topo_upload_graph", n_nodes, link_start, link)) return rc;
+    if (int rc = check_csr("samroad_topo_upload_graph", n_nodes, rlink_start, rlink)) return rc;
   }
   for (int32_t i = 0; i < n_nodes; ++i) {
     SRB_REQUIRE(std::isfinite(latlon[2 * i]) && std::isfinite(latlon[2 * i + 1]) && std::isfinite(cos_lat[i]),
@@ -588,25 +539,18 @@ extern "C" int samroad_topo_upload_graph(samroad_topo_t T, int which, int32_t n_
   const size_t m0 = link_start[n_nodes], m1 = rlink_start[n_nodes];
   const size_t sizes[] = {16 * n, 8 * n, 4 * (n + 1), 4 * m0, 4 * (n + 1), 4 * m1};
   const void* src[] = {latlon, cos_lat, link_start, link, rlink_start, rlink};
-  size_t total = 0;
-  for (size_t b : sizes) total += align_up(std::max<size_t>(b, 1));
-  if (total > T->gcap[which]) {   // runs are synchronous, so nothing of this handle still reads the old buffer
-    free_graph(T, which);
-    if (cudaMalloc(&T->gbuf[which], total) != cudaSuccess) {
-      cudaGetLastError();
-      T->gbuf[which] = nullptr;
-      set_last_error("samroad_topo_upload_graph: out of device memory for a graph of %d nodes", n_nodes);
-      return 1;
-    }
-    T->gcap[which] = total;
-  }
-  char* base = static_cast<char*>(T->gbuf[which]);
+  // each array gets a region of at least one byte
+  auto carve = [&](void* base, void** dst) {
+    Layout L(base);
+    for (int i = 0; i < 6; ++i) dst[i] = L.take<char>(std::max<size_t>(sizes[i], 1));
+    return L.bytes();
+  };
   void* dst[6];
-  for (int i = 0; i < 6; ++i) {
-    dst[i] = base;
+  // runs are synchronous, so nothing of this handle still reads the old buffer
+  if (T->gbuf[which].reserve(carve(nullptr, dst), "samroad_topo_upload_graph")) return 1;
+  carve(T->gbuf[which].get(), dst);
+  for (int i = 0; i < 6; ++i)
     if (sizes[i]) SRB_CUDA_OK(cudaMemcpyAsync(dst[i], src[i], sizes[i], cudaMemcpyHostToDevice, T->stream));
-    base += align_up(std::max<size_t>(sizes[i], 1));
-  }
   SRB_CUDA_OK(cudaStreamSynchronize(T->stream));
   GraphDev g;
   g.ll = static_cast<const double*>(dst[0]);
@@ -659,48 +603,48 @@ extern "C" int samroad_topo_run(samroad_topo_t T, int32_t n_pairs, const int32_t
   p.cap_cand = c.max_candidates;
   p.npairs = n_pairs;
   const int slots = std::min(n_pairs, c.slots);
+  auto walk_bytes = [&](int32_t n) {
+    Layout L(nullptr);
+    walk_ws(L, p, n);
+    return L.bytes();
+  };
   Ws ws;
-  ws.walk_bytes_prop = walk_bytes(p, p.prop.n);
-  ws.walk_bytes_gt = walk_bytes(p, p.gt.n);
+  ws.walk_bytes_prop = walk_bytes(p.prop.n);
+  ws.walk_bytes_gt = walk_bytes(p.gt.n);
   ws.slot_walk_bytes = ws.walk_bytes_prop + 2 * ws.walk_bytes_gt;
-  ws.slot_match_bytes = 2 * match_side_bytes(c.max_marbles, c.max_candidates);
-  const size_t io_bytes = align_up(16ull * n_pairs) + align_up(32ull * n_pairs) + align_up(24ull * n_pairs) +
-                          2 * align_up(12ull * slots);
-  const size_t need = (ws.slot_walk_bytes + ws.slot_match_bytes) * slots + io_bytes;
-  bool fresh = false;
-  if (need > T->work_bytes) {
-    if (T->work) cudaFree(T->work);   // the previous run has finished: runs are synchronous
-    T->work = nullptr;
-    T->work_bytes = 0;
-    if (cudaMalloc(&T->work, need) != cudaSuccess) {
-      cudaGetLastError();
-      set_last_error("%s: out of device memory (%zu bytes for %d pair slots); lower the slot count", what, need, slots);
-      return 1;
-    }
-    T->work_bytes = need;
-    fresh = true;
+  Layout match(nullptr);
+  match_ws(match, p);
+  match_ws(match, p);
+  ws.slot_match_bytes = match.bytes();
+  // the run's workspace: every slot's walks, every slot's matchings, the pairs in, the counts and walk status out
+  int32_t* d_pn = nullptr;
+  double* d_pd = nullptr;
+  auto carve = [&](void* base) {
+    Layout L(base);
+    ws.walk = L.take<char>(ws.slot_walk_bytes * slots);
+    ws.match = L.take<char>(ws.slot_match_bytes * slots);
+    d_pn = L.take<int32_t>(4ull * n_pairs);
+    d_pd = L.take<double>(4ull * n_pairs);
+    p.out = L.take<int32_t>(6ull * n_pairs);
+    p.wcount = L.take<int32_t>(3ull * slots);
+    p.wstatus = L.take<int32_t>(3ull * slots);
+    return L.bytes();
+  };
+  const size_t need = carve(nullptr);
+  const bool fresh = need > T->work.capacity();
+  // the previous run has finished: runs are synchronous
+  if (T->work.reserve(need, what)) {
+    set_last_error("%s: out of device memory (%zu bytes for %d pair slots); lower the slot count", what, need, slots);
+    return 1;
   }
-  char* base = static_cast<char*>(T->work);
-  ws.walk = base;
-  base += ws.slot_walk_bytes * slots;
-  ws.match = base;
-  base += ws.slot_match_bytes * slots;
-  int32_t* d_pn = reinterpret_cast<int32_t*>(base);
-  base += align_up(16ull * n_pairs);
-  double* d_pd = reinterpret_cast<double*>(base);
-  base += align_up(32ull * n_pairs);
-  p.out = reinterpret_cast<int32_t*>(base);
-  base += align_up(24ull * n_pairs);
-  p.wcount = reinterpret_cast<int32_t*>(base);
-  base += align_up(12ull * slots);
-  p.wstatus = reinterpret_cast<int32_t*>(base);
+  carve(T->work.get());
   p.pn = d_pn;
   p.pd = d_pd;
   // the stamps of the dense distance maps and covered-edge tables must start below every serial in use
   const int chunks = (n_pairs + slots - 1) / slots;
   const size_t layout[3] = {ws.walk_bytes_prop, ws.walk_bytes_gt, static_cast<size_t>(slots)};
   if (fresh || !std::equal(layout, layout + 3, T->layout) || T->serial > 0xFFFFFFF0u - static_cast<uint32_t>(chunks)) {
-    SRB_CUDA_OK(cudaMemsetAsync(T->work, 0, ws.slot_walk_bytes * slots, T->stream));
+    SRB_CUDA_OK(cudaMemsetAsync(T->work.get(), 0, ws.slot_walk_bytes * slots, T->stream));
     std::copy(layout, layout + 3, T->layout);
     T->serial = 0;
   }

@@ -856,8 +856,6 @@ __global__ void keep_kernel(Dropout d, int layer, int site, long long n, uint8_t
   } while (0)
 
 // ---- workspace --------------------------------------------------------------------------------------------
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 struct Dims {
   int B, N, Ns, Np, P, s, T, topo_version;
   long long M, R1, R2, R3, R4, pts, tok, rows;
@@ -908,40 +906,43 @@ struct TrainWs {
 };
 
 TrainWs layout_train(const Dims& d, void* base) {
-  size_t off = 0;
-  char* b = static_cast<char*>(base);
-  auto f = [&](long long n) { float* p = reinterpret_cast<float*>(b + off); off += align_up(n * 4, 256); return p; };
-  auto i32 = [&](long long n) { int* p = reinterpret_cast<int*>(b + off); off += align_up(n * 4, 256); return p; };
+  Layout L(base);
   TrainWs w{};
   const long long tok = d.tok, pts = d.pts;
-  w.emb = f(d.M * 256);
-  w.f0 = f(d.M * 256);
-  w.xh1 = f(d.R1 * 128); w.rs1 = f(d.R1); w.a1 = f(d.R1 * 128);
-  w.z2 = f(d.R2 * 64); w.a2 = f(d.R2 * 64);
-  w.z3 = f(d.R3 * 32); w.a3 = f(d.R3 * 32);
-  w.dl = f(d.R4 * 2);
-  w.fs = f(pts * 256); w.pf = f(pts * 128); w.pst = f(pts * 256); w.off = f(tok * 2);
-  w.src = i32(tok); w.tgt = i32(tok);
-  w.src_start = i32(pts + 1); w.tgt_start = i32(pts + 1);
-  w.src_list = i32(tok); w.tgt_list = i32(tok); w.cursor = i32(pts); w.sort_tmp = i32(tok);
-  w.vf = reinterpret_cast<uint8_t*>(b + off); off += align_up(tok, 256);
+  w.emb = L.take<float>(d.M * 256);
+  w.f0 = L.take<float>(d.M * 256);
+  w.xh1 = L.take<float>(d.R1 * 128); w.rs1 = L.take<float>(d.R1); w.a1 = L.take<float>(d.R1 * 128);
+  w.z2 = L.take<float>(d.R2 * 64); w.a2 = L.take<float>(d.R2 * 64);
+  w.z3 = L.take<float>(d.R3 * 32); w.a3 = L.take<float>(d.R3 * 32);
+  w.dl = L.take<float>(d.R4 * 2);
+  w.fs = L.take<float>(pts * 256); w.pf = L.take<float>(pts * 128); w.pst = L.take<float>(pts * 256);
+  w.off = L.take<float>(tok * 2);
+  w.src = L.take<int>(tok); w.tgt = L.take<int>(tok);
+  w.src_start = L.take<int>(pts + 1); w.tgt_start = L.take<int>(pts + 1);
+  w.src_list = L.take<int>(tok); w.tgt_list = L.take<int>(tok); w.cursor = L.take<int>(pts);
+  w.sort_tmp = L.take<int>(tok);
+  w.vf = L.take<uint8_t>(tok);
   const int nx = d.tf ? 4 : 1;
-  for (int l = 0; l < 4; ++l) w.x[l] = l < nx ? f(tok * 128) : nullptr;
+  for (int l = 0; l < 4; ++l) w.x[l] = l < nx ? L.take<float>(tok * 128) : nullptr;
   for (int l = 0; l < (d.tf ? 3 : 0); ++l) {
-    LayerWs& L = w.L[l];
-    L.qkv = f(tok * 384); L.att = f(tok * 128);
-    L.xh1 = f(tok * 128); L.rs1 = f(tok); L.x1 = f(tok * 128); L.h = f(tok * 128);
-    L.xh2 = f(tok * 128); L.rs2 = f(tok);
+    LayerWs& y = w.L[l];
+    y.qkv = L.take<float>(tok * 384); y.att = L.take<float>(tok * 128);
+    y.xh1 = L.take<float>(tok * 128); y.rs1 = L.take<float>(tok); y.x1 = L.take<float>(tok * 128);
+    y.h = L.take<float>(tok * 128);
+    y.xh2 = L.take<float>(tok * 128); y.rs2 = L.take<float>(tok);
   }
-  w.dlt = f(tok);
-  w.part = reinterpret_cast<double*>(b + off); off += align_up(3 * kLossBlocks * 8, 256);
-  w.stats = f(1);
-  w.scale = f(2); w.g3 = f(d.R3 * 32); w.g2 = f(d.R2 * 64); w.g1 = f(d.R1 * 128);
-  w.gx = f(tok * 128); w.gr = f(tok * 128); w.gy = f(tok * 128); w.gh = f(tok * 128);
-  w.gq = f(tok * 384); w.gp = f(pts * 128); w.gps = f(pts * 128); w.gpt = f(pts * 128);
-  w.wpart = f(static_cast<long long>(kWgradChunks) * 257 * 512 > kColChunks * 256LL
+  w.dlt = L.take<float>(tok);
+  w.part = L.take<double>(3 * kLossBlocks);
+  w.stats = L.take<float>(1);
+  w.scale = L.take<float>(2); w.g3 = L.take<float>(d.R3 * 32); w.g2 = L.take<float>(d.R2 * 64);
+  w.g1 = L.take<float>(d.R1 * 128);
+  w.gx = L.take<float>(tok * 128); w.gr = L.take<float>(tok * 128); w.gy = L.take<float>(tok * 128);
+  w.gh = L.take<float>(tok * 128);
+  w.gq = L.take<float>(tok * 384); w.gp = L.take<float>(pts * 128); w.gps = L.take<float>(pts * 128);
+  w.gpt = L.take<float>(pts * 128);
+  w.wpart = L.take<float>(static_cast<long long>(kWgradChunks) * 257 * 512 > kColChunks * 256LL
                   ? static_cast<long long>(kWgradChunks) * 257 * 512 : kColChunks * 256LL);
-  w.total = off;
+  w.total = L.bytes();
   return w;
 }
 

@@ -309,21 +309,14 @@ class LabelScenes:
         self.lc, self.image_size, self.margin, self.cap = lc, image_size, margin, max(1, int(max_patch_points))
         cfg = _lib.SamRoadLabelCfg(lc["P"], image_size, margin, lc["S"], lc["Np"], self.cap, lc["r_nms"],
                                    lc["r_nbr"])
-        h = C.c_void_p()
-        _lib.check(_lib.load().samroad_labels_create(idx, C.byref(cfg), C.byref(h)), "samroad_labels_create")
-        self._h = h.value
+        self._h = _lib.Handle("samroad_labels_create", "samroad_labels_destroy", idx, C.byref(cfg))
         self.n_scenes = 0
-
-    def __del__(self):
-        try:
-            if self.__dict__.get("_h"):
-                from . import _lib
-                _lib.load().samroad_labels_destroy(self._h)
-        except Exception:
-            pass
 
     def __getstate__(self):
         raise TypeError("LabelScenes holds device state and cannot be copied or pickled")
+
+    def close(self) -> None:
+        self._h.close()
 
     def upload(self, scene: SceneLabels, rgb: np.ndarray, keypoint_mask: np.ndarray, road_mask: np.ndarray) -> int:
         from . import _lib

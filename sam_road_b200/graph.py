@@ -60,20 +60,16 @@ class SceneGraph:
             raise RuntimeError(f"SceneGraph runs on CUDA only, got '{device}' (there is no CPU path)")
         self.device = device
         self._idx = device.index if device.index is not None else torch.cuda.current_device()
-        h = C.c_void_p()
-        _lib.check(_lib.load().samroad_graph_create(self._idx, C.byref(h)), "samroad_graph_create")
-        self._h = h.value
+        self._h = _lib.Handle("samroad_graph_create", "samroad_graph_destroy", self._idx)
         self._points_buf: Optional[torch.Tensor] = None
         self._edges_buf: Optional[torch.Tensor] = None
         self._counts: Optional[np.ndarray] = None
         self.stats: dict = {}
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                _lib.load().samroad_graph_destroy(self._h)
-        except Exception:
-            pass
+    __getstate__ = _lib.refuse_copy
+
+    def close(self) -> None:
+        self._h.close()
 
     # ---- keypoints ----------------------------------------------------------------------------------
     def extract_graph_points(self, keypoint_mask: torch.Tensor, road_mask: torch.Tensor, itsc_threshold,

@@ -30,28 +30,20 @@ class PrecisionRecallCurve:
         if device.type != "cuda":
             raise RuntimeError(f"PrecisionRecallCurve runs on CUDA only; got '{device}'. There is no CPU path.")
         self.device = torch.device("cuda", device.index if device.index is not None else torch.cuda.current_device())
-        h = C.c_void_p()
-        _lib.check(_lib.load().samroad_prc_create(self.device.index, C.byref(h)), "samroad_prc_create")
-        self._h = h.value
+        self._h = _lib.Handle("samroad_prc_create", "samroad_prc_destroy", self.device.index)
         self._curve_h = self._h     # the handle the last compute ran on (a gathered one under distributed)
         self._best = None
 
-    def __del__(self):
-        try:
-            self._drop_gathered()
-            if self.__dict__.get("_h"):
-                _lib.load().samroad_prc_destroy(self._h)
-        except Exception:
-            pass
+    __getstate__ = _lib.refuse_copy
+
+    def close(self) -> None:
+        self._drop_gathered()
+        self._h.close()
 
     def _drop_gathered(self):
-        h = self.__dict__.get("_curve_h")
-        if h and h != self.__dict__.get("_h"):
-            _lib.load().samroad_prc_destroy(h)
-        self._curve_h = self.__dict__.get("_h")
-
-    def __getstate__(self):
-        raise TypeError("PrecisionRecallCurve holds device state and cannot be copied or pickled")
+        if self._curve_h is not self._h:
+            self._curve_h.close()
+        self._curve_h = self._h
 
     def reset(self) -> None:
         with torch.cuda.device(self.device):
@@ -95,7 +87,7 @@ class PrecisionRecallCurve:
                 self._h, flat.data_ptr(), stride, tgt.data_ptr(), tdt, _lib.ptr(val), n,
                 _lib.current_stream_ptr()), "samroad_prc_update")
 
-    def _gathered_handle(self, dist) -> int:
+    def _gathered_handle(self, dist) -> _lib.Handle:
         """A new accumulator holding the accepted keys of every rank.  Every rank takes part in the same
         collectives even when one of them fails, so a refusal on one rank raises on all of them instead of
         leaving the others waiting."""
@@ -121,17 +113,16 @@ class PrecisionRecallCurve:
         send = local.to(comm_dev)
         parts = [torch.empty(m, dtype=torch.int32, device=comm_dev) for _ in range(world)]
         dist.all_gather(parts, send)
-        h = C.c_void_p()
-        _lib.check(lib.samroad_prc_create(self.device.index, C.byref(h)), "samroad_prc_create")
+        h = _lib.Handle("samroad_prc_create", "samroad_prc_destroy", self.device.index)
         try:
             for part, c in zip(parts, counts):
                 part = part[:c].to(self.device)
-                _lib.check(lib.samroad_prc_append_keys(h.value, part.data_ptr(), c, stream), "samroad_prc_append_keys")
+                _lib.check(lib.samroad_prc_append_keys(h, part.data_ptr(), c, stream), "samroad_prc_append_keys")
             torch.cuda.current_stream().synchronize()    # `parts` are freed on return
         except Exception:
-            lib.samroad_prc_destroy(h.value)
+            h.close()
             raise
-        return h.value
+        return h
 
     def _compute(self):
         counts = (C.c_int64 * 4)()
@@ -214,19 +205,12 @@ class ValidationMetrics:
             raise RuntimeError(f"ValidationMetrics runs on CUDA only; got '{device}'. There is no CPU path.")
         self.device = torch.device("cuda", device.index if device.index is not None else torch.cuda.current_device())
         self.loss_kind = _lib.LOSS_FOCAL if focal else _lib.LOSS_BCE
-        h = C.c_void_p()
-        _lib.check(_lib.load().samroad_val_create(self.device.index, C.byref(h)), "samroad_val_create")
-        self._h = h.value
+        self._h = _lib.Handle("samroad_val_create", "samroad_val_destroy", self.device.index)
 
-    def __del__(self):
-        try:
-            if self.__dict__.get("_h"):
-                _lib.load().samroad_val_destroy(self._h)
-        except Exception:
-            pass
+    __getstate__ = _lib.refuse_copy
 
-    def __getstate__(self):
-        raise TypeError("ValidationMetrics holds device state and cannot be copied or pickled")
+    def close(self) -> None:
+        self._h.close()
 
     def reset(self) -> None:
         with torch.cuda.device(self.device):

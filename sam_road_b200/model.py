@@ -208,7 +208,7 @@ class SAMRoad(_Base):
                 _register(self, key, nn.Parameter(init, requires_grad=False))
         self.register_buffer("pixel_mean", torch.tensor([123.675, 116.28, 103.53]).view(-1, 1, 1), False)
         self.register_buffer("pixel_std", torch.tensor([58.395, 57.12, 57.375]).view(-1, 1, 1), False)
-        self._handles: Dict[int, int] = {}     # cuda device index -> samroad_handle_t
+        self._handles: Dict[int, _lib.Handle] = {}     # cuda device index -> samroad_handle_t
         self._weights_version = 0
         self._synced_version: Dict[int, int] = {}
         self._packed_versions: Dict[int, Dict[str, int]] = {}   # device -> key -> _version at the last pack
@@ -261,7 +261,7 @@ class SAMRoad(_Base):
         """Call after mutating parameters in place so the packed device weights are rebuilt."""
         self._weights_version += 1
 
-    def _handle(self, device: torch.device) -> int:
+    def _handle(self, device: torch.device) -> _lib.Handle:
         if device.type != "cuda":
             raise RuntimeError(
                 f"sam_road_b200.SAMRoad runs on CUDA (sm_90a) only; got input on '{device}'. "
@@ -280,9 +280,7 @@ class SAMRoad(_Base):
                 _cfg_get(self.config, "TOPONET_VERSION", "normal"), _lib.TOPO_NORMAL)
             cfg.lora_rank = (int(_cfg_get(self.config, "LORA_RANK", 0))
                              if _cfg_get(self.config, "ENCODER_LORA", False) else 0)
-            h = C.c_void_p()
-            _lib.check(lib.samroad_create(C.byref(cfg), idx, C.byref(h)), "samroad_create")
-            self._handles[idx] = h.value
+            self._handles[idx] = _lib.Handle("samroad_create", "samroad_destroy", C.byref(cfg), idx)
         # parameters that require grad (the trained heads) are watched through their autograd version
         # counter: an optimizer step changes them in place, and only those are repacked, on the device
         watched = [(k, p) for k, p in self._head_params() if p.requires_grad]
@@ -313,14 +311,6 @@ class SAMRoad(_Base):
         for k, p in watched:
             seen[k] = p._version
         return self._handles[idx]
-
-    def __del__(self):
-        try:
-            lib = _lib.load()
-            for h in self.__dict__.get("_handles", {}).values():
-                lib.samroad_destroy(h)
-        except Exception:
-            pass
 
     # C handles are owned by exactly one Python object: copies / unpickled objects create their own
     # on first use (copy.deepcopy of a module would otherwise destroy the same handle twice).

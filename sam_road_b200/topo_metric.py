@@ -310,20 +310,12 @@ class TopoDevice:
         c = dict(DEFAULT_CAPS, **caps)
         self._lib = _lib.load()
         self.caps = _lib.SamRoadTopoCaps(**c)
-        h = C.c_void_p()
-        _lib.check(self._lib.samroad_topo_create(device, C.byref(self.caps), C.byref(h)), "samroad_topo_create")
-        self._h = h
+        self._h = _lib.Handle("samroad_topo_create", "samroad_topo_destroy", device, C.byref(self.caps))
+
+    __getstate__ = _lib.refuse_copy
 
     def close(self):
-        if self._h:
-            self._lib.samroad_topo_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._h.close()
 
     def upload(self, which: int, g: RoadGraph):
         ll = np.ascontiguousarray(np.asarray(g.nodes, dtype=np.float64).reshape(-1, 2))

@@ -451,7 +451,7 @@ def test_coincident_survivors():
 # ---- 8. one object across batch sizes --------------------------------------------------------------------------
 
 def test_one_object_across_batch_sizes():
-    """ensure_work: B = 2, 40, 5, 1 on one LabelScenes re-grows the work buffers and the pinned read-back once and
+    """The work area: B = 2, 40, 5, 1 on one LabelScenes re-grows the work buffers and the pinned read-back once and
     then reuses them.  The status word is read with the survivor counts for every B up to the allocated one; each
     batch equals the oracle and a fresh object's batch, and a bad patch in a smaller batch is still refused."""
     lc = _lc(P=128, S=7, Np=8, r_nms=16, r_nbr=64)
