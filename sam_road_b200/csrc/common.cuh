@@ -79,6 +79,9 @@ using PinnedBuffer = Buffer<true>;
 
 __host__ __device__ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// Blocks of `per` elements that cover n elements: a grid size.
+inline int blocks_for(long long n, int per) { return static_cast<int>((n + per - 1) / per); }
+
 // Bump allocator over a workspace.  Each workspace has one function that takes its regions in order; called
 // with a null base it only counts (bytes() is then the size to allocate, and what take() returns is an
 // offset, not a pointer), called with the allocation it carves the same regions.  Every region starts at a

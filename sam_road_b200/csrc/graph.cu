@@ -34,6 +34,7 @@
 
 #include "common.cuh"
 #include "ops.h"
+#include "scan.cuh"
 
 using namespace srb;
 
@@ -51,7 +52,6 @@ int grow(DeviceBuffer& b, size_t bytes) {
 // use them clear them all on entry.
 struct Counters {
   int cand[2];       // candidates per mask
-  int sort_total;    // counting sort: scan total
   int order_err;     // visiting order: 1 = host index out of range, 2 = not non-increasing
   int n_mortal;      // entries of an NMS pass that can be suppressed
   int survivors;     // entries an NMS pass keeps
@@ -69,14 +69,14 @@ struct samroad_graph_ctx {
   int device = 0;
   DeviceBuffer counters;                  // one Counters
   // keypoint extraction
-  DeviceBuffer blk_cnt, blk_off;          // compaction scratch
+  DeviceBuffer blk;                       // compaction: counts of the chunks, scanned in place, + scan scratch
   DeviceBuffer cand_pix[2], cand_score[2]; // candidates of the two masks, np.where order
   DeviceBuffer order, sorted_pix, immune; // visiting order of one NMS pass
   DeviceBuffer list[3];                   // kept pixels of passes 1 / 2 / 3, visiting order
   DeviceBuffer cand3, cls3;               // pass 3 input: concatenation + class (1 = keypoint mask)
   DeviceBuffer cell;                      // scene-sized rank/state image
   DeviceBuffer tile_und, round_cnt;       // NMS rounds
-  DeviceBuffer ghist;                     // counting sort
+  DeviceBuffer ghist;                     // counting sort: histogram + scan scratch (host order: its permutation)
   PinnedBuffer h_pin;                     // kPinBytes of pinned host memory for small read-backs
   // pair queries
   DeviceBuffer pts32, t_cnt, t_off, members, nbr, tile_xy;
@@ -87,7 +87,7 @@ struct samroad_graph_ctx {
   int max_nbr = 0;                        // K the plan was made for (fill / aggregate take K <= max_nbr)
   int nbr_stride = 16;                    // row length of nbr: 16 for max_nbr <= 16, else 32
   // aggregation
-  DeviceBuffer adj_deg, adj_off, adj_src, adj_tgt, adj_sum, adj_cnt, adj_first, eflags, tile_soff;
+  DeviceBuffer adj_off, adj_src, adj_tgt, adj_sum, adj_cnt, adj_first, eflags, tile_soff;
 };
 
 namespace {
@@ -96,38 +96,7 @@ constexpr uint32_t kNone = 0xFFFFFFFFu;
 constexpr uint32_t kUndecided = 0u, kKept = 1u, kSuppressed = 2u;
 
 // ---------------------------------------------------------------------------------------------------
-// block-wide exclusive scan of one int per thread (blockDim.x multiple of 32, <= 1024)
-// ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int block_excl_scan(int v, int* sw /*[33]*/, int& total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) sw[wid] = inc;
-  __syncthreads();
-  if (wid == 0) {
-    const int w = lane < nw ? sw[lane] : 0;
-    int wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, wi, o);
-      if (lane >= o) wi += t;
-    }
-    sw[lane] = wi - w;
-    if (lane == 31) sw[32] = wi;
-  }
-  __syncthreads();
-  const int res = inc - v + sw[wid];
-  total = sw[32];
-  __syncthreads();
-  return res;
-}
-
-// ---------------------------------------------------------------------------------------------------
-// ordered stream compaction: count per 1024-element chunk -> scan of chunk counts -> fill.
+// ordered stream compaction: count per 1024-element chunk -> exclusive scan of the counts -> fill.
 // F provides   __device__ bool pred(int i) const;   __device__ void emit(int i, int pos) const;
 // Output positions follow the input order (what np.where / boolean indexing produce).
 // ---------------------------------------------------------------------------------------------------
@@ -142,25 +111,8 @@ __global__ void __launch_bounds__(256) compact_count_kernel(F f, int n, int* __r
   for (int e = 0; e < 4; ++e)
     if (base + e < n && f.pred(base + e)) ++c;
   int total;
-  block_excl_scan(c, sw, total);
+  block_exclusive_scan(c, sw, total);
   if (threadIdx.x == 0) blk_cnt[blockIdx.x] = total;
-}
-
-// exclusive scan of `n` ints by one block; writes the grand total to *total_out
-__global__ void __launch_bounds__(1024) scan_single_block_kernel(const int* __restrict__ in, int n,
-                                                                 int* __restrict__ out,
-                                                                 int* __restrict__ total_out) {
-  __shared__ int sw[33];
-  int carry = 0;
-  for (int base = 0; base < n; base += 1024) {
-    const int i = base + threadIdx.x;
-    const int v = i < n ? in[i] : 0;
-    int total;
-    const int ex = block_excl_scan(v, sw, total);
-    if (i < n) out[i] = carry + ex;
-    carry += total;
-  }
-  if (threadIdx.x == 0) *total_out = carry;
 }
 
 template <class F>
@@ -175,7 +127,7 @@ __global__ void __launch_bounds__(256) compact_fill_kernel(F f, int n, const int
     c += p[e] ? 1 : 0;
   }
   int total;
-  int pos = blk_off[blockIdx.x] + block_excl_scan(c, sw, total);
+  int pos = blk_off[blockIdx.x] + block_exclusive_scan(c, sw, total);
 #pragma unroll
   for (int e = 0; e < 4; ++e)
     if (p[e]) f.emit(base + e, pos++);
@@ -184,18 +136,20 @@ __global__ void __launch_bounds__(256) compact_fill_kernel(F f, int n, const int
 // host driver: returns the number of emitted elements in *n_out_dev (device int) -- no sync
 template <class F>
 int compact(samroad_graph_ctx* g, const F& f, int n, int* n_out_dev, cudaStream_t st) {
-  const int nblk = (n + kChunk - 1) / kChunk;
+  const int nblk = blocks_for(n, kChunk);
   if (nblk == 0) {
     SRB_CUDA_OK(cudaMemsetAsync(n_out_dev, 0, sizeof(int), st));
     return 0;
   }
-  if (int rc = grow(g->blk_cnt, sizeof(int) * nblk)) return rc;
-  if (int rc = grow(g->blk_off, sizeof(int) * nblk)) return rc;
-  compact_count_kernel<F><<<nblk, 256, 0, st>>>(f, n, g->blk_cnt.as<int>());
-  scan_single_block_kernel<<<1, 1024, 0, st>>>(g->blk_cnt.as<int>(), nblk, g->blk_off.as<int>(), n_out_dev);
-  compact_fill_kernel<F><<<nblk, 256, 0, st>>>(f, n, g->blk_off.as<int>());
+  if (int rc = grow(g->blk, sizeof(int) * (nblk + scan_scratch_elems(nblk)))) return rc;
+  int* blk = g->blk.as<int>();
+  compact_count_kernel<F><<<nblk, 256, 0, st>>>(f, n, blk);
   SRB_CUDA_OK(cudaGetLastError());
-  note_launch(3);
+  note_launch(1);
+  if (int rc = exclusive_scan(blk, blk, nblk, n_out_dev, blk + nblk, st)) return rc;
+  compact_fill_kernel<F><<<nblk, 256, 0, st>>>(f, n, blk);
+  SRB_CUDA_OK(cudaGetLastError());
+  note_launch(1);
   return 0;
 }
 
@@ -233,49 +187,16 @@ struct EdgeFlag {    // edges in dict-insertion (first occurrence) order, infere
   }
 };
 
-// ---------------------------------------------------------------------------------------------------
-// device visiting order:  np.argsort(scores, kind='stable')[::-1]  for uint8 scores
-// (descending score, equal scores in descending candidate index).  Stable counting sort: one warp
-// per chunk of 1024 elements, per-(key, chunk) histogram -> scan -> ordered scatter.
-// ---------------------------------------------------------------------------------------------------
-constexpr int kSortChunk = 1024;
-
-__global__ void __launch_bounds__(32) sort_hist_kernel(const uint8_t* __restrict__ key, int n, int nchunks,
-                                                       int* __restrict__ ghist) {
-  __shared__ int hist[256];
-  for (int i = threadIdx.x; i < 256; i += 32) hist[i] = 0;
-  __syncwarp();
-  const int base = blockIdx.x * kSortChunk;
-  for (int it = 0; it < kSortChunk / 32; ++it) {
-    const int i = base + it * 32 + threadIdx.x;
-    if (i < n) atomicAdd(&hist[key[i]], 1);
-  }
-  __syncwarp();
-  for (int k = threadIdx.x; k < 256; k += 32) ghist[k * nchunks + blockIdx.x] = hist[k];
-}
-
-__global__ void __launch_bounds__(32) sort_scatter_kernel(const uint8_t* __restrict__ key, int n, int nchunks,
-                                                          const int* __restrict__ goff,
-                                                          int32_t* __restrict__ order) {
-  __shared__ int off[256];
-  for (int k = threadIdx.x; k < 256; k += 32) off[k] = goff[k * nchunks + blockIdx.x];
-  __syncwarp();
-  const int base = blockIdx.x * kSortChunk;
-  const unsigned lane = threadIdx.x;
-  for (int it = 0; it < kSortChunk / 32; ++it) {
-    const int i = base + it * 32 + static_cast<int>(lane);
-    const bool ok = i < n;
-    const unsigned k = ok ? key[i] : (256u + lane);      // out-of-range lanes match only themselves
-    const unsigned peers = __match_any_sync(0xffffffffu, k);
-    const int r = __popc(peers & ((1u << lane) - 1u));
-    int asc = 0;
-    if (ok) asc = off[k] + r;
-    __syncwarp();
-    if (ok && r == 0) off[k] += __popc(peers);
-    __syncwarp();
-    if (ok) order[n - 1 - asc] = i;
-  }
-}
+// device visiting order:  np.argsort(scores, kind='stable')[::-1]  for uint8 scores (descending score,
+// equal scores in descending candidate index): one stable counting-sort pass on the score, ranks reversed.
+struct ReversedOrder {
+  const uint8_t* score;
+  int n;
+  int32_t* order;
+  __device__ uint32_t key(long long i) const { return __ldg(score + i); }
+  __device__ unsigned digit(uint32_t k) const { return k; }
+  __device__ void emit(long long i, uint32_t, uint32_t pos) const { order[n - 1 - pos] = static_cast<int32_t>(i); }
+};
 
 // host permutation (ascending argsort, int64) -> visiting order (its reverse, int32)
 __global__ void order_from_host_kernel(const int64_t* __restrict__ asc, int n, int32_t* __restrict__ order,
@@ -482,8 +403,6 @@ __global__ void pix_to_xy_kernel(const int32_t* __restrict__ pix, int n, int W, 
   out[2 * static_cast<size_t>(i) + 1] = p / W;    // y
 }
 
-inline int blocks_for(long n, int per = 256) { return static_cast<int>((n + per - 1) / per); }
-
 // read a small device object back (synchronises the stream)
 template <typename T>
 int read_back(samroad_graph_ctx* g, const T* dev, T* host, cudaStream_t st) {
@@ -528,25 +447,18 @@ int host_order(samroad_graph_ctx* g, const uint8_t* key, int n, int key_dtype, s
   const std::vector<int64_t>& asc = pre_asc ? *pre_asc : own;
   if (int rc = grow(g->ghist, sizeof(int64_t) * n)) return rc;
   SRB_CUDA_OK(cudaMemcpyAsync(g->ghist.get(), asc.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
-  order_from_host_kernel<<<blocks_for(n), 256, 0, st>>>(g->ghist.as<int64_t>(), n, order, err);
+  order_from_host_kernel<<<blocks_for(n, 256), 256, 0, st>>>(g->ghist.as<int64_t>(), n, order, err);
   note_launch();
   SRB_CUDA_OK(cudaStreamSynchronize(st));   // `asc` is pageable host memory: keep it alive until copied
   return 0;
 }
 
 // Visiting order on the device: np.argsort(key, kind='stable')[::-1] by the counting sort
-int stable_order(samroad_graph_ctx* g, const uint8_t* key, int n, int32_t* order, int* scan_total,
-                 cudaStream_t st) {
-  const int nchunks = (n + kSortChunk - 1) / kSortChunk;
-  if (int rc = grow(g->ghist, sizeof(int) * 256 * static_cast<size_t>(nchunks) * 2 + 16)) return rc;
-  int* hist = g->ghist.as<int>();
-  int* off = hist + 256 * static_cast<size_t>(nchunks);
-  sort_hist_kernel<<<nchunks, 32, 0, st>>>(key, n, nchunks, hist);
-  scan_single_block_kernel<<<1, 1024, 0, st>>>(hist, 256 * nchunks, off, scan_total);
-  sort_scatter_kernel<<<nchunks, 32, 0, st>>>(key, n, nchunks, off, order);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(3);
-  return 0;
+int stable_order(samroad_graph_ctx* g, const uint8_t* key, int n, int32_t* order, cudaStream_t st) {
+  const long long m = digit_hist_elems<1024>(n);
+  if (int rc = grow(g->ghist, sizeof(uint32_t) * (m + scan_scratch_elems(m)))) return rc;
+  uint32_t* hist = g->ghist.as<uint32_t>();
+  return stable_digit_pass<1024>(ReversedOrder{key, n, order}, n, hist, hist + m, st);
 }
 
 struct PassStats {
@@ -573,11 +485,11 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
   Counters* ctr = g->counters.as<Counters>();
   clk::time_point t0 = clk::now();
   if (int rc = cb ? host_order(g, key, n, key_dtype, cb, user, pre_asc, order, &ctr->order_err, st)
-                  : stable_order(g, key, n, order, &ctr->sort_total, st))
+                  : stable_order(g, key, n, order, st))
     return rc;
   SRB_CUDA_OK(cudaMemsetAsync(&ctr->n_mortal, 0, sizeof(int), st));
-  gather_sorted_kernel<<<blocks_for(n), 256, 0, st>>>(pix, key, order, n, sorted_pix, immune, &ctr->n_mortal,
-                                                      &ctr->order_err);
+  gather_sorted_kernel<<<blocks_for(n, 256), 256, 0, st>>>(pix, key, order, n, sorted_pix, immune, &ctr->n_mortal,
+                                                           &ctr->order_err);
   note_launch();
   Counters c;
   if (int rc = read_back(g, ctr, &c, st)) return rc;
@@ -599,7 +511,7 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
   if (int rc = grow(g->cell, npx * 4)) return rc;
   uint32_t* cell = g->cell.as<uint32_t>();
   SRB_CUDA_OK(cudaMemsetAsync(cell, 0xFF, npx * 4, st));
-  cell_build_kernel<<<blocks_for(n), 256, 0, st>>>(sorted_pix, immune, n, cell);
+  cell_build_kernel<<<blocks_for(n, 256), 256, 0, st>>>(sorted_pix, immune, n, cell);
   note_launch();
   const int tx = (W + kNmsTile - 1) / kNmsTile, ty = (H + kNmsTile - 1) / kNmsTile;
   constexpr int kMaxRounds = 4096;
@@ -622,8 +534,8 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
         nms_round_kernel<<<dim3(tx, ty), 256, smem, st>>>(cell, H, W, halo, d2max, g->tile_und.as<int>(),
                                                           round_cnt + round);
       else
-        nms_round_generic_kernel<<<blocks_for(n), 256, 0, st>>>(cell, sorted_pix, n, H, W, halo, d2max,
-                                                                round_cnt + round);
+        nms_round_generic_kernel<<<blocks_for(n, 256), 256, 0, st>>>(cell, sorted_pix, n, H, W, halo, d2max,
+                                                                     round_cnt + round);
       note_launch();
     }
     SRB_CUDA_OK(cudaGetLastError());
@@ -748,8 +660,8 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
     if (int rc = grow(g->cand3, sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
     if (int rc = grow(g->cls3, static_cast<size_t>(n3))) return rc;
     if (int rc = grow(g->list[2], sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
-    concat_kernel<<<blocks_for(n3), 256, 0, st>>>(g->list[0].as<int32_t>(), m0, g->list[1].as<int32_t>(), m1,
-                                                  g->cand3.as<int32_t>(), g->cls3.as<uint8_t>());
+    concat_kernel<<<blocks_for(n3, 256), 256, 0, st>>>(g->list[0].as<int32_t>(), m0, g->list[1].as<int32_t>(), m1,
+                                                       g->cand3.as<int32_t>(), g->cls3.as<uint8_t>());
     note_launch();
     const bool pre3 = have_pre && m0 == n_cand[0] && m1 == n_cand[1];
     if (int rc = nms_pass(g, g->cand3.as<int32_t>(), g->cls3.as<uint8_t>(), n3, SAMROAD_F64, argsort, user,
@@ -761,7 +673,7 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
   SRB_REQUIRE(points_xy != nullptr || n_out == 0, "samroad_extract_graph_points: null output");
   SRB_REQUIRE(n_out <= cap, "samroad_extract_graph_points: %d keypoints exceed the output capacity %d", n_out, cap);
   if (n_out > 0) {
-    pix_to_xy_kernel<<<blocks_for(n_out), 256, 0, st>>>(g->list[2].as<int32_t>(), n_out, W, points_xy);
+    pix_to_xy_kernel<<<blocks_for(n_out, 256), 256, 0, st>>>(g->list[2].as<int32_t>(), n_out, W, points_xy);
     note_launch();
     SRB_CUDA_OK(cudaGetLastError());
   }
@@ -801,7 +713,7 @@ tile_count_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restr
   int c = 0;
   for (int i = threadIdx.x; i < N; i += 256) c += in_tile(pts[2 * i], pts[2 * i + 1], x0, y0, P) ? 1 : 0;
   int total;
-  block_excl_scan(c, sw, total);
+  block_exclusive_scan(c, sw, total);
   if (threadIdx.x == 0) cnt[t] = total;
 }
 
@@ -817,7 +729,7 @@ tile_fill_kernel(const int32_t* __restrict__ pts, int N, const int32_t* __restri
     const int i = b + threadIdx.x;
     const bool in = i < N && in_tile(pts[2 * i], pts[2 * i + 1], x0, y0, P);
     int total;
-    const int pos = block_excl_scan(in ? 1 : 0, sw, total);
+    const int pos = block_exclusive_scan(in ? 1 : 0, sw, total);
     if (in) members[base + pos] = i;
     base += total;
   }
@@ -944,7 +856,7 @@ extern "C" int samroad_pair_queries_plan_k(samroad_graph_t g, const int64_t* poi
     return 0;
   }
   if (int rc = grow(g->pts32, sizeof(int32_t) * 2 * static_cast<size_t>(N))) return rc;
-  points_to_i32_kernel<<<blocks_for(2L * N), 256, 0, st>>>(points_xy, 2 * N, g->pts32.as<int32_t>());
+  points_to_i32_kernel<<<blocks_for(2L * N, 256), 256, 0, st>>>(points_xy, 2 * N, g->pts32.as<int32_t>());
   tile_count_kernel<<<n_tiles, 256, 0, st>>>(g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P, g->t_cnt.as<int>());
   note_launch(2);
   SRB_CUDA_OK(cudaMemcpyAsync(g->h_cnt.data(), g->t_cnt.get(), sizeof(int) * n_tiles, cudaMemcpyDeviceToHost, st));
@@ -999,7 +911,7 @@ extern "C" int samroad_pair_queries_fill(samroad_graph_t g, int tile_begin, int 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long total = static_cast<long>(B) * nmax * K;
   auto* fill = g->nbr_stride == 16 ? fill_batch_kernel<16> : fill_batch_kernel<32>;
-  fill<<<blocks_for(total), 256, 0, st>>>(
+  fill<<<blocks_for(total, 256), 256, 0, st>>>(
       g->pts32.as<int32_t>(), g->tile_xy.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
       g->members.as<int32_t>(), g->nbr.as<int32_t>(), tile_begin, B, nmax, K, points, pairs, valid);
   SRB_CUDA_OK(cudaGetLastError());
@@ -1202,21 +1114,21 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
               "planned for %d", K, g->max_nbr);
   SRB_REQUIRE(topo_scores != nullptr, "samroad_aggregate_edges: null scores");
   const int32_t* pts = g->pts32.as<int32_t>();
-  if (int rc = grow(g->adj_deg, sizeof(int) * static_cast<size_t>(N))) return rc;
-  if (int rc = grow(g->adj_off, sizeof(int) * (static_cast<size_t>(N) + 1))) return rc;
+  // adj_off: the degrees, scanned in place into N + 1 offsets, then the scan's scratch
+  if (int rc = grow(g->adj_off, sizeof(int) * (N + 1 + scan_scratch_elems(N)))) return rc;
   if (int rc = grow(g->tile_soff, sizeof(int64_t) * g->n_tiles)) return rc;
   SRB_CUDA_OK(cudaMemcpyAsync(g->tile_soff.get(), tile_score_offset_host, sizeof(int64_t) * g->n_tiles,
                               cudaMemcpyHostToDevice, st));
   Counters* ctr = g->counters.as<Counters>();
   SRB_CUDA_OK(cudaMemsetAsync(ctr, 0, sizeof(Counters), st));
-  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, nullptr, g->adj_deg.as<int>(), nullptr, nullptr,
-                                                 &ctr->max_deg);
-  scan_single_block_kernel<<<1, 1024, 0, st>>>(g->adj_deg.as<int>(), N, g->adj_off.as<int>(), &ctr->nnz);
-  note_launch(2);
+  int* adj_off = g->adj_off.as<int>();
+  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, nullptr, adj_off, nullptr, nullptr, &ctr->max_deg);
+  note_launch(1);
+  if (int rc = exclusive_scan(adj_off, adj_off, N, &ctr->nnz, adj_off + N + 1, st)) return rc;
   Counters c;
   if (int rc = read_back(g, ctr, &c, st)) return rc;
   const int max_deg = c.max_deg, nnz = c.nnz;
-  SRB_CUDA_OK(cudaMemcpyAsync(g->adj_off.as<int>() + N, &ctr->nnz, sizeof(int), cudaMemcpyDeviceToDevice, st));
+  SRB_CUDA_OK(cudaMemcpyAsync(adj_off + N, &ctr->nnz, sizeof(int), cudaMemcpyDeviceToDevice, st));
   if (nnz == 0) return 0;
   const size_t nz = static_cast<size_t>(nnz);
   if (int rc = grow(g->adj_src, 4 * nz)) return rc;
@@ -1230,19 +1142,19 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
   SRB_CUDA_OK(cudaMemsetAsync(g->adj_cnt.get(), 0, 4 * nz, st));
   SRB_CUDA_OK(cudaMemsetAsync(g->adj_first.get(), 0xFF, 4 * nz, st));
   SRB_CUDA_OK(cudaMemsetAsync(g->eflags.get(), 0xFF, 4 * static_cast<size_t>(n_entries), st));
-  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, g->adj_off.as<int>(), nullptr,
+  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, adj_off, nullptr,
                                                  g->adj_src.as<int32_t>(), g->adj_tgt.as<int32_t>(), nullptr);
   const AggArgs args{pts, N, g->tile_xy.as<int32_t>(), g->n_tiles, g->P, g->t_cnt.as<int>(), g->t_off.as<int>(),
                      g->members.as<int32_t>(), g->nbr.as<int32_t>(), topo_scores, g->tile_soff.as<int64_t>(), K,
-                     g->adj_off.as<int>(), g->adj_tgt.as<int32_t>(), g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
+                     adj_off, g->adj_tgt.as<int32_t>(), g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
                      g->adj_first.as<int32_t>(), &ctr->bad_score};
   if (g->nbr_stride == 16)
     launch_aggregate<16>(max_deg, args, st);
   else
     launch_aggregate<32>(max_deg, args, st);
-  edge_select_kernel<<<blocks_for(nnz), 256, 0, st>>>(g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
-                                                      g->adj_first.as<int32_t>(), nnz, threshold,
-                                                      g->eflags.as<int32_t>());
+  edge_select_kernel<<<blocks_for(nnz, 256), 256, 0, st>>>(g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
+                                                           g->adj_first.as<int32_t>(), nnz, threshold,
+                                                           g->eflags.as<int32_t>());
   note_launch(3);
   EdgeFlag ef{g->eflags.as<int32_t>(), g->adj_src.as<int32_t>(), g->adj_tgt.as<int32_t>(), edges, edges ? cap : 0};
   if (int rc = compact(g, ef, static_cast<int>(n_entries), &ctr->n_edges, st)) return rc;

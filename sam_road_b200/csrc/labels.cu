@@ -30,6 +30,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "scan.cuh"
 
 using namespace srb;
 
@@ -176,34 +177,6 @@ __global__ void crop_kernel(Params p, const int32_t* patch, float* rgb, float* k
   road[o] = __fdiv_rn(static_cast<float>(sc.road[s]), 255.0f);
 }
 
-// exclusive prefix sum of v over the block; *total gets the block sum.  All threads must call it.
-__device__ int block_scan_excl(int v, int* warp_tot, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_tot[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    const int t = lane < nw ? warp_tot[lane] : 0;
-    int s = t;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += y;
-    }
-    if (lane < nw) warp_tot[lane] = s - t;
-    if (lane == 31) *total = s;
-  }
-  __syncthreads();
-  const int r = warp_tot[wid] + x - v;
-  __syncthreads();
-  return r;
-}
-
 // sort order of the NMS visit: score descending, then id ascending
 __device__ __forceinline__ bool precedes(unsigned long long ka, int ia, unsigned long long kb, int ib) {
   return ka > kb || (ka == kb && ia < ib);
@@ -227,8 +200,7 @@ size_t patch_smem_bytes(int cap) {
 
 __global__ void __launch_bounds__(kPatchThreads) patch_kernel(Params p, Work w) {
   extern __shared__ __align__(16) unsigned char smem[];
-  __shared__ int warp_tot[32];
-  __shared__ int s_total;
+  __shared__ int scan_sm[33];
   const int b = blockIdx.x, tid = threadIdx.x;
   const int32_t* pa = w.patch + 4 * b;
   if (!patch_ok(p, pa)) {
@@ -252,8 +224,8 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(Params p, Work w) 
       const double x = sc.pts[2 * i], y = sc.pts[2 * i + 1];
       keep = x >= bx0 && x <= bx1 && y >= by0 && y <= by1 && !(sc.flags[i] & kExcluded);
     }
-    const int pos = block_scan_excl(keep, warp_tot, &s_total);
-    const int tot = s_total;
+    int tot;
+    const int pos = block_exclusive_scan(keep, scan_sm, tot);
     if (keep && M + pos < p.cap) cand[M + pos] = i;
     M += tot;
   }
@@ -344,9 +316,10 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(Params p, Work w) 
     for (int base = 0; base < nc * nc + 1; base += blockDim.x) {
       const int c = base + tid;
       const int v = c < nc * nc + 1 ? cstart[c] : 0;
-      const int ex = block_scan_excl(v, warp_tot, &s_total);
+      int tot;
+      const int ex = block_exclusive_scan(v, scan_sm, tot);
       if (c < nc * nc + 1) cstart[c] = carry + ex + v;
-      carry += s_total;
+      carry += tot;
     }
   }
   for (int c = tid; c < nc * nc; c += blockDim.x) ccur[c] = cstart[c];

@@ -27,6 +27,7 @@
 #include "common.cuh"
 #include "loss_terms.cuh"
 #include "ops.h"
+#include "scan.cuh"
 
 using namespace srb;
 
@@ -56,10 +57,9 @@ constexpr unsigned kBadPred = 1u, kBadTarget = 2u;
 const char* const kPrcBadText[] = {" a prediction is NaN or outside [0, 1]",
                                    " a target is not 0 or 1 after truncation to int32"};
 
-// Tile sizes.  The radix sort gives one warp a chunk of kSortChunk keys (stable within the warp by
-// __match_any_sync ranks); scans and the curve kernel give a 256-thread block kTile elements.
+// The radix sort gives one warp a chunk of kSortChunk keys; the curve kernels give a 256-thread block kTile
+// keys.
 constexpr int kSortChunk = 4096;
-constexpr int kSortWarps = 8;
 constexpr int kTile = 4096;
 constexpr int kTileItems = kTile / 256;
 
@@ -74,9 +74,8 @@ struct samroad_prc_ctx {
   size_t reserved = 0;             // host upper bound of state->committed
   long long n_updates = 0;         // updates since the last reset
   // scratch of compute
-  DeviceBuffer hist;               // per (digit, chunk) counts, scanned in place
-  DeviceBuffer tile_sums;
-  DeviceBuffer tile_cnt;           // curve: (starts << 32 | positives) per tile, then scanned
+  DeviceBuffer hist;               // per (digit, chunk) counts, scanned in place, + scan scratch
+  DeviceBuffer tile_cnt;           // curve: (starts << 32 | positives) per tile, then scanned; total; scan scratch
   // the curve of the last successful compute: thr [T], prec [T+1], rec [T+1], tps [T], fps [T]
   DeviceBuffer thr, prec, rec, tps, fps;
   size_t curve_cap = 0;
@@ -92,8 +91,6 @@ struct samroad_prc_ctx {
 };
 
 namespace {
-
-inline int grid_for(long long n, int per) { return static_cast<int>((n + per - 1) / per); }
 
 // Grows a scratch buffer of compute to n elements of T, with 25 % + 64 elements of slack.  No
 // synchronisation: compute synchronises before it returns, so no earlier work still reads the old block.
@@ -205,132 +202,15 @@ __global__ void prc_commit_kernel(PrcState* st, long long serial) {
   st->staged = st->committed;
 }
 
-// ---------------------------------------------------------------------------------------------------
-// LSD radix sort of 32-bit keys, 8 bits per pass: per (digit, warp chunk) histogram, one exclusive scan
-// of the digit-major histogram (global offsets of every digit in every chunk), ordered scatter.  A warp
-// walks its chunk in 32-key steps; __match_any_sync ranks equal digits within a step in lane order, so
-// each pass is stable and the result does not depend on scheduling.
-// ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(32 * kSortWarps) radix_hist_kernel(const uint32_t* __restrict__ keys, long long n,
-                                                                    int nchunks, int shift,
-                                                                    uint32_t* __restrict__ hist) {
-  __shared__ uint32_t h[kSortWarps][256];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int chunk = blockIdx.x * kSortWarps + w;
-  for (int d = lane; d < 256; d += 32) h[w][d] = 0;
-  __syncwarp();
-  if (chunk < nchunks) {
-    const long long base = static_cast<long long>(chunk) * kSortChunk;
-    for (int it = 0; it < kSortChunk / 32; ++it) {
-      const long long i = base + it * 32 + lane;
-      if (i < n) atomicAdd(&h[w][(keys[i] >> shift) & 255u], 1u);
-    }
-    __syncwarp();
-    for (int d = lane; d < 256; d += 32) hist[static_cast<size_t>(d) * nchunks + chunk] = h[w][d];
-  }
-}
-
-__global__ void __launch_bounds__(32 * kSortWarps) radix_scatter_kernel(const uint32_t* __restrict__ in, long long n,
-                                                                       int nchunks, int shift,
-                                                                       const uint32_t* __restrict__ off,
-                                                                       uint32_t* __restrict__ out) {
-  __shared__ uint32_t o[kSortWarps][256];
-  const int w = threadIdx.x >> 5;
-  const unsigned lane = threadIdx.x & 31;
-  const int chunk = blockIdx.x * kSortWarps + w;
-  if (chunk >= nchunks) return;
-  for (int d = lane; d < 256; d += 32) o[w][d] = off[static_cast<size_t>(d) * nchunks + chunk];
-  __syncwarp();
-  const long long base = static_cast<long long>(chunk) * kSortChunk;
-  for (int it = 0; it < kSortChunk / 32; ++it) {
-    const long long i = base + it * 32 + lane;
-    const bool ok = i < n;
-    const uint32_t key = ok ? in[i] : 0u;
-    const unsigned d = ok ? ((key >> shift) & 255u) : (256u + lane);   // idle lanes match only themselves
-    const unsigned peers = __match_any_sync(0xffffffffu, d);
-    const unsigned r = __popc(peers & ((1u << lane) - 1u));
-    uint32_t pos = 0;
-    if (ok) pos = o[w][d] + r;
-    __syncwarp();
-    if (ok && r == 0) o[w][d] += __popc(peers);
-    __syncwarp();
-    if (ok) out[pos] = key;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// exclusive scans: 256-thread block scan, tile sums -> one-block scan of the sums -> tile scan
-// ---------------------------------------------------------------------------------------------------
-template <typename T>
-__device__ __forceinline__ T block_excl_scan256(T v, T* sw /*[9]*/, T& total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  T inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const T t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) sw[wid] = inc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    T acc = 0;
-    for (int k = 0; k < 8; ++k) {
-      const T t = sw[k];
-      sw[k] = acc;
-      acc += t;
-    }
-    sw[8] = acc;
-  }
-  __syncthreads();
-  const T res = inc - v + sw[wid];
-  total = sw[8];
-  __syncthreads();
-  return res;
-}
-
-__global__ void __launch_bounds__(256) tile_sum_kernel(const uint32_t* __restrict__ a, long long m,
-                                                       uint32_t* __restrict__ sums) {
-  __shared__ uint32_t sw[9];
-  const long long base = static_cast<long long>(blockIdx.x) * kTile;
-  uint32_t s = 0;
-  for (int it = 0; it < kTileItems; ++it) {
-    const long long i = base + it * 256 + threadIdx.x;
-    if (i < m) s += a[i];
-  }
-  uint32_t total;
-  block_excl_scan256(s, sw, total);
-  if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-
-// in-place exclusive scan of m values by one block
-template <typename T>
-__global__ void __launch_bounds__(256) scan_one_block_kernel(T* __restrict__ a, int m) {
-  __shared__ T sw[9];
-  T carry = 0;
-  for (int base = 0; base < m; base += 256) {
-    const int i = base + threadIdx.x;
-    const T v = i < m ? a[i] : T(0);
-    T total;
-    const T ex = block_excl_scan256(v, sw, total);
-    if (i < m) a[i] = carry + ex;
-    carry += total;
-  }
-}
-
-__global__ void __launch_bounds__(256) tile_scan_kernel(uint32_t* __restrict__ a, long long m,
-                                                        const uint32_t* __restrict__ tile_off) {
-  __shared__ uint32_t sw[9];
-  const long long base = static_cast<long long>(blockIdx.x) * kTile;
-  uint32_t carry = tile_off[blockIdx.x];
-  for (int it = 0; it < kTileItems; ++it) {
-    const long long i = base + it * 256 + threadIdx.x;
-    const uint32_t v = i < m ? a[i] : 0u;
-    uint32_t total;
-    const uint32_t ex = block_excl_scan256(v, sw, total);
-    if (i < m) a[i] = carry + ex;
-    carry += total;
-  }
-}
+// One LSD radix sort pass over 32-bit keys: the keys move themselves, stably, by the 8-bit digit at `shift`.
+struct RadixPass {
+  const uint32_t* in;
+  uint32_t* out;
+  int shift;
+  __device__ uint32_t key(long long i) const { return __ldg(in + i); }   // read-only: loads run ahead of the stores
+  __device__ unsigned digit(uint32_t k) const { return (k >> shift) & 255u; }
+  __device__ void emit(long long, uint32_t k, uint32_t pos) const { out[pos] = k; }
+};
 
 // ---------------------------------------------------------------------------------------------------
 // curve over the sorted keys.  Element i starts a run when its score differs from element i-1's; run j
@@ -344,7 +224,7 @@ __device__ __forceinline__ bool run_start(const uint32_t* keys, long long i) {
 
 __global__ void __launch_bounds__(256) curve_count_kernel(const uint32_t* __restrict__ keys, long long n,
                                                           unsigned long long* __restrict__ tile_cnt) {
-  __shared__ unsigned long long sw[9];
+  __shared__ unsigned long long sw[33];
   const long long base = static_cast<long long>(blockIdx.x) * kTile;
   unsigned long long c = 0;
   for (int it = 0; it < kTileItems; ++it) {
@@ -352,7 +232,7 @@ __global__ void __launch_bounds__(256) curve_count_kernel(const uint32_t* __rest
     if (i < n) c += (run_start(keys, i) ? (1ull << 32) : 0ull) + (keys[i] & 1u);
   }
   unsigned long long total;
-  block_excl_scan256(c, sw, total);
+  block_exclusive_scan(c, sw, total);
   if (threadIdx.x == 0) tile_cnt[blockIdx.x] = total;
 }
 
@@ -374,7 +254,7 @@ __global__ void __launch_bounds__(256) curve_fill_kernel(const uint32_t* __restr
                                                          long long* __restrict__ tps_out,
                                                          long long* __restrict__ fps_out,
                                                          PrcState* __restrict__ st) {
-  __shared__ unsigned long long sw[9];
+  __shared__ unsigned long long sw[33];
   __shared__ unsigned long long best_sh;
   if (threadIdx.x == 0) best_sh = 0;
   const long long base = static_cast<long long>(blockIdx.x) * kTile;
@@ -388,7 +268,7 @@ __global__ void __launch_bounds__(256) curve_fill_kernel(const uint32_t* __restr
     const bool start = in && run_start(keys, i);
     const unsigned long long c = (start ? (1ull << 32) : 0ull) + (in ? (key & 1u) : 0u);
     unsigned long long total;
-    const unsigned long long ex = carry + block_excl_scan256(c, sw, total);
+    const unsigned long long ex = carry + block_exclusive_scan(c, sw, total);
     carry += total;
     if (start) {
       const long long j = static_cast<long long>(ex >> 32);
@@ -478,36 +358,16 @@ int grow_keys(samroad_prc_ctx* p, long long n, const char* what, cudaStream_t st
   return 0;
 }
 
-// exclusive scan of m uint32 in place (values and their total < 2^32)
-int scan_u32(samroad_prc_ctx* p, uint32_t* a, long long m, cudaStream_t st) {
-  const int tiles = grid_for(m, kTile);
-  if (int rc = grow<uint32_t>(p->tile_sums, static_cast<size_t>(tiles))) return rc;
-  uint32_t* sums = p->tile_sums.as<uint32_t>();
-  tile_sum_kernel<<<tiles, 256, 0, st>>>(a, m, sums);
-  scan_one_block_kernel<uint32_t><<<1, 256, 0, st>>>(sums, tiles);
-  tile_scan_kernel<<<tiles, 256, 0, st>>>(a, m, sums);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(3);
-  return 0;
-}
-
+// LSD radix sort of the n keys, 8 bits per pass; each pass is stable, so the result is deterministic
 int radix_sort(samroad_prc_ctx* p, long long n, cudaStream_t st) {
   if (int rc = grow<uint32_t>(p->alt, static_cast<size_t>(n))) return rc;
-  const int nchunks = grid_for(n, kSortChunk);
-  const long long m = 256LL * nchunks;
-  if (int rc = grow<uint32_t>(p->hist, static_cast<size_t>(m))) return rc;
+  const long long m = digit_hist_elems<kSortChunk>(n);
+  if (int rc = grow<uint32_t>(p->hist, static_cast<size_t>(m + scan_scratch_elems(m)))) return rc;
   uint32_t* hist = p->hist.as<uint32_t>();
-  const int blocks = grid_for(nchunks, kSortWarps);
   uint32_t* src = p->keys;
   uint32_t* dst = p->alt.as<uint32_t>();
   for (int shift = 0; shift < 32; shift += 8) {    // 4 passes: the sorted keys end up back in p->keys
-    radix_hist_kernel<<<blocks, 32 * kSortWarps, 0, st>>>(src, n, nchunks, shift, hist);
-    SRB_CUDA_OK(cudaGetLastError());
-    note_launch(1);
-    if (int rc = scan_u32(p, hist, m, st)) return rc;
-    radix_scatter_kernel<<<blocks, 32 * kSortWarps, 0, st>>>(src, n, nchunks, shift, hist, dst);
-    SRB_CUDA_OK(cudaGetLastError());
-    note_launch(1);
+    if (int rc = stable_digit_pass<kSortChunk>(RadixPass{src, dst, shift}, n, hist, hist + m, st)) return rc;
     uint32_t* t = src;
     src = dst;
     dst = t;
@@ -565,9 +425,9 @@ extern "C" int samroad_prc_update(samroad_prc_t p, const float* preds, int64_t p
   PrcState* state = p->state.as<PrcState>();
   prc_begin_kernel<<<1, 1, 0, st>>>(state);
   if (target_dtype == SAMROAD_U8)
-    prc_append_kernel<true><<<grid_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
+    prc_append_kernel<true><<<blocks_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
   else
-    prc_append_kernel<false><<<grid_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
+    prc_append_kernel<false><<<blocks_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
   prc_commit_kernel<<<1, 1, 0, st>>>(state, p->n_updates);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(3);
@@ -585,7 +445,7 @@ extern "C" int samroad_prc_append_keys(samroad_prc_t p, const uint32_t* keys, in
   if (int rc = grow_keys(p, n, "samroad_prc_append_keys", st)) return rc;
   PrcState* state = p->state.as<PrcState>();
   prc_begin_kernel<<<1, 1, 0, st>>>(state);
-  prc_append_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(keys, n, p->keys, state);
+  prc_append_keys_kernel<<<blocks_for(n, 256), 256, 0, st>>>(keys, n, p->keys, state);
   prc_commit_kernel<<<1, 1, 0, st>>>(state, p->n_updates);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch(3);
@@ -616,14 +476,14 @@ extern "C" int samroad_prc_compute(samroad_prc_t p, int64_t* counts, float* best
   if (int rc = take_refusals(p, "samroad_prc_compute", &n, st)) return rc;
   SRB_REQUIRE(n > 0, "samroad_prc_compute: no entries (nothing was updated since the last reset)");
   if (int rc = radix_sort(p, n, st)) return rc;
-  const int tiles = grid_for(n, kTile);
-  if (int rc = grow<unsigned long long>(p->tile_cnt, static_cast<size_t>(tiles) + 1)) return rc;
+  const int tiles = blocks_for(n, kTile);
+  if (int rc = grow<unsigned long long>(p->tile_cnt, static_cast<size_t>(tiles + 1 + scan_scratch_elems(tiles))))
+    return rc;
   unsigned long long* tile_cnt = p->tile_cnt.as<unsigned long long>();
   curve_count_kernel<<<tiles, 256, 0, st>>>(p->keys, n, tile_cnt);
-  SRB_CUDA_OK(cudaMemsetAsync(tile_cnt + tiles, 0, sizeof(unsigned long long), st));
-  scan_one_block_kernel<unsigned long long><<<1, 256, 0, st>>>(tile_cnt, tiles + 1);
   SRB_CUDA_OK(cudaGetLastError());
-  note_launch(2);
+  note_launch(1);
+  if (int rc = exclusive_scan(tile_cnt, tile_cnt, tiles, tile_cnt + tiles, tile_cnt + tiles + 1, st)) return rc;
   unsigned long long tot = 0;
   SRB_CUDA_OK(cudaMemcpyAsync(&tot, tile_cnt + tiles, sizeof(tot), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
@@ -956,8 +816,8 @@ extern "C" int samroad_val_update(samroad_val_t v, const float* mask_logits, con
   SRB_CUDA_OK(cudaSetDevice(v->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long npix = static_cast<long long>(B) * P * P;
-  const int g_mask = static_cast<int>(std::min<long long>(grid_for(npix, 256), v->max_blocks));
-  const int g_pair = static_cast<int>(std::min<long long>(grid_for(n_pairs, 256), v->max_blocks));
+  const int g_mask = static_cast<int>(std::min<long long>(blocks_for(npix, 256), v->max_blocks));
+  const int g_pair = static_cast<int>(std::min<long long>(blocks_for(n_pairs, 256), v->max_blocks));
   ValState* state = v->state.as<ValState>();
   ValPartial* mask_part = v->part.as<ValPartial>();
   ValPartial* pair_part = mask_part + v->max_blocks;

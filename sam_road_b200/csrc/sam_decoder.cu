@@ -453,8 +453,6 @@ __global__ void sam_upsample4_kernel(const float* __restrict__ lr, int S4, long 
   }
 }
 
-inline int blocks_for(long n, int t) { return static_cast<int>((n + t - 1) / t); }
-
 }  // namespace
 
 struct SamDecoderWs {

@@ -28,6 +28,7 @@
 #include "common.cuh"
 #include "loss_terms.cuh"
 #include "ops.h"
+#include "scan.cuh"
 #include "toponet_tc.cuh"   // load_coord, resolve_pair
 
 using namespace srb;
@@ -779,31 +780,6 @@ __global__ void outer_kernel(const float* __restrict__ g, const float* __restric
 __global__ void csr_count_kernel(const int* __restrict__ idx, long long n, int* __restrict__ cnt) {
   GRID_STRIDE(i, n) atomicAdd(cnt + idx[i], 1);
 }
-// exclusive scan of cnt[0..n) into start[0..n], one block of 1024 threads
-__global__ void __launch_bounds__(1024) csr_scan_kernel(const int* __restrict__ cnt, int n, int* __restrict__ start) {
-  __shared__ int sh[1024];
-  const int per = (n + 1023) / 1024;
-  const int b = threadIdx.x * per, e = b + per < n ? b + per : n;
-  int s = 0;
-  for (int i = b; i < e; ++i) s += cnt[i];
-  sh[threadIdx.x] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int acc = 0;
-    for (int t = 0; t < 1024; ++t) {
-      const int v = sh[t];
-      sh[t] = acc;
-      acc += v;
-    }
-    start[n] = acc;
-  }
-  __syncthreads();
-  int acc = sh[threadIdx.x];
-  for (int i = b; i < e; ++i) {
-    start[i] = acc;
-    acc += cnt[i];
-  }
-}
 __global__ void csr_fill_kernel(const int* __restrict__ idx, long long n, const int* __restrict__ start,
                                 int* __restrict__ cursor, int* __restrict__ list) {
   GRID_STRIDE(i, n) {
@@ -892,7 +868,7 @@ struct TrainWs {
   float* emb;                           // [B, 256, T] image embeddings
   float *f0, *xh1, *rs1, *a1, *z2, *a2, *z3, *a3, *dl;   // decoder (dl: unscaled dlogits [R4, 2])
   float *fs, *pf, *pst, *off;           // TopoNet: sampled features, relu(feature_proj), Ws f | Wt f, offsets
-  int *src, *tgt, *src_start, *tgt_start, *src_list, *tgt_list, *cursor, *sort_tmp;
+  int *src, *tgt, *src_start, *tgt_start, *src_list, *tgt_list, *cursor, *sort_tmp, *scan_tmp;
   uint8_t* vf;                          // fixed key-padding mask
   float* x[4];                          // layer inputs / outputs [tok, 128]
   LayerWs L[3];
@@ -920,7 +896,7 @@ TrainWs layout_train(const Dims& d, void* base) {
   w.src = L.take<int>(tok); w.tgt = L.take<int>(tok);
   w.src_start = L.take<int>(pts + 1); w.tgt_start = L.take<int>(pts + 1);
   w.src_list = L.take<int>(tok); w.tgt_list = L.take<int>(tok); w.cursor = L.take<int>(pts);
-  w.sort_tmp = L.take<int>(tok);
+  w.sort_tmp = L.take<int>(tok); w.scan_tmp = L.take<int>(scan_scratch_elems(pts));
   w.vf = L.take<uint8_t>(tok);
   const int nx = d.tf ? 4 : 1;
   for (int l = 0; l < 4; ++l) w.x[l] = l < nx ? L.take<float>(tok * 128) : nullptr;
@@ -950,12 +926,10 @@ const float* LP(const HeadPtrs& hp, int l, int k) { return hp.p[HP_LAYER0 + 12 *
 
 // CSR of tokens by their point index
 int build_csr(const int* idx, long long tok, long long pts, int* start, int* list, int* cursor, int* tmp,
-              cudaStream_t st) {
+              int* scan_tmp, cudaStream_t st) {
   SRB_CUDA_OK(cudaMemsetAsync(cursor, 0, pts * 4, st));
   EW(csr_count_kernel, tok, idx, tok, cursor);
-  csr_scan_kernel<<<1, 1024, 0, st>>>(cursor, static_cast<int>(pts), start);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_TRY(exclusive_scan(cursor, start, pts, start + pts, scan_tmp, st));
   SRB_CUDA_OK(cudaMemsetAsync(cursor, 0, pts * 4, st));
   EW(csr_fill_kernel, tok, idx, tok, start, cursor, list);
   csr_sort_kernel<<<static_cast<unsigned>(pts), 256, 0, st>>>(start, list, tmp);
@@ -1037,8 +1011,8 @@ extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs*
   tr_pair_kernel<<<static_cast<unsigned>(d.tok), 128, 0, st>>>(pin, P_[HP_PP_W], w.x[0], w.off, w.src, w.tgt);
   SRB_CUDA_OK(cudaGetLastError());
   note_launch();
-  SRB_TRY(build_csr(w.src, d.tok, d.pts, w.src_start, w.src_list, w.cursor, w.sort_tmp, st));
-  SRB_TRY(build_csr(w.tgt, d.tok, d.pts, w.tgt_start, w.tgt_list, w.cursor, w.sort_tmp, st));
+  SRB_TRY(build_csr(w.src, d.tok, d.pts, w.src_start, w.src_list, w.cursor, w.sort_tmp, w.scan_tmp, st));
+  SRB_TRY(build_csr(w.tgt, d.tok, d.pts, w.tgt_start, w.tgt_list, w.cursor, w.sort_tmp, w.scan_tmp, st));
   SRB_TRY(topo_fix_valid(valid, static_cast<int>(d.rows), d.Np, w.vf, st));
   const float* xl = w.x[0];
   if (d.tf) {

@@ -49,6 +49,8 @@ def test_keypoints_golden_masks(gx, tie):
     ((300, 517), (0.95, 0.90), (3, 7)),         # non-square, odd width, small radii
     ((257, 129), (0.90, 0.80), (16, 40)),       # radius 40 > shared-memory halo: generic kernel
     ((128, 128), (0.5, 0.5), (8, 32)),          # dense candidates, halo 32 (largest tiled radius)
+    ((256, 256), (0.7, 0.6), (8, 16)),          # > 16 384 candidates: the stable order's histogram spans scan tiles
+    ((2048, 2052), (0.996, 0.99), (8, 16)),     # > 4096 x 1024 pixels: the compaction's chunk counts span scan tiles
 ])
 def test_keypoints_noise_masks(gx, tie, shape, thr, radii):
     rng = np.random.RandomState(shape[0] + shape[1])

@@ -96,6 +96,18 @@ def test_split_and_permutation_invariance():
     _check(split, preds[:1000].numpy(), target[:1000].numpy())
 
 
+@pytest.mark.parametrize("n", [1, 4095, 4096, 4097, 65_537])
+def test_entry_counts_around_one_scan_tile(n):
+    """One and two 4096-key sort chunks and curve tiles, and 17 chunks, whose 256 x 17 histogram is scanned in
+    more than one tile."""
+    gen = torch.Generator().manual_seed(n)
+    preds = _tied(gen, (n,))
+    target = (torch.rand(n, generator=gen) < preds * 0.7).to(torch.uint8)
+    curve = PrecisionRecallCurve(DEV)
+    curve.update(preds.to(DEV), target.to(DEV))
+    _check(curve, preds.numpy(), target.numpy())
+
+
 def test_exact_counts_past_2_24():
     # 3e7 entries, ~1.8e7 positives: float32 partial sums would round above 2^24
     n = 30_000_000

@@ -3,6 +3,7 @@
 
 Cases: decoder rows that are not a multiple of the 64-row GEMM tile and a 25 x 25 token grid (@400); the benched
 shape with dropout (B*N = 8192 points in the CSR scan, 128-chunk weight gradients over 131 072 pair tokens);
+B*N = 4098 points, one more tile of the CSR scan holding two;
 pair batches drawn the way the reference's dataset draws them (sources with replacement, (src, src) padding, so
 CSR segments that are long, empty or hold a point both as src and as tgt); the other input dtypes; one point, one
 sample, one pair; ViT-L; a batch without a valid slot; and decoder GEMMs of more than 65 535 row tiles.
@@ -220,13 +221,20 @@ def test_partial_row_tiles_at_400(B, version, focal):
 
 
 def test_benched_shape_with_dropout():
-    """B=16 @512, N = Ns = 512, Np = 16 with dropout, the shape tools/train_bench.py times: 8192 points (the
-    scan's several-elements-per-thread path), 131 072 pair tokens (weight gradients in 128 chunks of 1024 rows)."""
+    """B=16 @512, N = Ns = 512, Np = 16 with dropout, the shape tools/train_bench.py times: 8192 points (two
+    4096-point tiles of the CSR scan), 131 072 pair tokens (weight gradients in 128 chunks of 1024 rows)."""
     net = _net(_cfg(512))
     b = _dev(_knn_batch(16, 512, 512, 512, 16, seed=16))
     keep = _keep_masks(b, seed=77)
     got = _engine_step(net, b, dropout_p=0.1, seed=77)
     _check("bench B=16 @512 dropout", net, got, b, "normal", keep=keep, dropout_p=0.1)
+
+
+def test_csr_scan_with_a_partial_tile():
+    """B*N = 3 * 1366 = 4098 points: the CSR offsets are scanned in two 4096-point tiles, the second holding two."""
+    net = _net(_cfg(256))
+    b = _dev(_knn_batch(3, 256, 1366, 24, 8, seed=3))
+    _check("B*N = 4098", net, _engine_step(net, b), b, "normal")
 
 
 @pytest.mark.parametrize("Np,version", [(1, "normal"), (2, "no_offset"), (16, "normal"), (31, "normal")])
