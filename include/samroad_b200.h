@@ -446,6 +446,19 @@ int samroad_apls_candidates(samroad_apls_t A, int which, int32_t n_queries, cons
 int samroad_apls_one_way(samroad_apls_t A, int gt_role, int32_t n_cp, const int32_t* cp_gt, const int32_t* cp_match,
                          double min_distance_filter, SamRoadAplsResult* out, int32_t* dist_gt, int32_t* dist_prop);
 
+/* ---- label masks of the datasets (sam_road_b200/label_masks.py, DESIGN.md §16) ----
+ * cityscale/generate_labels.py and spacenet/generate_labels.py for T tiles of size x size pixels at once,
+ * pixel-identical to OpenCV 4.x: cv2.circle(kp, p, keypoint_radius, 255, -1) at every keypoint and
+ * cv2.line(road, p0, p1, 255, road_width) for every edge.  All pointers are device memory.  nodes_xy [n, 2] int32
+ * (x, y) keypoint centres with node_off [T + 1] int64 (tile t owns rows node_off[t] .. node_off[t + 1] - 1);
+ * edges_xyxy [m, 4] int32 (x0, y0, x1, y1) with edge_off [T + 1] int64 likewise.  Centres and end points may lie
+ * outside the tile.  Writes uint8 [T, size, size] masks of 0 / 255, zeroed first.  Refuses, before any launch,
+ * road_width outside [2, 32767] (width 1 is another OpenCV path), keypoint_radius outside [0, 32767], size < 1,
+ * T < 0 and null pointers.  Stateless and asynchronous on `stream`. */
+int samroad_label_masks(int T, int size, const int32_t* nodes_xy, const int64_t* node_off, const int32_t* edges_xyxy,
+                        const int64_t* edge_off, int keypoint_radius, int road_width, uint8_t* keypoint_mask,
+                        uint8_t* road_mask, void* stream);
+
 /* Stream memory operations on a 32-bit flag word in device (or peer-mapped) memory, executed by the stream
  * front end without a kernel: an ordered write of `value`, and a wait until *addr >= value.  The exchange step
  * between ranks (sam_road_b200/exchange.py; no reference counterpart, the reference is single-GPU) builds its

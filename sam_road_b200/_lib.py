@@ -161,6 +161,7 @@ SIGNATURES = {
     "samroad_apls_upload_graph": (_i, [_vp, _i, C.c_int32, _vp, _vp, _vp, _vp]),
     "samroad_apls_candidates": (_i, [_vp, _i, C.c_int32, _vp, _vp]),
     "samroad_apls_one_way": (_i, [_vp, _i, C.c_int32, _vp, _vp, _d, C.POINTER(SamRoadAplsResult), _vp, _vp]),
+    "samroad_label_masks": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "samroad_stream_write_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_stream_wait_value32": (_i, [_vp, C.c_uint32, _vp]),
     "samroad_timing_enable": (_i, [_vp, _i]),

@@ -758,8 +758,79 @@ def topo_fixture():
     print(f"{path}: {os.path.getsize(path)} bytes")
 
 
+def _label_mask_special(size, spacenet):
+    """Adjacency entries that exercise the graph rules: a self-loop on a node with one other edge (degree 3), a
+    lone self-loop (degree 2), repeated and one-way entries, float nodes that truncate to one node, end points
+    outside the tile (negative, at the size and far beyond), and a key without neighbours."""
+    s = float(size)
+    adj = {
+        (10.0, 10.0): [(10.0, 10.0), (30.5, 40.25), (30.5, 40.25)],
+        (30.5, 40.25): [(10.0, 10.0)],
+        (60.0, 60.0): [(60.0, 60.0)],
+        (80.2, 20.7): [(95.0, 21.0)],                          # one-way
+        (80.9, 20.1): [(70.0, 45.0)],                          # merges with (80.2, 20.7)
+        (120.0, 5.0): [(-40.0, 2.0), (s - 1.0, s + 30.0)],
+        (s - 2.0, 3.0): [(s + 5000.0, -7000.0)],
+        (s * 0.5, s * 0.5): [],
+        (s * 0.5 + 3.0, -2.0): [(s * 0.5 + 3.0, -2.0), (s * 0.5 + 20.0, 17.0)],
+    }
+    if spacenet:   # rows that map to y = 400 - int(row) = 400 and beyond
+        adj[(0.0, 200.0)] = [(0.4, 230.0), (-3.0, 260.0)]
+    return adj
+
+
+def label_masks_fixture():
+    """The reference scripts' own drawing functions on synthetic graphs: CityScale 2048^2 tiles from
+    synth.city_tile (float nodes, diagonals), SpaceNet 400^2 tiles from synth.make_road_graph, the graph-rule
+    cases of _label_mask_special and an empty dict.  Stored per tile: the adjacency entries, the key of every
+    entry without neighbours and both masks as np.packbits."""
+    import cv2
+    import networkx as nx
+    from oracle import label_mask_oracle as LM
+    out = {"cv2_version": np.array(cv2.__version__), "networkx_version": np.array(nx.__version__)}
+    tiles = [("city0", "cityscale", synth.city_tile(2048, seed=0)[0]),
+             ("city1", "cityscale", synth.city_tile(2048, seed=1)[1]),
+             ("city_special", "cityscale", _label_mask_special(2048, False)),
+             ("city_empty", "cityscale", {}),
+             ("space0", "spacenet", synth.make_road_graph(384, seed=0)),
+             ("space1", "spacenet", synth.make_road_graph(400, seed=1, spacing=40, lo=0)),
+             ("space_special", "spacenet", _label_mask_special(400, True))]
+    for name, dataset, adj in tiles:
+        script = os.path.join(ref_loader.REF_ROOT, dataset, "generate_labels.py")
+        fns = _extract_functions(script, {"draw_points_on_image", "draw_line_segments_on_image"})
+        fns["cv2"] = cv2
+        size = 2048 if dataset == "cityscale" else 400
+        graph = nx.Graph()
+        for n, neis in adj.items():
+            for nei in neis:
+                if dataset == "cityscale":
+                    graph.add_edge((int(n[1]), int(n[0])), (int(nei[1]), int(nei[0])))
+                else:
+                    graph.add_edge((int(n[1]), size - int(n[0])), (int(nei[1]), size - int(nei[0])))
+        key_nodes = [node for node, degree in graph.degree() if degree != 2]
+        kp = fns["draw_points_on_image"](size=size, points=key_nodes, radius=3)
+        road = fns["draw_line_segments_on_image"](size=size, line_segments=graph.edges(), width=3)
+        okp, oroad = LM.tile_masks(adj, dataset, size)
+        assert np.array_equal(kp, okp) and np.array_equal(road, oroad), f"{name}: oracle disagrees with cv2"
+        pairs = [(*n, *m) for n, neis in adj.items() for m in neis]
+        out[f"{name}/dataset"] = np.array(dataset)
+        out[f"{name}/pairs"] = np.array(pairs, np.float64).reshape(-1, 4)
+        out[f"{name}/lonely"] = np.array([n for n, neis in adj.items() if not neis], np.float64).reshape(-1, 2)
+        out[f"{name}/keypoint"] = np.packbits(kp > 0)
+        out[f"{name}/road"] = np.packbits(road > 0)
+        print(f"label masks {name}: {len(key_nodes)} keypoints, {graph.number_of_edges()} edges, "
+              f"{int((kp > 0).sum())} / {int((road > 0).sum())} pixels set")
+    path = os.path.join(OUT, "label_masks.npz")
+    np.savez_compressed(path, **out)
+    print(f"{path}: {os.path.getsize(path)} bytes")
+
+
 def main():
     assert ref_loader.available(), "needs /root/reference"
+    if "--label-masks" in sys.argv:   # generate_labels.py's masks of CityScale and SpaceNet graphs
+        os.makedirs(OUT, exist_ok=True)
+        label_masks_fixture()
+        return
     if "--topo" in sys.argv:          # the TOPO metric on three synthetic tiles, both drivers and aggregators
         os.makedirs(OUT, exist_ok=True)
         topo_fixture()
