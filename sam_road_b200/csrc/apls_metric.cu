@@ -379,7 +379,7 @@ extern "C" int samroad_apls_create(int device, const SamRoadAplsCaps* caps, samr
   if (int rc = open_device(device)) return rc;
   int optin = 0;
   SRB_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
-  SRB_CUDA_OK(cudaFuncSetAttribute(sssp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+  SRB_TRY(allow_dynamic_smem(sssp_kernel, optin));
   cudaStream_t st = nullptr;
   SRB_CUDA_OK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   samroad_apls_ctx* A = new samroad_apls_ctx();
@@ -512,10 +512,8 @@ extern "C" int samroad_apls_candidates(samroad_apls_t A, int which, int32_t n_qu
   carve(A->work.get());
   cudaStream_t st = A->stream;
   SRB_CUDA_OK(cudaMemcpyAsync(dq, query_latlon, 16ull * n_queries, cudaMemcpyHostToDevice, st));
-  knn_kernel<<<(n_queries + kKnnWarps - 1) / kKnnWarps, 32 * kKnnWarps, 0, st>>>(A->ll[which].as<double>(), n, dq,
-                                                                                  n_queries, dout);
-  note_launch(1);
-  SRB_CUDA_OK(cudaGetLastError());
+  SRB_LAUNCH(knn_kernel, (n_queries + kKnnWarps - 1) / kKnnWarps, 32 * kKnnWarps, 0, st, A->ll[which].as<double>(), n,
+             dq, n_queries, dout);
   SRB_CUDA_OK(cudaMemcpyAsync(out, dout, 4ull * kK * n_queries, cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   return 0;
@@ -606,13 +604,10 @@ extern "C" int samroad_apls_one_way(samroad_apls_t A, int gt_role, int32_t n_cp,
   SsspGraph s0{dptr[0], dptr[1], dptr[2], dptr[3], dmg, ntg, ng};
   SsspGraph s1{dptr[4], dptr[5], dptr[6], dptr[7], dmp, ntp, np_};
   if (njobs > 0) {
-    sssp_kernel<<<sssp_grid, kSsspThreads, in_smem ? per_cta : 0, st>>>(s0, s1, dscratch, per_cta);
-    note_launch(1);
+    SRB_LAUNCH(sssp_kernel, sssp_grid, kSsspThreads, in_smem ? per_cta : 0, st, s0, s1, dscratch, per_cta);
   }
-  pair_kernel<<<pair_grid, kPairThreads, 0, st>>>(n_cp, dptr[8], dptr[9], dmg, ng, dmp, np_, min_distance_filter,
-                                                  dpart);
-  note_launch(1);
-  SRB_CUDA_OK(cudaGetLastError());
+  SRB_LAUNCH(pair_kernel, pair_grid, kPairThreads, 0, st, n_cp, dptr[8], dptr[9], dmg, ng, dmp, np_,
+             min_distance_filter, dpart);
   std::vector<PairPartial> part(pair_grid);
   SRB_CUDA_OK(cudaMemcpyAsync(part.data(), dpart, sizeof(PairPartial) * pair_grid, cudaMemcpyDeviceToHost, st));
   if (dist_gt && ng) SRB_CUDA_OK(cudaMemcpyAsync(dist_gt, dmg, 4ull * ng * ng, cudaMemcpyDeviceToHost, st));

@@ -18,8 +18,6 @@
 #include "common.cuh"
 #include "ops.h"
 
-#define SRB_TRY_RC(expr) do { int _rc = (expr); if (_rc != 0) return _rc; } while (0)
-
 namespace srb {
 
 constexpr int kAttThreads = 128;
@@ -189,14 +187,10 @@ static int launch_attention_simt(const __half* qkv, const float* qkv_bias, const
   const int nwin = (s + win - 1) / win;
   const size_t smem = (2 * kAttChunk * HD + kAttThreads * 2 * win) * sizeof(float);
   auto kern = encoder_attention_simt_kernel<HD>;
-  SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(smem)));
+  SRB_TRY(allow_dynamic_smem(kern, smem));
   dim3 grid((win * win + kAttThreads - 1) / kAttThreads, B * nwin * nwin * heads);
   const float scale = 1.0f / sqrtf(static_cast<float>(HD));
-  kern<<<grid, kAttThreads, smem, st>>>(qkv, qkv_bias, rel_h, rel_w, B, s, win, nwin, heads, scale,
-                                        out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(kern, grid, kAttThreads, smem, st, qkv, qkv_bias, rel_h, rel_w, B, s, win, nwin, heads, scale, out);
   return 0;
 }
 

@@ -794,13 +794,6 @@ attention_wide_kernel(const __half* __restrict__ qkv, const float* __restrict__ 
   for (int m = 0; m < 2; ++m) am_store<HD>(t[m], row0 + rA + m * 16, nreal, rx, s, D, out0, lane);
 }
 
-// One bit per CUDA device (function attributes are per device) for each head dim.  Internal linkage,
-// unlike a static local of the launcher template: two builds of the library loaded into one process
-// (tools/attention_bench.py --lib-b) each keep their own flags.
-static uint64_t g_am_attr_devs[2] = {0, 0};
-static uint64_t g_au_attr_devs[2] = {0, 0};
-static uint64_t g_aw_attr_devs[2] = {0, 0};
-
 // Warps of a one-CTA-per-unit block, and the shared memory that still lets two such CTAs share an SM
 // (228 KB per SM, 1 KB reserved per CTA).  A full 14 x 14 window is 13 m-tiles: 5 warps walk them in three
 // rounds (13 of 15 slots used, 4 warps 13 of 16) at 10 warps per SM; 6 warps need a fourth of the time for one
@@ -827,28 +820,20 @@ int launch_attention_mma(const __half* qkv, const float* qkv_bias, const float* 
   const unsigned grid = static_cast<unsigned>(blocks);
   if (resident) {
     auto kern = attention_unit_kernel<HD, NW>;
-    if (first_use_on_device(&g_au_attr_devs[HD == 80])) {
-      SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kAuMaxBytes));
-    }
-    kern<<<grid, NW * 32, ly.unit_bytes(NW), st>>>(qkv, qkv_bias, rel_h, rel_w, s, win, nwin, heads, scale_log2e,
-                                                   out);
+    SRB_TRY(allow_dynamic_smem(kern, ly.unit_bytes(NW)));
+    SRB_LAUNCH(kern, grid, NW * 32, ly.unit_bytes(NW), st, qkv, qkv_bias, rel_h, rel_w, s, win, nwin, heads,
+               scale_log2e, out);
   } else if (wide) {
     auto kern = attention_wide_kernel<HD>;
-    if (first_use_on_device(&g_aw_attr_devs[HD == 80])) {
-      SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LY(64).wide_bytes()));
-    }
-    kern<<<grid, kAmWarps * 32, ly.wide_bytes(), st>>>(qkv, qkv_bias, rel_h, rel_w, s, win, heads, qblocks,
-                                                      scale_log2e, out);
+    SRB_TRY(allow_dynamic_smem(kern, ly.wide_bytes()));
+    SRB_LAUNCH(kern, grid, kAmWarps * 32, ly.wide_bytes(), st, qkv, qkv_bias, rel_h, rel_w, s, win, heads, qblocks,
+               scale_log2e, out);
   } else {
     auto kern = attention_mma_kernel<HD>;
-    if (first_use_on_device(&g_am_attr_devs[HD == 80])) {   // the largest window the encoder supports (s <= 64)
-      SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LY(64).bytes));
-    }
-    kern<<<grid, kAmWarps * 32, ly.bytes, st>>>(qkv, qkv_bias, rel_h, rel_w, s, win, nwin, heads, qblocks,
-                                                scale_log2e, out);
+    SRB_TRY(allow_dynamic_smem(kern, ly.bytes));
+    SRB_LAUNCH(kern, grid, kAmWarps * 32, ly.bytes, st, qkv, qkv_bias, rel_h, rel_w, s, win, nwin, heads, qblocks,
+               scale_log2e, out);
   }
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
   return 0;
 }
 

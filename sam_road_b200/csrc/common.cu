@@ -1,11 +1,14 @@
-// sam_road_b200 :: host-side common pieces: last-error slot, SM count, TMA descriptor encoding.
+// sam_road_b200 :: host-side common pieces: last-error slot, launch check and count, shared-memory opt-in,
+// SM count, TMA descriptor encoding.
 #include "common.cuh"
 #include "ops.h"
 
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <map>
 #include <mutex>
+#include <utility>
 
 namespace srb {
 
@@ -20,9 +23,32 @@ void set_last_error(const char* fmt, ...) {
 const char* get_last_error() { return g_last_error; }
 
 static std::atomic<uint64_t> g_launches{0};
-void note_launch(int n) { g_launches.fetch_add(static_cast<uint64_t>(n), std::memory_order_relaxed); }
+static void note_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 uint64_t launch_count(bool reset) {
   return reset ? g_launches.exchange(0) : g_launches.load();
+}
+
+int launched(const char* file, int line, const char* call) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_last_error("%s:%d: SRB_LAUNCH(%s) -> %s", file, line, call, cudaGetErrorString(e));
+    return 1;
+  }
+  note_launch();
+  return 0;
+}
+
+int allow_dynamic_smem(const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> allowed;   // (device, kernel) -> bytes set
+  int dev = 0;
+  SRB_CUDA_OK(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& have = allowed[{dev, kernel}];
+  if (bytes <= have) return 0;
+  SRB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
+  have = bytes;
+  return 0;
 }
 
 template <bool kPinned>
@@ -80,15 +106,6 @@ int device_sm_count() {
     cached[dev] = n;
   }
   return cached[dev];
-}
-
-bool first_use_on_device(uint64_t* device_mask) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return true;
-  const uint64_t bit = 1ull << dev;
-  if (*device_mask & bit) return false;
-  *device_mask |= bit;
-  return true;
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,

@@ -18,7 +18,6 @@ namespace srb {
 // error plumbing (C-ABI never throws: every entry point returns an int and stores a message)
 // ----------------------------------------------------------------------------------------------
 void set_last_error(const char* fmt, ...);
-void note_launch(int n);
 
 #define SRB_CUDA_OK(expr)                                                                  \
   do {                                                                                     \
@@ -37,6 +36,41 @@ void note_launch(int n);
       return 2;                                                                            \
     }                                                                                      \
   } while (0)
+
+// Return the status of a call that already set the error message, when it is not 0.
+#define SRB_TRY(expr)                                                                      \
+  do {                                                                                     \
+    if (int _rc = (expr)) return _rc;                                                      \
+  } while (0)
+
+// ----------------------------------------------------------------------------------------------
+// kernel launch: every kernel goes on a stream through SRB_LAUNCH
+// ----------------------------------------------------------------------------------------------
+// Reads the launch's error right away, so that a bad configuration is reported at its own call site and not
+// by the next unrelated check, and counts one launch when it was enqueued (samroad_launch_count).  Returns 0,
+// or 1 with "<file>:<line>: SRB_LAUNCH(<arguments>) -> <error>" set.
+int launched(const char* file, int line, const char* call);
+
+template <typename... Params, typename... Args>
+int launch(const char* file, int line, const char* call, void (*kernel)(Params...), dim3 grid, dim3 block,
+           size_t smem, cudaStream_t stream, Args&&... args) {
+  kernel<<<grid, block, smem, stream>>>(static_cast<Args&&>(args)...);
+  return launched(file, line, call);
+}
+
+// SRB_LAUNCH(kernel, grid, block, smem, stream, kernel arguments...) launches with <<<grid, block, smem, stream>>>
+// and returns the error status from the calling function when the launch fails.  The kernel may be a template
+// specialisation with commas in its argument list, or a pointer.
+#define SRB_LAUNCH(...) SRB_TRY(::srb::launch(__FILE__, __LINE__, #__VA_ARGS__, __VA_ARGS__))
+
+// Lets `kernel` take `bytes` of dynamic shared memory on the current device.  The attribute is only ever
+// raised, once per size above what was set before for that kernel and device, so launchers may call it before
+// every launch, from any host thread.
+int allow_dynamic_smem(const void* kernel, size_t bytes);
+template <typename... Params>
+int allow_dynamic_smem(void (*kernel)(Params...), size_t bytes) {
+  return allow_dynamic_smem(reinterpret_cast<const void*>(kernel), bytes);
+}
 
 // ----------------------------------------------------------------------------------------------
 // resources: every handle owns its memory through these, so destructors free it

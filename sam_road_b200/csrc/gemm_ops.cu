@@ -97,9 +97,7 @@ __global__ void gemm_ref_simt_kernel(const __half* __restrict__ A, int lda,
 int gemm_ref_simt(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
                   float* out, int ldo, cudaStream_t st) {
   dim3 grid((N + 127) / 128, M);
-  gemm_ref_simt_kernel<<<grid, 128, 0, st>>>(A, lda, W, ldw, M, N, K, out, ldo);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(gemm_ref_simt_kernel, grid, 128, 0, st, A, lda, W, ldw, M, N, K, out, ldo);
   return 0;
 }
 

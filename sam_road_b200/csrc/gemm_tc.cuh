@@ -627,15 +627,10 @@ int launch_gemm_tc(const __half* A, int lda, const __half* W, int ldw, int M, in
   }
   if (int rc = make_tmap_f16_2d(&tmB, W, N, K, ldw, BN)) return rc;
   auto kern = gemm_tc_kernel<BN, STAGES, Epi>;
-  static uint64_t attr_devs = 0;          // one bit per CUDA device: function attributes are per device   // per template instantiation
-  if (first_use_on_device(&attr_devs)) {
-    SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
-  }
+  SRB_TRY(allow_dynamic_smem(kern, SM::kTotal));
   const int num_tiles = ((M + kGemmBM - 1) / kGemmBM) * ((N + BN - 1) / BN);
   const int grid = num_tiles < device_sm_count() ? num_tiles : device_sm_count();
-  kern<<<grid, kGemmThreads, SM::kTotal, stream>>>(tmA, tmB, M, N, K, ep, conv_s);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(kern, grid, kGemmThreads, SM::kTotal, stream, tmA, tmB, M, N, K, ep, conv_s);
   return 0;
 }
 
@@ -787,15 +782,10 @@ int launch_gemm_pp(const __half* A, int lda, const __half* W, int ldw, int M, in
   if (int rc = make_tmap_f16_2d(&tmA, A, M, K, lda, kGemmBM)) return rc;
   if (int rc = make_tmap_f16_2d(&tmB, W, N, K, ldw, 128)) return rc;
   auto kern = gemm_pp_kernel<kStages, Epi>;
-  static uint64_t attr_devs = 0;          // one bit per CUDA device: function attributes are per device
-  if (first_use_on_device(&attr_devs)) {
-    SRB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
-  }
+  SRB_TRY(allow_dynamic_smem(kern, SM::kTotal));
   const int num_tiles = ((M + kGemmBM - 1) / kGemmBM) * ((N + 127) / 128);
   const int grid = num_tiles < device_sm_count() ? num_tiles : device_sm_count();
-  kern<<<grid, kGemmThreads, SM::kTotal, stream>>>(tmA, tmB, M, N, K, ep);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(kern, grid, kGemmThreads, SM::kTotal, stream, tmA, tmB, M, N, K, ep);
   return 0;
 }
 

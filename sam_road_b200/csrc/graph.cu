@@ -143,13 +143,9 @@ int compact(samroad_graph_ctx* g, const F& f, int n, int* n_out_dev, cudaStream_
   }
   if (int rc = grow(g->blk, sizeof(int) * (nblk + scan_scratch_elems(nblk)))) return rc;
   int* blk = g->blk.as<int>();
-  compact_count_kernel<F><<<nblk, 256, 0, st>>>(f, n, blk);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(compact_count_kernel<F>, nblk, 256, 0, st, f, n, blk);
   if (int rc = exclusive_scan(blk, blk, nblk, n_out_dev, blk + nblk, st)) return rc;
-  compact_fill_kernel<F><<<nblk, 256, 0, st>>>(f, n, blk);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(compact_fill_kernel<F>, nblk, 256, 0, st, f, n, blk);
   return 0;
 }
 
@@ -447,8 +443,7 @@ int host_order(samroad_graph_ctx* g, const uint8_t* key, int n, int key_dtype, s
   const std::vector<int64_t>& asc = pre_asc ? *pre_asc : own;
   if (int rc = grow(g->ghist, sizeof(int64_t) * n)) return rc;
   SRB_CUDA_OK(cudaMemcpyAsync(g->ghist.get(), asc.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
-  order_from_host_kernel<<<blocks_for(n, 256), 256, 0, st>>>(g->ghist.as<int64_t>(), n, order, err);
-  note_launch();
+  SRB_LAUNCH(order_from_host_kernel, blocks_for(n, 256), 256, 0, st, g->ghist.as<int64_t>(), n, order, err);
   SRB_CUDA_OK(cudaStreamSynchronize(st));   // `asc` is pageable host memory: keep it alive until copied
   return 0;
 }
@@ -488,9 +483,8 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
                   : stable_order(g, key, n, order, st))
     return rc;
   SRB_CUDA_OK(cudaMemsetAsync(&ctr->n_mortal, 0, sizeof(int), st));
-  gather_sorted_kernel<<<blocks_for(n, 256), 256, 0, st>>>(pix, key, order, n, sorted_pix, immune, &ctr->n_mortal,
-                                                           &ctr->order_err);
-  note_launch();
+  SRB_LAUNCH(gather_sorted_kernel, blocks_for(n, 256), 256, 0, st, pix, key, order, n, sorted_pix, immune,
+             &ctr->n_mortal, &ctr->order_err);
   Counters c;
   if (int rc = read_back(g, ctr, &c, st)) return rc;
   SRB_REQUIRE(c.order_err == 0, "argsort callback returned an invalid permutation (code %d) for %s", c.order_err,
@@ -511,8 +505,7 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
   if (int rc = grow(g->cell, npx * 4)) return rc;
   uint32_t* cell = g->cell.as<uint32_t>();
   SRB_CUDA_OK(cudaMemsetAsync(cell, 0xFF, npx * 4, st));
-  cell_build_kernel<<<blocks_for(n, 256), 256, 0, st>>>(sorted_pix, immune, n, cell);
-  note_launch();
+  SRB_LAUNCH(cell_build_kernel, blocks_for(n, 256), 256, 0, st, sorted_pix, immune, n, cell);
   const int tx = (W + kNmsTile - 1) / kNmsTile, ty = (H + kNmsTile - 1) / kNmsTile;
   constexpr int kMaxRounds = 4096;
   if (int rc = grow(g->round_cnt, sizeof(int) * kMaxRounds)) return rc;
@@ -523,22 +516,18 @@ int nms_pass(samroad_graph_ctx* g, const int32_t* pix, const uint8_t* key, int n
   const bool tiled = halo <= kNmsMaxHalo;
   const int SH = kNmsTile + 2 * halo;
   const size_t smem = tiled ? (static_cast<size_t>(SH) * (SH + 1) + 2 * halo + 1) * 4 + kNmsTile * kNmsTile * 2 : 0;
-  if (tiled && smem > 48 * 1024)
-    SRB_CUDA_OK(cudaFuncSetAttribute(nms_round_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     static_cast<int>(smem)));
+  if (tiled && smem > 48 * 1024) SRB_TRY(allow_dynamic_smem(nms_round_kernel, smem));
   int round = 0;
   while (true) {
     const int burst = round == 0 ? 2 : 4;
     for (int b = 0; b < burst && round < kMaxRounds; ++b, ++round) {
       if (tiled)
-        nms_round_kernel<<<dim3(tx, ty), 256, smem, st>>>(cell, H, W, halo, d2max, g->tile_und.as<int>(),
-                                                          round_cnt + round);
+        SRB_LAUNCH(nms_round_kernel, dim3(tx, ty), 256, smem, st, cell, H, W, halo, d2max, g->tile_und.as<int>(),
+                   round_cnt + round);
       else
-        nms_round_generic_kernel<<<blocks_for(n, 256), 256, 0, st>>>(cell, sorted_pix, n, H, W, halo, d2max,
-                                                                     round_cnt + round);
-      note_launch();
+        SRB_LAUNCH(nms_round_generic_kernel, blocks_for(n, 256), 256, 0, st, cell, sorted_pix, n, H, W, halo, d2max,
+                   round_cnt + round);
     }
-    SRB_CUDA_OK(cudaGetLastError());
     int open = 0;
     if (int rc = read_back(g, round_cnt + round - 1, &open, st)) return rc;
     if (open == 0) break;
@@ -660,9 +649,8 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
     if (int rc = grow(g->cand3, sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
     if (int rc = grow(g->cls3, static_cast<size_t>(n3))) return rc;
     if (int rc = grow(g->list[2], sizeof(int32_t) * static_cast<size_t>(n3))) return rc;
-    concat_kernel<<<blocks_for(n3, 256), 256, 0, st>>>(g->list[0].as<int32_t>(), m0, g->list[1].as<int32_t>(), m1,
-                                                       g->cand3.as<int32_t>(), g->cls3.as<uint8_t>());
-    note_launch();
+    SRB_LAUNCH(concat_kernel, blocks_for(n3, 256), 256, 0, st, g->list[0].as<int32_t>(), m0, g->list[1].as<int32_t>(),
+               m1, g->cand3.as<int32_t>(), g->cls3.as<uint8_t>());
     const bool pre3 = have_pre && m0 == n_cand[0] && m1 == n_cand[1];
     if (int rc = nms_pass(g, g->cand3.as<int32_t>(), g->cls3.as<uint8_t>(), n3, SAMROAD_F64, argsort, user,
                           pre3 ? &pre_asc[2] : nullptr, "the merged pass", H, W, road_radius, g->list[2].as<int32_t>(),
@@ -673,9 +661,7 @@ extern "C" int samroad_extract_graph_points(samroad_graph_t g, const uint8_t* ke
   SRB_REQUIRE(points_xy != nullptr || n_out == 0, "samroad_extract_graph_points: null output");
   SRB_REQUIRE(n_out <= cap, "samroad_extract_graph_points: %d keypoints exceed the output capacity %d", n_out, cap);
   if (n_out > 0) {
-    pix_to_xy_kernel<<<blocks_for(n_out, 256), 256, 0, st>>>(g->list[2].as<int32_t>(), n_out, W, points_xy);
-    note_launch();
-    SRB_CUDA_OK(cudaGetLastError());
+    SRB_LAUNCH(pix_to_xy_kernel, blocks_for(n_out, 256), 256, 0, st, g->list[2].as<int32_t>(), n_out, W, points_xy);
   }
   *n_points = n_out;
   if (stats) {
@@ -856,9 +842,9 @@ extern "C" int samroad_pair_queries_plan_k(samroad_graph_t g, const int64_t* poi
     return 0;
   }
   if (int rc = grow(g->pts32, sizeof(int32_t) * 2 * static_cast<size_t>(N))) return rc;
-  points_to_i32_kernel<<<blocks_for(2L * N, 256), 256, 0, st>>>(points_xy, 2 * N, g->pts32.as<int32_t>());
-  tile_count_kernel<<<n_tiles, 256, 0, st>>>(g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P, g->t_cnt.as<int>());
-  note_launch(2);
+  SRB_LAUNCH(points_to_i32_kernel, blocks_for(2L * N, 256), 256, 0, st, points_xy, 2 * N, g->pts32.as<int32_t>());
+  SRB_LAUNCH(tile_count_kernel, n_tiles, 256, 0, st, g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P,
+             g->t_cnt.as<int>());
   SRB_CUDA_OK(cudaMemcpyAsync(g->h_cnt.data(), g->t_cnt.get(), sizeof(int) * n_tiles, cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   int max_cnt = 0;
@@ -873,17 +859,15 @@ extern "C" int samroad_pair_queries_plan_k(samroad_graph_t g, const int64_t* poi
   if (g->total == 0) { SRB_CUDA_OK(cudaStreamSynchronize(st)); return 0; }
   if (int rc = grow(g->members, sizeof(int32_t) * static_cast<size_t>(g->total))) return rc;
   if (int rc = grow(g->nbr, sizeof(int32_t) * g->nbr_stride * static_cast<size_t>(g->total))) return rc;
-  tile_fill_kernel<<<n_tiles, 256, 0, st>>>(g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P, g->t_off.as<int>(),
-                                            g->members.as<int32_t>());
+  SRB_LAUNCH(tile_fill_kernel, n_tiles, 256, 0, st, g->pts32.as<int32_t>(), N, g->tile_xy.as<int32_t>(), P,
+             g->t_off.as<int>(), g->members.as<int32_t>());
   const dim3 knn_grid(n_tiles, (max_cnt + 127) / 128);
   if (g->nbr_stride == 16)
-    knn_kernel<16><<<knn_grid, 128, 0, st>>>(g->pts32.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
-                                             g->members.as<int32_t>(), g->d2lt, g->nbr.as<int32_t>());
+    SRB_LAUNCH(knn_kernel<16>, knn_grid, 128, 0, st, g->pts32.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
+               g->members.as<int32_t>(), g->d2lt, g->nbr.as<int32_t>());
   else
-    knn_kernel<32><<<knn_grid, 128, 0, st>>>(g->pts32.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
-                                             g->members.as<int32_t>(), g->d2lt, g->nbr.as<int32_t>());
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(2);
+    SRB_LAUNCH(knn_kernel<32>, knn_grid, 128, 0, st, g->pts32.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
+               g->members.as<int32_t>(), g->d2lt, g->nbr.as<int32_t>());
   SRB_CUDA_OK(cudaStreamSynchronize(st));    // h_off was copied from pageable memory
   return 0;
 }
@@ -911,11 +895,9 @@ extern "C" int samroad_pair_queries_fill(samroad_graph_t g, int tile_begin, int 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long total = static_cast<long>(B) * nmax * K;
   auto* fill = g->nbr_stride == 16 ? fill_batch_kernel<16> : fill_batch_kernel<32>;
-  fill<<<blocks_for(total, 256), 256, 0, st>>>(
-      g->pts32.as<int32_t>(), g->tile_xy.as<int32_t>(), g->t_cnt.as<int>(), g->t_off.as<int>(),
-      g->members.as<int32_t>(), g->nbr.as<int32_t>(), tile_begin, B, nmax, K, points, pairs, valid);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(fill, blocks_for(total, 256), 256, 0, st, g->pts32.as<int32_t>(), g->tile_xy.as<int32_t>(),
+             g->t_cnt.as<int>(), g->t_off.as<int>(), g->members.as<int32_t>(), g->nbr.as<int32_t>(), tile_begin, B,
+             nmax, K, points, pairs, valid);
   return 0;
 }
 
@@ -1078,15 +1060,16 @@ __global__ void __launch_bounds__(128) aggregate_kernel(const AggArgs a) {
 }
 
 template <int NS>
-void launch_aggregate(int max_deg, const AggArgs& a, cudaStream_t st) {
+int launch_aggregate(int max_deg, const AggArgs& a, cudaStream_t st) {
   if (max_deg <= 32)
-    aggregate_warp_kernel<1, NS><<<blocks_for(32L * a.N, 256), 256, 0, st>>>(a);
+    SRB_LAUNCH(aggregate_warp_kernel<1, NS>, blocks_for(32L * a.N, 256), 256, 0, st, a);
   else if (max_deg <= 64)
-    aggregate_warp_kernel<2, NS><<<blocks_for(32L * a.N, 256), 256, 0, st>>>(a);
+    SRB_LAUNCH(aggregate_warp_kernel<2, NS>, blocks_for(32L * a.N, 256), 256, 0, st, a);
   else if (max_deg <= 128)
-    aggregate_warp_kernel<4, NS><<<blocks_for(32L * a.N, 256), 256, 0, st>>>(a);
+    SRB_LAUNCH(aggregate_warp_kernel<4, NS>, blocks_for(32L * a.N, 256), 256, 0, st, a);
   else
-    aggregate_kernel<NS><<<blocks_for(a.N, 128), 128, 0, st>>>(a);
+    SRB_LAUNCH(aggregate_kernel<NS>, blocks_for(a.N, 128), 128, 0, st, a);
+  return 0;
 }
 
 __global__ void edge_select_kernel(const float* __restrict__ sum, const float* __restrict__ num,
@@ -1122,8 +1105,8 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
   Counters* ctr = g->counters.as<Counters>();
   SRB_CUDA_OK(cudaMemsetAsync(ctr, 0, sizeof(Counters), st));
   int* adj_off = g->adj_off.as<int>();
-  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, nullptr, adj_off, nullptr, nullptr, &ctr->max_deg);
-  note_launch(1);
+  SRB_LAUNCH(adj_kernel, blocks_for(N, 128), 128, 0, st, pts, N, g->d2lt, nullptr, adj_off, nullptr, nullptr,
+             &ctr->max_deg);
   if (int rc = exclusive_scan(adj_off, adj_off, N, &ctr->nnz, adj_off + N + 1, st)) return rc;
   Counters c;
   if (int rc = read_back(g, ctr, &c, st)) return rc;
@@ -1142,20 +1125,18 @@ extern "C" int samroad_aggregate_edges(samroad_graph_t g, const float* topo_scor
   SRB_CUDA_OK(cudaMemsetAsync(g->adj_cnt.get(), 0, 4 * nz, st));
   SRB_CUDA_OK(cudaMemsetAsync(g->adj_first.get(), 0xFF, 4 * nz, st));
   SRB_CUDA_OK(cudaMemsetAsync(g->eflags.get(), 0xFF, 4 * static_cast<size_t>(n_entries), st));
-  adj_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts, N, g->d2lt, adj_off, nullptr,
-                                                 g->adj_src.as<int32_t>(), g->adj_tgt.as<int32_t>(), nullptr);
+  SRB_LAUNCH(adj_kernel, blocks_for(N, 128), 128, 0, st, pts, N, g->d2lt, adj_off, nullptr, g->adj_src.as<int32_t>(),
+             g->adj_tgt.as<int32_t>(), nullptr);
   const AggArgs args{pts, N, g->tile_xy.as<int32_t>(), g->n_tiles, g->P, g->t_cnt.as<int>(), g->t_off.as<int>(),
                      g->members.as<int32_t>(), g->nbr.as<int32_t>(), topo_scores, g->tile_soff.as<int64_t>(), K,
                      adj_off, g->adj_tgt.as<int32_t>(), g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
                      g->adj_first.as<int32_t>(), &ctr->bad_score};
   if (g->nbr_stride == 16)
-    launch_aggregate<16>(max_deg, args, st);
+    SRB_TRY(launch_aggregate<16>(max_deg, args, st));
   else
-    launch_aggregate<32>(max_deg, args, st);
-  edge_select_kernel<<<blocks_for(nnz, 256), 256, 0, st>>>(g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
-                                                           g->adj_first.as<int32_t>(), nnz, threshold,
-                                                           g->eflags.as<int32_t>());
-  note_launch(3);
+    SRB_TRY(launch_aggregate<32>(max_deg, args, st));
+  SRB_LAUNCH(edge_select_kernel, blocks_for(nnz, 256), 256, 0, st, g->adj_sum.as<float>(), g->adj_cnt.as<float>(),
+             g->adj_first.as<int32_t>(), nnz, threshold, g->eflags.as<int32_t>());
   EdgeFlag ef{g->eflags.as<int32_t>(), g->adj_src.as<int32_t>(), g->adj_tgt.as<int32_t>(), edges, edges ? cap : 0};
   if (int rc = compact(g, ef, static_cast<int>(n_entries), &ctr->n_edges, st)) return rc;
   if (int rc = read_back(g, ctr, &c, st)) return rc;

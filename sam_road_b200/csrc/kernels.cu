@@ -62,9 +62,7 @@ int layernorm_f16(const float* x, const float* gamma, const float* beta, float e
                   __half* out, bool reverse, cudaStream_t st) {
   SRB_REQUIRE(D % 128 == 0 && D <= 128 * kLNMaxVec, "layernorm: D=%d unsupported", D);
   if (M <= 0) return 0;
-  layernorm_f16_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, gamma, beta, eps, M, D, out, reverse ? 1 : 0);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(layernorm_f16_kernel, (M + 7) / 8, 256, 0, st, x, gamma, beta, eps, M, D, out, reverse ? 1 : 0);
   return 0;
 }
 
@@ -127,15 +125,11 @@ int im2col_patch16(const void* rgb, int dtype, int B, int P, const float* mean,
   const long total = static_cast<long>(B) * s * s * 96;
   const int blocks = static_cast<int>((total + 255) / 256);
   if (dtype == 0)
-    im2col_patch16_kernel<float><<<blocks, 256, 0, st>>>(
-        static_cast<const float*>(rgb), B, P, mean[0], mean[1], mean[2], inv_std[0], inv_std[1],
-        inv_std[2], out);
+    SRB_LAUNCH(im2col_patch16_kernel<float>, blocks, 256, 0, st, static_cast<const float*>(rgb), B, P, mean[0], mean[1],
+               mean[2], inv_std[0], inv_std[1], inv_std[2], out);
   else
-    im2col_patch16_kernel<uint8_t><<<blocks, 256, 0, st>>>(
-        static_cast<const uint8_t*>(rgb), B, P, mean[0], mean[1], mean[2], inv_std[0], inv_std[1],
-        inv_std[2], out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+    SRB_LAUNCH(im2col_patch16_kernel<uint8_t>, blocks, 256, 0, st, static_cast<const uint8_t*>(rgb), B, P, mean[0],
+               mean[1], mean[2], inv_std[0], inv_std[1], inv_std[2], out);
   return 0;
 }
 
@@ -166,9 +160,7 @@ int crop_tiles(const uint8_t* scene, int H, int W, const int* tile_xy, int B, in
   SRB_REQUIRE(P % 4 == 0 && P > 0 && P <= H && P <= W, "crop_tiles: P=%d vs scene %dx%d", P, H, W);
   if (B <= 0) return 0;
   const long total = static_cast<long>(B) * P * (P * 3 / 4);
-  crop_tiles_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, st>>>(scene, W, tile_xy, B, P, out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(crop_tiles_kernel, static_cast<int>((total + 255) / 256), 256, 0, st, scene, W, tile_xy, B, P, out);
   return 0;
 }
 
@@ -198,9 +190,7 @@ int im2col_3x3(const __half* x, int B, int s, int C, __half* out, cudaStream_t s
   SRB_REQUIRE(C % 8 == 0, "im2col_3x3: C=%d must be a multiple of 8", C);
   if (B <= 0) return 0;
   const long total = static_cast<long>(B) * s * s * 9 * (C / 8);
-  im2col_3x3_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, st>>>(x, B, s, C, out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(im2col_3x3_kernel, static_cast<int>((total + 255) / 256), 256, 0, st, x, B, s, C, out);
   return 0;
 }
 
@@ -219,9 +209,7 @@ convert_f32_f16_kernel(const float* __restrict__ x, long n8, __half* __restrict_
 int convert_f32_f16(const float* x, long n, __half* out, cudaStream_t st) {
   SRB_REQUIRE(n % 8 == 0, "convert_f32_f16: n=%ld must be a multiple of 8", n);
   if (n <= 0) return 0;
-  convert_f32_f16_kernel<<<static_cast<int>((n / 8 + 255) / 256), 256, 0, st>>>(x, n / 8, out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(convert_f32_f16_kernel, static_cast<int>((n / 8 + 255) / 256), 256, 0, st, x, n / 8, out);
   return 0;
 }
 
@@ -301,10 +289,7 @@ int fuse_masks(const float* scores, int n_tiles, int P, const int* tile_x0, cons
   SRB_REQUIRE(H > 0 && W > 0 && P > 0 && n_tiles >= 0, "fuse_masks: bad sizes H=%d W=%d P=%d n=%d",
               H, W, P, n_tiles);
   dim3 grid((W + 255) / 256, H);
-  fuse_masks_kernel<<<grid, 256, 0, st>>>(scores, n_tiles, P, tile_x0, tile_y0, H, W, keypoint_u8,
-                                          road_u8);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(fuse_masks_kernel, grid, 256, 0, st, scores, n_tiles, P, tile_x0, tile_y0, H, W, keypoint_u8, road_u8);
   return 0;
 }
 

@@ -277,9 +277,7 @@ extern "C" int samroad_label_masks(int T, int size, const int32_t* nodes_xy, con
   SRB_CUDA_OK(cudaMemsetAsync(keypoint_mask, 0, bytes, s));
   SRB_CUDA_OK(cudaMemsetAsync(road_mask, 0, bytes, s));
   const dim3 grid(T, std::min(65535, std::max(1, blocks_for(kTargetBlocks, T))));
-  label_masks_kernel<<<grid, kWarps * 32, 0, s>>>(size, nodes_xy, node_off, edges_xyxy, edge_off, keypoint_radius,
-                                                  road_width, keypoint_mask, road_mask);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(label_masks_kernel, grid, kWarps * 32, 0, s, size, nodes_xy, node_off, edges_xyxy, edge_off,
+             keypoint_radius, road_width, keypoint_mask, road_mask);
   return 0;
 }

@@ -660,16 +660,14 @@ int run_batch(samroad_labels_ctx* L, int B, unsigned long long seed, const int32
   } else {
     if (patches) SRB_CUDA_OK(cudaMemcpyAsync(w.patch, patches, 16 * B, cudaMemcpyDefault, st));
     const unsigned gx = std::min<unsigned>(grid_of(std::max(p.cap, p.S), 256), 64u);
-    draw_kernel<<<dim3(gx, B), 256, 0, st>>>(w, p, patches == nullptr, seed);
-    note_launch(1);
+    SRB_LAUNCH(draw_kernel, dim3(gx, B), 256, 0, st, w, p, patches == nullptr, seed);
   }
   SRB_CUDA_OK(cudaMemsetAsync(w.status, 0, sizeof(int32_t), st));
-  crop_kernel<<<dim3(grid_of(static_cast<long long>(p.P) * p.P, 256), B), 256, 0, st>>>(p, w.patch, rgb, kp, road);
-  patch_kernel<<<B, kPatchThreads, L->smem_patch, st>>>(p, w);
-  pairs_kernel<<<dim3(grid_of(p.S, kPairWarps), B), 32 * kPairWarps, sizeof(BfsSmem) * kPairWarps, st>>>(
-      p, w, pairs, connected, valid);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(3);
+  SRB_LAUNCH(crop_kernel, dim3(grid_of(static_cast<long long>(p.P) * p.P, 256), B), 256, 0, st, p, w.patch, rgb, kp,
+             road);
+  SRB_LAUNCH(patch_kernel, B, kPatchThreads, L->smem_patch, st, p, w);
+  SRB_LAUNCH(pairs_kernel, dim3(grid_of(p.S, kPairWarps), B), 32 * kPairWarps, sizeof(BfsSmem) * kPairWarps, st, p, w,
+             pairs, connected, valid);
   SRB_CUDA_OK(cudaMemcpyAsync(h_read, w.status, sizeof(int32_t) * (B + 1), cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   const int status = h_read[0];
@@ -680,9 +678,7 @@ int run_batch(samroad_labels_ctx* L, int B, unsigned long long seed, const int32
               "steps", what, kBfsList, p.depth);
   int N = 1;
   for (int b = 0; b < B; ++b) N = std::max(N, h_read[1 + b]);
-  points_kernel<<<dim3(grid_of(N, 128), B), 128, 0, st>>>(p, w, N, points);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(points_kernel, dim3(grid_of(N, 128), B), 128, 0, st, p, w, N, points);
   if (export_to) {
     SRB_CUDA_OK(cudaMemcpyAsync(export_to[0], w.patch, 16 * B, cudaMemcpyDefault, st));
     SRB_CUDA_OK(cudaMemcpyAsync(export_to[1], w.score_u, 8 * cap * B, cudaMemcpyDefault, st));
@@ -705,9 +701,8 @@ extern "C" int samroad_labels_create(int device, const SamRoadLabelCfg* cfg, sam
   SRB_REQUIRE(smem + 32 * 4 + 64 <= static_cast<size_t>(optin),
               "samroad_labels_create: a patch window holds up to %d labelled points; the on-chip NMS of one patch "
               "takes %zu bytes of shared memory and this device allows %d", cfg->max_patch_points, smem, optin);
-  SRB_CUDA_OK(cudaFuncSetAttribute(patch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  SRB_CUDA_OK(cudaFuncSetAttribute(pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(sizeof(BfsSmem) * kPairWarps)));
+  SRB_TRY(allow_dynamic_smem(patch_kernel, smem));
+  SRB_TRY(allow_dynamic_smem(pairs_kernel, sizeof(BfsSmem) * kPairWarps));
   samroad_labels_ctx* L = new samroad_labels_ctx();
   L->cfg = *cfg;
   L->device = device;

@@ -423,14 +423,14 @@ extern "C" int samroad_prc_update(samroad_prc_t p, const float* preds, int64_t p
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = grow_keys(p, n, "samroad_prc_update", st)) return rc;
   PrcState* state = p->state.as<PrcState>();
-  prc_begin_kernel<<<1, 1, 0, st>>>(state);
+  SRB_LAUNCH(prc_begin_kernel, 1, 1, 0, st, state);
   if (target_dtype == SAMROAD_U8)
-    prc_append_kernel<true><<<blocks_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
+    SRB_LAUNCH(prc_append_kernel<true>, blocks_for(n, 256), 256, 0, st, preds, pred_stride, target, valid, n, p->keys,
+               state);
   else
-    prc_append_kernel<false><<<blocks_for(n, 256), 256, 0, st>>>(preds, pred_stride, target, valid, n, p->keys, state);
-  prc_commit_kernel<<<1, 1, 0, st>>>(state, p->n_updates);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(3);
+    SRB_LAUNCH(prc_append_kernel<false>, blocks_for(n, 256), 256, 0, st, preds, pred_stride, target, valid, n, p->keys,
+               state);
+  SRB_LAUNCH(prc_commit_kernel, 1, 1, 0, st, state, p->n_updates);
   p->reserved += static_cast<size_t>(n);
   ++p->n_updates;
   return 0;
@@ -444,11 +444,9 @@ extern "C" int samroad_prc_append_keys(samroad_prc_t p, const uint32_t* keys, in
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = grow_keys(p, n, "samroad_prc_append_keys", st)) return rc;
   PrcState* state = p->state.as<PrcState>();
-  prc_begin_kernel<<<1, 1, 0, st>>>(state);
-  prc_append_keys_kernel<<<blocks_for(n, 256), 256, 0, st>>>(keys, n, p->keys, state);
-  prc_commit_kernel<<<1, 1, 0, st>>>(state, p->n_updates);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(3);
+  SRB_LAUNCH(prc_begin_kernel, 1, 1, 0, st, state);
+  SRB_LAUNCH(prc_append_keys_kernel, blocks_for(n, 256), 256, 0, st, keys, n, p->keys, state);
+  SRB_LAUNCH(prc_commit_kernel, 1, 1, 0, st, state, p->n_updates);
   p->reserved += static_cast<size_t>(n);
   ++p->n_updates;
   return 0;
@@ -480,9 +478,7 @@ extern "C" int samroad_prc_compute(samroad_prc_t p, int64_t* counts, float* best
   if (int rc = grow<unsigned long long>(p->tile_cnt, static_cast<size_t>(tiles + 1 + scan_scratch_elems(tiles))))
     return rc;
   unsigned long long* tile_cnt = p->tile_cnt.as<unsigned long long>();
-  curve_count_kernel<<<tiles, 256, 0, st>>>(p->keys, n, tile_cnt);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(curve_count_kernel, tiles, 256, 0, st, p->keys, n, tile_cnt);
   if (int rc = exclusive_scan(tile_cnt, tile_cnt, tiles, tile_cnt + tiles, tile_cnt + tiles + 1, st)) return rc;
   unsigned long long tot = 0;
   SRB_CUDA_OK(cudaMemcpyAsync(&tot, tile_cnt + tiles, sizeof(tot), cudaMemcpyDeviceToHost, st));
@@ -498,11 +494,9 @@ extern "C" int samroad_prc_compute(samroad_prc_t p, int64_t* counts, float* best
     p->curve_cap = c;
   }
   SRB_CUDA_OK(cudaMemsetAsync(&p->state.as<PrcState>()->best, 0, sizeof(unsigned long long), st));
-  curve_fill_kernel<<<tiles, 256, 0, st>>>(p->keys, n, tile_cnt, n_pos, T, p->thr.as<float>(), p->prec.as<float>(),
-                                           p->rec.as<float>(), p->tps.as<long long>(), p->fps.as<long long>(),
-                                           p->state.as<PrcState>());
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(curve_fill_kernel, tiles, 256, 0, st, p->keys, n, tile_cnt, n_pos, T, p->thr.as<float>(),
+             p->prec.as<float>(), p->rec.as<float>(), p->tps.as<long long>(), p->fps.as<long long>(),
+             p->state.as<PrcState>());
   if (int rc = read_state(p, st)) return rc;
   const unsigned long long bk = p->h_state.as<PrcState>()->best;
   const long long bi = static_cast<long long>(0xFFFFFFFFull - (bk & 0xFFFFFFFFull));
@@ -770,12 +764,11 @@ extern "C" int samroad_val_create(int device, samroad_val_t* out) {
   if (v->state.reserve(sizeof(ValState), what) || v->part.reserve(sizeof(ValPartial) * 2 * v->max_blocks, what) ||
       v->h_state.reserve(sizeof(ValState), what))
     return 1;
-  val_reset_kernel<<<1, 1>>>(v->state.as<ValState>());
-  if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
+  SRB_LAUNCH(val_reset_kernel, 1, 1, 0, 0, v->state.as<ValState>());
+  if (cudaDeviceSynchronize() != cudaSuccess) {
     set_last_error("samroad_val_create: initialising the state failed");
     return 1;
   }
-  note_launch(1);
   *out = v.release();
   return 0;
 }
@@ -791,9 +784,7 @@ extern "C" int samroad_val_destroy(samroad_val_t v) {
 extern "C" int samroad_val_reset(samroad_val_t v, void* stream) {
   SRB_REQUIRE(v != nullptr, "samroad_val_reset: null handle");
   SRB_CUDA_OK(cudaSetDevice(v->device));
-  val_reset_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(v->state.as<ValState>());
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(val_reset_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), v->state.as<ValState>());
   v->n_updates = 0;
   return 0;
 }
@@ -822,19 +813,15 @@ extern "C" int samroad_val_update(samroad_val_t v, const float* mask_logits, con
   ValPartial* mask_part = v->part.as<ValPartial>();
   ValPartial* pair_part = mask_part + v->max_blocks;
   if (loss_kind == SAMROAD_LOSS_FOCAL)
-    val_mask_kernel<true><<<g_mask, 256, 0, st>>>(reinterpret_cast<const float2*>(mask_logits),
-                                                  reinterpret_cast<const float2*>(mask_scores), keypoint_mask,
-                                                  road_mask, npix, mask_part, &state->ref);
+    SRB_LAUNCH(val_mask_kernel<true>, g_mask, 256, 0, st, reinterpret_cast<const float2*>(mask_logits),
+               reinterpret_cast<const float2*>(mask_scores), keypoint_mask, road_mask, npix, mask_part, &state->ref);
   else
-    val_mask_kernel<false><<<g_mask, 256, 0, st>>>(reinterpret_cast<const float2*>(mask_logits),
-                                                   reinterpret_cast<const float2*>(mask_scores), keypoint_mask,
-                                                   road_mask, npix, mask_part, &state->ref);
+    SRB_LAUNCH(val_mask_kernel<false>, g_mask, 256, 0, st, reinterpret_cast<const float2*>(mask_logits),
+               reinterpret_cast<const float2*>(mask_scores), keypoint_mask, road_mask, npix, mask_part, &state->ref);
   if (g_pair > 0)
-    val_pair_kernel<<<g_pair, 256, 0, st>>>(topo_logits, topo_scores, connected, valid, n_pairs,
-                                            static_cast<unsigned long long>(2 * npix), pair_part, &state->ref);
-  val_finish_kernel<<<1, 256, 0, st>>>(mask_part, g_mask, pair_part, g_pair, npix, B, out, state, v->n_updates);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(g_pair > 0 ? 3 : 2);
+    SRB_LAUNCH(val_pair_kernel, g_pair, 256, 0, st, topo_logits, topo_scores, connected, valid, n_pairs,
+               static_cast<unsigned long long>(2 * npix), pair_part, &state->ref);
+  SRB_LAUNCH(val_finish_kernel, 1, 256, 0, st, mask_part, g_mask, pair_part, g_pair, npix, B, out, state, v->n_updates);
   ++v->n_updates;
   return 0;
 }

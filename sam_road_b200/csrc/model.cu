@@ -319,12 +319,6 @@ TopoWs layout_topo(int B, int N, int Ns, int Np, void* base) {
     if (_rc != 0) return _rc;                                            \
   } while (0)
 
-#define SRB_TRY(expr)            \
-  do {                           \
-    int _rc = (expr);            \
-    if (_rc != 0) return _rc;    \
-  } while (0)
-
 int check_handle(samroad_handle_t h, bool need_weights) {
   SRB_REQUIRE(h != nullptr, "null samroad handle");
   SRB_REQUIRE(!need_weights || h->finalized,
@@ -752,10 +746,8 @@ extern "C" int samroad_update_tensor_device(samroad_handle_t h, const char* key,
   SRB_REQUIRE(same, "samroad_update_tensor_device: '%s' has the wrong shape", key);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   for (const Target& t : tg) {
-    repack_kernel<<<static_cast<unsigned>((t.n + 255) / 256), 256, 0, st>>>(dev_data, t.mode, t.cin, t.cout, t.n,
-                                                                            t.d32, t.d16);
-    SRB_CUDA_OK(cudaGetLastError());
-    note_launch();
+    SRB_LAUNCH(repack_kernel, static_cast<unsigned>((t.n + 255) / 256), 256, 0, st, dev_data, t.mode, t.cin, t.cout,
+               t.n, t.d32, t.d16);
   }
   return 0;
 }

@@ -10,12 +10,8 @@ namespace srb {
 
 enum Act : int { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2 };
 
-void set_last_error(const char* fmt, ...);
 const char* get_last_error();
 int device_sm_count();
-// true the first time it is called with this mask on the current CUDA device (then sets the bit)
-bool first_use_on_device(uint64_t* device_mask);
-void note_launch(int n = 1);
 // stream memory operations on a 32-bit flag word (no kernel): ordered write / wait until *addr >= value
 int stream_write_value32(void* addr, uint32_t value, cudaStream_t st);
 int stream_wait_value32_geq(void* addr, uint32_t value, cudaStream_t st);

@@ -214,9 +214,7 @@ int tok_gemm(const float* A, int lda, const float* pe, const float* W, const flo
   SRB_REQUIRE(K % 4 == 0 && lda % 4 == 0 && (reinterpret_cast<uintptr_t>(A) & 15u) == 0,
               "tok_gemm: K=%d lda=%d must be multiples of 4 and A 16-byte aligned", K, lda);
   dim3 grid((N + 63) / 64, (M + 31) / 32);
-  tok_gemm_kernel<<<grid, 256, 0, st>>>(A, lda, pe, kC, W, bias, M, N, K, relu ? 1 : 0, out, ldo);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(tok_gemm_kernel, grid, 256, 0, st, A, lda, pe, kC, W, bias, M, N, K, relu ? 1 : 0, out, ldo);
   return 0;
 }
 
@@ -530,29 +528,27 @@ int sam_decoder_forward(const SamDecoderWeights& W, const float* emb_nchw, int B
   const int Mi = static_cast<int>(M);
   const int Bt = 4 * B;
   const float* pe = w.tokens;            // query_pe = the output tokens themselves (transformer.py:95,101)
-  auto LN = [&](float* x, const float* add, const float* g, const float* bb) {
-    tok_add_layernorm_kernel<<<(Bt + 7) / 8, 256, 0, st>>>(x, nullptr, add, g, bb, Bt);
-    note_launch();
+  auto LN = [&](float* x, const float* add, const float* g, const float* bb) -> int {
+    SRB_LAUNCH(tok_add_layernorm_kernel, (Bt + 7) / 8, 256, 0, st, x, nullptr, add, g, bb, Bt);
+    return 0;
   };
   auto t2i = [&](const AttnW& a, const float* g, const float* bb) -> int {
     // queries = norm(queries + out_proj(softmax(q_proj(queries + pe) K^T / 4) V))   (transformer.py:168-172,99-104)
     if (int rc = tok_gemm(b.X, kC, pe, a.qw, a.qb, Bt, 128, kC, false, b.Qc, 128, st)) return rc;
-    tok_t2i_attention_kernel<<<dim3(B, 8), kThreads, 0, st>>>(b.Qc, b.K32, b.V32, T, b.A2);
-    note_launch();
+    SRB_LAUNCH(tok_t2i_attention_kernel, dim3(B, 8), kThreads, 0, st, b.Qc, b.K32, b.V32, T, b.A2);
     if (int rc = tok_gemm(b.A2, 128, nullptr, a.ow, a.ob, Bt, kC, 128, false, b.T1, kC, st)) return rc;
-    LN(b.X, b.T1, g, bb);
+    SRB_TRY(LN(b.X, b.T1, g, bb));
     return 0;
   };
 
-  sam_keys_init_kernel<<<blocks_for(M * 256, 256), 256, 0, st>>>(emb_nchw, w.no_mask_embed, T, M * 256, b.keys32);
-  tok_broadcast_kernel<<<blocks_for(static_cast<long>(Bt) * kC, 256), 256, 0, st>>>(W.q0, static_cast<long>(Bt) * kC, b.X);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(2);
+  SRB_LAUNCH(sam_keys_init_kernel, blocks_for(M * 256, 256), 256, 0, st, emb_nchw, w.no_mask_embed, T, M * 256,
+             b.keys32);
+  SRB_LAUNCH(tok_broadcast_kernel, blocks_for(static_cast<long>(Bt) * kC, 256), 256, 0, st, W.q0,
+             static_cast<long>(Bt) * kC, b.X);
   for (int l = 0; l < 2; ++l) {
     const SamLayerW& L = w.layer[l];
-    sam_keys_prep_kernel<<<blocks_for(M * 256, 256), 256, 0, st>>>(b.keys32, w.dense_pe, T, M * 256, b.ka16, b.va16);
-    SRB_CUDA_OK(cudaGetLastError());
-    note_launch();
+    SRB_LAUNCH(sam_keys_prep_kernel, blocks_for(M * 256, 256), 256, 0, st, b.keys32, w.dense_pe, T, M * 256, b.ka16,
+               b.va16);
     if (int rc = gemm_f32out(b.ka16, 256, w.t2i_kw[l], 256, Mi, 128, 256, w.t2i_kb[l], nullptr, nullptr, 0, b.K32, 128, st)) return rc;
     if (int rc = gemm_f32out(b.va16, 256, w.t2i_vw[l], 256, Mi, 128, 256, w.t2i_vb[l], nullptr, nullptr, 0, b.V32, 128, st)) return rc;
     if (int rc = gemm_f32out(b.ka16, 256, w.i2t_qw[l], 256, Mi, 128, 256, w.i2t_qb[l], nullptr, nullptr, 0, b.Q32, 128, st)) return rc;
@@ -560,31 +556,27 @@ int sam_decoder_forward(const SamDecoderWeights& W, const float* emb_nchw, int B
       if (int rc = tok_gemm(b.X, kC, pe, L.self_attn.qw, L.self_attn.qb, Bt, kC, kC, false, b.T1, kC, st)) return rc;
       if (int rc = tok_gemm(b.X, kC, pe, L.self_attn.kw, L.self_attn.kb, Bt, kC, kC, false, b.T2, kC, st)) return rc;
       if (int rc = tok_gemm(b.X, kC, nullptr, L.self_attn.vw, L.self_attn.vb, Bt, kC, kC, false, b.T3, kC, st)) return rc;
-      tok_self_attention_kernel<<<blocks_for(static_cast<long>(Bt) * kC, 256), 256, 0, st>>>(
-          b.T1, b.T2, b.T3, static_cast<long>(Bt) * kC, b.T0);
-      note_launch();
+      SRB_LAUNCH(tok_self_attention_kernel, blocks_for(static_cast<long>(Bt) * kC, 256), 256, 0, st, b.T1, b.T2, b.T3,
+                 static_cast<long>(Bt) * kC, b.T0);
       if (int rc = tok_gemm(b.T0, kC, nullptr, L.self_attn.ow, L.self_attn.ob, Bt, kC, kC, false, b.T1, kC, st)) return rc;
-      LN(b.X, b.T1, L.n1g, L.n1b);
+      SRB_TRY(LN(b.X, b.T1, L.n1g, L.n1b));
     }
     if (int rc = t2i(L.t2i, L.n2g, L.n2b)) return rc;
     // MLP (transformer.py:174-177): queries = norm3(queries + lin2(relu(lin1(queries))))
     if (int rc = tok_gemm(b.X, kC, nullptr, L.l1w, L.l1b, Bt, 2048, kC, true, b.Hd, 2048, st)) return rc;
     if (int rc = tok_gemm(b.Hd, 2048, nullptr, L.l2w, L.l2b, Bt, kC, 2048, false, b.T1, kC, st)) return rc;
-    LN(b.X, b.T1, L.n3g, L.n3b);
+    SRB_TRY(LN(b.X, b.T1, L.n3g, L.n3b));
     // image -> token attention (transformer.py:179-182): k = k_proj(queries + pe), v = v_proj(queries)
     if (int rc = tok_gemm(b.X, kC, pe, L.i2t.kw, L.i2t.kb, Bt, 128, kC, false, b.k4, 128, st)) return rc;
     if (int rc = tok_gemm(b.X, kC, nullptr, L.i2t.vw, L.i2t.vb, Bt, 128, kC, false, b.v4, 128, st)) return rc;
-    sam_i2t_attention_kernel<<<blocks_for(M * 8, 256), 256, 0, st>>>(b.Q32, b.k4, b.v4, T, M, b.att16);
-    SRB_CUDA_OK(cudaGetLastError());
-    note_launch();
+    SRB_LAUNCH(sam_i2t_attention_kernel, blocks_for(M * 8, 256), 256, 0, st, b.Q32, b.k4, b.v4, T, M, b.att16);
     // keys = norm4(keys + out_proj(attn))
     if (int rc = gemm_ln(b.att16, 128, w.i2t_ow[l], 128, Mi, 256, 128, w.i2t_ob[l], b.keys32, w.n4g[l], w.n4b[l],
                          1e-5f, 256, ACT_NONE, nullptr, b.keys32, nullptr, 1, 256, st)) return rc;
   }
   // final token -> image attention + norm_final_attn (transformer.py:99-106), then the hypernetwork MLPs
-  sam_keys_prep_kernel<<<blocks_for(M * 256, 256), 256, 0, st>>>(b.keys32, w.dense_pe, T, M * 256, b.ka16, b.va16);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(sam_keys_prep_kernel, blocks_for(M * 256, 256), 256, 0, st, b.keys32, w.dense_pe, T, M * 256, b.ka16,
+             b.va16);
   if (int rc = gemm_f32out(b.ka16, 256, w.t2i_kw[2], 256, Mi, 128, 256, w.t2i_kb[2], nullptr, nullptr, 0, b.K32, 128, st)) return rc;
   if (int rc = gemm_f32out(b.va16, 256, w.t2i_vw[2], 256, Mi, 128, 256, w.t2i_vb[2], nullptr, nullptr, 0, b.V32, 128, st)) return rc;
   if (int rc = t2i(w.fin.attn, w.fin.ng, w.fin.nb)) return rc;
@@ -596,16 +588,13 @@ int sam_decoder_forward(const SamDecoderWeights& W, const float* emb_nchw, int B
     if (int rc = tok_gemm(b.T0, kC, nullptr, w.fin.hw[mi][1], w.fin.hb[mi][1], B, kC, kC, true, b.T2, kC, st)) return rc;
     if (int rc = tok_gemm(b.T2, kC, nullptr, w.fin.hw[mi][2], w.fin.hb[mi][2], B, 32, kC, false, b.hyper + mi * 32, 64, st)) return rc;
   }
-  SRB_CUDA_OK(cudaGetLastError());
   // upscaler: ConvT(256->64)+LN2d+GELU, ConvT(64->32)+GELU as GEMMs (va16 = fp16(keys))
   if (int rc = gemm_ln(b.va16, 256, w.up1_w, 256, Mi, 256, 256, w.up1_b, nullptr, w.up1_g, w.up1_beta, 1e-6f, 64,
                        ACT_GELU, b.u1, nullptr, nullptr, 1, 256, st)) return rc;
   if (int rc = gemm_f16out(b.u1, 64, w.up2_w, 64, 4 * Mi, 128, 64, w.up2_b, ACT_GELU, b.u2, 128, st)) return rc;
-  sam_lowres_masks_kernel<<<blocks_for(16 * M, 256), 256, 0, st>>>(b.u2, b.hyper, s, 16 * M, b.lr);
-  sam_upsample4_kernel<<<blocks_for(static_cast<long>(B) * P * P, 256), 256, 0, st>>>(
-      b.lr, 4 * s, static_cast<long>(B) * P * P, mask_logits, mask_scores);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(2);
+  SRB_LAUNCH(sam_lowres_masks_kernel, blocks_for(16 * M, 256), 256, 0, st, b.u2, b.hyper, s, 16 * M, b.lr);
+  SRB_LAUNCH(sam_upsample4_kernel, blocks_for(static_cast<long>(B) * P * P, 256), 256, 0, st, b.lr, 4 * s,
+             static_cast<long>(B) * P * P, mask_logits, mask_scores);
   return 0;
 }
 
@@ -615,9 +604,7 @@ int sam_decoder_forward(const SamDecoderWeights& W, const float* emb_nchw, int B
 int sam_decoder_prepare(const SamDecoderWeights& W, float* q0, cudaStream_t st) {
   AttnW a{W.self_attn[0].qw, W.self_attn[0].qb, W.self_attn[0].kw, W.self_attn[0].kb,
           W.self_attn[0].vw, W.self_attn[0].vb, W.self_attn[0].ow, W.self_attn[0].ob};
-  sam_tokens_init_kernel<<<1, kThreads, 0, st>>>(W.tokens, a, W.n1g[0], W.n1b[0], q0);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(sam_tokens_init_kernel, 1, kThreads, 0, st, W.tokens, a, W.n1g[0], W.n1b[0], q0);
   return 0;
 }
 

@@ -3,7 +3,7 @@
 // stable 8-bit digit sort.
 //
 // None of them allocates or synchronises: each caller sizes the scratch with the *_elems helpers and grows it
-// under its own policy.  Every launch is counted with note_launch.  The sums are integer sums, so a scan's
+// under its own policy.  Every launch goes through SRB_LAUNCH.  The sums are integer sums, so a scan's
 // result does not depend on how it is split over threads and blocks.
 #pragma once
 
@@ -163,16 +163,13 @@ __global__ void __launch_bounds__(32 * kDigitWarps) digit_scatter_kernel(const F
 template <typename T>
 int exclusive_scan(const T* in, T* out, long long n, T* total_dev, T* scratch, cudaStream_t st) {
   if (n <= kScanTile) {
-    scan_block_kernel<T><<<1, kScanBlock, 0, st>>>(in, out, n, total_dev);
-    note_launch(1);
+    SRB_LAUNCH(scan_block_kernel<T>, 1, kScanBlock, 0, st, in, out, n, total_dev);
   } else {
     const int tiles = blocks_for(n, kScanTile);
-    scan_sums_kernel<T><<<tiles, 256, 0, st>>>(in, n, scratch);
-    scan_block_kernel<T><<<1, kScanBlock, 0, st>>>(scratch, scratch, tiles, total_dev);
-    scan_tile_kernel<T><<<tiles, 256, 0, st>>>(in, out, n, scratch);
-    note_launch(3);
+    SRB_LAUNCH(scan_sums_kernel<T>, tiles, 256, 0, st, in, n, scratch);
+    SRB_LAUNCH(scan_block_kernel<T>, 1, kScanBlock, 0, st, scratch, scratch, tiles, total_dev);
+    SRB_LAUNCH(scan_tile_kernel<T>, tiles, 256, 0, st, in, out, n, scratch);
   }
-  SRB_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
@@ -189,13 +186,9 @@ int stable_digit_pass(const F& f, long long n, uint32_t* hist, uint32_t* scratch
   static_assert(kChunk % 32 == 0, "a warp walks its chunk 32 elements at a time");
   const int nchunks = blocks_for(n, kChunk);
   const int blocks = blocks_for(nchunks, kDigitWarps);
-  digit_hist_kernel<kChunk, F><<<blocks, 32 * kDigitWarps, 0, st>>>(f, n, nchunks, hist);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(digit_hist_kernel<kChunk, F>, blocks, 32 * kDigitWarps, 0, st, f, n, nchunks, hist);
   if (int rc = exclusive_scan<uint32_t>(hist, hist, 256LL * nchunks, nullptr, scratch, st)) return rc;
-  digit_scatter_kernel<kChunk, F><<<blocks, 32 * kDigitWarps, 0, st>>>(f, n, nchunks, hist);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(1);
+  SRB_LAUNCH(digit_scatter_kernel<kChunk, F>, blocks, 32 * kDigitWarps, 0, st, f, n, nchunks, hist);
   return 0;
 }
 

@@ -654,11 +654,9 @@ extern "C" int samroad_topo_run(samroad_topo_t T, int32_t n_pairs, const int32_t
   for (int ch = 0; ch < chunks; ++ch) {
     p.first_pair = ch * slots;
     p.serial = ++T->serial;
-    walk_kernel<<<dim3(slots, 3), 32, 0, st>>>(p, ws);
-    match_kernel<<<slots, kMatchThreads, 0, st>>>(p, ws);
-    note_launch(2);
+    SRB_LAUNCH(walk_kernel, dim3(slots, 3), 32, 0, st, p, ws);
+    SRB_LAUNCH(match_kernel, slots, kMatchThreads, 0, st, p, ws);
   }
-  SRB_CUDA_OK(cudaGetLastError());
   SRB_CUDA_OK(cudaMemcpyAsync(counts, p.out, 24ull * n_pairs, cudaMemcpyDeviceToHost, st));
   SRB_CUDA_OK(cudaStreamSynchronize(st));
   for (int32_t i = 0; i < n_pairs; ++i) {

@@ -59,10 +59,8 @@ int topo_sample_launch(const float* feat_nchw, int B, int C, int s, int P, const
                        int pts_dtype, int N, T* out, cudaStream_t st) {
   SRB_REQUIRE(pts_dtype >= 0 && pts_dtype <= 2, "topo_sample: points dtype %d", pts_dtype);
   if (B * N <= 0) return 0;
-  topo_sample_kernel<T><<<B * N, 256, 0, st>>>(feat_nchw, C, s, static_cast<float>(P), points,
-                                               pts_dtype, N, out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(topo_sample_kernel<T>, B * N, 256, 0, st, feat_nchw, C, s, static_cast<float>(P), points, pts_dtype, N,
+             out);
   return 0;
 }
 
@@ -95,9 +93,7 @@ topo_pair_kernel(const TopoPairInputs in, float* __restrict__ x32, __half* __res
 int topo_pair_features(const TopoPairInputs& in, int tokens, float* x32, __half* x16, cudaStream_t st) {
   SRB_REQUIRE(in.pairs_dtype == 1 || in.pairs_dtype == 2, "topo_pair: pairs dtype %d", in.pairs_dtype);
   if (tokens <= 0) return 0;
-  topo_pair_kernel<<<static_cast<unsigned>(tokens), 128, 0, st>>>(in, x32, x16);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(topo_pair_kernel, static_cast<unsigned>(tokens), 128, 0, st, in, x32, x16);
   return 0;
 }
 
@@ -113,9 +109,7 @@ __global__ void topo_fix_valid_kernel(const uint8_t* __restrict__ valid, int row
 }
 int topo_fix_valid(const uint8_t* valid, int rows, int Np, uint8_t* out, cudaStream_t st) {
   if (rows <= 0) return 0;
-  topo_fix_valid_kernel<<<(rows + 255) / 256, 256, 0, st>>>(valid, rows, Np, out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(topo_fix_valid_kernel, (rows + 255) / 256, 256, 0, st, valid, rows, Np, out);
   return 0;
 }
 
@@ -193,9 +187,7 @@ int topo_attention(const __half* qkv, const uint8_t* valid, int rows, int Np, __
   if (rows <= 0) return 0;
   const int per_block = 128 / (4 * Np);
   auto* kernel = Np <= 16 ? topo_attention_kernel<16> : topo_attention_kernel<32>;
-  kernel<<<(rows + per_block - 1) / per_block, 128, 0, st>>>(qkv, valid, rows, Np, out);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(kernel, (rows + per_block - 1) / per_block, 128, 0, st, qkv, valid, rows, Np, out);
   return 0;
 }
 
@@ -225,10 +217,7 @@ topo_output_kernel(const float* __restrict__ x32, const uint8_t* __restrict__ va
 int topo_output(const float* x32, const uint8_t* valid_fixed, const float* w, const float* b,
                 int tokens, float* logits, float* scores, cudaStream_t st) {
   if (tokens <= 0) return 0;
-  topo_output_kernel<<<(tokens + 7) / 8, 256, 0, st>>>(x32, valid_fixed, w, b, tokens, logits,
-                                                       scores);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(topo_output_kernel, (tokens + 7) / 8, 256, 0, st, x32, valid_fixed, w, b, tokens, logits, scores);
   return 0;
 }
 
@@ -245,12 +234,8 @@ int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, con
   SRB_REQUIRE(in.pairs_dtype == 1 || in.pairs_dtype == 2, "topo fused: pairs dtype %d", in.pairs_dtype);
   CUtensorMap tmW;
   if (int rc = make_tmap_f16_2d(&tmW, w_chunks, 18 * 128, 128, 128, 128)) return rc;
-  // one bit per CUDA device and instantiation: function attributes are per device and function
-  static uint64_t attr_devs[2] = {0, 0};
   auto* kernel = Np == 16 ? toponet_tc_kernel<16> : toponet_tc_kernel<32>;
-  if (first_use_on_device(&attr_devs[Np == 32])) {
-    SRB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTtcSmemBytes));
-  }
+  SRB_TRY(allow_dynamic_smem(kernel, kTtcSmemBytes));
   TtcParams p;
   for (int l = 0; l < 3; ++l) p.layer[l] = layers[l];
   p.in = in;
@@ -258,9 +243,7 @@ int topo_transformer_fused(const TopoPairInputs& in, const __half* w_chunks, con
   p.logits = logits; p.scores = scores; p.tokens = tokens;
   p.num_tiles = (tokens + 127) / 128;
   const int grid = p.num_tiles < device_sm_count() ? p.num_tiles : device_sm_count();
-  kernel<<<grid, kTtcThreads, kTtcSmemBytes, st>>>(tmW, p);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(kernel, grid, kTtcThreads, kTtcSmemBytes, st, tmW, p);
   return 0;
 }
 

@@ -36,12 +36,6 @@ using namespace srb;
 // model.cu: the parts of the handle's configuration the heads need
 int samroad_handle_head_config(samroad_handle_t h, int* patch_size, int* toponet_version, int* use_sam_decoder);
 
-#define SRB_TRY(expr)            \
-  do {                           \
-    int _rc = (expr);            \
-    if (_rc != 0) return _rc;    \
-  } while (0)
-
 namespace {
 
 // ---- head parameters in the reference layout ------------------------------------------------------------
@@ -293,9 +287,7 @@ int tc_gemm(LA A, LB Bm, OUT out, long long M, long long N, long long K, int chu
   // make_dims bounds every GEMM of a step far below these limits
   SRB_REQUIRE(nt < 65536 && z < 65536, "train: GEMM of %lld x %lld (%lld chunks) is too large", M, N, z);
   const dim3 grid(static_cast<unsigned>(nt), static_cast<unsigned>(mt < 65535 ? mt : 65535), static_cast<unsigned>(z));
-  gemm_mma_kernel<<<grid, 256, 0, st>>>(A, Bm, out, M, N, K, kchunk);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(gemm_mma_kernel<LA, LB, OUT>, grid, 256, 0, st, A, Bm, out, M, N, K, kchunk);
   return 0;
 }
 
@@ -353,10 +345,8 @@ int wgrad(Mat a, int K0, LG g, int N, long long R, int mode, int cout, long long
   const long long Z = wgrad_chunks(R);
   SRB_TRY(tc_gemm(at, g, Partial{part, M, N}, M, N, R, kWgradChunks, st));
   const long long MN = static_cast<long long>(M) * N;
-  wgrad_finish_kernel<<<static_cast<unsigned>((MN + 255) / 256), 256, 0, st>>>(part, static_cast<int>(Z), K0, M, N,
-                                                                              mode, cout, ld, col0, dW, db, scale);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(wgrad_finish_kernel, static_cast<unsigned>((MN + 255) / 256), 256, 0, st, part, static_cast<int>(Z), K0, M,
+             N, mode, cout, ld, col0, dW, db, scale);
   return 0;
 }
 
@@ -506,10 +496,8 @@ int ln_param_grads(const float* g, const float* xh, long long rows, float* part,
                    const float* scale, cudaStream_t st) {
   const long long chunk = rows > 0 ? (rows + kColChunks - 1) / kColChunks : 1;
   const int Z = static_cast<int>(rows > 0 ? (rows + chunk - 1) / chunk : 1);
-  colsum_kernel<<<Z, 128, 0, st>>>(g, xh, rows, chunk, part);
-  colsum_finish_kernel<<<1, 128, 0, st>>>(part, Z, dg, db, scale);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(2);
+  SRB_LAUNCH(colsum_kernel, Z, 128, 0, st, g, xh, rows, chunk, part);
+  SRB_LAUNCH(colsum_finish_kernel, 1, 128, 0, st, part, Z, dg, db, scale);
   return 0;
 }
 
@@ -816,19 +804,10 @@ __global__ void keep_kernel(Dropout d, int layer, int site, long long n, uint8_t
   GRID_STRIDE(i, n) out[i] = drop_mul(d, layer, site, static_cast<unsigned long long>(i)) != 0.0f;
 }
 
-#define EW(kernel, n, ...)                                                     \
-  do {                                                                         \
-    kernel<<<ew_grid(n), 256, 0, st>>>(__VA_ARGS__);                           \
-    SRB_CUDA_OK(cudaGetLastError());                                           \
-    note_launch();                                                             \
-  } while (0)
-#define ROWS8(kernel, rows, ...)                                               \
-  do {                                                                         \
-    if ((rows) > 0) {                                                          \
-      kernel<<<static_cast<unsigned>(((rows) + 7) / 8), 256, 0, st>>>(__VA_ARGS__); \
-      SRB_CUDA_OK(cudaGetLastError());                                         \
-      note_launch();                                                           \
-    }                                                                          \
+#define EW(kernel, n, ...) SRB_LAUNCH(kernel, ew_grid(n), 256, 0, st, __VA_ARGS__)
+#define ROWS8(kernel, rows, ...)                                                                     \
+  do {                                                                                              \
+    if ((rows) > 0) SRB_LAUNCH(kernel, static_cast<unsigned>(((rows) + 7) / 8), 256, 0, st, __VA_ARGS__); \
   } while (0)
 
 // ---- workspace --------------------------------------------------------------------------------------------
@@ -932,9 +911,7 @@ int build_csr(const int* idx, long long tok, long long pts, int* start, int* lis
   SRB_TRY(exclusive_scan(cursor, start, pts, start + pts, scan_tmp, st));
   SRB_CUDA_OK(cudaMemsetAsync(cursor, 0, pts * 4, st));
   EW(csr_fill_kernel, tok, idx, tok, start, cursor, list);
-  csr_sort_kernel<<<static_cast<unsigned>(pts), 256, 0, st>>>(start, list, tmp);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(csr_sort_kernel, static_cast<unsigned>(pts), 256, 0, st, start, list, tmp);
   return 0;
 }
 
@@ -994,10 +971,8 @@ extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs*
   SRB_TRY(tc_gemm(rowmajor(w.a2, 64), ConvTW{P_[HP_DEC5_W], 32, false}, Store{w.z3, 128}, d.R2, 128, 64, 1, st));
   EW(bias_act_kernel, d.R3 * 32, w.z3, P_[HP_DEC5_B], 32, d.R3 * 32, 1, w.a3);
   SRB_TRY(tc_gemm(rowmajor(w.a3, 32), ConvTW{P_[HP_DEC7_W], 2, false}, Store{w.dl, 8}, d.R3, 8, 32, 1, st));
-  mask_loss_kernel<<<kLossBlocks, 256, 0, st>>>(w.dl, P_[HP_DEC7_B], keypoint_mask, road_mask, d.R4, d.T, d.s, d.P,
-                                                args->loss_kind == SAMROAD_LOSS_FOCAL, w.part);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(mask_loss_kernel, kLossBlocks, 256, 0, st, w.dl, P_[HP_DEC7_B], keypoint_mask, road_mask, d.R4, d.T, d.s,
+             d.P, args->loss_kind == SAMROAD_LOSS_FOCAL, w.part);
 
   // ---- TopoNet (model.py:88-148), slow-path semantics ----
   SRB_TRY(topo_sample_features_f32(w.emb, d.B, 256, d.s, d.P, points, pts_dtype, d.N, w.fs, st));
@@ -1008,9 +983,7 @@ extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs*
                 st));
   const TopoPairInputs pin{w.pst, nullptr, P_[HP_PP_B], points, pairs, pts_dtype, pairs_dtype, d.N, d.Ns * d.Np,
                            d.topo_version == SAMROAD_TOPO_NO_OFFSET};
-  tr_pair_kernel<<<static_cast<unsigned>(d.tok), 128, 0, st>>>(pin, P_[HP_PP_W], w.x[0], w.off, w.src, w.tgt);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(tr_pair_kernel, static_cast<unsigned>(d.tok), 128, 0, st, pin, P_[HP_PP_W], w.x[0], w.off, w.src, w.tgt);
   SRB_TRY(build_csr(w.src, d.tok, d.pts, w.src_start, w.src_list, w.cursor, w.sort_tmp, w.scan_tmp, st));
   SRB_TRY(build_csr(w.tgt, d.tok, d.pts, w.tgt_start, w.tgt_list, w.cursor, w.sort_tmp, w.scan_tmp, st));
   SRB_TRY(topo_fix_valid(valid, static_cast<int>(d.rows), d.Np, w.vf, st));
@@ -1020,9 +993,7 @@ extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs*
       const LayerWs& L = w.L[l];
       SRB_TRY(tc_gemm(rowmajor(xl, 128), colmajor(LP(hp, l, LP_IN_W), 128), Store{L.qkv, 384}, d.tok, 384, 128, 1, st));
       EW(bias_act_kernel, d.tok * 384, L.qkv, LP(hp, l, LP_IN_B), 384, d.tok * 384, 0, nullptr);
-      tr_attn_fwd_kernel<<<static_cast<unsigned>(d.rows * 4), 32, 0, st>>>(L.qkv, w.vf, d.Np, drop, l, L.att);
-      SRB_CUDA_OK(cudaGetLastError());
-      note_launch();
+      SRB_LAUNCH(tr_attn_fwd_kernel, static_cast<unsigned>(d.rows * 4), 32, 0, st, L.qkv, w.vf, d.Np, drop, l, L.att);
       SRB_TRY(tc_gemm(rowmajor(L.att, 128), colmajor(LP(hp, l, LP_OUT_W), 128), Store{w.gy, 128}, d.tok, 128, 128, 1, st));
       ROWS8(ln_fwd_kernel, d.tok, w.gy, LP(hp, l, LP_OUT_B), xl, drop, l, 1, LP(hp, l, LP_N1_G), LP(hp, l, LP_N1_B),
             1e-5f, 0, d.tok, L.xh1, L.rs1, L.x1);
@@ -1036,11 +1007,9 @@ extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs*
     }
   }
   ROWS8(topo_logit_kernel, d.tok, xl, P_[HP_OUT_W], P_[HP_OUT_B], d.tok, w.dlt);
-  topo_loss_kernel<<<kLossBlocks, 256, 0, st>>>(w.dlt, connected, valid, d.tok, w.part + kLossBlocks);
-  loss_finish_kernel<<<1, 32, 0, st>>>(w.part, w.part + kLossBlocks, kLossBlocks, 2.0 * static_cast<double>(d.R4),
-                                       losses, w.stats);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(2);
+  SRB_LAUNCH(topo_loss_kernel, kLossBlocks, 256, 0, st, w.dlt, connected, valid, d.tok, w.part + kLossBlocks);
+  SRB_LAUNCH(loss_finish_kernel, 1, 32, 0, st, w.part, w.part + kLossBlocks, kLossBlocks,
+             2.0 * static_cast<double>(d.R4), losses, w.stats);
   return 0;
 }
 
@@ -1066,9 +1035,7 @@ extern "C" int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs
   const float* const* P_ = hp.p;
 
   // ---- map decoder ----
-  loss_scale_kernel<<<1, 1, 0, st>>>(g, 2.0 * static_cast<double>(d.R4), w.stats, w.scale);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch();
+  SRB_LAUNCH(loss_scale_kernel, 1, 1, 0, st, g, 2.0 * static_cast<double>(d.R4), w.stats, w.scale);
   SRB_TRY(wgrad(rowmajor(w.a3, 32), 32, rowmajor(w.dl, 8), 8, d.R3, 1, 2, 0, 0, G[HP_DEC7_W], G[HP_DEC7_B], w.wpart, w.scale, st));
   SRB_TRY(tc_gemm(rowmajor(w.dl, 8), ConvTW{P_[HP_DEC7_W], 2, true}, Store{w.g3, 32}, d.R3, 32, 8, 1, st));
   EW(act_grad_kernel, d.R3 * 32, w.g3, w.z3, d.R3 * 32, 1, drop, 0, 0);
@@ -1116,9 +1083,8 @@ extern "C" int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs
       SRB_TRY(wgrad(rowmajor(L.att, 128), 128, gy1, 128, d.tok, 0, 0, 128, 0, G[HP_LAYER0 + 12 * l + LP_OUT_W],
                     G[HP_LAYER0 + 12 * l + LP_OUT_B], w.wpart, w.scale + 1, st));
       SRB_TRY(tc_gemm(gy1, rowmajor(LP(hp, l, LP_OUT_W), 128), Store{w.gy, 128}, d.tok, 128, 128, 1, st));
-      tr_attn_bwd_kernel<<<static_cast<unsigned>(d.rows * 4), 32, 0, st>>>(L.qkv, w.vf, w.gy, d.Np, drop, l, w.gq);
-      SRB_CUDA_OK(cudaGetLastError());
-      note_launch();
+      SRB_LAUNCH(tr_attn_bwd_kernel, static_cast<unsigned>(d.rows * 4), 32, 0, st, L.qkv, w.vf, w.gy, d.Np, drop, l,
+                 w.gq);
       // in_proj: dWin = gq^T x; gx = gr + gq Win (gradient of the layer input)
       const float* xin = w.x[l];
       SRB_TRY(wgrad(rowmajor(xin, 128), 128, rowmajor(w.gq, 384), 384, d.tok, 0, 0, 128, 0,
@@ -1132,10 +1098,8 @@ extern "C" int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs
   SRB_TRY(wgrad(rowmajor(w.off, 2), 2, rowmajor(w.gx, 128), 128, d.tok, 0, 0, 258, 256, G[HP_PP_W], G[HP_PP_B],
                 w.wpart, w.scale + 1, st));
   // per-point sums of the token gradients by src and by tgt, then Ws / Wt over the points
-  segsum_kernel<<<static_cast<unsigned>(d.pts), 128, 0, st>>>(w.src_start, w.src_list, w.gx, w.gps);
-  segsum_kernel<<<static_cast<unsigned>(d.pts), 128, 0, st>>>(w.tgt_start, w.tgt_list, w.gx, w.gpt);
-  SRB_CUDA_OK(cudaGetLastError());
-  note_launch(2);
+  SRB_LAUNCH(segsum_kernel, static_cast<unsigned>(d.pts), 128, 0, st, w.src_start, w.src_list, w.gx, w.gps);
+  SRB_LAUNCH(segsum_kernel, static_cast<unsigned>(d.pts), 128, 0, st, w.tgt_start, w.tgt_list, w.gx, w.gpt);
   SRB_TRY(wgrad(rowmajor(w.pf, 128), 128, rowmajor(w.gps, 128), 128, d.pts, 0, 0, 258, 0, G[HP_PP_W], nullptr,
                 w.wpart, w.scale + 1, st));
   SRB_TRY(wgrad(rowmajor(w.pf, 128), 128, rowmajor(w.gpt, 128), 128, d.pts, 0, 0, 258, 128, G[HP_PP_W], nullptr,
