@@ -503,6 +503,14 @@ int samroad_op_layernorm(const float* x, const float* gamma, const float* beta, 
 int samroad_op_attention(const void* qkv16, const float* qkv_bias, const float* rel_h,
                          const float* rel_w, int B, int s, int win, int heads, int head_dim,
                          void* out16, void* stream);
+/* The SAM mask decoder alone (USE_SAM_DECODER handles): the forward of samroad_encode_masks on caller-given
+ * fp32 NCHW embeddings [B,256,s,s] with the handle's weights, then stream-ordered copies of four of its
+ * intermediates (each may be NULL): queries [B,4,256] after norm_final_attn, keys [B,T,256] after the last
+ * norm4, hyper [B,2,32] (hypernetworks of mask tokens 1, 2) and the low-res masks lowres [B,4s,4s,2].
+ * Refused before any launch: a handle without the decoder, unfinalised weights, a NULL emb_nchw, B <= 0
+ * and both mask outputs NULL. */
+int samroad_op_sam_decoder(samroad_handle_t h, const float* emb_nchw, int B, float* queries, float* keys,
+                           float* hyper, float* lowres, float* mask_scores, float* mask_logits, void* stream);
 
 /* Test hook: bit 0 routes samroad_op_attention / the encoder through the fp32 SIMT attention
  * kernel (the independent on-device checker of the tensor-core kernel).  Not for production use. */

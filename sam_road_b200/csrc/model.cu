@@ -1173,5 +1173,21 @@ extern "C" int samroad_op_attention(const void* qkv16, const float* qkv_bias, co
                            win, heads, head_dim, static_cast<__half*>(out16),
                            static_cast<cudaStream_t>(stream));
 }
+extern "C" int samroad_op_sam_decoder(samroad_handle_t h, const float* emb_nchw, int B, float* queries,
+                                      float* keys, float* hyper, float* lowres, float* mask_scores,
+                                      float* mask_logits, void* stream) {
+  SRB_TRY(check_handle(h, false));
+  SRB_REQUIRE(h->cfg.use_sam_decoder, "samroad_op_sam_decoder: the handle has no SAM mask decoder");
+  SRB_TRY(check_handle(h, true));
+  SRB_REQUIRE(emb_nchw, "samroad_op_sam_decoder: null emb_nchw");
+  SRB_REQUIRE(B > 0, "samroad_op_sam_decoder: B=%d (want > 0)", B);
+  SRB_REQUIRE(mask_scores || mask_logits, "samroad_op_sam_decoder: mask_scores and mask_logits are both null");
+  SRB_REQUIRE(static_cast<long>(B) * h->T * 16 < 2147483647L, "batch of %d tiles is too large for one call", B);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SRB_TRY(grow(h->sam_ws, sam_decoder_ws_bytes(B, h->T), "samroad_op_sam_decoder"));
+  SRB_TRY(sam_decoder_forward(h->sam, emb_nchw, B, h->s, h->cfg.patch_size, h->sam_ws.get(), mask_scores,
+                              mask_logits, st));
+  return sam_decoder_checkpoints(B, h->T, h->sam_ws.get(), queries, keys, hyper, lowres, st);
+}
 extern "C" void samroad_debug_force_simt_attention(int on) { attention_force_simt(on); }
 extern "C" void samroad_debug_disable_2cta_gemm(int off) { g_ln_ascending = (off & 16) != 0; }

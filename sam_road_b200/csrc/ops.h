@@ -117,6 +117,11 @@ size_t sam_decoder_ws_bytes(int B, int T);
 int sam_decoder_prepare(const SamDecoderWeights& w, float* q0_out, cudaStream_t st);
 int sam_decoder_forward(const SamDecoderWeights& w, const float* emb_nchw, int B, int s, int P, void* ws,
                         float* mask_scores, float* mask_logits, cudaStream_t st);
+// stream-ordered copies of the forward's final intermediates out of its workspace (test hook; any may be null):
+// queries [B][4][256] after norm_final_attn, keys [B][T][256] after the last norm4, hyper [B][2][32],
+// lowres [B][4s][4s][2]
+int sam_decoder_checkpoints(int B, int T, void* ws, float* queries, float* keys, float* hyper, float* lowres,
+                            cudaStream_t st);
 
 // ---- mask fusion (kernels.cu) : inferencer.py:79-110 --------------------------------------------------------
 int fuse_masks(const float* scores, int n_tiles, int P, const int* tile_x0, const int* tile_y0,

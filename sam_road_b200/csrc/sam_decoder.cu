@@ -492,6 +492,18 @@ SamDecoderWs layout_sam_decoder(int B, int T, void* base) {
 
 size_t sam_decoder_ws_bytes(int B, int T) { return layout_sam_decoder(B, T, nullptr).total; }
 
+int sam_decoder_checkpoints(int B, int T, void* ws, float* queries, float* keys, float* hyper, float* lowres,
+                            cudaStream_t st) {
+  const SamDecoderWs b = layout_sam_decoder(B, T, ws);
+  const size_t M = static_cast<size_t>(B) * T;
+  const struct { float* dst; const float* src; size_t n; } cp[] = {
+      {queries, b.X, static_cast<size_t>(B) * kTok * kC}, {keys, b.keys32, M * kC},
+      {hyper, b.hyper, static_cast<size_t>(B) * 64}, {lowres, b.lr, M * 16 * 2}};
+  for (const auto& c : cp)
+    if (c.dst) SRB_CUDA_OK(cudaMemcpyAsync(c.dst, c.src, c.n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
 int sam_decoder_forward(const SamDecoderWeights& W, const float* emb_nchw, int B, int s, int P, void* ws,
                         float* mask_scores, float* mask_logits, cudaStream_t st) {
   const int T = s * s;

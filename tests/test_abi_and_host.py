@@ -45,6 +45,16 @@ def test_gemm_rejects_unknown_activation(act):
     assert rc != 0 and f"act={act}" in _lib.last_error()
 
 
+def test_sam_decoder_hook_rejects_null_handle():
+    # the handle is checked before any CUDA call, so this needs no GPU
+    lib = _lib.load()
+    out = ctypes.c_void_p(16)
+    assert lib.samroad_op_sam_decoder(None, out, 1, None, None, None, None, out, out, None) != 0
+    assert "null samroad handle" in _lib.last_error()
+    assert lib.samroad_op_sam_decoder(None, None, 0, None, None, None, None, None, None, None) != 0
+    assert "null samroad handle" in _lib.last_error()
+
+
 def test_cfg_struct_matches_header():
     src = open(os.path.join(ROOT, "include", "samroad_b200.h")).read()
     body = re.search(r"typedef struct SamRoadCfg \{(.*?)\} SamRoadCfg;", src, flags=re.S).group(1)
