@@ -23,6 +23,7 @@ int gemm_f16out(const __half* A, int lda, const __half* W, int ldw, int M, int N
               "gemm_f16out: act=%d must be 0 (none), 1 (GELU) or 2 (ReLU)", act);
   EpiF16::Params p{out, bias, ldo, act};
   SRB_REQUIRE(ldo % 8 == 0, "gemm_f16out: ldo=%d must be a multiple of 8", ldo);
+  SRB_REQUIRE(reinterpret_cast<uintptr_t>(out) % 16 == 0, "gemm_f16out: out must be 16-byte aligned");
   return launch_gemm_pp<EpiF16>(A, lda, W, ldw, M, N, K, p, st);
 }
 
@@ -102,3 +103,12 @@ int gemm_ref_simt(const __half* A, int lda, const __half* W, int ldw, int M, int
 }
 
 }  // namespace srb
+
+#ifdef SRB_GEMM_TRACE
+// Points the ping-pong kernel's phase trace at buf [ctas][tiles][kGemmTraceEvents] int64 (device memory), or off
+// with buf = null.  Only in the traced build of tools/gemm_trace.py, so not part of the C ABI.
+extern "C" int samroad_debug_gemm_trace(long long* buf, int ctas, int tiles) {
+  const srb::GemmTrace t{buf, ctas, tiles};
+  return cudaMemcpyToSymbol(srb::g_gemm_trace, &t, sizeof(t)) == cudaSuccess ? 0 : 1;
+}
+#endif

@@ -59,9 +59,9 @@ struct AccRow {
 // consumer warpgroup's 128x128 tile: d[h] is the m64n128 fragment of tile rows 64h .. 64h+63, so a
 // thread (warp w of the warpgroup, lane l) holds, per n8 block j, the two adjacent columns
 // 8j + 2(l&3) .. +1 of rows 16w + l/4 and 16w + l/4 + 8 of each half.  The four lanes of a quad
-// cover 32 contiguous bytes of an fp32 row (one sector) and 16 of an fp16 row; every output element
-// is read (residual) and written by the one thread that holds its accumulator, which keeps `out`
-// aliasing `resid` legal.
+// cover 32 contiguous bytes of an fp32 row (one sector) and 16 of an fp16 row.  In EpiF32 every output
+// element is read (residual) and written by the one thread that holds its accumulator, which keeps
+// `out` aliasing `resid` legal.
 // ------------------------------------------------------------------------------------------------
 struct FragPos {
   int r0;       // first of this thread's four rows r0, r0 + 8, r0 + 64, r0 + 72
@@ -81,6 +81,10 @@ struct FragPos {
 // consumer's mainloop).
 
 // Epilogue 1: out16[m,n] = act(acc + bias[n])                       (qkv, MLP lin1, TopoNet lin)
+// Per 32-column chunk and row, the quad's four lanes transpose their packed half2 pairs with two shuffles so that
+// lane t holds all eight columns of n8 block 4c + t: one 16-byte store per lane, 64 contiguous bytes per quad.
+// Stored straight from the fragment as 4-byte half2s (half-sector writes), the same output nearly doubled the
+// other consumer's TMA-fed mainloop at K = 768 (tools/gemm_trace.py, DESIGN.md).  Needs `out` 16-byte aligned.
 struct EpiF16 {
   struct Params {
     __half* out;          // [M, ldo]
@@ -96,22 +100,36 @@ struct EpiF16 {
       b[j] = make_float2(0.f, 0.f);
       if (p.bias && f.cols_in(32 * (j >> 2), N)) b[j] = __ldg(reinterpret_cast<const float2*>(p.bias + f.c0 + 8 * j));
     }
+    const int t = threadIdx.x & 3;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       if (!f.cols_in(32 * c, N)) continue;
+      const int n = f.n_tile + 8 * (4 * c + t);
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int j = 4 * c + jj;
-        const int n = f.c0 + 8 * j;
+      for (int q = 0; q < 4; ++q) {
+        uint32_t x[4];                         // x[u]: this lane's column pair of n8 block 4c + u
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float2 x = make_float2(d[q >> 1][4 * j + 2 * (q & 1)], d[q >> 1][4 * j + 2 * (q & 1) + 1]);
-          if (p.bias) { x.x += b[j].x; x.y += b[j].y; }
-          if (p.act == ACT_GELU) x = gelu_erf_fast2(x);
-          else if (p.act == ACT_RELU) x = make_float2(fmaxf(x.x, 0.0f), fmaxf(x.y, 0.0f));
-          const int m = f.row(q);
-          if (m < M) *reinterpret_cast<uint32_t*>(p.out + static_cast<size_t>(m) * p.ldo + n) = pack_half2(x.x, x.y);
+        for (int u = 0; u < 4; ++u) {
+          const int j = 4 * c + u;
+          float2 v = make_float2(d[q >> 1][4 * j + 2 * (q & 1)], d[q >> 1][4 * j + 2 * (q & 1) + 1]);
+          if (p.bias) { v.x += b[j].x; v.y += b[j].y; }
+          if (p.act == ACT_GELU) v = gelu_erf_fast2(v);
+          else if (p.act == ACT_RELU) v = make_float2(fmaxf(v.x, 0.0f), fmaxf(v.y, 0.0f));
+          x[u] = pack_half2(v.x, v.y);
         }
+        // 4x4 transpose across the quad: afterwards x[s] is lane s's column pair of n8 block 4c + t
+#pragma unroll
+        for (int k = 0; k < 4; k += 2) {
+          const uint32_t r = __shfl_xor_sync(0xffffffffu, (t & 1) ? x[k] : x[k + 1], 1);
+          if (t & 1) x[k] = r; else x[k + 1] = r;
+        }
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const uint32_t r = __shfl_xor_sync(0xffffffffu, (t & 2) ? x[k] : x[k + 2], 2);
+          if (t & 2) x[k] = r; else x[k + 2] = r;
+        }
+        const int m = f.row(q);
+        if (m < M) *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(m) * p.ldo + n) = make_uint4(x[0], x[1], x[2], x[3]);
       }
     }
   }
@@ -653,6 +671,28 @@ int launch_gemm_tc(const __half* A, int lda, const __half* W, int ldw, int M, in
 // before), so fill n - 1 of the slot is complete and fill n + 1 cannot start before this consumer
 // releases fill n: the slot's full barrier is exactly one phase from the waited parity, never two.
 // ------------------------------------------------------------------------------------------------
+// Phase trace (built only with -DSRB_GEMM_TRACE, by tools/gemm_trace.py): clock64 stamps per CTA and local tile i
+// into buf[(cta * tiles + i) * kGemmTraceEvents + event], CTAs < ctas and tiles < tiles only.  The consumer that
+// owns tile i stamps, from lane 0 of its first warp, TR_* events 0..5; the producer adds up the clocks it spent
+// waiting on empty_bar for the tile's k-blocks (TR_EMPTY_WAIT).
+enum { TR_ORDER_WAIT, TR_ORDER_DONE, TR_FIRST_FULL, TR_LAST_ISSUE, TR_DRAINED, TR_EPI_DONE, TR_EMPTY_WAIT,
+       kGemmTraceEvents = 8 };
+#ifdef SRB_GEMM_TRACE
+struct GemmTrace {
+  long long* buf;
+  int ctas, tiles;
+};
+static __device__ GemmTrace g_gemm_trace;
+__device__ __forceinline__ long long* gemm_trace_slot(int i) {
+  const GemmTrace t = g_gemm_trace;
+  if (t.buf == nullptr || static_cast<int>(blockIdx.x) >= t.ctas || i >= t.tiles) return nullptr;
+  return t.buf + (static_cast<size_t>(blockIdx.x) * t.tiles + i) * kGemmTraceEvents;
+}
+#define GEMM_TRACE(...) __VA_ARGS__
+#else
+#define GEMM_TRACE(...)
+#endif
+
 template <int STAGES>
 struct GemmPPSmem {
   static constexpr int kABytes = kGemmBM * kGemmBK * 2;
@@ -702,16 +742,21 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
+      GEMM_TRACE(int ti = 0);
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile / num_n, n_blk = tile % num_n;
+        GEMM_TRACE(long long stall = 0);
         for (int kb = 0; kb < num_k; ++kb) {
+          GEMM_TRACE(const long long t0 = clock64());
           mbar_wait(&empty_bar[stage], phase ^ 1u);
+          GEMM_TRACE(stall += clock64() - t0);
           uint8_t* sa = smem + stage * SM::kStageBytes;
           mbar_arrive_expect_tx(&full_bar[stage], SM::kStageBytes);
           tma_load_2d(sa, &tmA, &full_bar[stage], kb * kGemmBK, m_blk * kGemmBM);
           tma_load_2d(sa + SM::kABytes, &tmB, &full_bar[stage], kb * kGemmBK, n_blk * 128);
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
+        GEMM_TRACE(if (long long* t = gemm_trace_slot(ti++)) t[TR_EMPTY_WAIT] = stall);
       }
     }
   } else {
@@ -723,10 +768,13 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     int i = g;                                 // local tile index
     for (int tile = blockIdx.x + g * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, i += 2) {
       const int m_blk = tile / num_n, n_blk = tile % num_n;
+      GEMM_TRACE(long long* tr = w == 0 && lane == 0 ? gemm_trace_slot(i) : nullptr;
+                 if (tr) tr[TR_ORDER_WAIT] = clock64());
       if (i > 0) {                             // the other consumer has issued tile i - 1
         mbar_wait(&order_bar[g], order_phase);
         order_phase ^= 1u;
       }
+      GEMM_TRACE(if (tr) tr[TR_ORDER_DONE] = clock64());
       const int pos = i * num_k;
       int stage = pos % STAGES;
       uint32_t phase = static_cast<uint32_t>(pos / STAGES) & 1u;
@@ -738,6 +786,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       int prev = -1;
       for (int kb = 0; kb < num_k; ++kb) {
         mbar_wait(&full_bar[stage], phase);
+        GEMM_TRACE(if (tr && kb == 0) tr[TR_FIRST_FULL] = clock64());
         const uint32_t a_addr = smem_u32(smem + stage * SM::kStageBytes);
         const uint64_t adesc0 = wgmma_desc_k128(a_addr);
         const uint64_t adesc1 = wgmma_desc_k128(a_addr + 64 * kGemmBK * 2);
@@ -752,6 +801,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           wgmma_m64n128k16(d[1], adesc1 + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), acc);
         }
         wgmma_commit();
+        GEMM_TRACE(if (tr && kb == num_k - 1) tr[TR_LAST_ISSUE] = clock64());
         wgmma_wait<1>();                       // the previous k-block's MMAs have read their stage
         wgmma_fence_operand(d[0]);
         wgmma_fence_operand(d[1]);
@@ -763,8 +813,10 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_wait<0>();
       wgmma_fence_operand(d[0]);
       wgmma_fence_operand(d[1]);
+      GEMM_TRACE(if (tr) tr[TR_DRAINED] = clock64());
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
       Epi::run(ep, M, N, FragPos(m_blk * kGemmBM, n_blk * 128, w, lane), d);
+      GEMM_TRACE(if (tr) tr[TR_EPI_DONE] = clock64());
     }
   }
 }
