@@ -486,7 +486,8 @@ int samroad_abi_version(void);
 /* out16[M,N] = act(A[M,K] W[N,K]^T + bias)      act: 0 none, 1 GELU(erf), 2 ReLU; others are rejected */
 int samroad_op_gemm_f16(const void* A, int lda, const void* W, int ldw, int M, int N, int K,
                         const float* bias, int act, void* out16, int ldo, void* stream);
-/* out32[M,N] = A W^T + bias + resid + pos[m % pos_rows]   (bias/resid/pos may be NULL) */
+/* out32[M,N] = A W^T + bias + resid + pos[m % pos_rows]   (bias/resid/pos may be NULL; resid, [M, ldo], may be
+   out32; out32 and resid 16-byte aligned, ldo a multiple of 4 and >= N) */
 int samroad_op_gemm_f32(const void* A, int lda, const void* W, int ldw, int M, int N, int K,
                         const float* bias, const float* resid, const float* pos, int pos_rows,
                         float* out32, int ldo, void* stream);

@@ -149,6 +149,27 @@ int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t
   return 0;
 }
 
+int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems,
+                     uint32_t box_rows) {
+  PFN_encodeTiled fn = get_encode_fn();
+  SRB_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled driver entry point not available");
+  SRB_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15u) == 0, "TMA base %p not 16-byte aligned",
+              base);
+  SRB_REQUIRE((ld_elems * 4) % 16 == 0, "TMA row pitch %llu B not a multiple of 16",
+              (unsigned long long)(ld_elems * 4));
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstr[1] = {ld_elems * 4};
+  cuuint32_t box[2] = {32, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim, gstr, box,
+                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  SRB_REQUIRE(r == CUDA_SUCCESS,
+              "cuTensorMapEncodeTiled(f32) failed (%d) rows=%llu cols=%llu ld=%llu box=%ux32", (int)r,
+              (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld_elems, box_rows);
+  return 0;
+}
+
 int make_tmap_f16_4d(CUtensorMap* out, const void* base, const uint64_t dims[4],
                      const uint64_t strides_elems[3], const uint32_t box[4]) {
   PFN_encodeTiled fn = get_encode_fn();

@@ -258,6 +258,11 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, const void* 
                "r"(c3)
                : "memory");
 }
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() {
   asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
@@ -397,6 +402,10 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_
 // [box_rows][64 cols], 128B swizzle.  Out-of-bounds elements read as zero.
 int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                      uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols = 64);
+
+// 2D fp32 row-major tensor [rows][cols] (row pitch `ld` elements), box [box_rows][32 cols] (128 B), 128B swizzle.
+int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems,
+                     uint32_t box_rows);
 
 // 4D fp16 view [d3][d2][d1][d0] (d0 contiguous; strides in elements for d1..d3), box {b0,b1,b2,b3},
 // 128B swizzle (b0 * 2 bytes must be 128).  Out-of-bounds elements read as zero.

@@ -30,8 +30,20 @@ int gemm_f16out(const __half* A, int lda, const __half* W, int ldw, int M, int N
 int gemm_f32out(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
                 const float* bias, const float* resid, const float* pos, int pos_rows, float* out,
                 int ldo, cudaStream_t st) {
-  EpiF32::Params p{out, bias, resid, pos, ldo, pos_rows > 0 ? pos_rows : 1, N};
   SRB_REQUIRE(ldo % 4 == 0, "gemm_f32out: ldo=%d must be a multiple of 4", ldo);
+  SRB_REQUIRE(reinterpret_cast<uintptr_t>(out) % 16 == 0 && reinterpret_cast<uintptr_t>(resid) % 16 == 0,
+              "gemm_f32out: out and resid must be 16-byte aligned");
+  SRB_REQUIRE(N <= ldo, "gemm_f32out: N=%d wider than the output row pitch ldo=%d", N, ldo);
+  EpiF32::Params p;
+  memset(&p, 0, sizeof(p));
+  // TMA residual loads and stores of 16-row x 32-column boxes, staged 128B-swizzled (gemm_tc.cuh EpiF32)
+  if (int rc = make_tmap_f32_2d(&p.tm_out, out, M, N, ldo, 16)) return rc;
+  if (resid) { if (int rc = make_tmap_f32_2d(&p.tm_resid, resid, M, N, ldo, 16)) return rc; }
+  p.bias = bias;
+  p.resid = resid;
+  p.pos = pos;
+  p.pos_rows = pos_rows > 0 ? pos_rows : 1;
+  p.n_total = N;
   return launch_gemm_pp<EpiF32>(A, lda, W, ldw, M, N, K, p, st);
 }
 

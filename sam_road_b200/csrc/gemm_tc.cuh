@@ -75,31 +75,93 @@ struct FragPos {
   __device__ __forceinline__ bool cols_in(int col, int N) const { return n_tile + col < N; }
 };
 
-// Both epilogues load every operand of a chunk before they store an earlier one: the compiler may not
-// move a load above a store to `out`, which it must assume aliases the operand, and a load issued
-// after the stores costs one L2 round trip each (at K = 768 the epilogue then outlasts the other
-// consumer's mainloop).
+// Phase trace (built only with -DSRB_GEMM_TRACE, by tools/gemm_trace.py): clock64 stamps per CTA and local tile i
+// into buf[(cta * tiles + i) * kGemmTraceEvents + event], CTAs < ctas and tiles < tiles only.  The consumer that
+// owns tile i stamps, from lane 0 of its first warp, TR_* events 0..5 and the epilogue's sub-phases (TR_EPI_LOADED:
+// its first operands are in registers; TR_EPI_STAGED: the tile is packed into the staging buffer); the producer adds
+// up the clocks it spent waiting on empty_bar for the tile's k-blocks (TR_EMPTY_WAIT).  With -DSRB_GEMM_TRACE_NOSTORE
+// as well, the epilogues issue no global stores, which leaves the length of their loads and math (the values that
+// are not stored still feed TR_EPI_STAGED, so the compiler keeps their computation).
+enum { TR_ORDER_WAIT, TR_ORDER_DONE, TR_FIRST_FULL, TR_LAST_ISSUE, TR_DRAINED, TR_EPI_DONE, TR_EMPTY_WAIT,
+       TR_EPI_LOADED, TR_EPI_STAGED, kGemmTraceEvents = 10 };
+#ifdef SRB_GEMM_TRACE
+struct GemmTrace {
+  long long* buf;
+  int ctas, tiles;
+};
+static __device__ GemmTrace g_gemm_trace;
+__device__ __forceinline__ long long* gemm_trace_slot(int i) {
+  const GemmTrace t = g_gemm_trace;
+  if (t.buf == nullptr || static_cast<int>(blockIdx.x) >= t.ctas || i >= t.tiles) return nullptr;
+  return t.buf + (static_cast<size_t>(blockIdx.x) * t.tiles + i) * kGemmTraceEvents;
+}
+// Stamps `event` once `dep` (a value the phase produced) is in a register: the store of dep has to wait for it,
+// and the clock read is not moved above that store.
+__device__ __forceinline__ void gemm_trace_stamp(long long* tr, int event, float dep) {
+  if (tr == nullptr) return;
+  tr[kGemmTraceEvents - 1] = __float_as_int(dep);
+  long long t;
+  asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)::"memory");
+  tr[event] = t;
+}
+#define GEMM_TRACE(...) __VA_ARGS__
+#else
+#define GEMM_TRACE(...)
+#endif
+#if defined(SRB_GEMM_TRACE) && defined(SRB_GEMM_TRACE_NOSTORE)
+#define GEMM_STORE(...)
+#else
+#define GEMM_STORE(...) __VA_ARGS__
+#endif
+
+// Each epilogue gets its warp's part of the consumer's staging buffer (Epi::kStageBytes per consumer, a quarter
+// per warp; EpiF16 has none) and two mbarriers of the warp for loads into it.  Epi::prefetch runs on lane 0 of
+// each warp once the tile's first k-block is issued, Epi::run after the tile's last MMAs, Epi::drain at the end.
+// Operands read from global memory are loaded before the stores that the compiler must assume alias them: a load
+// issued after those stores costs one L2 round trip each, and at K = 768 the epilogue then outlasts the other
+// consumer's mainloop.
 
 // Epilogue 1: out16[m,n] = act(acc + bias[n])                       (qkv, MLP lin1, TopoNet lin)
 // Per 32-column chunk and row, the quad's four lanes transpose their packed half2 pairs with two shuffles so that
 // lane t holds all eight columns of n8 block 4c + t: one 16-byte store per lane, 64 contiguous bytes per quad.
 // Stored straight from the fragment as 4-byte half2s (half-sector writes), the same output nearly doubled the
 // other consumer's TMA-fed mainloop at K = 768 (tools/gemm_trace.py, DESIGN.md).  Needs `out` 16-byte aligned.
+// Bias and activation are template arguments of the tile loop: tested per column pair, each pair's add, activation,
+// pack and shuffles ran as a block of their own, back to back, and the epilogue outlasted the other consumer's
+// mainloop; as one branch-free block the compiler interleaves the independent pairs.
 struct EpiF16 {
+  static constexpr int kStageBytes = 0;
   struct Params {
     __half* out;          // [M, ldo]
     const float* bias;    // [N] or null
     int ldo;
     int act;
   };
-  static __device__ __forceinline__ void run(const Params& p, int M, int N, const FragPos& f,
-                                             float (&d)[2][64]) {
+  static __device__ __forceinline__ void prefetch(const Params&, int, int, int, int, uint8_t*, uint64_t*) {}
+  static __device__ __forceinline__ void run(const Params& p, int M, int N, const FragPos& f, float (&d)[2][64],
+                                             uint8_t* /*stage*/, uint64_t* /*bar*/, uint32_t (&)[2], long long* tr) {
     float2 b[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       b[j] = make_float2(0.f, 0.f);
       if (p.bias && f.cols_in(32 * (j >> 2), N)) b[j] = __ldg(reinterpret_cast<const float2*>(p.bias + f.c0 + 8 * j));
     }
+    GEMM_TRACE(float dep = 0.f; for (int j = 0; j < 16; ++j) dep += b[j].x + b[j].y;
+               gemm_trace_stamp(tr, TR_EPI_LOADED, dep));
+    if (p.bias) {
+      if (p.act == ACT_GELU) tile<true, ACT_GELU>(p, M, N, f, d, b, tr);
+      else if (p.act == ACT_RELU) tile<true, ACT_RELU>(p, M, N, f, d, b, tr);
+      else tile<true, ACT_NONE>(p, M, N, f, d, b, tr);
+    } else {
+      if (p.act == ACT_GELU) tile<false, ACT_GELU>(p, M, N, f, d, b, tr);
+      else if (p.act == ACT_RELU) tile<false, ACT_RELU>(p, M, N, f, d, b, tr);
+      else tile<false, ACT_NONE>(p, M, N, f, d, b, tr);
+    }
+  }
+  template <bool kBias, int kAct>
+  static __device__ __forceinline__ void tile(const Params& p, int M, int N, const FragPos& f, float (&d)[2][64],
+                                              const float2 (&b)[16], long long* tr) {
+    GEMM_TRACE(uint32_t sink = 0);             // every value the tile computes feeds the last stamp
     const int t = threadIdx.x & 3;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
@@ -112,9 +174,9 @@ struct EpiF16 {
         for (int u = 0; u < 4; ++u) {
           const int j = 4 * c + u;
           float2 v = make_float2(d[q >> 1][4 * j + 2 * (q & 1)], d[q >> 1][4 * j + 2 * (q & 1) + 1]);
-          if (p.bias) { v.x += b[j].x; v.y += b[j].y; }
-          if (p.act == ACT_GELU) v = gelu_erf_fast2(v);
-          else if (p.act == ACT_RELU) v = make_float2(fmaxf(v.x, 0.0f), fmaxf(v.y, 0.0f));
+          if (kBias) { v.x += b[j].x; v.y += b[j].y; }
+          if (kAct == ACT_GELU) v = gelu_erf_fast2(v);
+          else if (kAct == ACT_RELU) v = make_float2(fmaxf(v.x, 0.0f), fmaxf(v.y, 0.0f));
           x[u] = pack_half2(v.x, v.y);
         }
         // 4x4 transpose across the quad: afterwards x[s] is lane s's column pair of n8 block 4c + t
@@ -129,54 +191,81 @@ struct EpiF16 {
           if (t & 2) x[k] = r; else x[k + 2] = r;
         }
         const int m = f.row(q);
-        if (m < M) *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(m) * p.ldo + n) = make_uint4(x[0], x[1], x[2], x[3]);
+        GEMM_STORE(if (m < M) *reinterpret_cast<uint4*>(p.out + static_cast<size_t>(m) * p.ldo + n) = make_uint4(x[0], x[1], x[2], x[3]));
+        GEMM_TRACE(sink ^= x[0] ^ x[1] ^ x[2] ^ x[3];
+                   if (c == 3 && q == 3) gemm_trace_stamp(tr, TR_EPI_STAGED, __uint_as_float(sink)));
       }
     }
   }
+  static __device__ __forceinline__ void drain(int /*lane*/) {}
 };
 
 // Epilogue 2: out32[m,n] = acc + resid[m,n] + bias[n] + pos[m % pos_rows, n]
 //             (patch-embed + pos_embed, attention proj + shortcut, MLP lin2 + shortcut; plain f32)
-// fp32 in/out makes this epilogue HBM-bound for short K (attention proj): the residual of 16-column
-// chunk c+1 is loaded into registers before chunk c is stored (it never touches an element chunk c
-// stores).  Bias and pos-embed (L1- / L2-resident) are loaded when their chunk starts, all before its
-// first store.  (Double-buffering pos-embed too spills next to the 128 accumulators.)
+// fp32 in/out makes this epilogue HBM-bound for short K (attention proj).  Each warp works in slabs of 32
+// columns of its 32 rows (16 of each 64-row half), through its 8 KB of the staging buffer: two 4 KB slab buffers
+// used in turn, each two 16-row x 32-column boxes (half h at 2 KB * h), 128B-swizzled (16-byte chunk k of row r
+// at k ^ (r & 7)).  The residual of a slab arrives in its buffer by TMA: slabs 0 and 1 are requested while the
+// tile's mainloop runs (prefetch), slab s + 2 as soon as the stores of slab s have read the buffer.  Each thread
+// reads the residual of its accumulator's element from the buffer and writes the sum back to the same place;
+// lane 0 then stores the slab with TMA through the output map (N x M, row pitch ldo), which clips the M tail and
+// the columns >= N.  A slab's residual has been read before the slab is stored, and the tiles of a launch do not
+// overlap, so `out` may alias `resid`.  Bias and pos-embed (L1- / L2-resident) are loaded per 16-column chunk.
 struct EpiF32 {
+  static constexpr int kStageBytes = 4 * 8192;
   struct Params {
-    float* out;           // [M, ldo]
+    CUtensorMap tm_out;   // [M, N] fp32, row pitch ldo; box 32 columns x 16 rows, 128B swizzle
+    CUtensorMap tm_resid; // the same for resid, when there is one
     const float* bias;    // [N] or null
-    const float* resid;   // [M, ldo] or null (may alias out)
+    const float* resid;   // [M, ldo] or null (may alias the output)
     const float* pos;     // [pos_rows, N] or null
-    int ldo;
     int pos_rows;
     int n_total;
   };
-  // residuals of n8 blocks 2c + jj, jj = 0, 1: r[4 * jj + q] for row pair q
-  static __device__ __forceinline__ void load_resid(const Params& p, int M, int N, const FragPos& f, int c,
-                                                    float2 (&r)[8]) {
-    const bool in_n = f.cols_in(16 * c, N);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int m = f.row(i & 3);
-      r[i] = make_float2(0.f, 0.f);
-      if (p.resid && in_n && m < M)
-        r[i] = *reinterpret_cast<const float2*>(p.resid + static_cast<size_t>(m) * p.ldo + f.c0 + 8 * (2 * c + (i >> 2)));
-    }
+  // residual of slab s of the warp's rows (row0 .. +15 and row0 + 64 .. +15) into slab buffer s & 1, completing on
+  // bar[s & 1]; a box wholly below M is not loaded (its rows are not stored), and with neither box the arrive
+  // alone completes the barrier's phase.  One thread.
+  static __device__ __forceinline__ void load_slab(const Params& p, int M, int N, int n_tile, int row0, int s,
+                                                   uint8_t* stage, uint64_t* bar) {
+    if (n_tile + 32 * s >= N) return;
+    const int boxes = (row0 < M) + (row0 + 64 < M);
+    mbar_arrive_expect_tx(&bar[s & 1], 2048 * boxes);
+    for (int h = 0; h < boxes; ++h)
+      tma_load_2d(stage + 4096 * (s & 1) + 2048 * h, &p.tm_resid, &bar[s & 1], n_tile + 32 * s, row0 + 64 * h);
   }
-  static __device__ __forceinline__ void run(const Params& p, int M, int N, const FragPos& f,
-                                             float (&d)[2][64]) {
+  // Called by lane 0 of each warp once the tile's first k-block is issued: the buffers are free when the stores of
+  // the warp's previous tile have read them.
+  static __device__ __forceinline__ void prefetch(const Params& p, int M, int N, int n_tile, int row0, uint8_t* stage,
+                                                  uint64_t* bar) {
+    if (p.resid == nullptr) return;
+    bulk_wait_group_read<0>();
+    load_slab(p, M, N, n_tile, row0, 0, stage, bar);
+    load_slab(p, M, N, n_tile, row0, 1, stage, bar);
+  }
+  static __device__ __forceinline__ void run(const Params& p, int M, int N, const FragPos& f, float (&d)[2][64],
+                                             uint8_t* stage, uint64_t* bar, uint32_t (&bar_phase)[2], long long* tr) {
+    const int lane = threadIdx.x & 31;
+    const int row0 = f.r0 - (lane >> 2);         // the first of the warp's 16 rows in half 0
     int pos_row[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) pos_row[q] = p.pos ? f.row(q) % p.pos_rows : 0;
-    float2 nxt[8];
-    load_resid(p, M, N, f, 0, nxt);
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
-      float2 cur[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) cur[i] = nxt[i];
-      if (c + 1 < 8) load_resid(p, M, N, f, c + 1, nxt);
       if (!f.cols_in(16 * c, N)) continue;
+      float* slab = reinterpret_cast<float*>(stage + 4096 * ((c >> 1) & 1));
+      if ((c & 1) == 0) {
+        if (p.resid) {                           // the slab's residual has arrived
+          mbar_wait(&bar[(c >> 1) & 1], bar_phase[(c >> 1) & 1]);
+          bar_phase[(c >> 1) & 1] ^= 1u;
+        } else {                                 // the stores of the slab before last (at c = 0: of the previous
+          if (lane == 0) {                       // tile) have read the buffer
+            if (c == 0) bulk_wait_group_read<0>();
+            else bulk_wait_group_read<1>();
+          }
+          __syncwarp();
+        }
+        GEMM_TRACE(if (c == 0) gemm_trace_stamp(tr, TR_EPI_LOADED, slab[0]));
+      }
       float2 b[2], e[8];
 #pragma unroll
       for (int jj = 0; jj < 2; ++jj) {
@@ -190,19 +279,40 @@ struct EpiF32 {
       }
 #pragma unroll
       for (int jj = 0; jj < 2; ++jj) {
-        const int n = f.c0 + 8 * (2 * c + jj);
         const int j = 2 * c + jj;
+        // 16-byte chunk of this lane's column pair inside the slab row, and the pair's half of it
+        const int k = 4 * (c & 1) + 2 * jj + ((lane & 3) >> 1);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const int m = f.row(q);
-          const float2 r = cur[4 * jj + q];
+          const int row = (lane >> 2) + 8 * (q & 1);
+          float2* at = reinterpret_cast<float2*>(slab + 512 * (q >> 1) + 32 * row + 4 * (k ^ (row & 7)) + 2 * (lane & 1));
+          const float2 r = p.resid ? *at : make_float2(0.f, 0.f);
           float2 x = make_float2(d[q >> 1][4 * j + 2 * (q & 1)] + r.x, d[q >> 1][4 * j + 2 * (q & 1) + 1] + r.y);
           if (p.bias) { x.x += b[jj].x; x.y += b[jj].y; }
           if (p.pos) { x.x += e[4 * jj + q].x; x.y += e[4 * jj + q].y; }
-          if (m < M) *reinterpret_cast<float2*>(p.out + static_cast<size_t>(m) * p.ldo + n) = x;
+          *at = x;
+        }
+      }
+      if (c & 1) {                               // the slab is complete (N is a multiple of 32)
+        fence_proxy_async_smem();                // the slab's writes are visible to the TMA unit
+        __syncwarp();
+        GEMM_TRACE(if (c == 7) gemm_trace_stamp(tr, TR_EPI_STAGED, 0.f));
+        if (lane == 0) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (row0 + 64 * h < M)
+              GEMM_STORE(tma_store_2d(&p.tm_out, slab + 512 * h, f.n_tile + 32 * (c >> 1), row0 + 64 * h));
+          bulk_commit_group();
+          if (c < 4 && p.resid) {                // slab c/2 + 2 reuses this buffer once the stores have read it
+            bulk_wait_group_read<0>();
+            load_slab(p, M, N, f.n_tile, row0, (c >> 1) + 2, stage, bar);
+          }
         }
       }
     }
+  }
+  static __device__ __forceinline__ void drain(int lane) {
+    if (lane == 0) bulk_wait_group<0>();
   }
 };
 
@@ -658,7 +768,7 @@ int launch_gemm_tc(const __half* A, int lda, const __half* W, int ldw, int M, in
 // tiles: two wgmma m64n128k16 per k16 step, 2 x 64 fp32 accumulators per thread.  The CTA's tiles
 // t0, t1, t2, ... alternate between the consumers (t0, t2, ... and t1, t3, ...), and an ordering
 // mbarrier pair starts a consumer's mainloop when the other's has issued its last MMAs, so one
-// warpgroup is on the tensor cores while the other runs its epilogue from registers.  The ring
+// warpgroup is on the tensor cores while the other runs its epilogue (EpiF32 through its own staging buffer).  The ring
 // holds operands only; the producer never waits for an epilogue.
 //
 // Ring bookkeeping.  The producer fills ring positions p = 0, 1, 2, ... in CTA tile order: local
@@ -671,42 +781,25 @@ int launch_gemm_tc(const __half* A, int lda, const __half* W, int ldw, int M, in
 // before), so fill n - 1 of the slot is complete and fill n + 1 cannot start before this consumer
 // releases fill n: the slot's full barrier is exactly one phase from the waited parity, never two.
 // ------------------------------------------------------------------------------------------------
-// Phase trace (built only with -DSRB_GEMM_TRACE, by tools/gemm_trace.py): clock64 stamps per CTA and local tile i
-// into buf[(cta * tiles + i) * kGemmTraceEvents + event], CTAs < ctas and tiles < tiles only.  The consumer that
-// owns tile i stamps, from lane 0 of its first warp, TR_* events 0..5; the producer adds up the clocks it spent
-// waiting on empty_bar for the tile's k-blocks (TR_EMPTY_WAIT).
-enum { TR_ORDER_WAIT, TR_ORDER_DONE, TR_FIRST_FULL, TR_LAST_ISSUE, TR_DRAINED, TR_EPI_DONE, TR_EMPTY_WAIT,
-       kGemmTraceEvents = 8 };
-#ifdef SRB_GEMM_TRACE
-struct GemmTrace {
-  long long* buf;
-  int ctas, tiles;
-};
-static __device__ GemmTrace g_gemm_trace;
-__device__ __forceinline__ long long* gemm_trace_slot(int i) {
-  const GemmTrace t = g_gemm_trace;
-  if (t.buf == nullptr || static_cast<int>(blockIdx.x) >= t.ctas || i >= t.tiles) return nullptr;
-  return t.buf + (static_cast<size_t>(blockIdx.x) * t.tiles + i) * kGemmTraceEvents;
-}
-#define GEMM_TRACE(...) __VA_ARGS__
-#else
-#define GEMM_TRACE(...)
-#endif
-
-template <int STAGES>
+// Shared memory: the operand ring, then each consumer's epilogue staging buffer (kEpiBytes, 1024-aligned for the
+// 128B swizzle), then the barriers.
+template <int STAGES, int kEpiBytes>
 struct GemmPPSmem {
   static constexpr int kABytes = kGemmBM * kGemmBK * 2;
   static constexpr int kBBytes = 128 * kGemmBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kBarOffset = STAGES * kStageBytes;
+  static constexpr int kEpiOffset = STAGES * kStageBytes;
+  static constexpr int kBarOffset = kEpiOffset + 2 * kEpiBytes;
   static constexpr int kTotal = kBarOffset + 256 + 1024;
+  static_assert(kTotal <= 227 * 1024, "gemm_pp_kernel: shared memory over the 227 KB an H100 block may use");
+  static_assert((2 * STAGES + 2 + 16) * 8 <= 256, "gemm_pp_kernel: barriers (full, empty, order, staging) over 256 B");
 };
 
 template <int STAGES, class Epi>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                int M, int N, int K, const __grid_constant__ typename Epi::Params ep) {
-  using SM = GemmPPSmem<STAGES>;
+  using SM = GemmPPSmem<STAGES, Epi::kStageBytes>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
@@ -714,6 +807,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* order_bar = empty_bar + STAGES;       // [g]: the other consumer has issued its mainloop
+  uint64_t* stage_bar = order_bar + 2;            // [4g + w][2]: loads into warp w's staging buffers (EpiF32)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -732,6 +826,8 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     mbar_init(&order_bar[0], 4);
     mbar_init(&order_bar[1], 4);
+    if (Epi::kStageBytes > 0)
+      for (int i = 0; i < 16; ++i) mbar_init(&stage_bar[i], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -764,11 +860,14 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     setmaxnreg_inc<232>();
     const int g = wg - 1;
     const int w = warp & 3;
-    uint32_t order_phase = 0;
+    uint8_t* staging = smem + SM::kEpiOffset + g * Epi::kStageBytes + w * (Epi::kStageBytes / 4);
+    uint64_t* bar = stage_bar + 2 * (4 * g + w);
+    uint32_t order_phase = 0, bar_phase[2] = {0u, 0u};
     int i = g;                                 // local tile index
     for (int tile = blockIdx.x + g * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, i += 2) {
       const int m_blk = tile / num_n, n_blk = tile % num_n;
-      GEMM_TRACE(long long* tr = w == 0 && lane == 0 ? gemm_trace_slot(i) : nullptr;
+      long long* tr = nullptr;
+      GEMM_TRACE(if (w == 0 && lane == 0) tr = gemm_trace_slot(i);
                  if (tr) tr[TR_ORDER_WAIT] = clock64());
       if (i > 0) {                             // the other consumer has issued tile i - 1
         mbar_wait(&order_bar[g], order_phase);
@@ -802,6 +901,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         wgmma_commit();
         GEMM_TRACE(if (tr && kb == num_k - 1) tr[TR_LAST_ISSUE] = clock64());
+        if (kb == 0 && lane == 0) Epi::prefetch(ep, M, N, n_blk * 128, m_blk * kGemmBM + 16 * w, staging, bar);
         wgmma_wait<1>();                       // the previous k-block's MMAs have read their stage
         wgmma_fence_operand(d[0]);
         wgmma_fence_operand(d[1]);
@@ -815,9 +915,10 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_fence_operand(d[1]);
       GEMM_TRACE(if (tr) tr[TR_DRAINED] = clock64());
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      Epi::run(ep, M, N, FragPos(m_blk * kGemmBM, n_blk * 128, w, lane), d);
+      Epi::run(ep, M, N, FragPos(m_blk * kGemmBM, n_blk * 128, w, lane), d, staging, bar, bar_phase, tr);
       GEMM_TRACE(if (tr) tr[TR_EPI_DONE] = clock64());
     }
+    Epi::drain(lane);
   }
 }
 
@@ -825,7 +926,7 @@ template <class Epi>
 int launch_gemm_pp(const __half* A, int lda, const __half* W, int ldw, int M, int N, int K,
                    const typename Epi::Params& ep, cudaStream_t stream) {
   constexpr int kStages = 5;
-  using SM = GemmPPSmem<kStages>;
+  using SM = GemmPPSmem<kStages, Epi::kStageBytes>;
   SRB_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
   SRB_REQUIRE(N % 32 == 0, "gemm: N=%d must be a multiple of 32", N);
   SRB_REQUIRE(K % 8 == 0 && lda % 8 == 0 && ldw % 8 == 0,

@@ -1,6 +1,6 @@
-"""Per-tile phase trace of the ping-pong GEMM (`gemm_pp_kernel`) at the c2 encoder shapes.
+"""Per-tile phase trace of the ping-pong GEMM (`gemm_pp_kernel`) at the c2 and c5 encoder shapes.
 
-    python tools/gemm_trace.py [--lib PATH] [--shapes c2_qkv,c2_lin1] [--out FILE]
+    python tools/gemm_trace.py [--lib PATH] [--no-store] [--shapes c2_qkv,c2_lin1] [--out FILE]
 
 The trace is compiled in only with -DSRB_GEMM_TRACE.  Without --lib, this tool compiles gemm_ops.cu with it into a
 temporary directory and links it with the other objects of this tree's build (`python -m sam_road_b200.build`
@@ -12,11 +12,17 @@ tiles:
                 tensor-core time of 8 wgmma m64n128k16 per k-block at 4096 FLOP per clock)
   first_full    order_bar passed -> first full_bar wait passed (the tile's first stage not yet loaded)
   drain         last MMAs issued -> wgmma_wait<0> returned
-  epilogue      wgmma_wait<0> returned -> last store of the epilogue issued
+  epilogue      wgmma_wait<0> returned -> last store of the epilogue issued, in three parts:
+    epi_loads   wgmma_wait<0> returned -> the epilogue's first operands (bias, residual) in registers
+    epi_math    -> the tile's last values computed and packed (staged in shared memory, where it is)
+    epi_stores  -> last store issued
   order_wait    epilogue done -> the other consumer has issued its mainloop (this consumer idles)
   tensor_idle   max(0, first MMA of tile i - tile i-1's MMAs complete): tensor cores idle at the handoff
   producer_stall  clocks the producer waited on empty_bar for the tile's k-blocks
   period        between the last MMA issues of consecutive tiles of a CTA (the CTA's time per tile)
+
+With --no-store the library is built with -DSRB_GEMM_TRACE_NOSTORE as well: the epilogues compute everything but
+issue no global stores (the output is not written), which gives the length of their loads and math alone.
 """
 from __future__ import annotations
 
@@ -37,18 +43,19 @@ from tools.attention_bench import card_info, load_lib  # noqa: E402
 from tools.gemm_bench import POS_ROWS, SHAPES  # noqa: E402
 
 DEV = "cuda:0"
-EVENTS = 8                     # kGemmTraceEvents
-ORDER_WAIT, ORDER_DONE, FIRST_FULL, LAST_ISSUE, DRAINED, EPI_DONE, EMPTY_WAIT = range(7)
+EVENTS = 10                    # kGemmTraceEvents
+ORDER_WAIT, ORDER_DONE, FIRST_FULL, LAST_ISSUE, DRAINED, EPI_DONE, EMPTY_WAIT, EPI_LOADED, EPI_STAGED = range(9)
 MAX_TILES = 128                # local tiles traced per CTA
 
 
-def build_traced(out_dir):
+def build_traced(out_dir, no_store=False):
     """gemm_ops.cu with -DSRB_GEMM_TRACE, linked with the tree's other objects, as out_dir/libsamroad_b200_trace.so."""
     B.build()
     nvcc = B._nvcc()
     obj = os.path.join(out_dir, "gemm_ops_trace.o")
     lib = os.path.join(out_dir, "libsamroad_b200_trace.so")
-    subprocess.run([nvcc, *B.NVCC_FLAGS, "-DSRB_GEMM_TRACE", "-c", str(B.CSRC / "gemm_ops.cu"), "-o", obj], check=True)
+    defs = ["-DSRB_GEMM_TRACE"] + (["-DSRB_GEMM_TRACE_NOSTORE"] if no_store else [])
+    subprocess.run([nvcc, *B.NVCC_FLAGS, *defs, "-c", str(B.CSRC / "gemm_ops.cu"), "-o", obj], check=True)
     objs = [obj if s == "gemm_ops.cu" else str(B.OBJ_DIR / (s + ".o")) for s in B.SOURCES]
     subprocess.run([nvcc, "-shared", "-o", lib, *objs, "-lcudart"], check=True)
     return lib
@@ -61,8 +68,8 @@ def median(xs):
 
 def phases(tr, num_k):
     """Medians of the phase durations over tr [ctas, tiles, EVENTS] (int64 clocks, zero = not reached)."""
-    q = {k: [] for k in ("mainloop", "first_full", "drain", "epilogue", "order_wait", "tensor_idle",
-                         "producer_stall", "period")}
+    q = {k: [] for k in ("mainloop", "first_full", "drain", "epilogue", "epi_loads", "epi_math", "epi_stores",
+                         "order_wait", "tensor_idle", "producer_stall", "period")}
     for cta in tr.tolist():
         n = sum(1 for t in cta if t[EPI_DONE] != 0)
         for i in range(n):
@@ -71,6 +78,9 @@ def phases(tr, num_k):
             q["first_full"].append(t[FIRST_FULL] - t[ORDER_DONE])
             q["drain"].append(t[DRAINED] - t[LAST_ISSUE])
             q["epilogue"].append(t[EPI_DONE] - t[DRAINED])
+            q["epi_loads"].append(t[EPI_LOADED] - t[DRAINED])
+            q["epi_math"].append(t[EPI_STAGED] - t[EPI_LOADED])
+            q["epi_stores"].append(t[EPI_DONE] - t[EPI_STAGED])
             q["producer_stall"].append(t[EMPTY_WAIT])
             if i >= 1:
                 p = cta[i - 1]
@@ -87,20 +97,21 @@ def phases(tr, num_k):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=None, help="a library built with -DSRB_GEMM_TRACE (default: build one)")
-    ap.add_argument("--shapes", default="c2_qkv,c2_proj,c2_lin1,c2_lin2,c2_patch_embed")
+    ap.add_argument("--no-store", action="store_true", help="build without the epilogues' global stores")
+    ap.add_argument("--shapes", default="c2_qkv,c2_proj,c2_lin1,c2_lin2,c2_patch_embed,c5_qkv,c5_lin1")
     ap.add_argument("--out", default=None, help="write the results as JSON to this file")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "gemm_trace needs a CUDA device"
 
     with tempfile.TemporaryDirectory() as tmp:
-        path = args.lib or build_traced(tmp)
+        path = args.lib or build_traced(tmp, args.no_store)
         lib = load_lib(path)
         lib.samroad_debug_gemm_trace.restype = C.c_int
         lib.samroad_debug_gemm_trace.argtypes = [C.c_void_p, C.c_int, C.c_int]
         st = torch.cuda.current_stream().cuda_stream
         ctas = torch.cuda.get_device_properties(0).multi_processor_count
         buf = torch.zeros(ctas, MAX_TILES, EVENTS, dtype=torch.int64, device=DEV)
-        result = {"card": card_info(), "lib": args.lib, "unit": "SM clocks", "shapes": {}}
+        result = {"card": card_info(), "lib": args.lib, "no_store": args.no_store, "unit": "SM clocks", "shapes": {}}
         wanted = args.shapes.split(",")
         for name, M, N, K, epi in SHAPES:
             if name not in wanted:
