@@ -13,7 +13,8 @@ rot90, box query, NMS, source sampling, kNN, BFS labels, point transform and col
         loss = net.training_step(batch, i)
 
 Randomness is Philox on the device keyed by a 62-bit seed drawn from torch's default generator per
-batch, so torch.manual_seed reproduces a batch bit for bit.  NumPy's streams are not reproduced.
+batch, so torch.manual_seed reproduces a batch bit for bit.  NumPy's streams are not reproduced.  Under
+torch.distributed the drawn seed is made per rank and each rank's loader serves its share (BatchLoader).
 """
 from __future__ import annotations
 
@@ -340,7 +341,8 @@ class LabelScenes:
         """One collated batch of B patches (dict of device tensors, graph_collate_fn's layout).  patches: [B,4]
         int32 (scene, x0, y0, rot) or None to draw them; seed: 62-bit Philox key (None: from torch's default
         generator).  Test hooks: draws = {"patches", "score_u", "source_u", "noise"} arrays are used instead of
-        drawing; export_draws=True draws everything and returns (batch, draws)."""
+        drawing; export_draws=True draws everything and returns (batch, draws).  A drawn seed is made per rank
+        under torch.distributed (ranks.rank_seed; rank 0 keeps it)."""
         import torch
         from . import _lib
         lc, dev = self.lc, self.device
@@ -359,7 +361,8 @@ class LabelScenes:
         want = {"patches": ((B, 4), torch.int32), "score_u": ((B, self.cap), torch.float64),
                 "source_u": ((B, S), torch.float64), "noise": ((B, self.cap, 2), torch.float64)}
         if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (), dtype=torch.int64).item())
+            from .ranks import draw_seed
+            seed = draw_seed()
         seed = int(seed) & 0xFFFFFFFFFFFFFFFF
         lib = _lib.load()
         with torch.cuda.device(dev):
@@ -459,8 +462,13 @@ class SatMapDataset:
 
     def patches(self, first: int, count: int) -> np.ndarray:
         """[count, 4] int32 (scene, x0, y0, rot 0) of eval patches first .. first + count - 1."""
-        out = np.zeros((count, 4), dtype=np.int32)
-        for k, (img, (x0, y0), _) in enumerate(self.eval_patches[first:first + count]):
+        return self.patches_at(range(first, first + count))
+
+    def patches_at(self, indices) -> np.ndarray:
+        """[len(indices), 4] int32 (scene, x0, y0, rot 0) of the eval patches at `indices`."""
+        out = np.zeros((len(indices), 4), dtype=np.int32)
+        for k, i in enumerate(indices):
+            img, (x0, y0), _ = self.eval_patches[i]
             out[k, :3] = (img, x0, y0)
         return out
 
@@ -474,19 +482,46 @@ class SatMapDataset:
         return BatchLoader(self, batch_size)
 
 
+def eval_shard(n: int, rank: int, world: int) -> np.ndarray:
+    """Indices of rank `rank` of `world` into n samples, as DistributedSampler(shuffle=False, drop_last=False)
+    gives them: the list 0 .. n-1 is padded to ceil(n / world) * world by repeating it from its start, and the
+    rank takes every world-th index from `rank` on."""
+    if not 0 <= rank < world:
+        raise ValueError(f"rank {rank} is not in [0, {world})")
+    per_rank = -(-n // world)
+    return np.resize(np.arange(n, dtype=np.int64), per_rank * world)[rank::world]
+
+
 class BatchLoader:
-    """Re-iterable batches of a SatMapDataset, already collated on the device.  len() is ceil(len(ds) / B); the
-    last batch is short when B does not divide len(ds), as DataLoader(drop_last=False) makes it."""
+    """Re-iterable batches of a SatMapDataset, already collated on the device.  The last batch is short when B
+    does not divide the sample count, as DataLoader(drop_last=False) makes it.
+
+    In one process len() is ceil(len(ds) / B).  Under torch.distributed each rank gets what Lightning's
+    DistributedSampler would give it: ceil(len(ds) / world) samples, so len() is ceil(ceil(len(ds) / world) / B);
+    evaluation takes this rank's eval_shard of the patch list, in order; training draws its own patches (the
+    seeds differ per rank, LabelScenes.batch)."""
 
     def __init__(self, ds: SatMapDataset, batch_size: int):
         if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size < 1:
             raise ValueError(f"batch_size must be a positive integer (got {batch_size!r})")
         self.ds, self.batch_size = ds, int(batch_size)
 
+    def _samples(self) -> int:
+        from .ranks import rank_and_world
+        return -(-len(self.ds) // rank_and_world()[1])
+
     def __len__(self):
-        return (len(self.ds) + self.batch_size - 1) // self.batch_size
+        return (self._samples() + self.batch_size - 1) // self.batch_size
 
     def __iter__(self):
-        n = len(self.ds)
-        for first in range(0, n, self.batch_size):
-            yield self.ds.batch(min(self.batch_size, n - first), first)
+        from .ranks import rank_and_world
+        B = self.batch_size
+        if self.ds.is_train:
+            n = self._samples()
+            for first in range(0, n, B):
+                yield self.ds.batch(min(B, n - first))
+            return
+        idx = eval_shard(len(self.ds), *rank_and_world())
+        for first in range(0, len(idx), B):
+            rows = self.ds.patches_at(idx[first:first + B])
+            yield self.ds._scenes.batch(rows.shape[0], patches=rows)

@@ -490,13 +490,22 @@ class SAMRoad(_Base):
                 p.requires_grad_(True)
             self._training_enabled = True
 
+    def setup(self, stage: Optional[str] = None) -> None:
+        """Lightning's setup hook, which runs before its DDP strategy wraps the module: for stage "fit" the head
+        parameters start requiring grad here, since DistributedDataParallel only reduces (and only accepts a
+        module with) parameters that require grad at wrap time.  Unsupported configurations raise here."""
+        if stage == "fit":
+            self._enable_training()
+
     def training_step(self, batch, batch_idx):
         """model.py:511-544 for FREEZE_ENCODER: True with the naive decoder: the encoder as the inference calls run
         it, then the map decoder and TopoNet (dropout 0.1 at torch's four sites when self.training) on the device,
         mask loss (BCEWithLogitsLoss, or sigmoid_focal_loss with FOCAL_LOSS) + the valid-slot topology BCE.  Returns
         the 0-dim fp32 loss, differentiable with respect to the map_decoder.* and topo_net.* parameters; its
         backward writes their .grad on the device (DESIGN.md §12).  Other configurations raise NotImplementedError
-        before the batch is read.  The dropout seed is drawn from torch's default generator."""
+        before the batch is read.  The dropout seed is drawn from torch's default generator and, under
+        torch.distributed, made per rank (ranks.rank_seed; rank 0 keeps it).  Wrapped in DistributedDataParallel
+        (after setup("fit")), DDP's averaged gradients land in the heads' .grad."""
         from . import train as T
         self._enable_training()
         heads = self._head_params()
@@ -506,7 +515,8 @@ class SAMRoad(_Base):
         b = T.validate_batch(batch, self.image_size, dev)
         h = self._handle(dev)
         dropout_p = 0.1 if self.training else 0.0
-        seed = int(torch.randint(0, 2 ** 62, (), dtype=torch.int64).item()) if dropout_p > 0 else 0
+        from .ranks import draw_seed
+        seed = draw_seed() if dropout_p > 0 else 0
         args = T.make_args(b, self.focal_loss, dropout_p, seed)
         mask_loss, topo_loss = T.head_losses(h, b, args, [k for k, _ in heads], [p for _, p in heads])
         loss = mask_loss + topo_loss

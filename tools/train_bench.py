@@ -8,12 +8,21 @@ Phases (CUDA events, each ends in a synchronise): encoder (samroad_encode_masks,
 with the card name and power limit.
 
     python tools/train_bench.py [--rounds 3] [--batch 16]
+
+With --gpus N, run under torchrun on N GPUs of one box: DDP training of the heads (NCCL) as Lightning's DDP strategy
+runs it, at the same workload per rank, with batches from each rank's SatMapDataset loader over synthetic
+2048^2 cityscale scenes (a street grid every 48 pixels), then one sharded validation epoch of the test split
+(dev_run: 4 scenes, 64 patches of 512^2).  Rank 0 prints one JSON object: the step time of every rank, the
+aggregate training samples/s (world x B x steps over the slowest rank's wall time) and the validation epoch time.
+
+    torchrun --nproc_per_node N tools/train_bench.py --gpus N [--steps 20] [--warmup 3]
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import time
 
 import torch
 
@@ -32,11 +41,117 @@ def _card():
         return f"unknown ({e})"
 
 
+class _StepModule(torch.nn.Module):
+    """What Lightning's DDP strategy wraps: a module whose forward is the LightningModule's training_step."""
+
+    def __init__(self, net):
+        super().__init__()
+        self.module = net
+
+    def forward(self, batch, batch_idx):
+        return self.module.training_step(batch, batch_idx)
+
+
+def ddp_main(a):
+    """--gpus N: one process per GPU, started by torchrun."""
+    import shutil
+    import tempfile
+    import torch.distributed as dist
+    from sam_road_b200 import dataset as D
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    rank, local = int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0"))
+    if world != a.gpus:
+        sys.exit(f"train_bench --gpus {a.gpus}: start it with torchrun --nproc_per_node {a.gpus} "
+                 f"(WORLD_SIZE is {world})")
+    B, P, Ns, Np = a.batch, 512, 512, 16
+    cfg = dict(DATASET="cityscale", SAM_VERSION="vit_b", PATCH_SIZE=P, TOPO_SAMPLE_NUM=Ns, MAX_NEIGHBOR_QUERIES=Np,
+               NEIGHBOR_RADIUS=64, ROAD_NMS_RADIUS=16, FREEZE_ENCODER=True, BASE_LR=1e-4, TOPONET_VERSION="normal",
+               FOCAL_LOSS=False)
+    if a.steps < 1 or a.warmup < 0:
+        sys.exit("train_bench --gpus: needs --steps >= 1 and --warmup >= 0")
+    if not torch.cuda.is_available() or torch.cuda.device_count() <= local:
+        sys.exit(f"train_bench --gpus {a.gpus}: rank {rank} needs CUDA device {local}, found "
+                 f"{torch.cuda.device_count() if torch.cuda.is_available() else 0}")
+    dev = torch.device("cuda", local)
+    torch.cuda.set_device(dev)
+    dist.init_process_group("nccl", device_id=dev)
+    try:
+        # synthetic scenes, written once by rank 0 to a temporary directory every rank reads
+        box = [tempfile.mkdtemp(prefix="train_bench_") if rank == 0 else None]
+        if rank == 0:
+            synth.write_label_scenes(box[0], "cityscale", (0, 1, 2, 3, 8, 9, 19, 28), 2048, seed=1, extent=2032)
+        dist.broadcast_object_list(box)
+        cwd = os.getcwd()
+        os.chdir(box[0])
+        try:
+            train_ds = D.SatMapDataset(cfg, is_train=True, dev_run=True, device=dev)
+            val_ds = D.SatMapDataset(cfg, is_train=False, dev_run=True, device=dev)
+        finally:
+            os.chdir(cwd)
+        dist.barrier()
+        if rank == 0:
+            shutil.rmtree(box[0], ignore_errors=True)
+        net = SAMRoad(cfg)
+        net.load_state_dict(synth.make_state_dict(cfg, seed=0, logit_gain=4.0))
+        net = net.to(dev).train()
+        net.setup("fit")
+        ddp = torch.nn.parallel.DistributedDataParallel(_StepModule(net), device_ids=[local])
+        opt = net.configure_optimizers()["optimizer"]
+        torch.manual_seed(0)
+        batches = iter(train_ds.loader(B))
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        steps_ms = []
+        for it in range(a.warmup + a.steps):
+            if it == a.warmup:
+                torch.cuda.synchronize()
+                dist.barrier()
+                t0 = time.perf_counter()
+            ev[0].record()
+            loss = ddp(next(batches), it)
+            opt.zero_grad(set_to_none=True)
+            loss.backward()
+            opt.step()
+            ev[1].record()
+            ev[1].synchronize()
+            if it >= a.warmup:
+                steps_ms.append(ev[0].elapsed_time(ev[1]))
+        wall = time.perf_counter() - t0
+        net.eval()
+        torch.cuda.synchronize()
+        dist.barrier()
+        v0 = time.perf_counter()
+        loader = val_ds.loader(B)
+        for j, b in enumerate(loader):
+            net.validation_step(b, j)
+        metrics = net.on_validation_epoch_end()       # the all-reduce ends in a device synchronise
+        torch.cuda.synchronize()
+        val_s = time.perf_counter() - v0
+        mine = {"rank": rank, "step_ms_median": sorted(steps_ms)[len(steps_ms) // 2],
+                "step_ms_min": min(steps_ms), "step_ms_max": max(steps_ms),
+                "wall_s": wall, "val_epoch_ms": 1e3 * val_s, "val_batches": len(loader)}
+        every = [None] * world
+        dist.all_gather_object(every, mine)
+        if rank == 0:
+            slowest = max(r["wall_s"] for r in every)
+            print(json.dumps({"card": _card(), "world": world, "B_per_rank": B, "patch": P, "Ns": Ns, "Np": Np,
+                              "steps": a.steps, "warmup": a.warmup,
+                              "samples_per_s": world * B * a.steps / slowest,
+                              "val_patches": len(val_ds), "val_epoch_ms_max": max(r["val_epoch_ms"] for r in every),
+                              "val_metrics": metrics, "ranks": every}))
+    finally:
+        dist.destroy_process_group()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--batch", type=int, default=16)
+    ap.add_argument("--gpus", type=int, default=0, help="DDP over this many GPUs (run under torchrun)")
+    ap.add_argument("--steps", type=int, default=20, help="--gpus: timed training steps per rank")
+    ap.add_argument("--warmup", type=int, default=3, help="--gpus: untimed training steps first")
     a = ap.parse_args()
+    if a.gpus:
+        return ddp_main(a)
     assert torch.cuda.is_available(), "needs a CUDA device"
     dev = torch.device("cuda:0")
     B, P, Ns, Np = a.batch, 512, 512, 16
