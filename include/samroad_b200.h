@@ -513,6 +513,33 @@ int samroad_op_attention(const void* qkv16, const float* qkv_bias, const float* 
 int samroad_op_sam_decoder(samroad_handle_t h, const float* emb_nchw, int B, float* queries, float* keys,
                            float* hyper, float* lowres, float* mask_scores, float* mask_logits, void* stream);
 
+/* Caller buffers (device) for the intermediates of samroad_op_encoder_taps; every pointer may be NULL.
+ * M = B * (P/16)^2 token rows, D = embed_dim; fp16 buffers are IEEE half. */
+typedef struct SamroadEncoderTaps {
+  float* tokens0;          /* [M, D] fp32: X after patch embed + pos_embed                                 */
+  uint64_t block_mask;     /* bit i: copy X after block i                                                  */
+  float* blocks;           /* [popcount(block_mask), M, D] fp32, the selected blocks in ascending order   */
+  int32_t detail_block;    /* block whose operands go to the six buffers below; -1: none                  */
+  void* ln1;               /* [M, D] fp16: norm1 output                                                    */
+  void* qkv;               /* [M, 3D] fp16: qkv linear (LoRA merged), columns (q|k|v) x head x hd          */
+  void* att;               /* [M, D] fp16: attention output, before proj                                   */
+  float* x_attn;           /* [M, D] fp32: X after proj + residual                                         */
+  void* ln2;               /* [M, D] fp16: norm2 output                                                    */
+  void* h;                 /* [M, 4D] fp16: GELU(lin1)                                                     */
+  void* n1;                /* [M, 256] fp16 NHWC: neck conv1 + LayerNorm2d                                 */
+  void* feat16;            /* [M, 256] fp16 NHWC: neck output (the map decoder's A operand)                */
+  void* d1;                /* [4M, 128] fp16: naive decoder stage 1, row (m * 4 + d), d = di * 2 + dj      */
+  void* d2;                /* [16M, 64] fp16: naive decoder stage 2, row ((m * 4 + d1) * 4 + d2)           */
+} SamroadEncoderTaps;
+
+/* Test hook: exactly samroad_encode_masks, plus stream-ordered copies (no kernels) of the intermediates
+ * `taps` selects, each made right after the launch that produces it.  taps == NULL is samroad_encode_masks.
+ * d1 / d2 are written only when the naive decoder runs (a mask output is requested, no SAM decoder).
+ * Refused before any launch: a NULL handle, a block_mask bit or a detail_block >= depth. */
+int samroad_op_encoder_taps(samroad_handle_t h, const void* rgb, int rgb_dtype, int B,
+                            const SamroadEncoderTaps* taps, float* mask_scores, float* mask_logits,
+                            float* image_embeddings, void* stream);
+
 /* Test hook: bit 0 routes samroad_op_attention / the encoder through the fp32 SIMT attention
  * kernel (the independent on-device checker of the tensor-core kernel).  Not for production use. */
 void samroad_debug_force_simt_attention(int on);

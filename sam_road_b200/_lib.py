@@ -34,6 +34,25 @@ class SamRoadCfg(C.Structure):
     ]
 
 
+class SamroadEncoderTaps(C.Structure):
+    _fields_ = [
+        ("tokens0", C.c_void_p),
+        ("block_mask", C.c_uint64),
+        ("blocks", C.c_void_p),
+        ("detail_block", C.c_int32),
+        ("ln1", C.c_void_p),
+        ("qkv", C.c_void_p),
+        ("att", C.c_void_p),
+        ("x_attn", C.c_void_p),
+        ("ln2", C.c_void_p),
+        ("h", C.c_void_p),
+        ("n1", C.c_void_p),
+        ("feat16", C.c_void_p),
+        ("d1", C.c_void_p),
+        ("d2", C.c_void_p),
+    ]
+
+
 class SamRoadTrainArgs(C.Structure):
     _fields_ = [
         ("B", C.c_int32),
@@ -180,6 +199,7 @@ SIGNATURES = {
     "samroad_debug_disable_2cta_gemm": (None, [_i]),
     "samroad_op_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "samroad_op_sam_decoder": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "samroad_op_encoder_taps": (_i, [_vp, _vp, _i, _i, C.POINTER(SamroadEncoderTaps), _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -132,6 +132,7 @@ struct samroad_ctx {
   HostSlot slots[2];
   cudaStream_t s_h2d = nullptr, s_compute = nullptr, s_copy = nullptr;   // upload / compute / download
   cudaEvent_t ev_emb_hook = nullptr;                     // recorded once the embeddings are final (after the neck)
+  const SamroadEncoderTaps* taps = nullptr;              // set for the duration of samroad_op_encoder_taps
 };
 
 namespace {
@@ -278,6 +279,13 @@ EncWs layout_enc(const samroad_ctx* h, int B, void* base) {
   w.RGB = L.take<uint8_t>(M * 768);    // B * P * P * 3 = M * 256 * 3
   w.total = L.bytes();
   return w;
+}
+
+// samroad_op_encoder_taps: copy a workspace tensor into a caller's buffer (NULL: not requested) before
+// a later launch reuses that workspace
+int tap_copy(void* dst, const void* src, size_t bytes, cudaStream_t st) {
+  if (dst) SRB_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st));
+  return 0;
 }
 
 struct TopoWs {
@@ -784,6 +792,9 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
         im2col_patch16(rgb, rgb_dtype == SAMROAD_U8 ? 1 : 0, B, P, kPixelMean, inv_std, w.XN, st));
   SRB_T(KT_GEMM_PATCH, 2 * Md * Dd * 768, Md * 768 * 2 + Md * Dd * 4,
         gemm_f32out(w.XN, 768, h->pe_w, 768, M, D, 768, h->pe_b, nullptr, h->pos, T, w.X, D, st));
+  const SamroadEncoderTaps* tp = h->taps;
+  const size_t MD = static_cast<size_t>(M) * D;
+  if (tp) SRB_TRY(tap_copy(tp->tokens0, w.X, MD * 4, st));
 
   // transformer blocks (image_encoder.py:166-182).  Both LayerNorms of block i walk the token rows
   // descending when i is even and ascending when i is odd (all ascending under the test hook); the
@@ -803,20 +814,31 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
         }
       att_flops *= static_cast<double>(B) * h->cfg.num_heads;
     }
+    const bool det = tp && tp->detail_block == i;
     SRB_T(KT_LAYERNORM, 0, Md * Dd * 6, layernorm_f16(w.X, b.ln1_g, b.ln1_b, 1e-6f, M, D, w.XN, ln_reverse, st));
+    if (det) SRB_TRY(tap_copy(tp->ln1, w.XN, MD * 2, st));
     SRB_T(KT_GEMM_QKV, 2 * Md * 3 * Dd * Dd, Md * Dd * 2 + Md * 3 * Dd * 2,
           gemm_f16out(w.XN, D, b.qkv_w, D, M, 3 * D, D, b.qkv_b, ACT_NONE, w.QKV, 3 * D, st));
+    if (det) SRB_TRY(tap_copy(tp->qkv, w.QKV, MD * 6, st));
     SRB_T(b.win == s ? KT_ATTN_GLOBAL : KT_ATTN_WINDOW, att_flops, Md * 4 * Dd * 2,
           encoder_attention(w.QKV, b.qkv_b, b.rel_h, b.rel_w, B, s, b.win,
                             h->cfg.num_heads, h->hd, w.ATT, st));
+    if (det) SRB_TRY(tap_copy(tp->att, w.ATT, MD * 2, st));
     SRB_T(KT_GEMM_PROJ, 2 * Md * Dd * Dd, Md * Dd * 2 + Md * Dd * 8,
           gemm_f32out(w.ATT, D, b.proj_w, D, M, D, D, b.proj_b, w.X, nullptr, 0, w.X, D, st));
+    if (det) SRB_TRY(tap_copy(tp->x_attn, w.X, MD * 4, st));
     SRB_T(KT_LAYERNORM, 0, Md * Dd * 6, layernorm_f16(w.X, b.ln2_g, b.ln2_b, 1e-6f, M, D, w.XN, ln_reverse, st));
+    if (det) SRB_TRY(tap_copy(tp->ln2, w.XN, MD * 2, st));
     SRB_T(KT_GEMM_LIN1, 2 * Md * 4 * Dd * Dd, Md * Dd * 2 + Md * 4 * Dd * 2,
           gemm_f16out(w.XN, D, b.lin1_w, D, M, 4 * D, D, b.lin1_b, ACT_GELU, w.H, 4 * D, st));
+    if (det) SRB_TRY(tap_copy(tp->h, w.H, MD * 8, st));
     SRB_T(KT_GEMM_LIN2, 2 * Md * 4 * Dd * Dd, Md * 4 * Dd * 2 + Md * Dd * 8,
           gemm_f32out(w.H, 4 * D, b.lin2_w, 4 * D, M, D, 4 * D, b.lin2_b, w.X, nullptr, 0, w.X, D,
                       st));
+    if (tp && tp->blocks && (tp->block_mask >> i & 1)) {
+      const int slot = __builtin_popcountll(tp->block_mask & ((uint64_t{1} << i) - 1));
+      SRB_TRY(tap_copy(tp->blocks + slot * MD, w.X, MD * 4, st));
+    }
   }
 
   // neck (image_encoder.py:88-104,114): 1x1 conv -> LN2d -> 3x3 conv -> LN2d
@@ -824,6 +846,7 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
   SRB_T(KT_NECK, 2 * Md * 256 * Dd, Md * Dd * 2 + Md * 256 * 2,
         gemm_ln(w.XN, D, h->neck0_w, D, M, 256, D, nullptr, nullptr, h->neck1_g, h->neck1_b, 1e-6f,
                 256, ACT_NONE, w.N1, nullptr, nullptr, T, 256, st));
+  if (tp) SRB_TRY(tap_copy(tp->n1, w.N1, static_cast<size_t>(M) * 256 * 2, st));
   if (128 % s == 0 && T % 128 == 0) {
     // 3x3 conv as an implicit GEMM: the TMA producer reads the nine tap-shifted slabs of the NHWC
     // tensor directly (zero fill outside the image), no im2col buffer
@@ -837,6 +860,7 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
           gemm_ln(IM2, 2304, h->neck2_w, 2304, M, 256, 2304, nullptr, nullptr, h->neck3_g, h->neck3_b,
                   1e-6f, 256, ACT_NONE, w.FEAT, nullptr, image_embeddings, T, 256, st));
   }
+  if (tp) SRB_TRY(tap_copy(tp->feat16, w.FEAT, static_cast<size_t>(M) * 256 * 2, st));
 
   // naive map decoder (model.py:286-295, 490-491) as three GEMMs, pixel shuffle by row indexing
   if (h->ev_emb_hook) SRB_CUDA_OK(cudaEventRecord(h->ev_emb_hook, st));   // embeddings are final here
@@ -849,9 +873,11 @@ extern "C" int samroad_encode_masks(samroad_handle_t h, const void* rgb, int rgb
     SRB_T(KT_DECODER, 2 * Md * 512 * 256, Md * 256 * 2 + Md * 512 * 2,
           gemm_ln(w.FEAT, 256, h->dec1_w, 256, M, 512, 256, h->dec1_b, nullptr, h->dec_ln_g,
                   h->dec_ln_b, 1e-6f, 128, ACT_GELU, w.D1, nullptr, nullptr, T, 512, st));
+    if (tp) SRB_TRY(tap_copy(tp->d1, w.D1, static_cast<size_t>(M) * 512 * 2, st));
     __half* D2 = w.H;
     SRB_T(KT_DECODER, 2 * Md * 4 * 256 * 128, Md * 512 * 2 + Md * 1024 * 2,
           gemm_f16out(w.D1, 128, h->dec2_w, 128, 4 * M, 256, 128, h->dec2_b, ACT_GELU, D2, 256, st));
+    if (tp) SRB_TRY(tap_copy(tp->d2, D2, static_cast<size_t>(M) * 1024 * 2, st));
     SRB_T(KT_DECODER, 2 * Md * 16 * (128 * 64 + 4 * 32 * 8), Md * 1024 * 2 + Md * 512 * 4,
           gemm_dec_final(D2, 64, h->dec3_w, 64, 16 * M, 64, h->dec3_b, h->dec4_w, h->dec4_b, s, P,
                          mask_scores, mask_logits, st));
@@ -1188,6 +1214,24 @@ extern "C" int samroad_op_sam_decoder(samroad_handle_t h, const float* emb_nchw,
   SRB_TRY(sam_decoder_forward(h->sam, emb_nchw, B, h->s, h->cfg.patch_size, h->sam_ws.get(), mask_scores,
                               mask_logits, st));
   return sam_decoder_checkpoints(B, h->T, h->sam_ws.get(), queries, keys, hyper, lowres, st);
+}
+extern "C" int samroad_op_encoder_taps(samroad_handle_t h, const void* rgb, int rgb_dtype, int B,
+                                       const SamroadEncoderTaps* taps, float* mask_scores, float* mask_logits,
+                                       float* image_embeddings, void* stream) {
+  SRB_TRY(check_handle(h, false));
+  if (taps) {
+    const int depth = h->cfg.depth;
+    SRB_REQUIRE(depth >= 64 || (taps->block_mask >> depth) == 0,
+                "samroad_op_encoder_taps: block_mask 0x%llx selects a block >= depth %d",
+                static_cast<unsigned long long>(taps->block_mask), depth);
+    SRB_REQUIRE(taps->detail_block >= -1 && taps->detail_block < depth,
+                "samroad_op_encoder_taps: detail_block=%d (want -1 or a block < depth %d)", taps->detail_block,
+                depth);
+  }
+  h->taps = taps;
+  const int rc = samroad_encode_masks(h, rgb, rgb_dtype, B, mask_scores, mask_logits, image_embeddings, stream);
+  h->taps = nullptr;
+  return rc;
 }
 extern "C" void samroad_debug_force_simt_attention(int on) { attention_force_simt(on); }
 extern "C" void samroad_debug_disable_2cta_gemm(int off) { g_ln_ascending = (off & 16) != 0; }

@@ -55,6 +55,18 @@ def test_sam_decoder_hook_rejects_null_handle():
     assert "null samroad handle" in _lib.last_error()
 
 
+def test_encoder_taps_hook_rejects_null_handle():
+    # the handle is checked before any CUDA call, so this needs no GPU; the block index refusals need a
+    # handle and are in tests/test_gpu_encoder_stages.py
+    lib = _lib.load()
+    out = ctypes.c_void_p(16)
+    taps = _lib.SamroadEncoderTaps(detail_block=-1)
+    assert lib.samroad_op_encoder_taps(None, out, 0, 1, ctypes.byref(taps), None, None, out, None) != 0
+    assert "null samroad handle" in _lib.last_error()
+    assert lib.samroad_op_encoder_taps(None, out, 0, 1, None, None, None, out, None) != 0
+    assert "null samroad handle" in _lib.last_error()
+
+
 def test_cfg_struct_matches_header():
     src = open(os.path.join(ROOT, "include", "samroad_b200.h")).read()
     body = re.search(r"typedef struct SamRoadCfg \{(.*?)\} SamRoadCfg;", src, flags=re.S).group(1)

@@ -19,6 +19,9 @@ from sam_road_b200 import SAMRoad  # noqa: E402
 
 DEV = "cuda:0"
 TOL_LOGIT = 1e-3
+# image embeddings against the fp32 oracle, max-abs relative to their max-abs: measured at most 8.4e-4 over
+# test_encode_and_topo_parity and test_tile_size_parity on an H100 80GB HBM3 at 700 W
+TOL_FEAT_REL = 3.5e-3
 _REPORT = {}
 
 
@@ -107,6 +110,7 @@ def test_encode_and_topo_parity(name, patch, version, B, lora):
     print(name, json.dumps(rep))
     assert torch.isfinite(logits).all() and torch.isfinite(t_logits).all()
     assert rep["mask_logit_maxabs"] <= TOL_LOGIT, rep
+    assert rep["feat_maxabs"] <= TOL_FEAT_REL * rep["feat_absmax"], rep
     # consumers read valid slots only (inferencer.py:213, model.py:536,587); masked slots are the
     # exact bias, rows with no valid pair (flipped to all-valid, model.py:128-130) are sanity-bounded
     assert rep["topo_logit_maxabs_valid"] <= TOL_LOGIT, rep
