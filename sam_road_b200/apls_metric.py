@@ -28,7 +28,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import _lib
+from . import _lib, ranks
 from .topo_metric import gt_path, tile_list, xy2latlon
 
 COVER_STEP = 4          # apls_one_way's graph_prop.propagate(nid, 4, ...): prop_step is not used there
@@ -371,11 +371,14 @@ def apls_tile(gt_adj: dict, prop_adj: dict, dataset: str = "cityscale", device: 
                        export=export)
 
 
-def run_tiles(savedir: str, dataset: str, gt_root: str, tiles=None, device: int = 0, scorer=None):
-    """apls.bash's loop: every tile of the dataset's list that has a proposal graph; each file is overwritten."""
+def run_tiles(savedir: str, dataset: str, gt_root: str, tiles=None, device: int = 0, scorer=None, rank: int = 0,
+              world: int = 1):
+    """apls.bash's loop: every tile of the dataset's list that has a proposal graph; each file is overwritten.  With
+    world > 1 only the tiles rank::world of the list."""
     tiles = tile_list(dataset, gt_root) if tiles is None else tiles
+    tiles = [tiles[i] for i in ranks.shard(len(tiles), rank, world)]
     os.makedirs(os.path.join(savedir, "results", "apls"), exist_ok=True)
-    dev = AplsDevice(device) if scorer is None else None
+    dev = AplsDevice(device) if scorer is None and tiles else None
     try:
         for tile in tiles:
             prop_path = os.path.join(savedir, "graph", "%s.p" % tile)
@@ -435,12 +438,15 @@ def main(argv=None):
     ap.add_argument("--gt-root", default=None,
                     help="the dataset directory: cityscale/ (with 20cities/) or spacenet/ (with RGB_1.0_meter/ and "
                          "data_split.json); default ./<dataset>")
-    ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--device", type=int, default=0, help="GPU index (GPU LOCAL_RANK under torchrun with several ranks)")
     a = ap.parse_args(argv)
     gt_root = a.gt_root or a.dataset
-    run_tiles(a.savedir, a.dataset, gt_root, device=a.device)
-    out = aggregate(a.savedir, a.dataset, verbose=True)
-    print('APLS', out['final_APLS'])
+    with ranks.process_group() as (rank, world):    # rank r of W scores the tiles r::W, rank 0 then aggregates
+        device = ranks.local_gpu() if world > 1 else a.device
+        ranks.run_checked(run_tiles, a.savedir, a.dataset, gt_root, device=device, rank=rank, world=world)
+        if rank == 0:
+            out = aggregate(a.savedir, a.dataset, verbose=True)
+            print('APLS', out['final_APLS'])
 
 
 if __name__ == "__main__":

@@ -343,20 +343,44 @@ def convert_to_sat2graph_format(nodes: np.ndarray, edges: np.ndarray) -> dict:
     return {int_nodes[i]: [int_nodes[j] for j in nbrs] for i, nbrs in enumerate(adj)}
 
 
+def output_dir(name: Optional[str]) -> str:
+    """The run directory `./save/<name>` (`./save/infer_<timestamp>` without a name, inferencer.py:265-269) with its
+    mask/, viz/ and graph/.  Rank 0 names and creates it; the other ranks get its name once it exists."""
+    from . import ranks
+    out_dir = None
+    if ranks.rank_and_world()[0] == 0:
+        out_dir = f"./save/{name}" if name else "./save/infer_" + time.strftime("%Y%m%d_%H%M%S")
+        for sub in ("mask", "viz", "graph"):
+            os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
+    return ranks.broadcast(out_dir)
+
+
 def main(argv=None):
+    """The reference's CLI.  Under torchrun with several ranks (one process per GPU) rank r of W infers the test
+    scenes r::W alone on GPU LOCAL_RANK, and rank 0 writes inference_time.txt with the slowest rank's loop time; every
+    other file is the one a single process writes (DESIGN.md §17)."""
+    from . import ranks
+    with ranks.process_group() as (rank, world):
+        _main(argv, rank, world)
+
+
+def _main(argv, rank: int, world: int):
     import pickle
     from argparse import ArgumentParser
 
     import cv2
+    from . import ranks
     from .model import SAMRoad
     ap = ArgumentParser()
     ap.add_argument("--checkpoint", default=None, help="checkpoint of the model to test.")
     ap.add_argument("--config", default=None, help="model config.")
     ap.add_argument("--output_dir", default=None, help="Name of the output dir under ./save/")
-    ap.add_argument("--device", default="cuda", help="device to use")
+    ap.add_argument("--device", default="cuda", help="device to use (a bare 'cuda' is GPU LOCAL_RANK under torchrun)")
     args = ap.parse_args(argv)
     config = load_config(args.config)
     device = torch.device(args.device)
+    if world > 1 and device.type == "cuda" and device.index is None:
+        device = torch.device("cuda", ranks.local_gpu())
     net = SAMRoad(config)
     ckpt = torch.load(args.checkpoint, map_location="cpu")
     print(f"##### Loading Trained CKPT {args.checkpoint} #####")
@@ -372,42 +396,44 @@ def main(argv=None):
         rgb_pattern = "./spacenet/RGB_1.0_meter/{}__rgb.png"
     else:
         raise SystemExit(f"config.DATASET must be 'cityscale' or 'spacenet', got {config.DATASET!r}")
-    out_dir = f"./save/{args.output_dir}" if args.output_dir else \
-        "./save/infer_" + time.strftime("%Y%m%d_%H%M%S")
-    for sub in ("mask", "viz", "graph"):
-        os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
+    out_dir = output_dir(args.output_dir)
+    mine = [test_ids[i] for i in ranks.shard(len(test_ids), rank, world)]
     loaded = {}
 
     def read_all():      # runs on infer_scenes' loader thread: decoding overlaps the GPU work of earlier scenes
-        for i in test_ids:
+        for i in mine:
             im = cv2.cvtColor(cv2.imread(rgb_pattern.format(i)), cv2.COLOR_BGR2RGB)
             loaded[i] = im
             yield im
 
-    t0 = time.time()
-    results = infer_scenes(net, read_all(), config, device=device)
-    for img_id, (nodes, edges, itsc_mask, road_mask) in zip(test_ids, results):
-        print(f"Processing {img_id}")
-        img = loaded.pop(img_id)
-        cv2.imwrite(os.path.join(out_dir, "mask", f"{img_id}_road.png"), road_mask)
-        cv2.imwrite(os.path.join(out_dir, "mask", f"{img_id}_itsc.png"), itsc_mask)
-        viz = cv2.cvtColor(img.copy(), cv2.COLOR_RGB2BGR)
-        for a, b in edges:
-            cv2.line(viz, (int(nodes[a][1]), int(nodes[a][0])), (int(nodes[b][1]), int(nodes[b][0])),
-                     (15, 160, 253), 4)
-        for r, c in nodes:
-            cv2.circle(viz, (int(c), int(r)), 4, (0, 255, 255), -1)
-        cv2.imwrite(os.path.join(out_dir, "viz", f"{img_id}.png"), viz)
-        if config.DATASET == "spacenet":    # r, c -> sat2graph convention (inferencer.py:332-334)
-            nodes = np.stack([400 - nodes[:, 0], nodes[:, 1]], axis=1)
-        with open(os.path.join(out_dir, "graph", f"{img_id}.p"), "wb") as f:
-            pickle.dump(convert_to_sat2graph_format(nodes, np.asarray(edges).reshape(-1, 2)), f)
-        print(f"Done for {img_id}.")
-    total = time.time() - t0      # wall time of the whole (pipelined) loop, output writing included
-    msg = f"Inference completed for {args.config} in {total} seconds."
-    print(msg)
-    with open(os.path.join(out_dir, "inference_time.txt"), "w") as f:
-        f.write(msg)
+    def run():
+        t0 = time.time()
+        results = infer_scenes(net, read_all(), config, device=device)
+        for img_id, (nodes, edges, itsc_mask, road_mask) in zip(mine, results):
+            print(f"Processing {img_id}")
+            img = loaded.pop(img_id)
+            cv2.imwrite(os.path.join(out_dir, "mask", f"{img_id}_road.png"), road_mask)
+            cv2.imwrite(os.path.join(out_dir, "mask", f"{img_id}_itsc.png"), itsc_mask)
+            viz = cv2.cvtColor(img.copy(), cv2.COLOR_RGB2BGR)
+            for a, b in edges:
+                cv2.line(viz, (int(nodes[a][1]), int(nodes[a][0])), (int(nodes[b][1]), int(nodes[b][0])),
+                         (15, 160, 253), 4)
+            for r, c in nodes:
+                cv2.circle(viz, (int(c), int(r)), 4, (0, 255, 255), -1)
+            cv2.imwrite(os.path.join(out_dir, "viz", f"{img_id}.png"), viz)
+            if config.DATASET == "spacenet":    # r, c -> sat2graph convention (inferencer.py:332-334)
+                nodes = np.stack([400 - nodes[:, 0], nodes[:, 1]], axis=1)
+            with open(os.path.join(out_dir, "graph", f"{img_id}.p"), "wb") as f:
+                pickle.dump(convert_to_sat2graph_format(nodes, np.asarray(edges).reshape(-1, 2)), f)
+            print(f"Done for {img_id}.")
+        return time.time() - t0      # wall time of the whole (pipelined) loop, output writing included
+
+    total = ranks.max_over_ranks(ranks.run_checked(run))      # the split's wall time: the slowest rank's loop
+    if rank == 0:
+        msg = f"Inference completed for {args.config} in {total} seconds."
+        print(msg)
+        with open(os.path.join(out_dir, "inference_time.txt"), "w") as f:
+            f.write(msg)
 
 
 if __name__ == "__main__":

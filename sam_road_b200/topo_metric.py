@@ -24,7 +24,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import _lib
+from . import _lib, ranks
 
 LAT_TOP_LEFT = 41.0
 LON_TOP_LEFT = -71.0
@@ -69,11 +69,22 @@ def distance(p1, p2):
     return math.sqrt(a * a + b * b)
 
 
+def carry_state(m: dict, state: TopoState):
+    """create_graph's update of state.min_lat / max_lon: from the keys of the adjacency dict m."""
+    for n1 in m:
+        lat1, lon1 = xy2latlon(n1[0], n1[1])
+        if lat1 < state.min_lat:
+            state.min_lat = lat1
+        if lon1 > state.max_lon:
+            state.max_lon = lon1
+
+
 def create_graph(m: dict, state: TopoState) -> RoadGraph:
     """main.py create_graph + RoadGraph.addEdge + ReverseDirectionLink; updates state.min_lat / max_lon."""
     g = RoadGraph()
     idmap = {}
     edge_set = set()
+    carry_state(m, state)
 
     def node(k, lat, lon):
         if k not in idmap:
@@ -84,10 +95,6 @@ def create_graph(m: dict, state: TopoState) -> RoadGraph:
 
     for n1, v in m.items():
         lat1, lon1 = xy2latlon(n1[0], n1[1])
-        if lat1 < state.min_lat:
-            state.min_lat = lat1
-        if lon1 > state.max_lon:
-            state.max_lon = lon1
         for n2 in v:
             lat2, lon2 = xy2latlon(n2[0], n2[1])
             id1 = node(n1, lat1, lon1)
@@ -461,19 +468,28 @@ def gt_path(dataset: str, gt_root: str, tile):
     return os.path.join(gt_root, "RGB_1.0_meter", "%s__gt_graph.p" % tile)
 
 
-def run_tiles(savedir: str, dataset: str, gt_root: str, tiles=None, device: int = 0, scorer=None):
-    """main.py: every tile of the dataset's list, in order, with min_lat / max_lon carried over."""
+def run_tiles(savedir: str, dataset: str, gt_root: str, tiles=None, device: int = 0, scorer=None, rank: int = 0,
+              world: int = 1):
+    """main.py: every tile of the dataset's list, in order, with min_lat / max_lon carried over.  With world > 1 this
+    scores and writes only the tiles rank::world; the graphs of the tiles before each of them are still read for the
+    carried min_lat / max_lon, so every file is the one a single process writes."""
     tiles = tile_list(dataset, gt_root) if tiles is None else tiles
+    mine = ranks.shard(len(tiles), rank, world)
     state = TopoState()
-    dev = TopoDevice(device) if scorer is None else None
+    dev = TopoDevice(device) if scorer is None and mine else None
     try:
-        for tile in tiles:
+        for i, tile in enumerate(tiles[:mine[-1] + 1] if mine else []):
             output = os.path.join(savedir, "results", "topo", "%s.txt" % tile)
-            os.makedirs(os.path.dirname(output), exist_ok=True)
+            if i in mine:
+                os.makedirs(os.path.dirname(output), exist_ok=True)
             with open(gt_path(dataset, gt_root, tile), "rb") as f:
                 gt_adj = pickle.load(f)
             with open(os.path.join(savedir, "graph", "%s.p" % tile), "rb") as f:
                 prop_adj = pickle.load(f)
+            if i not in mine:       # another rank's tile
+                carry_state(gt_adj, state)
+                carry_state(prop_adj, state)
+                continue
             _, _, d = topo_tile(gt_adj, prop_adj, state, dataset, device=dev, scorer=scorer)
             with open(output, "a") as fout:    # the reference appends
                 fout.write("".join(d.lines))
@@ -522,12 +538,15 @@ def main(argv=None):
     ap.add_argument("--gt-root", default=None,
                     help="the dataset directory: cityscale/ (with 20cities/) or spacenet/ (with RGB_1.0_meter/ and "
                          "data_split.json); default ./<dataset>")
-    ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--device", type=int, default=0, help="GPU index (GPU LOCAL_RANK under torchrun with several ranks)")
     a = ap.parse_args(argv)
     gt_root = a.gt_root or a.dataset
-    run_tiles(a.savedir, a.dataset, gt_root, device=a.device)
-    out = aggregate(a.savedir, a.dataset)
-    print('TOPO', out['mean topo'][0], 'Precision', out['mean topo'][1], 'Recall', out['mean topo'][2])
+    with ranks.process_group() as (rank, world):    # rank r of W scores the tiles r::W, rank 0 then aggregates
+        device = ranks.local_gpu() if world > 1 else a.device
+        ranks.run_checked(run_tiles, a.savedir, a.dataset, gt_root, device=device, rank=rank, world=world)
+        if rank == 0:
+            out = aggregate(a.savedir, a.dataset)
+            print('TOPO', out['mean topo'][0], 'Precision', out['mean topo'][1], 'Recall', out['mean topo'][2])
 
 
 if __name__ == "__main__":
