@@ -3,19 +3,17 @@
 //
 // Unit = (image, window, head).  Its real queries (the window's tokens inside the s x s grid, ry x rx
 // of them) are numbered j = qh * rx + qw and cut into 16-row m-tiles, one per warp at a time, so edge
-// windows run only the rows they have.  Three kernels run the same tile math and differ in who owns
-// what:
+// windows run only the rows they have.  Three kernels:
 //   attention_unit_kernel : window blocks (win < s) whose whole window fits in shared memory twice
 //              per SM.  One CTA per unit: K, V and the tables are staged once, and the CTA's warps
 //              walk the unit's m-tiles (tile = warp, warp + NW, ...).  After the one barrier that
 //              publishes K/V, a warp touches only its own scratch rows, so tiles need __syncwarp only.
-//   attention_wide_kernel : one window per image (global blocks, a window larger than the grid).  A
-//              unit is cut into CTAs of 2 * kAmWarps m-tiles, two per warp, so that every K and V
-//              fragment read from shared memory feeds two MMAs; each CTA streams the unit's K/V in
-//              double-buffered chunks.
-//   attention_mma_kernel  : windows too large to be resident.  As the wide kernel with one m-tile per
-//              warp; a CTA past the unit's last tile exits at once.  It keeps its own copy of the
-//              tile math (it predates the shared helpers and is left as measured).
+//   attention_global_kernel : global blocks (win == s), on TMA and wgmma; described at the kernel.
+//   attention_mma_kernel  : windows too large to be resident, the one padded window of a grid smaller
+//              than its window, and global blocks whose rings do not fit.  Each CTA streams the unit's
+//              K/V in double-buffered chunks for one m-tile per warp; a CTA past the unit's last tile
+//              exits at once.  It keeps its own copy of the tile math (it predates the shared helpers
+//              and is left as measured).
 // Keys sit in slots k = kh * winP + kw, winP = win rounded up to a power of two
 // (>= 8): a 64-key chunk then holds whole key rows, kh = k >> lg and kw = k & (winP - 1) need no
 // division, and each n8 tile of scores lies in one key row.
@@ -56,11 +54,6 @@ struct AmLayout {
   int tabRows;                    // 2 * win - 1 table rows, padded to n8 tiles
   int relOffset, padOffset, bytes;                // streamed kernel
   int kvSlots, uTabOffset, uWarpOffset, uWarpBytes;   // one-CTA-per-unit kernel: [K | V | tables | warp scratch]
-  int kvBytes;                                    // the streamed kernels' 2 stages of K, V (or the tables)
-  // streamed kernel with two m-tiles per warp: [Q 2 kRows | stages | rel 2 kRows | pad]
-  __host__ __device__ int wide_rel_offset() const { return 2 * kQBytes + kvBytes; }
-  __host__ __device__ int wide_pad_offset() const { return wide_rel_offset() + 2 * kRows * relPitch * 4; }
-  __host__ __device__ int wide_bytes() const { return wide_pad_offset() + 2 * HD * 2; }
   __host__ __device__ int unit_bytes(int nwarps) const { return uWarpOffset + nwarps * uWarpBytes; }
   __host__ __device__ explicit AmLayout(int win) {
     winP = 8; lg = 3;
@@ -72,7 +65,6 @@ struct AmLayout {
     tabRows = ((2 * win - 1 + 7) / 8) * 8;
     const int tab = 4 * tabRows * kPitch * 2;                   // [h hi | h lo | w hi | w lo]
     const int kv = tab > 2 * kStageBytes ? tab : 2 * kStageBytes;
-    kvBytes = kv;
     relOffset = kQBytes + kv;
     padOffset = relOffset + kRows * relPitch * 4;
     bytes = padOffset + 2 * HD * 2;
@@ -682,116 +674,364 @@ attention_unit_kernel(const __half* __restrict__ qkv, const float* __restrict__ 
   }
 }
 
-// Global blocks: the streamed kernel with two m-tiles per warp (128 query rows per CTA), so that every K and V
-// fragment read from shared memory feeds two MMAs and a unit's K/V is streamed by half as many CTAs.
+// Global blocks (win == s): one persistent CTA per SM, three warpgroups.  A work item is (image, head, block of
+// 128 query rows), the query block fastest, so that the CTAs reading one unit's K/V run together and share it in
+// L2.  Warpgroup 0 issues TMA loads: the item's Q (a [128 rows x HD] box of qkv viewed as [B s s, 3 D]) into a
+// ring of Q stages, and K and V of each 128-slot key block (a box {HD, winP, 128 / winP} of qkv viewed as
+// [B][s][s][3 D]; kw >= s and kh >= s arrive as zeros and are masked by the -inf of relw / relh) into a ring of
+// K/V stages.  Warpgroups 1 and 2 own the item's query rows 0..63 and 64..127: S = Q K^T on wgmma from shared
+// memory, the bias and online softmax of am_chunk on the accumulator (its per-warp row and column layout is that
+// of mma.sync), P rounded to fp16 and O += P V on wgmma with P from registers and V MN-major.  Within a
+// consumer the next block's Q K^T is issued with this block's P V, and both run under the softmax of the next
+// block; the two consumers take turns to issue (named barriers 2 and 3), so one's softmax runs under the
+// other's MMAs.  At head dim 80 each row is a 128B-swizzled 64-column box and a 32B-swizzled 16-column box.
+constexpr int kAgRows = 128;        // query rows per work item
+constexpr int kAgSlots = 128;       // key slots per K/V block
+constexpr int kAgThreads = 384;
+constexpr int kAgMaxBytes = 227 * 1024 - 1024;   // the dynamic limit, less the 1 KB alignment of the base
+
 template <int HD>
-__global__ void __launch_bounds__(kAmWarps * 32, 2)
-attention_wide_kernel(const __half* __restrict__ qkv, const float* __restrict__ qkv_bias,
-                      const float* __restrict__ rel_h, const float* __restrict__ rel_w, int s, int win,
-                      int heads, int qblocks, float scale_log2e, __half* __restrict__ out) {
-  using LY = AmLayout<HD>;
-  constexpr int NTH = kAmWarps * 32;
-  constexpr int P = LY::kPitch;
-  constexpr int NT = HD / 8;
-  constexpr int KS = HD / 16;
-  constexpr int RG = NTH / NT;        // key rows per pass of the chunk loader
-  constexpr int ROWS = 2 * LY::kRows;
-  const LY ly(win);
-  const int winP = ly.winP, lg = ly.lg, RP = ly.relPitch;
-  extern __shared__ __align__(16) uint8_t smem_am[];
-  __half* sQ = reinterpret_cast<__half*>(smem_am);
-  uint8_t* sKV = smem_am + 2 * LY::kQBytes;                                 // 2 stages of K, V
-  __half* sTab = reinterpret_cast<__half*>(sKV);                            // prologue only
-  float* sRel = reinterpret_cast<float*>(smem_am + ly.wide_rel_offset());  // [ROWS][relh | relw]
-  __half* sPad = reinterpret_cast<__half*>(smem_am + ly.wide_pad_offset());
-
-  const int D = heads * HD, ld = 3 * D;
-  const int unit = blockIdx.x / qblocks;           // (image, head), head fastest: one window per image
-  const int head = unit % heads, b = unit / heads;
-  const int ry = min(win, s), rx = ry, nreal = ry * rx;
-  const int row0 = (blockIdx.x - unit * qblocks) * ROWS;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const bool active = row0 + warp * 32 < nreal;    // warp-uniform; idle warps still load and sync
-  const __half* img = qkv + static_cast<size_t>(b) * s * s * ld + head * HD;
-
-  for (int idx = tid; idx < ROWS * NT; idx += NTH) {   // rows past the real queries repeat the last one
-    const int r = idx / NT, c8 = idx % NT;
-    const int j = min(row0 + r, nreal - 1), qh = j / rx, qw = j - qh * rx;
-    *reinterpret_cast<uint4*>(sQ + r * P + c8 * 8) =
-        *reinterpret_cast<const uint4*>(img + (qh * s + qw) * ld + c8 * 8);
+struct AgLayout {
+  static_assert(HD == 64 || HD == 80, "head dim 64 or 80");
+  static constexpr int kTailOffset = kAgRows * 128;            // the 16-column box of a Q, K or V buffer
+  static constexpr int kBoxBytes = kAgRows * HD * 2;           // one Q, K or V buffer
+  int winP, lg, nblocks, relH, relPitch, tabRows;
+  int qStages, kvStages;              // 0: shared memory does not hold even the smallest rings
+  int tabOffset, relOffset, barOffset, bytes;
+  __host__ __device__ explicit AgLayout(int s) {
+    winP = 8; lg = 3;
+    while (winP < s) { winP <<= 1; ++lg; }
+    nblocks = (s * winP + kAgSlots - 1) / kAgSlots;
+    relH = ((nblocks * kAgSlots / winP + 7) / 8) * 8;
+    relPitch = ((relH + winP - 8 + 31) / 32) * 32 + 8;
+    tabRows = ((2 * s - 1 + 7) / 8) * 8;
+    const int fixed = 4 * tabRows * AmLayout<HD>::kPitch * 2 + 2 * 64 * relPitch * 4 + 16 * 8;
+    // the deepest rings that fit: three K/V stages keep the next block's loads ahead of both consumers
+    const int cand[3][2] = {{2, 3}, {2, 2}, {1, 2}};
+    qStages = kvStages = 0;
+    for (int i = 0; i < 3 && qStages == 0; ++i)
+      if ((cand[i][0] + 2 * cand[i][1]) * kBoxBytes + fixed <= kAgMaxBytes) {
+        qStages = cand[i][0];
+        kvStages = cand[i][1];
+      }
+    tabOffset = (qStages + 2 * kvStages) * kBoxBytes;          // [Q stages | K, V stages | tables | rel | bars]
+    relOffset = tabOffset + 4 * tabRows * AmLayout<HD>::kPitch * 2;
+    barOffset = relOffset + 2 * 64 * relPitch * 4;
+    bytes = barOffset + 16 * 8 + 1024;
   }
-  am_stage_tables<HD, NTH>(sTab, rel_h, rel_w, win, ly.tabRows, tid);
-  if (tid < 2 * NT)
-    *reinterpret_cast<uint4*>(sPad + tid * 8) = am_bias8(qkv_bias + (1 + tid / NT) * D + head * HD + (tid % NT) * 8);
-  for (int r = tid; r < ROWS; r += NTH) {          // slots that are no key: -inf
-    for (int c = win; c < ly.relH; ++c) sRel[r * RP + c] = -INFINITY;
-    for (int c = win; c < winP; ++c) sRel[r * RP + ly.relH + c] = -INFINITY;
+};
+
+template <int HD>
+__global__ void __launch_bounds__(kAgThreads, 1)
+attention_global_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmQt,
+                        const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmKVt,
+                        const float* __restrict__ rel_h, const float* __restrict__ rel_w, int s, int heads,
+                        int nitems, float scale_log2e, __half* __restrict__ out) {
+  using LY = AgLayout<HD>;
+  constexpr bool kTail = HD == 80;
+  constexpr int KS = HD / 16;
+  const LY ly(s);
+  const int winP = ly.winP, lg = ly.lg, RP = ly.relPitch, nb = ly.nblocks;
+  const int QS = ly.qStages, KVS = ly.kvStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* sQ = smem;
+  uint8_t* sKV = smem + QS * LY::kBoxBytes;                      // stage i: K at 2 i, V at 2 i + 1 boxes
+  __half* sTab = reinterpret_cast<__half*>(smem + ly.tabOffset);
+  float* sRel = reinterpret_cast<float*>(smem + ly.relOffset);  // [2 consumers x 64 rows][relh | relw]
+  uint64_t* qfull = reinterpret_cast<uint64_t*>(smem + ly.barOffset);
+  uint64_t* qempty = qfull + 2;
+  uint64_t* kfull = qempty + 2;
+  uint64_t* kempty = kfull + 3;
+  uint64_t* vfull = kempty + 3;
+  uint64_t* vempty = vfull + 3;
+
+  const int D = heads * HD, nreal = s * s;
+  const int qblocks = (nreal + kAgRows - 1) / kAgRows;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < QS; ++i) {
+      mbar_init(&qfull[i], 1);
+      mbar_init(&qempty[i], 8);                                 // every consumer warp
+    }
+    for (int i = 0; i < KVS; ++i) {
+      mbar_init(&kfull[i], 1);
+      mbar_init(&kempty[i], 8);
+      mbar_init(&vfull[i], 1);
+      mbar_init(&vempty[i], 8);
+    }
+    fence_barrier_init();
   }
   __syncthreads();
 
-  uint32_t qa[2][KS][4];
-  const int rA = warp * 32 + (lane >> 2);          // this thread's query rows: rA, rA + 8 and those + 16
-#pragma unroll
-  for (int m = 0; m < 2; ++m) {
-#pragma unroll
-    for (int k = 0; k < KS; ++k)
-      ldsm_x4(smem_u32(sQ + (warp * 32 + m * 16 + (lane & 15)) * P + k * 16 + (lane >> 4) * 8), qa[m][k][0],
-              qa[m][k][1], qa[m][k][2], qa[m][k][3]);
-    if (active)
-      am_relpos<HD>(qa[m], sTab, ly.tabRows, win, rx, min(row0 + rA + m * 16, nreal - 1),
-                    min(row0 + rA + m * 16 + 8, nreal - 1), sRel + (rA + m * 16) * RP, RP, ly.relH, lane);
-  }
-
-  // ---- K/V chunk loader: thread owns column group c8 of key rows lr0, lr0 + RG, ... ----
-  const bool loader = tid < RG * NT;
-  const int c8 = tid % NT, lr0 = tid / NT;
-  const __half* ksrc = img + D + c8 * 8;
-  __half* kdst = reinterpret_cast<__half*>(sKV) + lr0 * P + c8 * 8;
-  const uint4* kpad = reinterpret_cast<const uint4*>(sPad) + c8;   // fp16 bias of k; of v at + NT
-  auto load_chunk = [&](int c) {
-    if (loader) {
-      __half* dk = kdst + (c & 1) * (LY::kStageBytes / 2);
-      for (int r = lr0; r < kAmKC; r += RG, dk += RG * P) {
-        const int k = c * kAmKC + r, kh = k >> lg, kw = k & (winP - 1);
-        __half* dv = dk + kAmKC * P;
-        if (kh < win && kw < win) {
-          if (kh < s && kw < s) {
-            const __half* src = ksrc + (kh * s + kw) * ld;
-            cp_async16(smem_u32(dk), src);
-            cp_async16(smem_u32(dv), src + D);
-          } else {
-            *reinterpret_cast<uint4*>(dk) = kpad[0];
-            *reinterpret_cast<uint4*>(dv) = kpad[NT];
-          }
-        } else {
-          *reinterpret_cast<uint4*>(dk) = make_uint4(0u, 0u, 0u, 0u);
-          *reinterpret_cast<uint4*>(dv) = make_uint4(0u, 0u, 0u, 0u);
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmKV);
+      int qs = 0, ks = 0;
+      uint32_t qph = 0, kph = 0;
+      for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+        const int qb = item % qblocks, unit = item / qblocks;
+        const int head = unit % heads, b = unit / heads;
+        uint8_t* q = sQ + qs * LY::kBoxBytes;
+        mbar_wait(&qempty[qs], qph ^ 1u);
+        mbar_arrive_expect_tx(&qfull[qs], LY::kBoxBytes);
+        tma_load_2d(q, &tmQ, &qfull[qs], head * HD, b * nreal + qb * kAgRows);
+        if (kTail) tma_load_2d(q + LY::kTailOffset, &tmQt, &qfull[qs], head * HD + 64, b * nreal + qb * kAgRows);
+        if (++qs == QS) { qs = 0; qph ^= 1u; }
+        for (int kb = 0; kb < nb; ++kb) {
+          const int kh0 = kb * (kAgSlots / winP);
+          uint8_t* k = sKV + 2 * ks * LY::kBoxBytes;
+          uint8_t* v = k + LY::kBoxBytes;
+          mbar_wait(&kempty[ks], kph ^ 1u);
+          mbar_arrive_expect_tx(&kfull[ks], LY::kBoxBytes);
+          tma_load_4d(k, &tmKV, &kfull[ks], D + head * HD, 0, kh0, b);
+          if (kTail) tma_load_4d(k + LY::kTailOffset, &tmKVt, &kfull[ks], D + head * HD + 64, 0, kh0, b);
+          mbar_wait(&vempty[ks], kph ^ 1u);
+          mbar_arrive_expect_tx(&vfull[ks], LY::kBoxBytes);
+          tma_load_4d(v, &tmKV, &vfull[ks], 2 * D + head * HD, 0, kh0, b);
+          if (kTail) tma_load_4d(v + LY::kTailOffset, &tmKVt, &vfull[ks], 2 * D + head * HD + 64, 0, kh0, b);
+          if (++ks == KVS) { ks = 0; kph ^= 1u; }
         }
       }
     }
-    cp_async_commit();
-  };
-  __syncthreads();                                 // tables consumed, sRel written
-  load_chunk(0);
-
-  const float* const rel[2] = {sRel + rA * RP, sRel + (rA + 16) * RP};
-  AmTile<HD> t[2];
-  t[0].reset();
-  t[1].reset();
-  for (int c = 0; c < ly.nchunks; ++c) {
-    cp_async_wait_all();
-    __syncthreads();                               // chunk c landed; chunk c - 1 consumed
-    if (c + 1 < ly.nchunks) load_chunk(c + 1);
-    if (!active) continue;
-    const __half* sK = reinterpret_cast<const __half*>(sKV + (c & 1) * LY::kStageBytes);
-    const int k0 = c * kAmKC;
-    am_chunk<HD, 2>(t, qa, sK, sK + kAmKC * P, k0, k0 + kAmKC / 2 < ly.nslots, rel, RP, ly.relH, lg, winP,
-                    scale_log2e, lane);
+    return;
   }
-  if (!active) return;
-  __half* out0 = out + static_cast<size_t>(b) * s * s * D + head * HD;
+
+  // ===================== consumers =====================
+  setmaxnreg_inc<232>();
+  const int g = wg - 1, w = warp & 3;
+  const int ctid = threadIdx.x - 128;
+  am_stage_tables<HD, 256>(sTab, rel_h, rel_w, s, ly.tabRows, ctid);
+  for (int r = ctid; r < 128; r += 256) {                       // slots that are no key: -inf
+    for (int c = s; c < ly.relH; ++c) sRel[r * RP + c] = -INFINITY;
+    for (int c = s; c < winP; ++c) sRel[r * RP + ly.relH + c] = -INFINITY;
+  }
+  named_bar_sync(1, 256);
+
+  const int rW = 64 * g + 16 * w;                               // the warp's first row of the item
+  const int cq = 2 * (lane & 3);
+  float* relA = sRel + (rW + (lane >> 2)) * RP;                 // the thread's rows A and B = A + 8
+  const float* relB = relA + 8 * RP;
+  if (g == 1) named_bar_arrive(2, 256);                         // consumer 0 issues first
+  int qs = 0, ks = 0;
+  uint32_t qph = 0, kph = 0;
+  for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+    const int qb = item % qblocks, unit = item / qblocks;
+    const int head = unit % heads, b = unit / heads;
+    const uint32_t q = smem_u32(sQ + qs * LY::kBoxBytes);
+    mbar_wait(&qfull[qs], qph);
+
+    // ---- rel-pos of the warp's 16 rows on mma.sync, from the swizzled Q box ----
+    {
+      uint32_t qa[KS][4];
+      const int r = rW + (lane & 15);
 #pragma unroll
-  for (int m = 0; m < 2; ++m) am_store<HD>(t[m], row0 + rA + m * 16, nreal, rx, s, D, out0, lane);
+      for (int k = 0; k < KS; ++k) {
+        const uint32_t a = k < 4 ? q + r * 128 + (((2 * k + (lane >> 4)) ^ (r & 7)) << 4)
+                                 : q + LY::kTailOffset + r * 32 + (((lane >> 4) ^ ((r >> 2) & 1)) << 4);
+        ldsm_x4(a, qa[k][0], qa[k][1], qa[k][2], qa[k][3]);
+      }
+      const int j = qb * kAgRows + rW + (lane >> 2);
+      am_relpos<HD>(qa, sTab, ly.tabRows, s, s, min(j, nreal - 1), min(j + 8, nreal - 1), relA, RP, ly.relH, lane);
+      __syncwarp();
+    }
+
+    const uint64_t qd = wgmma_desc_k128(q + g * 64 * 128);
+    const uint64_t qdt = wgmma_desc_k32(q + LY::kTailOffset + g * 64 * 32);
+    float sc[64];                     // S of one block: n8 tile n at sc[4 n ..], rows A (0, 1) and B (2, 3)
+    float o[32], ot[kTail ? 8 : 1];   // O columns 0..63 and, at head dim 80, 64..79
+    uint32_t pa[kAgSlots / 16][4];    // P (fp16) as the A operand of P V, one k16 step per row
+    float mA = -INFINITY, mB = -INFINITY, lA = 0.f, lB = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (kTail ? 8 : 1); ++i) ot[i] = 0.f;
+
+    auto issue_s = [&](int stage) {
+      const uint32_t k = smem_u32(sKV + 2 * stage * LY::kBoxBytes);
+      const uint64_t kd = wgmma_desc_k128(k);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_m64n128k16(sc, qd + static_cast<uint64_t>(2 * kk), kd + static_cast<uint64_t>(2 * kk), kk != 0);
+      if constexpr (kTail) wgmma_m64n128k16(sc, qdt, wgmma_desc_k32(k + LY::kTailOffset), 1u);
+      wgmma_commit();
+    };
+    // scale + bias, then P = 2^(S - m) in place; returns the rescale factors of the running state
+    auto softmax = [&](int kb, float& alA, float& alB) {
+      const int k0 = kb * kAgSlots;
+      float cmA = -INFINITY, cmB = -INFINITY;
+#pragma unroll
+      for (int n = 0; n < kAgSlots / 8; ++n) {
+        const int kh = (k0 + n * 8) >> lg;                      // one key row per n8 tile
+        const int kw = (n * 8 + cq) & (winP - 1);
+        const float hA = relA[kh], hB = relB[kh];
+        const float2 wA = *reinterpret_cast<const float2*>(relA + ly.relH + kw);
+        const float2 wB = *reinterpret_cast<const float2*>(relB + ly.relH + kw);
+        sc[4 * n + 0] = fmaf(sc[4 * n + 0], scale_log2e, hA + wA.x);
+        sc[4 * n + 1] = fmaf(sc[4 * n + 1], scale_log2e, hA + wA.y);
+        sc[4 * n + 2] = fmaf(sc[4 * n + 2], scale_log2e, hB + wB.x);
+        sc[4 * n + 3] = fmaf(sc[4 * n + 3], scale_log2e, hB + wB.y);
+        cmA = fmaxf(cmA, fmaxf(sc[4 * n + 0], sc[4 * n + 1]));
+        cmB = fmaxf(cmB, fmaxf(sc[4 * n + 2], sc[4 * n + 3]));
+      }
+#pragma unroll
+      for (int off = 1; off <= 2; off <<= 1) {
+        cmA = fmaxf(cmA, __shfl_xor_sync(0xffffffffu, cmA, off));
+        cmB = fmaxf(cmB, __shfl_xor_sync(0xffffffffu, cmB, off));
+      }
+      const float nmA = fmaxf(mA, cmA), nmB = fmaxf(mB, cmB);
+      alA = ex2_approx(mA - nmA);                               // first block: 2^-inf = 0
+      alB = ex2_approx(mB - nmB);
+      mA = nmA; mB = nmB;
+#pragma unroll
+      for (int n = 0; n < kAgSlots / 8; ++n) {
+        sc[4 * n + 0] = ex2_approx(sc[4 * n + 0] - mA);
+        sc[4 * n + 1] = ex2_approx(sc[4 * n + 1] - mA);
+        sc[4 * n + 2] = ex2_approx(sc[4 * n + 2] - mB);
+        sc[4 * n + 3] = ex2_approx(sc[4 * n + 3] - mB);
+      }
+    };
+    // once the previous P V has finished: rescale O and l, round P to fp16; l sums the rounded P
+    auto take_p = [&](float alA, float alB) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 4) { o[i] *= alA; o[i + 1] *= alA; o[i + 2] *= alB; o[i + 3] *= alB; }
+#pragma unroll
+      for (int i = 0; i < (kTail ? 8 : 0); i += 4) { ot[i] *= alA; ot[i + 1] *= alA; ot[i + 2] *= alB; ot[i + 3] *= alB; }
+      lA *= alA; lB *= alB;
+#pragma unroll
+      for (int kc = 0; kc < kAgSlots / 16; ++kc) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          pa[kc][e] = pack_half2(sc[8 * kc + 2 * e], sc[8 * kc + 2 * e + 1]);
+          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&pa[kc][e]));
+          if (e & 1) lB += f.x + f.y; else lA += f.x + f.y;
+        }
+      }
+    };
+
+    // ---- block 0 ----
+    mbar_wait(&kfull[ks], kph);
+    wgmma_fence();
+    issue_s(ks);
+    wgmma_wait<0>();
+    wgmma_fence_operand(sc);
+    if (lane == 0) mbar_arrive(&kempty[ks]);
+    {
+      float alA, alB;
+      softmax(0, alA, alB);
+      take_p(alA, alB);
+    }
+    // P V of the block in stage ks; issued in this consumer's turn, after the next block's Q K^T if any
+    auto issue_pv = [&]() {
+      mbar_wait(&vfull[ks], kph);
+      const uint32_t v = smem_u32(sKV + (2 * ks + 1) * LY::kBoxBytes);
+#pragma unroll
+      for (int kc = 0; kc < kAgSlots / 16; ++kc) {
+        wgmma_m64n64k16_rs_t(o, pa[kc], wgmma_desc_k128(v + kc * 16 * 128), 1u);
+        if constexpr (kTail)
+          wgmma_m64n16k16_rs_t(*reinterpret_cast<float(*)[8]>(ot), pa[kc],
+                               wgmma_desc_k32(v + LY::kTailOffset + kc * 16 * 32), 1u);
+      }
+      wgmma_commit();
+      named_bar_arrive(2 + (g ^ 1), 256);                       // the other consumer's turn
+    };
+    auto begin_turn = [&]() {
+      named_bar_sync(2 + g, 256);                               // this consumer's turn to issue
+      wgmma_fence_operand(o);
+      wgmma_fence_operand(ot);
+      wgmma_fence_operand(pa);
+      wgmma_fence();
+    };
+    auto end_pv = [&]() {
+      wgmma_fence_operand(o);
+      wgmma_fence_operand(ot);
+      wgmma_fence_operand(pa);
+      if (lane == 0) mbar_arrive(&vempty[ks]);
+    };
+    // every block but the last: the next block's S = Q K^T runs with this block's P V, its softmax under P V.
+    // The last block is peeled so that the number of MMA groups in flight never depends on a branch.
+    for (int kb = 0; kb + 1 < nb; ++kb) {
+      const int ks1 = ks + 1 == KVS ? 0 : ks + 1;
+      const uint32_t kph1 = ks1 == 0 ? kph ^ 1u : kph;
+      begin_turn();
+      mbar_wait(&kfull[ks1], kph1);
+      issue_s(ks1);
+      issue_pv();
+      wgmma_wait<1>();                                          // S of block kb + 1
+      wgmma_fence_operand(sc);
+      if (lane == 0) mbar_arrive(&kempty[ks1]);
+      float alA, alB;
+      softmax(kb + 1, alA, alB);
+      wgmma_wait<0>();                                          // P V of block kb
+      end_pv();
+      take_p(alA, alB);
+      ks = ks1;
+      kph = kph1;
+    }
+    begin_turn();
+    issue_pv();
+    wgmma_wait<0>();
+    end_pv();
+    if (++ks == KVS) { ks = 0; kph ^= 1u; }
+    if (lane == 0) mbar_arrive(&qempty[qs]);
+    if (++qs == QS) { qs = 0; qph ^= 1u; }
+
+    // ---- O / l -> fp16, real query rows only ----
+#pragma unroll
+    for (int off = 1; off <= 2; off <<= 1) {
+      lA += __shfl_xor_sync(0xffffffffu, lA, off);
+      lB += __shfl_xor_sync(0xffffffffu, lB, off);
+    }
+    const float invA = 1.0f / lA, invB = 1.0f / lB;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int j = qb * kAgRows + rW + (lane >> 2) + 8 * h;
+      if (j >= nreal) continue;
+      __half* op = out + (static_cast<size_t>(b) * nreal + j) * D + head * HD + cq;
+      const float inv = h ? invB : invA;
+#pragma unroll
+      for (int j8 = 0; j8 < 8; ++j8)
+        *reinterpret_cast<uint32_t*>(op + j8 * 8) = pack_half2(o[4 * j8 + 2 * h] * inv, o[4 * j8 + 2 * h + 1] * inv);
+#pragma unroll
+      for (int j8 = 0; j8 < (kTail ? 2 : 0); ++j8)
+        *reinterpret_cast<uint32_t*>(op + 64 + j8 * 8) =
+            pack_half2(ot[4 * j8 + 2 * h] * inv, ot[4 * j8 + 2 * h + 1] * inv);
+    }
+  }
+  if (g == 0) named_bar_sync(2, 256);                           // consumer 1's last turn handed back
+}
+
+template <int HD>
+int launch_attention_global(const __half* qkv, const float* rel_h, const float* rel_w, int B, int s, int heads,
+                            __half* out, cudaStream_t st) {
+  const AgLayout<HD> ly(s);
+  const uint64_t D = static_cast<uint64_t>(heads) * HD, tokens = static_cast<uint64_t>(B) * s * s;
+  CUtensorMap tmQ, tmQt, tmKV, tmKVt;
+  SRB_TRY(make_tmap_f16_2d(&tmQ, qkv, tokens, 3 * D, 3 * D, kAgRows, 64));
+  const uint64_t dims[4] = {3 * D, static_cast<uint64_t>(s), static_cast<uint64_t>(s), static_cast<uint64_t>(B)};
+  const uint64_t strides[3] = {3 * D, 3 * D * s, 3 * D * s * s};
+  const uint32_t box[4] = {64, static_cast<uint32_t>(ly.winP), static_cast<uint32_t>(kAgSlots / ly.winP), 1};
+  SRB_TRY(make_tmap_f16_4d(&tmKV, qkv, dims, strides, box));
+  tmQt = tmQ;
+  tmKVt = tmKV;
+  if (HD == 80) {
+    const uint32_t tbox[4] = {16, box[1], box[2], 1};
+    SRB_TRY(make_tmap_f16_2d(&tmQt, qkv, tokens, 3 * D, 3 * D, kAgRows, 16));
+    SRB_TRY(make_tmap_f16_4d(&tmKVt, qkv, dims, strides, tbox));
+  }
+  const long items = static_cast<long>(B) * heads * ((s * s + kAgRows - 1) / kAgRows);
+  SRB_REQUIRE(items <= 2147483647L, "attention: %ld work items exceed the int range (B=%d s=%d heads=%d)", items,
+              B, s, heads);
+  const int grid = items < device_sm_count() ? static_cast<int>(items) : device_sm_count();
+  const float scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(HD));
+  auto kern = attention_global_kernel<HD>;
+  SRB_TRY(allow_dynamic_smem(kern, ly.bytes));
+  SRB_LAUNCH(kern, grid, kAgThreads, ly.bytes, st, tmQ, tmQt, tmKV, tmKVt, rel_h, rel_w, s, heads,
+             static_cast<int>(items), scale_log2e, out);
+  return 0;
 }
 
 // Warps of a one-CTA-per-unit block, and the shared memory that still lets two such CTAs share an SM
@@ -807,13 +1047,14 @@ int launch_attention_mma(const __half* qkv, const float* qkv_bias, const float* 
                          int B, int s, int win, int heads, __half* out, cudaStream_t st) {
   using LY = AmLayout<HD>;
   constexpr int NW = kAuWarps<HD>;
+  if (win == s && AgLayout<HD>(s).qStages > 0)
+    return launch_attention_global<HD>(qkv, rel_h, rel_w, B, s, heads, out, st);
   const LY ly(win);
   const int nwin = (s + win - 1) / win;
   const float scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(HD));
   const bool resident = win < s && ly.unit_bytes(NW) <= kAuMaxBytes;
   const int w0 = win < s ? win : s;       // real queries of the fullest window: w0 x w0
-  const bool wide = win >= s;              // one window per image: two m-tiles per warp
-  const int qblocks = resident ? 1 : ((w0 * w0 + 15) / 16 + (wide ? 2 : 1) * kAmWarps - 1) / ((wide ? 2 : 1) * kAmWarps);
+  const int qblocks = resident ? 1 : ((w0 * w0 + 15) / 16 + kAmWarps - 1) / kAmWarps;
   const long blocks = static_cast<long>(qblocks) * B * nwin * nwin * heads;
   SRB_REQUIRE(blocks <= 2147483647L, "attention: %ld CTAs exceed the grid limit (B=%d s=%d win=%d heads=%d)",
               blocks, B, s, win, heads);
@@ -822,11 +1063,6 @@ int launch_attention_mma(const __half* qkv, const float* qkv_bias, const float* 
     auto kern = attention_unit_kernel<HD, NW>;
     SRB_TRY(allow_dynamic_smem(kern, ly.unit_bytes(NW)));
     SRB_LAUNCH(kern, grid, NW * 32, ly.unit_bytes(NW), st, qkv, qkv_bias, rel_h, rel_w, s, win, nwin, heads,
-               scale_log2e, out);
-  } else if (wide) {
-    auto kern = attention_wide_kernel<HD>;
-    SRB_TRY(allow_dynamic_smem(kern, ly.wide_bytes()));
-    SRB_LAUNCH(kern, grid, kAmWarps * 32, ly.wide_bytes(), st, qkv, qkv_bias, rel_h, rel_w, s, win, heads, qblocks,
                scale_log2e, out);
   } else {
     auto kern = attention_mma_kernel<HD>;

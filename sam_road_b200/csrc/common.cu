@@ -127,6 +127,11 @@ static PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
+// fp16 boxes of 16 columns are the 32-byte tails of 80-column rows, read by wgmma in its 32B-swizzled layout
+static CUtensorMapSwizzle f16_swizzle(uint32_t box_cols) {
+  return box_cols == 16 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B;
+}
+
 int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                      uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols) {
   PFN_encodeTiled fn = get_encode_fn();
@@ -140,7 +145,7 @@ int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), gdim, gstr, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, f16_swizzle(box_cols),
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SRB_REQUIRE(r == CUDA_SUCCESS,
               "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu ld=%llu box=%ux%u", (int)r,
@@ -184,7 +189,7 @@ int make_tmap_f16_4d(CUtensorMap* out, const void* base, const uint64_t dims[4],
   cuuint32_t bx[4] = {box[0], box[1], box[2], box[3]};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), gdim, gstr, bx,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, f16_swizzle(box[0]),
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SRB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(4D) failed (%d)", (int)r);
   return 0;

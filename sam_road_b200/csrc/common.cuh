@@ -299,6 +299,16 @@ __device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 62;                           // SWIZZLE_128B
   return d;
 }
+// The same for rows of 16 fp16 (32 B) written by a 32B-swizzled TMA box: 8-row atoms 256 B apart.  A
+// K-major operand covers one k16 step; an MN-major one (wgmma transpose bit) 16 columns of 8-row k groups.
+__device__ __forceinline__ uint64_t wgmma_desc_k32(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(256u >> 4) << 32;
+  d |= static_cast<uint64_t>(3) << 62;                           // SWIZZLE_32B
+  return d;
+}
 __device__ __forceinline__ void wgmma_fence() {
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
@@ -315,6 +325,14 @@ __device__ __forceinline__ void wgmma_fence_operand(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// the same for A fragments held in registers, which the MMA reads until it has completed
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operand(uint32_t (&a)[R][4]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
+}
 // register budget of a warpgroup (all its warps execute it): producers give registers to consumers
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() {
@@ -326,6 +344,9 @@ __device__ __forceinline__ void setmaxnreg_dec() {
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // Accumulator fragment of wgmma m64nNk16 (f32): register i of thread (warp w of the warpgroup, lane l)
@@ -394,12 +415,46 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_
       : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
+// D[64 x 64] (+)= A[64 x 16] * B[16 x 64]: A from registers (the m16n8k16 A fragment of each warp's 16 rows),
+// B MN-major in shared memory (transpose bit set)
+__device__ __forceinline__ void wgmma_m64n64k16_rs_t(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b,
+                                                   uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
+}
+
+// D[64 x 16] (+)= A[64 x 16] * B[16 x 16], as wgmma_m64n64k16_rs_t
+__device__ __forceinline__ void wgmma_m64n16k16_rs_t(float (&d)[8], const uint32_t (&a)[4], uint64_t desc_b,
+                                                   uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
+}
 
 // ----------------------------------------------------------------------------------------------
 // host: TMA descriptor construction (driver entry point fetched at run time; no -lcuda needed)
 // ----------------------------------------------------------------------------------------------
 // 2D fp16 row-major tensor [rows][cols] (cols contiguous, row pitch `ld` elements), box
-// [box_rows][64 cols], 128B swizzle.  Out-of-bounds elements read as zero.
+// [box_rows][box_cols], 128B swizzle (32B for a box of 16 columns).  Out-of-bounds elements read as zero.
 int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                      uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols = 64);
 
@@ -408,7 +463,7 @@ int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t
                      uint32_t box_rows);
 
 // 4D fp16 view [d3][d2][d1][d0] (d0 contiguous; strides in elements for d1..d3), box {b0,b1,b2,b3},
-// 128B swizzle (b0 * 2 bytes must be 128).  Out-of-bounds elements read as zero.
+// 128B swizzle for b0 = 64, 32B swizzle for b0 = 16.  Out-of-bounds elements read as zero.
 int make_tmap_f16_4d(CUtensorMap* out, const void* base, const uint64_t dims[4],
                      const uint64_t strides_elems[3], const uint32_t box[4]);
 int make_tmap_f32_4d_dense(CUtensorMap* out, const void* base, const uint64_t dims[4],

@@ -193,6 +193,7 @@ struct Partial {   // out[z][m][n] = v
 };
 
 constexpr int kTile = 64, kTk = 32, kLdh = kTk + 8;   // 64x64 tile, 32-deep k stage, padded fp16 rows
+constexpr float kLoScale = 2048.0f;                   // 2^11: the lo half of an operand split stays a normal fp16
 
 __device__ __forceinline__ uint32_t ld_h2(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
@@ -204,9 +205,11 @@ __device__ __forceinline__ void mma16816(float (&c)[4], uint32_t a0, uint32_t a1
       : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-// Each fp32 operand v is split into fp16 hi = fp16(v) and lo = fp16(v - hi); a product is hi*hi + hi*lo + lo*hi
-// (three mma.sync), which keeps about 21 bits of the operands: the forward tracks the fp32 reference closely
-// enough that ReLU / GELU decisions near zero agree with it, where plain fp16 operands flip them.
+// Each fp32 operand v is split into fp16 hi = fp16(v) and lo = fp16((v - hi) * 2^11); a product is hi*hi plus
+// 2^-11 (hi*lo + lo*hi) (three mma.sync, the cross terms in an accumulator of their own), which keeps about 21
+// bits of the operands: the forward tracks the fp32 reference closely enough that ReLU / GELU decisions near zero
+// agree with it, where plain fp16 operands flip them.  Unscaled, v - hi of a weight below about 0.06 falls into
+// fp16's subnormal range, whose fixed spacing of 2^-24 costs up to ten bits of the residual.
 // 8 warps in a 4 x 2 grid; each warp owns 16 x 32 of the tile = four m16n8 accumulators
 template <class LA, class LB, class OUT>
 __global__ void __launch_bounds__(256) gemm_mma_kernel(LA A, LB Bm, OUT out, long long M, long long N, long long K,
@@ -221,11 +224,11 @@ __global__ void __launch_bounds__(256) gemm_mma_kernel(LA A, LB Bm, OUT out, lon
   const bool a_kfast = A.second_unit(), b_kfast = Bm.first_unit();
   // one row tile per block unless M has more row tiles than grid.y holds
   for (long long m0 = static_cast<long long>(blockIdx.y) * kTile; m0 < M; m0 += static_cast<long long>(gridDim.y) * kTile) {
-    float acc[4][4];
+    float acc[4][4], acx[4][4];   // hi*hi; the scaled cross terms
 #pragma unroll
     for (int j = 0; j < 4; ++j)
 #pragma unroll
-      for (int r = 0; r < 4; ++r) acc[j][r] = 0.f;
+      for (int r = 0; r < 4; ++r) acc[j][r] = acx[j][r] = 0.f;
     for (long long k0 = kb; k0 < ke; k0 += kTk) {
       for (int i = threadIdx.x; i < kTk * kTile; i += 256) {
         int mm = a_kfast ? i / kTk : i % kTile, kk = a_kfast ? i % kTk : i / kTile;
@@ -233,7 +236,7 @@ __global__ void __launch_bounds__(256) gemm_mma_kernel(LA A, LB Bm, OUT out, lon
         float v = (r < M && k < ke) ? A(r, k) : 0.f;
         __half h = __float2half_rn(v);
         As[0][mm][kk] = h;
-        As[1][mm][kk] = __float2half_rn(v - __half2float(h));
+        As[1][mm][kk] = __float2half_rn((v - __half2float(h)) * kLoScale);
         mm = b_kfast ? i / kTk : i % kTile;
         kk = b_kfast ? i % kTk : i / kTile;
         r = n0 + mm;
@@ -241,7 +244,7 @@ __global__ void __launch_bounds__(256) gemm_mma_kernel(LA A, LB Bm, OUT out, lon
         v = (r < N && k < ke) ? Bm(k, r) : 0.f;
         h = __float2half_rn(v);
         Bs[0][mm][kk] = h;
-        Bs[1][mm][kk] = __float2half_rn(v - __half2float(h));
+        Bs[1][mm][kk] = __float2half_rn((v - __half2float(h)) * kLoScale);
       }
       __syncthreads();
 #pragma unroll
@@ -258,8 +261,8 @@ __global__ void __launch_bounds__(256) gemm_mma_kernel(LA A, LB Bm, OUT out, lon
         for (int j = 0; j < 4; ++j) {
           const uint32_t bh0 = ld_h2(&Bs[0][wn + 8 * j + g][ks + 2 * t]), bh1 = ld_h2(&Bs[0][wn + 8 * j + g][ks + 2 * t + 8]);
           const uint32_t bl0 = ld_h2(&Bs[1][wn + 8 * j + g][ks + 2 * t]), bl1 = ld_h2(&Bs[1][wn + 8 * j + g][ks + 2 * t + 8]);
-          mma16816(acc[j], a[1][0], a[1][1], a[1][2], a[1][3], bh0, bh1);   // small terms first
-          mma16816(acc[j], a[0][0], a[0][1], a[0][2], a[0][3], bl0, bl1);
+          mma16816(acx[j], a[1][0], a[1][1], a[1][2], a[1][3], bh0, bh1);
+          mma16816(acx[j], a[0][0], a[0][1], a[0][2], a[0][3], bl0, bl1);
           mma16816(acc[j], a[0][0], a[0][1], a[0][2], a[0][3], bh0, bh1);
         }
       }
@@ -270,7 +273,7 @@ __global__ void __launch_bounds__(256) gemm_mma_kernel(LA A, LB Bm, OUT out, lon
 #pragma unroll
       for (int r = 0; r < 4; ++r) {
         const long long m = m0 + wm + g + (r >> 1) * 8, n = n0 + wn + 8 * j + 2 * t + (r & 1);
-        if (m < M && n < N) out(z, m, n, acc[j][r]);
+        if (m < M && n < N) out(z, m, n, fmaf(acx[j][r], 1.0f / kLoScale, acc[j][r]));
       }
   }
 }

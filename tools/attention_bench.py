@@ -50,12 +50,15 @@ def att_flops(B, s, win, heads, hd):
 
 
 def score_ratio(s, win):
-    """Executed / needed scores of attention_mma.cuh: 16-row tiles of the real queries against
-    whole 64-slot chunks of win x winP key slots (an upper half with no key skipped)."""
+    """Executed / needed scores of attention_mma.cuh.  Global blocks (win == s): 128-row items of the
+    s x s queries against whole 128-slot blocks of s x winP key slots.  Window blocks: 16-row tiles of the
+    real queries against whole 64-slot chunks of win x winP key slots (an upper half with no key skipped)."""
     winp = 8
     while winp < win:
         winp *= 2
     slots = win * winp
+    if win == s:
+        return math.ceil(s * s / 128) * 128 * math.ceil(slots / 128) * 128 / (s * s) ** 2
     executed_keys = (slots // 64) * 64 + (0 if slots % 64 == 0 else (32 if slots % 64 <= 32 else 64))
     executed = needed = 0
     for ry, rx in windows(s, win):
