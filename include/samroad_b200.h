@@ -543,6 +543,12 @@ int samroad_op_encoder_taps(samroad_handle_t h, const void* rgb, int rgb_dtype, 
 /* Test hook: bit 0 routes samroad_op_attention / the encoder through the fp32 SIMT attention
  * kernel (the independent on-device checker of the tensor-core kernel).  Not for production use. */
 void samroad_debug_force_simt_attention(int on);
+/* Test hook: the kernel samroad_op_attention runs for grid s, window win and head_dim, as it would be chosen
+ * now (no launch, no device needed): 0 the one-CTA-per-window kernel, 1 the streamed kernel, 2 the global
+ * wgmma kernel, 3 the SIMT kernel (forced by samroad_debug_force_simt_attention).  *q_stages and *kv_stages
+ * (each may be NULL) get the global kernel's Q and K/V ring depths, 0 on the other paths.  Returns -1 (see
+ * samroad_last_error) for a shape or head_dim samroad_op_attention refuses. */
+int samroad_debug_attention_path(int s, int win, int head_dim, int* q_stages, int* kv_stages);
 /* Test hook (bit mask): bit 4 (16) makes the encoder's LayerNorms walk the token rows ascending
  * (by default those of even blocks walk them descending).  Other bits are ignored. */
 void samroad_debug_disable_2cta_gemm(int off);

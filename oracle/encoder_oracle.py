@@ -17,9 +17,10 @@ kernels.cu, attention_mma.cuh, gemm_tc.cuh), and nowhere else:
     every bias, LayerNorm parameter, pos_embed and the rel-pos tables stay as given;
   * ln1, ln2, qkv, the attention output and GELU(lin1);
   * the window padding tokens, whose q = k = v = fp16(qkv bias);
-  * the probabilities P fed to the P V product, taken against the row's global maximum, with the
-    softmax denominator summing the rounded P.  The device takes P against a running maximum over key
-    chunks; that difference is not modelled here and is part of the measured stage bounds;
+  * the probabilities P fed to the P V product, with the softmax denominator summing the rounded P.  With
+    `p_block(s, win, hd)` given, P is taken against the running maximum over key blocks of that many slots,
+    as the kernel that runs the block does (attention_oracle.softmax_pv; None: P unrounded, the SIMT
+    kernel); without it, against the row's global maximum;
   * fp16(X) into the neck, its two outputs n1 and feat16, and the decoder activations d1 and d2.
 The image embeddings (neck output before rounding), the residual stream X, dec3 + GELU + map_decoder.7
 and the logits stay in full precision.  With fp16=False the stages chained end to end are the algorithm of
@@ -27,11 +28,12 @@ samroad_oracle (tests/test_encoder_oracle_host.py).
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Callable, Dict, Optional
 
 import torch
 import torch.nn.functional as F
 
+from . import attention_oracle as A
 from .samroad_oracle import PIXEL_MEAN, PIXEL_STD, ModelSpec, layer_norm_2d, rel_pos_gather
 
 Tensor = torch.Tensor
@@ -76,8 +78,8 @@ class EncoderRef:
     """Weights of one model prepared for the stages (rounded to fp16 where the device packs fp16)."""
 
     def __init__(self, sd: Dict[str, Tensor], spec: ModelSpec, fp16: bool = False, dtype=torch.float64,
-                 device=None):
-        self.spec, self.fp16, self.dtype = spec, fp16, dtype
+                 device=None, p_block: Optional[Callable[[int, int, int], Optional[int]]] = None):
+        self.spec, self.fp16, self.dtype, self.p_block = spec, fp16, dtype, p_block
         self.r = _half if fp16 else _keep
         dev = device if device is not None else next(iter(sd.values())).device
         self.device = torch.device(dev)
@@ -184,8 +186,8 @@ class EncoderRef:
         rw = torch.einsum("nahwc,wkc->nahwk", qg, rel_pos_gather(win, win, rel_w))
         scores = (scores.view(n, heads, win, win, win, win) + rh[..., :, None] + rw[..., None, :]).view(n, heads, L, L)
         if self.fp16:
-            pr = _half(torch.exp(scores - scores.amax(-1, keepdim=True)))
-            o = (pr @ v) / pr.sum(-1, keepdim=True)
+            block = self.p_block(self.spec.grid, win, hd) if self.p_block else win * A.win_pitch(win)
+            o = A.softmax_pv(scores, v, A.key_blocks(win, block, scores.device))
         else:
             o = scores.softmax(-1) @ v
         return self.r(o.permute(0, 2, 1, 3).reshape(n, win, win, D))

@@ -196,6 +196,7 @@ SIGNATURES = {
     "samroad_op_gemm_ref": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "samroad_op_layernorm": (_i, [_vp, _vp, _vp, _f, _i, _i, _vp, _vp]),
     "samroad_debug_force_simt_attention": (None, [_i]),
+    "samroad_debug_attention_path": (_i, [_i, _i, _i, _vp, _vp]),
     "samroad_debug_disable_2cta_gemm": (None, [_i]),
     "samroad_op_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "samroad_op_sam_decoder": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -197,6 +197,24 @@ static int launch_attention_simt(const __half* qkv, const float* qkv_bias, const
 static bool g_force_simt = false;
 void attention_force_simt(int mode) { g_force_simt = (mode & 1) != 0; }
 
+int attention_path(int s, int win, int hd, int* q_stages, int* kv_stages) {
+  if (q_stages) *q_stages = 0;
+  if (kv_stages) *kv_stages = 0;
+  if (!(win > 0 && win <= 64 && s > 0 && s <= 64)) {
+    set_last_error("attention: win=%d s=%d unsupported", win, s);
+    return -1;
+  }
+  if (hd != 64 && hd != 80) {
+    set_last_error("attention: head_dim=%d unsupported (64 or 80)", hd);
+    return -1;
+  }
+  if (g_force_simt) return 3;
+  const AmChoice c = hd == 64 ? attention_mma_choice<64>(s, win) : attention_mma_choice<80>(s, win);
+  if (q_stages) *q_stages = c.qStages;
+  if (kv_stages) *kv_stages = c.kvStages;
+  return static_cast<int>(c.path);
+}
+
 int encoder_attention(const __half* qkv, const float* qkv_bias, const float* rel_h,
                       const float* rel_w, int B, int s, int win, int heads, int hd, __half* out,
                       cudaStream_t st) {

@@ -1042,17 +1042,35 @@ int launch_attention_global(const __half* qkv, const float* rel_h, const float* 
 template <int HD> constexpr int kAuWarps = HD == 64 ? 5 : 4;
 constexpr int kAuMaxBytes = (228 * 1024) / 2 - 1024;
 
+// The kernel launch_attention_mma runs for (s, win): global blocks whose rings fit take the wgmma kernel, window
+// blocks whose window is resident the unit kernel, everything else the streamed kernel.  Ring depths are those of
+// the global kernel (0 on the other paths).
+enum class AmPath { kUnit = 0, kStreamed = 1, kGlobal = 2 };
+struct AmChoice {
+  AmPath path;
+  int qStages, kvStages;
+};
+template <int HD>
+AmChoice attention_mma_choice(int s, int win) {
+  if (win == s) {
+    const AgLayout<HD> ag(s);
+    if (ag.qStages > 0) return {AmPath::kGlobal, ag.qStages, ag.kvStages};
+  }
+  const bool resident = win < s && AmLayout<HD>(win).unit_bytes(kAuWarps<HD>) <= kAuMaxBytes;
+  return {resident ? AmPath::kUnit : AmPath::kStreamed, 0, 0};
+}
+
 template <int HD>
 int launch_attention_mma(const __half* qkv, const float* qkv_bias, const float* rel_h, const float* rel_w,
                          int B, int s, int win, int heads, __half* out, cudaStream_t st) {
   using LY = AmLayout<HD>;
   constexpr int NW = kAuWarps<HD>;
-  if (win == s && AgLayout<HD>(s).qStages > 0)
-    return launch_attention_global<HD>(qkv, rel_h, rel_w, B, s, heads, out, st);
+  const AmPath path = attention_mma_choice<HD>(s, win).path;
+  if (path == AmPath::kGlobal) return launch_attention_global<HD>(qkv, rel_h, rel_w, B, s, heads, out, st);
   const LY ly(win);
   const int nwin = (s + win - 1) / win;
   const float scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(HD));
-  const bool resident = win < s && ly.unit_bytes(NW) <= kAuMaxBytes;
+  const bool resident = path == AmPath::kUnit;
   const int w0 = win < s ? win : s;       // real queries of the fullest window: w0 x w0
   const int qblocks = resident ? 1 : ((w0 * w0 + 15) / 16 + kAmWarps - 1) / kAmWarps;
   const long blocks = static_cast<long>(qblocks) * B * nwin * nwin * heads;

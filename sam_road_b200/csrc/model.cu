@@ -1234,4 +1234,7 @@ extern "C" int samroad_op_encoder_taps(samroad_handle_t h, const void* rgb, int 
   return rc;
 }
 extern "C" void samroad_debug_force_simt_attention(int on) { attention_force_simt(on); }
+extern "C" int samroad_debug_attention_path(int s, int win, int head_dim, int* q_stages, int* kv_stages) {
+  return attention_path(s, win, head_dim, q_stages, kv_stages);
+}
 extern "C" void samroad_debug_disable_2cta_gemm(int off) { g_ln_ascending = (off & 16) != 0; }

@@ -58,6 +58,9 @@ int encoder_attention(const __half* qkv, const float* qkv_bias, const float* rel
                       cudaStream_t st);
 // force the SIMT attention kernel (tests use it as the independent on-device checker)
 void attention_force_simt(int mode);   // bit 0: SIMT kernel
+// the kernel encoder_attention runs for (s, win, hd): 0 unit, 1 streamed, 2 global, 3 SIMT (forced); the global
+// kernel's Q and K/V ring depths (0 elsewhere); -1 (last error set) for a shape encoder_attention refuses
+int attention_path(int s, int win, int hd, int* q_stages, int* kv_stages);
 
 // ---- TopoNet pieces (toponet.cu) -----------------------------------------------------------------------------
 // points dtype: 0 = float32, 1 = int64, 2 = int32 ; pairs dtype: 1 = int64, 2 = int32

@@ -67,6 +67,34 @@ def test_encoder_taps_hook_rejects_null_handle():
     assert "null samroad handle" in _lib.last_error()
 
 
+def test_attention_path_hook():
+    # the kernel choice is host arithmetic on shared-memory layouts, so this needs no GPU.  Global blocks
+    # (win == s): the deepest rings that fit, and at head dim 80 from s = 41 on none, so the streamed kernel
+    lib = _lib.load()
+    q, kv = ctypes.c_int(), ctypes.c_int()
+
+    def path(s, win, hd):
+        return lib.samroad_debug_attention_path(s, win, hd, ctypes.byref(q), ctypes.byref(kv)), q.value, kv.value
+
+    for hd, runs in ((64, [(40, (2, 2, 3)), (52, (2, 2, 2)), (64, (2, 1, 2))]),
+                     (80, [(20, (2, 2, 3)), (36, (2, 2, 2)), (40, (2, 1, 2)), (64, (1, 0, 0))])):
+        lo = 1
+        for hi, want in runs:
+            for s in range(lo, hi + 1):
+                assert path(s, s, hd) == want, (hd, s)
+            lo = hi + 1
+    assert path(25, 14, 64) == (0, 0, 0) and path(32, 14, 80) == (0, 0, 0)     # window resident in one CTA
+    assert path(40, 20, 80) == (1, 0, 0) and path(12, 14, 64) == (1, 0, 0)     # streamed; padded window
+    lib.samroad_debug_force_simt_attention(1)
+    try:
+        assert path(32, 32, 64) == (3, 0, 0)
+    finally:
+        lib.samroad_debug_force_simt_attention(0)
+    assert lib.samroad_debug_attention_path(16, 0, 64, None, None) == -1 and "win=0" in _lib.last_error()
+    assert lib.samroad_debug_attention_path(65, 65, 64, None, None) == -1
+    assert lib.samroad_debug_attention_path(16, 16, 72, None, None) == -1 and "head_dim=72" in _lib.last_error()
+
+
 def test_cfg_struct_matches_header():
     src = open(os.path.join(ROOT, "include", "samroad_b200.h")).read()
     body = re.search(r"typedef struct SamRoadCfg \{(.*?)\} SamRoadCfg;", src, flags=re.S).group(1)

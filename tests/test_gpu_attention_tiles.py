@@ -1,5 +1,6 @@
 """Tensor-core encoder attention at tile boundaries of its layout (key rows padded to a power of two,
-64-slot chunks whose upper half may hold no key, 16-row tiles of a window's real queries), and the
+64-slot chunks whose upper half may hold no key, 16-row tiles of a window's real queries; 128-slot key blocks
+and 128-row work items in the global kernel), and the
 accuracy of its tensor-core rel-pos terms, each against the fp32 SIMT kernel."""
 import pytest
 import torch
@@ -37,12 +38,12 @@ def _run(lib, simt, B, s, win, heads, hd, qkv16, bias, rel_h, rel_w):
 
 
 @pytest.mark.parametrize("B,s,win,heads,hd", [
-    (2, 25, 25, 12, 64),    # global, key rows padded 25 -> 32, last chunk half empty
-    (2, 20, 20, 16, 80),    # global, padded key rows, whole chunks
+    (2, 25, 25, 12, 64),    # global, key rows padded 25 -> 32: 800 slots, a last key block of one key row
+    (2, 20, 20, 16, 80),    # global, padded key rows, five whole 128-slot blocks
     (3, 12, 14, 12, 64),    # one window larger than the grid: 144 real queries = 9 row tiles
     (4, 3, 3, 12, 64),      # 8-slot key rows, one half chunk
     (2, 5, 5, 16, 80),      # 8-slot key rows, one full chunk
-    (1, 40, 40, 12, 64),    # global, 64-slot key rows
+    (1, 40, 40, 12, 64),    # global, 64-slot key rows: two per key block
     (2, 48, 14, 16, 80),    # windows with 6-token edges
 ])
 def test_attention_tile_boundaries_tc_vs_simt(B, s, win, heads, hd):

@@ -1,6 +1,7 @@
 """Tensor-core encoder attention at the seams of its kernels: window blocks whose whole window is resident in one
-CTA (warps walking the window's 16-row tiles), global blocks with two 16-row tiles per warp, and the streamed
-one-tile kernel for windows too large to be resident, each against the fp32 SIMT kernel."""
+CTA (warps walking the window's 16-row tiles), global blocks on the persistent wgmma kernel (128-row work items,
+128-slot key blocks), and the streamed one-tile kernel for windows too large to be resident, each against the
+fp32 SIMT kernel."""
 import pytest
 import torch
 
@@ -38,9 +39,9 @@ def _run(lib, simt, B, s, win, heads, hd, qkv16, bias, rel_h, rel_w):
     (2, 25, 14, 12, 64),    # 14x11 edges (10 tiles, the last with 10 rows) and an 11x11 corner; s no multiple of 8
     (2, 28, 14, 16, 80),    # head dim 80: 13 tiles over 4 warps, no edge window
     (1, 64, 14, 12, 64),    # 25 windows per image, 14x8 edges
-    (1, 64, 64, 12, 64),    # global with 64-slot key rows: two tiles per warp at its largest shared memory
-    (2, 9, 9, 12, 64),      # global, 81 queries: a warp whose second tile has one row, a warp with no tile
-    (1, 23, 23, 16, 80),    # global at head dim 80: 529 queries, a last CTA of 17 rows
+    (1, 64, 64, 12, 64),    # global with 64-slot key rows: 32 items per head, 32 key blocks, 1 Q / 2 K/V stages
+    (2, 9, 9, 12, 64),      # global, 81 queries: one item of 128 rows, 47 never stored; one key block of 144 slots
+    (1, 23, 23, 16, 80),    # global at head dim 80: a last item of 17 rows, a last key block of 96 slots
     (1, 17, 14, 1, 64),     # one image, one head: 14x3 and 3x3 windows
     (1, 40, 20, 12, 64),    # a window too large to be resident: streamed, with CTAs past a unit's last tile
     (2, 30, 16, 16, 80),    # resident at head dim 64 only: head dim 80 streams 16x16 windows
