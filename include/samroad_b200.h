@@ -306,6 +306,23 @@ int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs* args, cons
 int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
                            const float* const* params, float* const* grads, int n_params, void* ws,
                            size_t ws_bytes, const float* g, void* stream);
+/* Forward of one step of the heads on caller-supplied image embeddings (device fp32 [B,256,P/16,P/16], NCHW,
+ * contiguous) in place of rgb: the encoder does not run; the embeddings are copied into ws and everything
+ * downstream is samroad_train_forward's.  Same arguments and outputs otherwise. */
+int samroad_train_forward_embeddings(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                                     const float* const* params, int n_params, const float* image_embeddings,
+                                     const void* points, int pts_dtype, const void* pairs, int pairs_dtype,
+                                     const uint8_t* valid, const uint8_t* connected, const float* keypoint_mask,
+                                     const float* road_mask, void* ws, size_t ws_bytes, float* losses,
+                                     void* stream);
+/* samroad_train_backward plus the gradient of the image embeddings, for a ws filled by either forward.
+ * grads == NULL skips the weight gradients; grad_embeddings (device fp32 [B,256,P/16,P/16], NCHW, overwritten)
+ * may be NULL, but not both.  The map decoder's and TopoNet's parts (through the bilinear sampler) are summed per
+ * element in that order and scaled by g[0] / (2 B P^2) and g[1] / sum(valid) in fp32; a part whose incoming
+ * gradient is exactly 0 adds nothing.  Deterministic: no float atomics. */
+int samroad_train_backward_embeddings(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                                      const float* const* params, float* const* grads, int n_params, void* ws,
+                                      size_t ws_bytes, const float* g, float* grad_embeddings, void* stream);
 /* Repacks one head tensor (map_decoder.* / topo_net.*) of finalized weights from DEVICE fp32 memory,
  * stream-ordered; the packed result equals what samroad_finalize_weights makes from the same values, bit for
  * bit.  Encoder tensors and the SAM mask decoder are refused. */

@@ -161,6 +161,9 @@ SIGNATURES = {
     "samroad_train_forward": (_i, [_vp, _targs, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp,
                                    C.c_size_t, _vp, _vp, _vp]),
     "samroad_train_backward": (_i, [_vp, _targs, _vp, _vp, _vp, _i, _vp, C.c_size_t, _vp, _vp]),
+    "samroad_train_forward_embeddings": (_i, [_vp, _targs, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp,
+                                              _vp, C.c_size_t, _vp, _vp]),
+    "samroad_train_backward_embeddings": (_i, [_vp, _targs, _vp, _vp, _vp, _i, _vp, C.c_size_t, _vp, _vp, _vp]),
     "samroad_update_tensor_device": (_i, [_vp, C.c_char_p, _vp, C.POINTER(C.c_int64), _i, _vp]),
     "samroad_debug_train_dropout_keep": (_i, [_f, C.c_uint64, _i, _i, C.c_int64, _vp, _vp]),
     "samroad_labels_create": (_i, [_i, C.POINTER(SamRoadLabelCfg), C.POINTER(_vp)]),

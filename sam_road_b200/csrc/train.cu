@@ -12,6 +12,8 @@
 //             rows in fixed chunks whose partials are summed in chunk order, then scaled in fp32; LayerNorm,
 //             GELU / ReLU, dropout and attention backward, and a segmented (CSR) reduction of the pair
 //             tokens onto their src / tgt points.  No float atomics: a step is bitwise reproducible.
+//   embeddings  optionally the forward from caller-supplied embeddings, and the gradient of the embeddings: the
+//             first ConvTranspose's input gradient plus the bilinear sampler's backward over taps sorted by texel.
 //
 // Layouts.  A ConvTranspose2d(k=2, s=2) is a per-pixel linear map Cin -> 4*Cout.  Decoder activations are
 // stored in "quad-tree" row order: the 4 children of row r are rows 4r+d, d = di*2+dj, so every stage is
@@ -340,6 +342,7 @@ __global__ void wgrad_finish_kernel(const float* __restrict__ part, int Z, int K
 template <class LG>
 int wgrad(Mat a, int K0, LG g, int N, long long R, int mode, int cout, long long ld, int col0, float* dW,
           float* db, float* part, const float* scale, cudaStream_t st) {
+  if (!dW && !db) return 0;   // a backward without weight gradients (samroad_train_backward_embeddings)
   a.ones = db ? K0 : -1;
   const int M = K0 + (db ? 1 : 0);
   // A(m, r) with m the input channel: swap the strides of the row-major activation
@@ -497,6 +500,7 @@ __global__ void colsum_finish_kernel(const float* __restrict__ part, int Z, floa
 }
 int ln_param_grads(const float* g, const float* xh, long long rows, float* part, float* dg, float* db,
                    const float* scale, cudaStream_t st) {
+  if (!dg && !db) return 0;
   const long long chunk = rows > 0 ? (rows + kColChunks - 1) / kColChunks : 1;
   const int Z = static_cast<int>(rows > 0 ? (rows + chunk - 1) / chunk : 1);
   SRB_LAUNCH(colsum_kernel, Z, 128, 0, st, g, xh, rows, chunk, part);
@@ -807,6 +811,120 @@ __global__ void keep_kernel(Dropout d, int layer, int site, long long n, uint8_t
   GRID_STRIDE(i, n) out[i] = drop_mul(d, layer, site, static_cast<unsigned long long>(i)) != 0.0f;
 }
 
+// ---- gradient of the image embeddings (DESIGN.md §12, "Gradients into the image embeddings") -------------
+// Bilinear sampler backward.  Tap 4p+k of point p is its corner k (0 (y0,x0), 1 (y0,x0+1), 2 (y0+1,x0),
+// 3 (y0+1,x0+1)) with the weight the forward sampled it with (topo_sample_kernel's arithmetic).  Its key is the
+// texel b*T + y*s + x, or M (past every texel) for a corner outside the map and for every corner of a point
+// that no pair token reads: such a point's feature gradient is exactly zero, and leaving it out keeps its
+// texels at zero where the loss scale is not finite.
+// the points as the sampler reads them, kept for backward
+__global__ void points_f32_kernel(const void* points, int pts_dtype, long long n, float* __restrict__ out) {
+  GRID_STRIDE(i, n) out[i] = load_coord(points, pts_dtype, static_cast<size_t>(i));
+}
+__global__ void emb_taps_kernel(const float* __restrict__ xy, int N, int s, float P, long long pts, long long M,
+                                const int* __restrict__ src_start, const int* __restrict__ tgt_start,
+                                uint32_t* __restrict__ key, float* __restrict__ wt) {
+  GRID_STRIDE(p, pts) {
+    const float px = xy[p * 2], py = xy[p * 2 + 1];
+    const float gx = (px / P) * 2.0f - 1.0f;
+    const float gy = (py / P) * 2.0f - 1.0f;
+    const float ux = ((gx + 1.0f) * static_cast<float>(s) - 1.0f) * 0.5f;
+    const float uy = ((gy + 1.0f) * static_cast<float>(s) - 1.0f) * 0.5f;
+    const float fx0 = floorf(ux), fy0 = floorf(uy);
+    const int x0 = static_cast<int>(fx0), y0 = static_cast<int>(fy0);
+    const float tx = ux - fx0, ty = uy - fy0;
+    const float w[4] = {(1.f - tx) * (1.f - ty), tx * (1.f - ty), (1.f - tx) * ty, tx * ty};
+    const bool read = src_start[p + 1] > src_start[p] || tgt_start[p + 1] > tgt_start[p];
+    const long long base = (p / N) * static_cast<long long>(s) * s;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int x = x0 + (k & 1), y = y0 + (k >> 1);
+      const bool in = read && x >= 0 && x < s && y >= 0 && y < s;
+      key[p * 4 + k] = static_cast<uint32_t>(in ? base + y * s + x : M);
+      wt[p * 4 + k] = w[k];
+    }
+  }
+}
+
+// One stable LSD pass of the taps by texel: the keys move with their tap ids (the ids are the identity on the
+// first pass), so equal texels keep the tap order: by point, then by corner.
+struct TapPass {
+  const uint32_t* kin;
+  const uint32_t* vin;   // null: tap i
+  uint32_t* kout;
+  uint32_t* vout;
+  int shift;
+  __device__ uint32_t key(long long i) const { return __ldg(kin + i); }
+  __device__ unsigned digit(uint32_t k) const { return (k >> shift) & 255u; }
+  __device__ void emit(long long i, uint32_t k, uint32_t pos) const {
+    kout[pos] = k;
+    vout[pos] = vin ? __ldg(vin + i) : static_cast<uint32_t>(i);
+  }
+};
+
+__device__ __forceinline__ long long lower_bound_u32(const uint32_t* __restrict__ a, long long n, uint32_t v) {
+  long long lo = 0, hi = n;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (a[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// dL/d(embeddings) [B,256,s,s] for 32 texels per block, one thread per channel:
+//   v = s_mask gm[m, c] + s_topo sum over m's taps, in sorted order, of w gfs[point, c]
+// gm: mask branch [M, 256] (unscaled); gfs: feature gradient [pts, 256] (unscaled).  A branch whose incoming
+// gradient is exactly zero adds nothing, and a texel no tap reaches gets no TopoNet term, so a non-finite scale
+// (a batch without a valid slot) reaches only the texels the reference's gradient is NaN at.  A segment is
+// walked 256 taps at a time from shared memory: its length is at most 4 N, and the channels run in parallel.
+constexpr int kEmbTexels = 32;
+constexpr int kTapChunk = 1024;   // taps per warp of a digit pass
+__global__ void __launch_bounds__(256) emb_grad_kernel(const float* __restrict__ gm, const float* __restrict__ gfs,
+                                                       const uint32_t* __restrict__ key,
+                                                       const uint32_t* __restrict__ tap, const float* __restrict__ wt,
+                                                       long long ntap, long long M, int T,
+                                                       const float* __restrict__ g, const float* __restrict__ scale,
+                                                       float* __restrict__ out) {
+  __shared__ float tile[kEmbTexels][257];
+  __shared__ uint32_t sp[256];
+  __shared__ float sw[256];
+  const int c = threadIdx.x;
+  const long long m0 = static_cast<long long>(blockIdx.x) * kEmbTexels;
+  const bool mask_on = g[0] != 0.0f, topo_on = g[1] != 0.0f;
+  const float s0 = scale[0], s1 = scale[1];
+  for (int j = 0; j < kEmbTexels && m0 + j < M; ++j) {
+    const long long m = m0 + j;
+    float v = mask_on ? __fmul_rn(s0, gm[m * 256 + c]) : 0.0f;
+    if (topo_on) {
+      const long long b = lower_bound_u32(key, ntap, static_cast<uint32_t>(m));
+      const long long e = lower_bound_u32(key, ntap, static_cast<uint32_t>(m + 1));
+      float a = 0.0f;
+      for (long long base = b; base < e; base += 256) {
+        const int cnt = static_cast<int>(e - base < 256 ? e - base : 256);
+        __syncthreads();
+        if (c < cnt) {
+          const uint32_t id = tap[base + c];
+          sp[c] = id >> 2;
+          sw[c] = wt[id];
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int k = 0; k < cnt; ++k) a = fmaf(sw[k], gfs[static_cast<long long>(sp[k]) * 256 + c], a);
+      }
+      if (e > b) v = __fadd_rn(v, __fmul_rn(s1, a));
+    }
+    tile[j][c] = v;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < kEmbTexels * 256; i += 256) {   // NCHW: consecutive threads walk texels
+    const int cc = i / kEmbTexels, j = i % kEmbTexels;
+    const long long m = m0 + j;
+    if (m >= M) continue;
+    const long long b = m / T, t = m % T;
+    out[(b * 256 + cc) * T + t] = tile[j][cc];
+  }
+}
+
 #define EW(kernel, n, ...) SRB_LAUNCH(kernel, ew_grid(n), 256, 0, st, __VA_ARGS__)
 #define ROWS8(kernel, rows, ...)                                                                     \
   do {                                                                                              \
@@ -850,6 +968,7 @@ struct TrainWs {
   float* emb;                           // [B, 256, T] image embeddings
   float *f0, *xh1, *rs1, *a1, *z2, *a2, *z3, *a3, *dl;   // decoder (dl: unscaled dlogits [R4, 2])
   float *fs, *pf, *pst, *off;           // TopoNet: sampled features, relu(feature_proj), Ws f | Wt f, offsets
+  float* xy;                            // the points in fp32 [pts, 2]
   int *src, *tgt, *src_start, *tgt_start, *src_list, *tgt_list, *cursor, *sort_tmp, *scan_tmp;
   uint8_t* vf;                          // fixed key-padding mask
   float* x[4];                          // layer inputs / outputs [tok, 128]
@@ -860,6 +979,11 @@ struct TrainWs {
   // backward scratch
   float* scale;                         // [2] loss scales of the decoder / TopoNet gradients
   float *g3, *g2, *g1, *gx, *gr, *gy, *gh, *gq, *gp, *gps, *gpt, *wpart;
+  // embeddings-gradient scratch: sampled-feature gradient, the bilinear taps sorted by texel
+  float* gfs;                           // [pts, 256]
+  uint32_t *tkey[2], *tid[2];           // [4 pts] each: keys and tap ids, ping-pong over the digit passes
+  float* twt;                           // [4 pts] tap weights
+  uint32_t* thist;                      // digit histogram + its scan scratch
   size_t total;
 };
 
@@ -875,6 +999,7 @@ TrainWs layout_train(const Dims& d, void* base) {
   w.dl = L.take<float>(d.R4 * 2);
   w.fs = L.take<float>(pts * 256); w.pf = L.take<float>(pts * 128); w.pst = L.take<float>(pts * 256);
   w.off = L.take<float>(tok * 2);
+  w.xy = L.take<float>(pts * 2);
   w.src = L.take<int>(tok); w.tgt = L.take<int>(tok);
   w.src_start = L.take<int>(pts + 1); w.tgt_start = L.take<int>(pts + 1);
   w.src_list = L.take<int>(tok); w.tgt_list = L.take<int>(tok); w.cursor = L.take<int>(pts);
@@ -900,6 +1025,11 @@ TrainWs layout_train(const Dims& d, void* base) {
   w.gpt = L.take<float>(pts * 128);
   w.wpart = L.take<float>(static_cast<long long>(kWgradChunks) * 257 * 512 > kColChunks * 256LL
                   ? static_cast<long long>(kWgradChunks) * 257 * 512 : kColChunks * 256LL);
+  w.gfs = L.take<float>(pts * 256);
+  for (int i = 0; i < 2; ++i) { w.tkey[i] = L.take<uint32_t>(4 * pts); w.tid[i] = L.take<uint32_t>(4 * pts); }
+  w.twt = L.take<float>(4 * pts);
+  const long long hist = digit_hist_elems<kTapChunk>(4 * pts);
+  w.thist = L.take<uint32_t>(hist + scan_scratch_elems(hist));
   w.total = L.bytes();
   return w;
 }
@@ -935,32 +1065,33 @@ extern "C" int samroad_train_workspace_bytes(samroad_handle_t h, const SamRoadTr
   return 0;
 }
 
-extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
-                                     const float* const* params, int n_params, const void* rgb, int rgb_dtype,
-                                     const void* points, int pts_dtype, const void* pairs, int pairs_dtype,
-                                     const uint8_t* valid, const uint8_t* connected, const float* keypoint_mask,
-                                     const float* road_mask, void* ws, size_t ws_bytes, float* losses,
-                                     float* image_embeddings, void* stream) {
-  Dims d;
-  SRB_TRY(make_dims(h, args, &d));
-  HeadPtrs hp;
-  SRB_TRY(resolve_params(keys, params, n_params, d.tf, &hp, nullptr));
-  SRB_REQUIRE(rgb && points && pairs && valid && connected && keypoint_mask && road_mask && ws && losses,
-              "samroad_train_forward: null input");
+namespace {
+
+// The checks both forward entry points share; fills the dims, the parameter table and the workspace layout.
+int prepare_forward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                    const float* const* params, int n_params, const void* input, const void* points, int pts_dtype,
+                    const void* pairs, int pairs_dtype, const uint8_t* valid, const uint8_t* connected,
+                    const float* keypoint_mask, const float* road_mask, void* ws, size_t ws_bytes, float* losses,
+                    const char* who, Dims* d, HeadPtrs* hp, TrainWs* w) {
+  SRB_TRY(make_dims(h, args, d));
+  SRB_TRY(resolve_params(keys, params, n_params, d->tf, hp, nullptr));
+  SRB_REQUIRE(input && points && pairs && valid && connected && keypoint_mask && road_mask && ws && losses,
+              "%s: null input", who);
   SRB_REQUIRE(pts_dtype == SAMROAD_F32 || pts_dtype == SAMROAD_I64 || pts_dtype == SAMROAD_I32,
-              "samroad_train_forward: points dtype %d", pts_dtype);
-  SRB_REQUIRE(pairs_dtype == SAMROAD_I64 || pairs_dtype == SAMROAD_I32, "samroad_train_forward: pairs dtype %d",
-              pairs_dtype);
-  const TrainWs w = layout_train(d, ws);
-  SRB_REQUIRE(ws_bytes >= w.total, "samroad_train_forward: workspace of %zu bytes, %zu needed", ws_bytes, w.total);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+              "%s: points dtype %d", who, pts_dtype);
+  SRB_REQUIRE(pairs_dtype == SAMROAD_I64 || pairs_dtype == SAMROAD_I32, "%s: pairs dtype %d", who, pairs_dtype);
+  *w = layout_train(*d, ws);
+  SRB_REQUIRE(ws_bytes >= w->total, "%s: workspace of %zu bytes, %zu needed", who, ws_bytes, w->total);
+  return 0;
+}
+
+// The heads' forward from the image embeddings in w.emb: map decoder, TopoNet and both losses.
+int heads_forward(const Dims& d, const HeadPtrs& hp, const TrainWs& w, const SamRoadTrainArgs* args,
+                  const void* points, int pts_dtype, const void* pairs, int pairs_dtype, const uint8_t* valid,
+                  const uint8_t* connected, const float* keypoint_mask, const float* road_mask, float* losses,
+                  cudaStream_t st) {
   const Dropout drop = make_dropout(args->dropout_p, args->seed);
   const Dropout none = make_dropout(0.0f, 0);
-
-  // encoder, exactly as the inference path (embeddings only)
-  SRB_TRY(samroad_encode_masks(h, rgb, rgb_dtype, d.B, nullptr, nullptr, w.emb, stream));
-  if (image_embeddings)
-    SRB_CUDA_OK(cudaMemcpyAsync(image_embeddings, w.emb, d.M * 256 * 4, cudaMemcpyDeviceToDevice, st));
 
   // ---- map decoder (model.py:286-295) in quad-tree rows ----
   const float* const* P_ = hp.p;
@@ -979,6 +1110,7 @@ extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs*
 
   // ---- TopoNet (model.py:88-148), slow-path semantics ----
   SRB_TRY(topo_sample_features_f32(w.emb, d.B, 256, d.s, d.P, points, pts_dtype, d.N, w.fs, st));
+  EW(points_f32_kernel, d.pts * 2, points, pts_dtype, d.pts * 2, w.xy);
   SRB_TRY(tc_gemm(rowmajor(w.fs, 256), colmajor(P_[HP_FP_W], 256), Store{w.pf, 128}, d.pts, 128, 256, 1, st));
   EW(bias_act_kernel, d.pts * 128, w.pf, P_[HP_FP_B], 128, d.pts * 128, 2, nullptr);
   SRB_TRY(tc_gemm(rowmajor(w.pf, 128), colmajor(P_[HP_PP_W], 258), Store{w.pst, 256}, d.pts, 128, 128, 1, st));
@@ -1016,26 +1148,73 @@ extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs*
   return 0;
 }
 
-extern "C" int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
-                                      const float* const* params, float* const* grads, int n_params, void* ws,
-                                      size_t ws_bytes, const float* g, void* stream) {
+}  // namespace
+
+extern "C" int samroad_train_forward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                                     const float* const* params, int n_params, const void* rgb, int rgb_dtype,
+                                     const void* points, int pts_dtype, const void* pairs, int pairs_dtype,
+                                     const uint8_t* valid, const uint8_t* connected, const float* keypoint_mask,
+                                     const float* road_mask, void* ws, size_t ws_bytes, float* losses,
+                                     float* image_embeddings, void* stream) {
+  Dims d;
+  HeadPtrs hp;
+  TrainWs w;
+  SRB_TRY(prepare_forward(h, args, keys, params, n_params, rgb, points, pts_dtype, pairs, pairs_dtype, valid,
+                          connected, keypoint_mask, road_mask, ws, ws_bytes, losses, "samroad_train_forward", &d, &hp,
+                          &w));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // encoder, exactly as the inference path (embeddings only)
+  SRB_TRY(samroad_encode_masks(h, rgb, rgb_dtype, d.B, nullptr, nullptr, w.emb, stream));
+  if (image_embeddings)
+    SRB_CUDA_OK(cudaMemcpyAsync(image_embeddings, w.emb, d.M * 256 * 4, cudaMemcpyDeviceToDevice, st));
+  return heads_forward(d, hp, w, args, points, pts_dtype, pairs, pairs_dtype, valid, connected, keypoint_mask,
+                       road_mask, losses, st);
+}
+
+extern "C" int samroad_train_forward_embeddings(samroad_handle_t h, const SamRoadTrainArgs* args,
+                                                const char* const* keys, const float* const* params, int n_params,
+                                                const float* image_embeddings, const void* points, int pts_dtype,
+                                                const void* pairs, int pairs_dtype, const uint8_t* valid,
+                                                const uint8_t* connected, const float* keypoint_mask,
+                                                const float* road_mask, void* ws, size_t ws_bytes, float* losses,
+                                                void* stream) {
+  Dims d;
+  HeadPtrs hp;
+  TrainWs w;
+  SRB_TRY(prepare_forward(h, args, keys, params, n_params, image_embeddings, points, pts_dtype, pairs, pairs_dtype,
+                          valid, connected, keypoint_mask, road_mask, ws, ws_bytes, losses,
+                          "samroad_train_forward_embeddings", &d, &hp, &w));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SRB_CUDA_OK(cudaMemcpyAsync(w.emb, image_embeddings, d.M * 256 * 4, cudaMemcpyDeviceToDevice, st));
+  return heads_forward(d, hp, w, args, points, pts_dtype, pairs, pairs_dtype, valid, connected, keypoint_mask,
+                       road_mask, losses, st);
+}
+
+namespace {
+
+// Backward of both entry points.  grads: null for no weight gradients, else one per parameter; grad_emb: null,
+// or the gradient of the image embeddings [B,256,s,s] (samroad_train_backward_embeddings).
+int train_backward_impl(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                        const float* const* params, float* const* grads, int n_params, void* ws, size_t ws_bytes,
+                        const float* g, float* grad_emb, void* stream, const char* who) {
   Dims d;
   SRB_TRY(make_dims(h, args, &d));
   HeadPtrs hp;
   int slot_of[HP_COUNT];
-  SRB_REQUIRE(n_params <= HP_COUNT, "samroad_train_backward: %d parameters", n_params);
+  SRB_REQUIRE(n_params <= HP_COUNT, "%s: %d parameters", who, n_params);
   SRB_TRY(resolve_params(keys, params, n_params, d.tf, &hp, slot_of));
-  SRB_REQUIRE(ws && g && (n_params == 0 || grads), "samroad_train_backward: null argument");
+  SRB_REQUIRE(ws && g, "%s: null argument", who);
   float* G[HP_COUNT] = {};
-  for (int i = 0; i < n_params; ++i) {
-    SRB_REQUIRE(grads[i], "samroad_train_backward: null gradient for '%s'", keys[i]);
+  for (int i = 0; grads && i < n_params; ++i) {
+    SRB_REQUIRE(grads[i], "%s: null gradient for '%s'", who, keys[i]);
     G[slot_of[i]] = grads[i];
   }
   const TrainWs w = layout_train(d, ws);
-  SRB_REQUIRE(ws_bytes >= w.total, "samroad_train_backward: workspace of %zu bytes, %zu needed", ws_bytes, w.total);
+  SRB_REQUIRE(ws_bytes >= w.total, "%s: workspace of %zu bytes, %zu needed", who, ws_bytes, w.total);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const Dropout drop = make_dropout(args->dropout_p, args->seed);
   const float* const* P_ = hp.p;
+  float* gm = w.g3;   // mask branch of the embeddings gradient [M, 256]: g3 is free once the decoder is done
 
   // ---- map decoder ----
   SRB_LAUNCH(loss_scale_kernel, 1, 1, 0, st, g, 2.0 * static_cast<double>(d.R4), w.stats, w.scale);
@@ -1054,6 +1233,10 @@ extern "C" int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs
   SRB_TRY(ln_param_grads(w.g1, w.xh1, d.R1, w.wpart, G[HP_DEC1_W], G[HP_DEC1_B], w.scale, st));
   SRB_TRY(wgrad(rowmajor(w.f0, 256), 256, rowmajor(w.g2, 512), 512, d.M, 1, 128, 0, 0, G[HP_DEC0_W], G[HP_DEC0_B],
                 w.wpart, w.scale, st));
+  // embeddings: g2 is the gradient of the first ConvTranspose's output, [M, 512] with column d*128 + co (the
+  // children of embedding row m are rows 4m + d), so the input gradient is g2 times the transposed weight
+  if (grad_emb)
+    SRB_TRY(tc_gemm(rowmajor(w.g2, 512), ConvTW{P_[HP_DEC0_W], 128, true}, Store{gm, 256}, d.M, 256, 512, 1, st));
 
   // ---- TopoNet ----
   const float* xl = d.tf ? w.x[3] : w.x[0];
@@ -1113,7 +1296,42 @@ extern "C" int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs
   EW(act_grad_kernel, d.pts * 128, w.gp, w.pf, d.pts * 128, 2, drop, 0, 0);
   SRB_TRY(wgrad(rowmajor(w.fs, 256), 256, rowmajor(w.gp, 128), 128, d.pts, 0, 0, 256, 0, G[HP_FP_W], G[HP_FP_B],
                 w.wpart, w.scale + 1, st));
+  if (!grad_emb) return 0;
+  // sampled features: gfs = (G_feature_proj * ReLU') W_feature_proj, then the sampler backward over the taps
+  // sorted by texel, and both branches into NCHW with the loss scales
+  SRB_TRY(tc_gemm(rowmajor(w.gp, 128), rowmajor(P_[HP_FP_W], 256), Store{w.gfs, 256}, d.pts, 256, 128, 1, st));
+  const long long ntap = 4 * d.pts;
+  EW(emb_taps_kernel, d.pts, w.xy, d.N, d.s, static_cast<float>(d.P), d.pts, d.M, w.src_start, w.tgt_start,
+     w.tkey[0], w.twt);
+  const long long hist = digit_hist_elems<kTapChunk>(ntap);
+  const int bits = 64 - __builtin_clzll(static_cast<unsigned long long>(d.M));   // keys run up to M
+  int cur = 0;
+  for (int shift = 0; shift < bits; shift += 8, cur ^= 1)
+    SRB_TRY(stable_digit_pass<kTapChunk>(TapPass{w.tkey[cur], shift ? w.tid[cur] : nullptr, w.tkey[cur ^ 1],
+                                                 w.tid[cur ^ 1], shift},
+                                         ntap, w.thist, w.thist + hist, st));
+  SRB_LAUNCH(emb_grad_kernel, static_cast<unsigned>((d.M + kEmbTexels - 1) / kEmbTexels), 256, 0, st, gm, w.gfs,
+             w.tkey[cur], w.tid[cur], w.twt, ntap, d.M, d.T, g, w.scale, grad_emb);
   return 0;
+}
+
+}  // namespace
+
+extern "C" int samroad_train_backward(samroad_handle_t h, const SamRoadTrainArgs* args, const char* const* keys,
+                                      const float* const* params, float* const* grads, int n_params, void* ws,
+                                      size_t ws_bytes, const float* g, void* stream) {
+  SRB_REQUIRE(n_params == 0 || grads, "samroad_train_backward: null argument");
+  return train_backward_impl(h, args, keys, params, grads, n_params, ws, ws_bytes, g, nullptr, stream,
+                             "samroad_train_backward");
+}
+
+extern "C" int samroad_train_backward_embeddings(samroad_handle_t h, const SamRoadTrainArgs* args,
+                                                 const char* const* keys, const float* const* params,
+                                                 float* const* grads, int n_params, void* ws, size_t ws_bytes,
+                                                 const float* g, float* grad_embeddings, void* stream) {
+  SRB_REQUIRE(grads || grad_embeddings, "samroad_train_backward_embeddings: no gradient requested");
+  return train_backward_impl(h, args, keys, params, grads, n_params, ws, ws_bytes, g, grad_embeddings, stream,
+                             "samroad_train_backward_embeddings");
 }
 
 extern "C" int samroad_debug_train_dropout_keep(float p, uint64_t seed, int layer, int site, int64_t n,

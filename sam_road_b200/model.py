@@ -526,6 +526,40 @@ class SAMRoad(_Base):
             self.log("train_loss", loss, **self._TRAIN_LOG)
         return loss
 
+    def head_losses(self, batch, image_embeddings: torch.Tensor):
+        """(mask_loss, topo_loss) of training_step's heads on caller-supplied image embeddings [B,256,P/16,P/16]
+        (fp32, fp16 or bf16, on the heads' CUDA device), e.g. the output of an encoder held in PyTorch.  No device
+        encoder runs, so FREEZE_ENCODER and ENCODER_LORA do not matter; USE_SAM_DECODER raises NotImplementedError.
+        Dropout, the seed and the batch checks are training_step's; nothing is logged.  Both losses are
+        differentiable with respect to the embeddings (the gradient comes back in their dtype and layout) and
+        the head parameters: only those that require grad get one (DESIGN.md §12)."""
+        from . import train as T
+        if _cfg_get(self.config, "USE_SAM_DECODER", False):
+            raise NotImplementedError(
+                "head_losses with USE_SAM_DECODER needs the TwoWayTransformer backward, which sam_road_b200 does "
+                "not implement; only the naive map decoder is served (DESIGN.md §12)")
+        heads = self._head_params()
+        dev = heads[0][1].device
+        if dev.type != "cuda":
+            raise RuntimeError(f"training runs on CUDA (sm_90a) only; the head parameters are on '{dev}'")
+        b = T.validate_batch(batch, self.image_size, dev)
+        emb = image_embeddings
+        s = self.image_size // 16
+        if not isinstance(emb, torch.Tensor):
+            raise ValueError(f"image_embeddings must be a tensor, got {type(emb).__name__}")
+        if tuple(emb.shape) != (b["B"], 256, s, s):
+            raise ValueError(f"image_embeddings must be [{b['B']},256,{s},{s}] for this batch, got {tuple(emb.shape)}")
+        if emb.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+            raise ValueError(f"image_embeddings must be float32, float16 or bfloat16, got {emb.dtype}")
+        if emb.device != dev:
+            raise ValueError(f"image_embeddings is on {emb.device}, the head parameters are on {dev}")
+        dropout_p = 0.1 if self.training else 0.0
+        from .ranks import draw_seed
+        seed = draw_seed() if dropout_p > 0 else 0
+        args = T.make_args(b, self.focal_loss, dropout_p, seed)
+        return T.head_losses(self._handle(dev), b, args, [k for k, _ in heads], [p for _, p in heads],
+                             image_embeddings=emb)
+
     def configure_optimizers(self):
         """model.py:637-685 for FREEZE_ENCODER: True with the naive decoder: Adam over map_decoder then topo_net,
         both at BASE_LR, and MultiStepLR(milestones=[9], gamma=0.1).  Prints the parameter count of each group as

@@ -3,7 +3,8 @@
 `head_losses` runs one step's forward on the device (the encoder as the inference path runs it, then the map
 decoder and TopoNet in fp32, saving their activations in a workspace tensor) and returns the differentiable
 0-dim fp32 (mask_loss, topo_loss).  Their backward writes one fp32 gradient per head parameter in the reference
-layout, so autograd, zero_grad, gradient accumulation and GradScaler work unmodified (DESIGN.md §12).
+layout, so autograd, zero_grad, gradient accumulation and GradScaler work unmodified (DESIGN.md §12).  Given image
+embeddings instead, the encoder does not run and the embeddings become a differentiable input of the step.
 """
 from __future__ import annotations
 
@@ -111,7 +112,7 @@ def make_args(b: Dict, focal: bool, dropout_p: float, seed: int) -> _lib.SamRoad
 
 class _HeadLosses(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, handle, b, args, keys, emb_out, *params):
+    def forward(ctx, handle, b, args, keys, emb_out, emb, *params):
         lib = _lib.load()
         dev = params[0].device
         nbytes = C.c_size_t()
@@ -123,13 +124,22 @@ class _HeadLosses(torch.autograd.Function):
         parr = _ptr_table(params)
         (x, xdt), (p, pdt), (q, qdt) = b["rgb"], b["points"], b["pairs"]
         with torch.cuda.device(dev):
-            _lib.check(lib.samroad_train_forward(
-                handle, C.byref(args), karr, parr, len(params), x.data_ptr(), xdt, p.data_ptr(), pdt, q.data_ptr(),
-                qdt, b["valid"].data_ptr(), b["connected"].data_ptr(), b["kp"].data_ptr(), b["road"].data_ptr(),
-                ws.data_ptr(), nbytes.value, losses.data_ptr(), _lib.ptr(emb_out), _lib.current_stream_ptr()),
-                "samroad_train_forward")
+            if emb is None:
+                _lib.check(lib.samroad_train_forward(
+                    handle, C.byref(args), karr, parr, len(params), x.data_ptr(), xdt, p.data_ptr(), pdt,
+                    q.data_ptr(), qdt, b["valid"].data_ptr(), b["connected"].data_ptr(), b["kp"].data_ptr(),
+                    b["road"].data_ptr(), ws.data_ptr(), nbytes.value, losses.data_ptr(), _lib.ptr(emb_out),
+                    _lib.current_stream_ptr()), "samroad_train_forward")
+            else:
+                e32 = emb.detach().to(torch.float32).contiguous()   # fp16 / bf16 from an autocast encoder
+                _lib.check(lib.samroad_train_forward_embeddings(
+                    handle, C.byref(args), karr, parr, len(params), e32.data_ptr(), p.data_ptr(), pdt, q.data_ptr(),
+                    qdt, b["valid"].data_ptr(), b["connected"].data_ptr(), b["kp"].data_ptr(), b["road"].data_ptr(),
+                    ws.data_ptr(), nbytes.value, losses.data_ptr(), _lib.current_stream_ptr()),
+                    "samroad_train_forward_embeddings")
         ctx.save_for_backward(*params)   # an in-place change before backward is reported by autograd
         ctx.handle, ctx.args, ctx.keys, ctx.ws = handle, args, keys, ws   # ws frees itself with the graph
+        ctx.emb = None if emb is None else torch.empty_like(emb, device="meta")   # dtype, shape and strides
         return losses[0].clone(), losses[1].clone()
 
     @staticmethod
@@ -140,20 +150,38 @@ class _HeadLosses(torch.autograd.Function):
         zero = torch.zeros((), dtype=torch.float32, device=dev)
         g = torch.stack([zero if g_mask is None else g_mask.to(torch.float32),
                          zero if g_topo is None else g_topo.to(torch.float32)]).contiguous()
-        grads = [torch.empty_like(p) for p in params]
+        want_params = any(ctx.needs_input_grad[6:])
+        want_emb = ctx.emb is not None and ctx.needs_input_grad[5]
+        grads = [torch.empty_like(p) for p in params] if want_params or ctx.emb is None else []
         karr, kref = _key_table(ctx.keys)
+        gemb = None
         with torch.cuda.device(dev):
-            _lib.check(lib.samroad_train_backward(
-                ctx.handle, C.byref(ctx.args), karr, _ptr_table(params), _ptr_table(grads), len(params),
-                ctx.ws.data_ptr(), ctx.ws.numel(), g.data_ptr(), _lib.current_stream_ptr()),
-                "samroad_train_backward")
-        return (None, None, None, None, None) + tuple(grads)
+            if ctx.emb is None:
+                _lib.check(lib.samroad_train_backward(
+                    ctx.handle, C.byref(ctx.args), karr, _ptr_table(params), _ptr_table(grads), len(params),
+                    ctx.ws.data_ptr(), ctx.ws.numel(), g.data_ptr(), _lib.current_stream_ptr()),
+                    "samroad_train_backward")
+            elif want_params or want_emb:
+                g32 = torch.empty(ctx.emb.shape, dtype=torch.float32, device=dev) if want_emb else None
+                _lib.check(lib.samroad_train_backward_embeddings(
+                    ctx.handle, C.byref(ctx.args), karr, _ptr_table(params),
+                    _ptr_table(grads) if want_params else None, len(params), ctx.ws.data_ptr(), ctx.ws.numel(),
+                    g.data_ptr(), _lib.ptr(g32), _lib.current_stream_ptr()),
+                    "samroad_train_backward_embeddings")
+                if want_emb:   # the input's dtype and layout
+                    gemb = torch.empty_like(ctx.emb, device=dev).copy_(g32)
+        if not grads:
+            return (None, None, None, None, None, gemb) + (None,) * len(params)
+        return (None, None, None, None, None, gemb) + tuple(grads)
 
 
 def head_losses(handle: int, b: Dict, args: _lib.SamRoadTrainArgs, keys: List[str], params: List[torch.Tensor],
-                emb_out=None):
-    """(mask_loss, topo_loss), differentiable with respect to `params` (the head parameters named by `keys`)."""
-    return _HeadLosses.apply(handle, b, args, keys, emb_out, *params)
+                emb_out=None, image_embeddings=None):
+    """(mask_loss, topo_loss), differentiable with respect to `params` (the head parameters named by `keys`).
+    With `image_embeddings` ([B,256,P/16,P/16] on the parameters' device, fp32, fp16 or bf16) the encoder does not
+    run: the heads take those embeddings, which are then a differentiable input too; their gradient comes back in
+    their dtype and layout (DESIGN.md §12).  Only the gradients autograd asks for are computed."""
+    return _HeadLosses.apply(handle, b, args, keys, emb_out, image_embeddings, *params)
 
 
 def dropout_keep(p: float, seed: int, layer: int, site: int, n: int, device) -> torch.Tensor:

@@ -266,6 +266,64 @@ def train_heads_fixture():
     np.savez_compressed(os.path.join(OUT, "train_heads_vitb_256.npz"), **out)
 
 
+EMB_GRAD_SAMPLES = 512   # gradient entries kept per loss kind (seeded positions)
+
+
+def emb_grad_fixture():
+    """d(loss)/d(image embeddings) of the reference's training_step + loss.backward() (the batch, weights and
+    configurations of train_heads_fixture), taken by a forward hook that makes the image encoder's output a leaf
+    which requires grad; the oracle must give the same gradient on the same embeddings."""
+    from oracle import train_oracle as TO
+    out = {}
+    for focal in (False, True):
+        cfg = dict(_cfg(256), FREEZE_ENCODER=True, FOCAL_LOSS=focal, BASE_LR=1e-3)
+        torch.manual_seed(0)
+        net = ref_loader.load_reference_model(cfg)
+        net.load_state_dict(synth.make_state_dict(cfg, seed=12, logit_gain=4.0), strict=True)
+        b = train_heads_batch()
+        tag = "focal" if focal else "bce"
+        taken = []
+
+        def leaf(module, inputs, output):
+            e = output.detach().requires_grad_(True)
+            taken.append(e)
+            return e
+
+        hook = net.image_encoder.register_forward_hook(leaf)
+        logged = {}
+        net.log = lambda name, v, **k: logged.__setitem__(name, v)
+        loss = net.training_step(b, 0)
+        hook.remove()
+        assert len(taken) == 1, len(taken)
+        # the mask loss alone (it is small next to the topology loss), then the step's own backward
+        gm, = torch.autograd.grad(logged["train_mask_loss"], taken[0], retain_graph=True)
+        loss.backward()
+        emb, g = taken[0].detach(), taken[0].grad
+        params = {k: p.detach().clone() for k, p in net.named_parameters()
+                  if k.startswith(("map_decoder.", "topo_net."))}
+        oemb = emb.clone().requires_grad_(True)
+        oml, otl = TO.heads_losses(params, oemb, b, 256, focal, "normal", None, 0.0)
+        ogm, = torch.autograd.grad(oml, oemb, retain_graph=True)
+        (oml + otl).backward()
+        rel = ((oemb.grad - g).abs().max() / g.abs().max()).item()
+        rel_m = ((ogm - gm).abs().max() / gm.abs().max()).item()
+        assert rel <= 2e-6 and rel_m <= 2e-6, (tag, rel, rel_m)   # fp32 against fp32, summation orders differ
+        dm = gm.double()
+        out[f"{tag}/mask_norm_maxabs"] = np.array([dm.norm().item(), dm.abs().max().item()])
+        out[f"{tag}/mask_texel_sum"] = dm.sum(1).numpy()
+        idx = torch.randint(0, g.numel(), (EMB_GRAD_SAMPLES,), generator=torch.Generator().manual_seed(98))
+        d = g.double()
+        out[f"{tag}/idx"] = idx.numpy().astype(np.int32)
+        out[f"{tag}/val"] = g.reshape(-1)[idx].numpy()
+        out[f"{tag}/norm_maxabs"] = np.array([d.norm().item(), d.abs().max().item()])
+        out[f"{tag}/channel_sum"] = d.sum((2, 3)).numpy()          # [B, 256]
+        out[f"{tag}/texel_sum"] = d.sum(1).numpy()                 # [B, s, s]
+        out[f"{tag}/emb_stats"] = _stats(emb)
+        print(f"emb_grad[{tag}]: |g|_2 {d.norm().item():.4e} (mask loss alone {dm.norm().item():.4e}), "
+              f"oracle-vs-reference max relative error {rel:.2e} ({rel_m:.2e})")
+    np.savez_compressed(os.path.join(OUT, "emb_grad_vitb_256.npz"), **out)
+
+
 LABEL_CFG = dict(PATCH_SIZE=256, TOPO_SAMPLE_NUM=24, MAX_NEIGHBOR_QUERIES=16, NEIGHBOR_RADIUS=64,
                  ROAD_NMS_RADIUS=16)
 LABEL_EXTENT = 360                 # the synthetic graph lies in [16, 360]^2: windows past it are empty
@@ -842,6 +900,10 @@ def main():
     if "--labels" in sys.argv:        # GraphLabelGenerator / sample_patch on a synthetic graph
         os.makedirs(OUT, exist_ok=True)
         labels_fixture()
+        return
+    if "--emb-grad" in sys.argv:      # the same step's gradient of the image embeddings
+        os.makedirs(OUT, exist_ok=True)
+        emb_grad_fixture()
         return
     if "--train-heads" in sys.argv:   # training_step / backward of the heads with a frozen encoder
         os.makedirs(OUT, exist_ok=True)
