@@ -43,6 +43,36 @@ struct BlockW {
   int win;   // attention window (14) or s for global blocks
 };
 
+// ---- one region of the packed weights (packed_regions) ----
+// Values samroad_finalize_weights computes on the host from a region's sources before it packs them.
+enum HostStep {
+  HS_NONE,
+  HS_LORA_QKV,   // sources qkv, A_q, B_q, A_v, B_v: the qkv weight with the LoRA products merged in
+  HS_DENSE_PE,   // source: the Gaussian matrix of the prompt encoder; the dense positional encoding [s, s, 256]
+};
+
+struct Source {
+  std::string key;              // state_dict key
+  std::vector<int64_t> shape;   // its required shape
+  int64_t at;                   // element offset of its values in the region
+};
+
+struct Region {
+  int pack;                  // Pack
+  int64_t n;                 // elements
+  int cin, cout;             // PK_CONVT: channels; PK_TILE4: bias length in cout
+  HostStep host;
+  bool refresh;              // samroad_update_tensor_device may rewrite it
+  std::vector<Source> src;
+};
+
+// Where samroad_update_tensor_device packs one key: a refreshable region, its storage and the key's source in it.
+struct RefreshTarget {
+  Region r;
+  void* dst;
+  Source src;
+};
+
 }  // namespace
 
 // Per-kernel-class CUDA-event timing (bench.py roofline): events are recorded on the launching
@@ -94,6 +124,8 @@ struct samroad_ctx {
 
   // device weight arena
   std::vector<DeviceBuffer> weight_allocs;
+  // the refreshable regions by state_dict key, filled by samroad_finalize_weights from packed_regions
+  std::map<std::string, std::vector<RefreshTarget>> refresh_targets;
 
   // encoder
   __half* pe_w = nullptr; float* pe_b = nullptr; float* pos = nullptr;
@@ -143,25 +175,319 @@ constexpr float kPixelStd[3] = {58.395f, 57.12f, 57.375f};      // model.py:230
 // test hook (bit 4 of samroad_debug_disable_2cta_gemm): every encoder LayerNorm walks its rows ascending
 bool g_ln_ascending = false;
 
-// ---- staged-tensor access -----------------------------------------------------------------------
+std::string fmt_key(const char* fmt, int i) {
+  char buf[256];
+  snprintf(buf, sizeof(buf), fmt, i);
+  return buf;
+}
+
+bool is_global_block(const SamRoadCfg& c, int i) {
+  for (int k = 0; k < 4; ++k)
+    if (c.global_attn_indexes[k] == i) return true;
+  return false;
+}
+
+// Grows a workspace or staging buffer to `need` bytes.  The handle's three streams may still read the old
+// block, so the device is synchronised before it is replaced.
+int grow(DeviceBuffer& b, size_t need, const char* what) {
+  if (need <= b.capacity()) return 0;
+  if (b.get()) SRB_CUDA_OK(cudaDeviceSynchronize());
+  return b.reserve(need, what);
+}
+
+// ---- packed weights ------------------------------------------------------------------------------------------
+// Every state_dict tensor reaches the device through one list (packed_regions) and one kernel (pack_kernel):
+// samroad_finalize_weights walks the list and packs the staged host values, and indexes the refreshable regions by
+// key; samroad_update_tensor_device packs one head tensor from device memory through that index.  So the two write
+// the same bytes, and a refresh costs one map lookup.
+
+// How a source is laid out in its region: dst[i] = src[j(i)], fp16 rounded to nearest even or fp32.
+enum Pack {
+  PK_F32,        // fp32 copy
+  PK_F16,        // fp16 copy: an nn.Linear weight [out, in] is already the K-major [N, K] operand
+  PK_PATCH,      // patch embed [D,3,16,16] -> fp16 [D, 768], k = ky*48 + kx*3 + c (matches im2col_patch16)
+  PK_NECK3,      // neck 3x3 conv [256,256,3,3] -> fp16 [256, 2304], k = tap*256 + c
+  PK_CONVT,      // ConvTranspose2d(k=2,s=2) [cin, cout, 2, 2] -> fp16 [N = (d, co), K = ci] with d = di*2 + dj, so that
+                 // output column block d is sub-pixel (di,dj) (SURVEY.md §8a P7)
+  PK_TILE4,      // bias [cout] once per sub-pixel d -> fp32 [4, cout]
+  PK_DEC4,       // map_decoder.7 [32, 2, 2, 2] -> fp32 [ci][d*2 + co]
+  PK_PAIR_ST,    // pair_proj.weight [128, 258] -> fp16 [256, 128]: rows 0..127 Ws, 128..255 Wt
+  PK_PAIR_OFF,   // pair_proj.weight [128, 258] -> fp32 [128, 2]: the two offset columns
+};
+
+bool packs_f16(int pack) {
+  return pack == PK_F16 || pack == PK_PATCH || pack == PK_NECK3 || pack == PK_CONVT || pack == PK_PAIR_ST;
+}
+
+__global__ void pack_kernel(const float* __restrict__ src, int pack, int cin, int cout, long long n, float* d32,
+                            __half* d16) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  long long j = i;
+  switch (pack) {
+    case PK_PATCH: {   // o[n*768 + ky*48 + kx*3 + c] = w[((n*3 + c)*16 + ky)*16 + kx]
+      const long long k = i % 768, ky = k / 48, kx = k % 48 / 3, c = k % 3;
+      j = ((i / 768 * 3 + c) * 16 + ky) * 16 + kx;
+      break;
+    }
+    case PK_NECK3: {   // o[n*2304 + tap*256 + c] = w[(n*256 + c)*9 + tap]
+      const long long k = i % 2304;
+      j = (i / 2304 * 256 + k % 256) * 9 + k / 256;
+      break;
+    }
+    case PK_CONVT: {   // o[(d*cout + co)*cin + ci] = w[(ci*cout + co)*4 + d]
+      const long long ci = i % cin, dc = i / cin, co = dc % cout, d = dc / cout;
+      j = (ci * cout + co) * 4 + d;
+      break;
+    }
+    case PK_TILE4: j = i % cout; break;
+    case PK_DEC4: {    // o[ci*8 + d*2 + co] = w[(ci*2 + co)*4 + d]
+      const long long ci = i / 8, d = (i % 8) / 2, co = i % 2;
+      j = (ci * 2 + co) * 4 + d;
+      break;
+    }
+    case PK_PAIR_ST: {   // o[r*128 + k] = w[(r % 128)*258 + (r / 128)*128 + k]
+      const long long r = i / 128, k = i % 128;
+      j = (r % 128) * 258 + (r / 128) * 128 + k;
+      break;
+    }
+    case PK_PAIR_OFF: j = (i / 2) * 258 + 256 + i % 2; break;
+    default: break;
+  }
+  const float v = src[j];
+  if (d16) d16[i] = __float2half_rn(v);
+  else d32[i] = v;
+}
+
+// The regions of the handle's packed weights in the order samroad_finalize_weights allocates them: visit(region,
+// field) with the handle member that holds the region's device address (a float* or __half* lvalue).  The blocks
+// must exist with their windows set.
+template <typename Visit>
+void packed_regions(samroad_ctx* h, Visit&& visit) {
+  const SamRoadCfg& c = h->cfg;
+  const int64_t D = h->D, s = h->s, hd = h->hd;
+  bool refresh = false;
+  auto region = [&](auto& field, int pack, int64_t n, std::vector<Source> src, int cin = 0, int cout = 0,
+                    HostStep host = HS_NONE) { visit(Region{pack, n, cin, cout, host, refresh, std::move(src)}, field); };
+  auto copy = [&](auto& field, int pack, const std::string& key, std::vector<int64_t> shape) {
+    int64_t n = 1;
+    for (int64_t d : shape) n *= d;
+    region(field, pack, n, {{key, std::move(shape), 0}});
+  };
+  auto f32 = [&](auto& field, const std::string& key, std::vector<int64_t> shape) {
+    copy(field, PK_F32, key, std::move(shape));
+  };
+  auto f16 = [&](auto& field, const std::string& key, std::vector<int64_t> shape) {
+    copy(field, PK_F16, key, std::move(shape));
+  };
+  auto convT = [&](auto& field, const std::string& key, int cin, int cout) {
+    region(field, PK_CONVT, 4LL * cin * cout, {{key, {cin, cout, 2, 2}, 0}}, cin, cout);
+  };
+  auto tile4 = [&](auto& field, const std::string& key, int cout) {
+    region(field, PK_TILE4, 4LL * cout, {{key, {cout}, 0}}, 0, cout);
+  };
+
+  // ---- image encoder ----
+  region(h->pe_w, PK_PATCH, D * 768, {{"image_encoder.patch_embed.proj.weight", {D, 3, 16, 16}, 0}});
+  f32(h->pe_b, "image_encoder.patch_embed.proj.bias", {D});
+  f32(h->pos, "image_encoder.pos_embed", {1, s, s, D});
+  for (int i = 0; i < c.depth; ++i) {
+    BlockW& b = h->blocks[i];
+    const std::string k = fmt_key("image_encoder.blocks.%d.", i);
+    const int64_t rel_rows = 2 * b.win - 1;
+    f32(b.ln1_g, k + "norm1.weight", {D});
+    f32(b.ln1_b, k + "norm1.bias", {D});
+    f32(b.ln2_g, k + "norm2.weight", {D});
+    f32(b.ln2_b, k + "norm2.bias", {D});
+    if (c.lora_rank > 0) {
+      const int64_t r = c.lora_rank;
+      const std::string q = k + "attn.qkv.";
+      region(b.qkv_w, PK_F16, 3 * D * D,
+             {{q + "weight", {3 * D, D}, 0}, {q + "linear_a_q.weight", {r, D}, 0}, {q + "linear_b_q.weight", {D, r}, 0},
+              {q + "linear_a_v.weight", {r, D}, 0}, {q + "linear_b_v.weight", {D, r}, 0}},
+             0, 0, HS_LORA_QKV);
+    } else {
+      f16(b.qkv_w, k + "attn.qkv.weight", {3 * D, D});
+    }
+    f32(b.qkv_b, k + "attn.qkv.bias", {3 * D});
+    f16(b.proj_w, k + "attn.proj.weight", {D, D});
+    f32(b.proj_b, k + "attn.proj.bias", {D});
+    f32(b.rel_h, k + "attn.rel_pos_h", {rel_rows, hd});
+    f32(b.rel_w, k + "attn.rel_pos_w", {rel_rows, hd});
+    f16(b.lin1_w, k + "mlp.lin1.weight", {4 * D, D});
+    f32(b.lin1_b, k + "mlp.lin1.bias", {4 * D});
+    f16(b.lin2_w, k + "mlp.lin2.weight", {D, 4 * D});
+    f32(b.lin2_b, k + "mlp.lin2.bias", {D});
+  }
+  // neck (image_encoder.py:88-104)
+  f16(h->neck0_w, "image_encoder.neck.0.weight", {256, D, 1, 1});
+  f32(h->neck1_g, "image_encoder.neck.1.weight", {256});
+  f32(h->neck1_b, "image_encoder.neck.1.bias", {256});
+  region(h->neck2_w, PK_NECK3, 256 * 2304, {{"image_encoder.neck.2.weight", {256, 256, 3, 3}, 0}});
+  f32(h->neck3_g, "image_encoder.neck.3.weight", {256});
+  f32(h->neck3_b, "image_encoder.neck.3.bias", {256});
+
+  if (!c.use_sam_decoder) {
+    // ---- naive map decoder (model.py:286-295) ----
+    refresh = true;
+    convT(h->dec1_w, "map_decoder.0.weight", 256, 128);
+    tile4(h->dec1_b, "map_decoder.0.bias", 128);
+    f32(h->dec_ln_g, "map_decoder.1.weight", {128});
+    f32(h->dec_ln_b, "map_decoder.1.bias", {128});
+    convT(h->dec2_w, "map_decoder.3.weight", 128, 64);
+    tile4(h->dec2_b, "map_decoder.3.bias", 64);
+    convT(h->dec3_w, "map_decoder.5.weight", 64, 32);
+    f32(h->dec3_b, "map_decoder.5.bias", {32});
+    region(h->dec4_w, PK_DEC4, 32 * 8, {{"map_decoder.7.weight", {32, 2, 2, 2}, 0}});
+    f32(h->dec4_b, "map_decoder.7.bias", {2});
+  } else {
+    // ---- SAM mask decoder + null-prompt encoder (model.py:260-282) ----
+    SamDecoderWeights& S = h->sam;
+    const std::string md = "mask_decoder.", tr = "mask_decoder.transformer.";
+    region(S.tokens, PK_F32, 4 * 256, {{md + "iou_token.weight", {1, 256}, 0}, {md + "mask_tokens.weight", {3, 256}, 256}});
+    f32(S.no_mask_embed, "prompt_encoder.no_mask_embed.weight", {1, 256});
+    region(S.dense_pe, PK_F32, s * s * 256,
+           {{"prompt_encoder.pe_layer.positional_encoding_gaussian_matrix", {2, 128}, 0}}, 0, 0, HS_DENSE_PE);
+    auto attn = [&](SamAttnW& a, const std::string& p, int64_t internal) {
+      f32(a.qw, p + "q_proj.weight", {internal, 256}); f32(a.qb, p + "q_proj.bias", {internal});
+      f32(a.kw, p + "k_proj.weight", {internal, 256}); f32(a.kb, p + "k_proj.bias", {internal});
+      f32(a.vw, p + "v_proj.weight", {internal, 256}); f32(a.vb, p + "v_proj.bias", {internal});
+      f32(a.ow, p + "out_proj.weight", {256, internal}); f32(a.ob, p + "out_proj.bias", {256});
+    };
+    for (int l = 0; l < 2; ++l) {
+      const std::string p = tr + "layers." + std::to_string(l) + ".";
+      attn(S.self_attn[l], p + "self_attn.", 256);
+      attn(S.t2i[l], p + "cross_attn_token_to_image.", 128);
+      attn(S.i2t[l], p + "cross_attn_image_to_token.", 128);
+      f32(S.n1g[l], p + "norm1.weight", {256}); f32(S.n1b[l], p + "norm1.bias", {256});
+      f32(S.n2g[l], p + "norm2.weight", {256}); f32(S.n2b[l], p + "norm2.bias", {256});
+      f32(S.n3g[l], p + "norm3.weight", {256}); f32(S.n3b[l], p + "norm3.bias", {256});
+      f32(S.n4g[l], p + "norm4.weight", {256}); f32(S.n4b[l], p + "norm4.bias", {256});
+      f32(S.l1w[l], p + "mlp.lin1.weight", {2048, 256}); f32(S.l1b[l], p + "mlp.lin1.bias", {2048});
+      f32(S.l2w[l], p + "mlp.lin2.weight", {256, 2048}); f32(S.l2b[l], p + "mlp.lin2.bias", {256});
+      f16(S.t2i_kw16[l], p + "cross_attn_token_to_image.k_proj.weight", {128, 256});
+      f16(S.t2i_vw16[l], p + "cross_attn_token_to_image.v_proj.weight", {128, 256});
+      f16(S.i2t_qw16[l], p + "cross_attn_image_to_token.q_proj.weight", {128, 256});
+      f16(S.i2t_ow16[l], p + "cross_attn_image_to_token.out_proj.weight", {256, 128});
+    }
+    attn(S.final_attn, tr + "final_attn_token_to_image.", 128);
+    f16(S.t2i_kw16[2], tr + "final_attn_token_to_image.k_proj.weight", {128, 256});
+    f16(S.t2i_vw16[2], tr + "final_attn_token_to_image.v_proj.weight", {128, 256});
+    f32(S.nfg, tr + "norm_final_attn.weight", {256}); f32(S.nfb, tr + "norm_final_attn.bias", {256});
+    for (int mi = 0; mi < 2; ++mi)
+      for (int j = 0; j < 3; ++j) {
+        const std::string k = md + "output_hypernetworks_mlps." + std::to_string(mi + 1) + ".layers." +
+                              std::to_string(j) + ".";
+        const int64_t out = j == 2 ? 32 : 256;
+        f32(S.hw[mi][j], k + "weight", {out, 256});
+        f32(S.hb[mi][j], k + "bias", {out});
+      }
+    convT(S.up1_w, md + "output_upscaling.0.weight", 256, 64);
+    tile4(S.up1_b, md + "output_upscaling.0.bias", 64);
+    f32(S.up1_g, md + "output_upscaling.1.weight", {64});
+    f32(S.up1_beta, md + "output_upscaling.1.bias", {64});
+    convT(S.up2_w, md + "output_upscaling.3.weight", 64, 32);
+    tile4(S.up2_b, md + "output_upscaling.3.bias", 32);
+  }
+
+  // ---- TopoNet (model.py:61-86) ----
+  refresh = true;
+  f16(h->tp_feat_w, "topo_net.feature_proj.weight", {128, 256});
+  f32(h->tp_feat_b, "topo_net.feature_proj.bias", {128});
+  region(h->tp_st_w, PK_PAIR_ST, 256 * 128, {{"topo_net.pair_proj.weight", {128, 258}, 0}});
+  region(h->tp_off_w, PK_PAIR_OFF, 128 * 2, {{"topo_net.pair_proj.weight", {128, 258}, 0}});
+  f32(h->tp_pair_b, "topo_net.pair_proj.bias", {128});
+  if (c.toponet_version != SAMROAD_TOPO_NO_TRANSFORMER) {
+    std::vector<Source> chunks;   // tp_chunks: per layer Wq|Wk|Wv, Wo, W1, W2 as [128, 128] blocks
+    for (int l = 0; l < 3; ++l) {
+      const std::string k = fmt_key("topo_net.transformer_encoder.layers.%d.", l);
+      const int64_t at = static_cast<int64_t>(l) * 6 * 128 * 128;
+      chunks.push_back({k + "self_attn.in_proj_weight", {384, 128}, at});
+      chunks.push_back({k + "self_attn.out_proj.weight", {128, 128}, at + 3 * 128 * 128});
+      chunks.push_back({k + "linear1.weight", {128, 128}, at + 4 * 128 * 128});
+      chunks.push_back({k + "linear2.weight", {128, 128}, at + 5 * 128 * 128});
+    }
+    region(h->tp_chunks, PK_F16, 18 * 128 * 128, std::move(chunks));
+    for (int l = 0; l < 3; ++l) {
+      TopoLayerParams& t = h->tp_layers[l];
+      const std::string k = fmt_key("topo_net.transformer_encoder.layers.%d.", l);
+      f32(t.in_b, k + "self_attn.in_proj_bias", {384});
+      f32(t.out_b, k + "self_attn.out_proj.bias", {128});
+      f32(t.l1_b, k + "linear1.bias", {128});
+      f32(t.l2_b, k + "linear2.bias", {128});
+      f32(t.n1_g, k + "norm1.weight", {128});
+      f32(t.n1_b, k + "norm1.bias", {128});
+      f32(t.n2_g, k + "norm2.weight", {128});
+      f32(t.n2_b, k + "norm2.bias", {128});
+    }
+  }
+  f32(h->tp_out_w, "topo_net.output_proj.weight", {1, 128});
+  f32(h->tp_out_b, "topo_net.output_proj.bias", {1});
+}
+
+// Packs n_src fp32 values at src (device memory) into region r, whose storage starts at dst, from element `at`
+// on; stream-ordered.  A copy writes n_src elements, every other packing the whole region.
+int pack_source(const Region& r, const float* src, int64_t n_src, void* dst, int64_t at, cudaStream_t st) {
+  const long long n = r.pack == PK_F32 || r.pack == PK_F16 ? n_src : r.n;
+  const bool f16 = packs_f16(r.pack);
+  SRB_LAUNCH(pack_kernel, blocks_for(n, 256), 256, 0, st, src, r.pack, r.cin, r.cout, n,
+             f16 ? nullptr : static_cast<float*>(dst) + at, f16 ? static_cast<__half*>(dst) + at : nullptr);
+  return 0;
+}
+
+// The fp32 values a region with a host step packs, computed from its sources' staged values.
+std::vector<float> host_values(const samroad_ctx* h, const Region& r, const std::vector<const HostTensor*>& in) {
+  const int64_t D = h->D, s = h->s;
+  if (r.host == HS_LORA_QKV) {
+    // qkv = xW^T + b ; q += B_q A_q x ; v += B_v A_v x   (model.py:179-186), merged into W in fp32
+    const int64_t rank = h->cfg.lora_rank;
+    const HostTensor *aq = in[1], *bq = in[2], *av = in[3], *bv = in[4];
+    std::vector<float> wf = in[0]->data;
+    for (int64_t n = 0; n < D; ++n)
+      for (int64_t j = 0; j < rank; ++j) {
+        const float bqv = bq->data[n * rank + j], bvv = bv->data[n * rank + j];
+        float* wq = &wf[n * D];
+        float* wv = &wf[(2 * D + n) * D];
+        const float* aqr = &aq->data[j * D];
+        const float* avr = &av->data[j * D];
+        for (int64_t k = 0; k < D; ++k) {
+          wq[k] += bqv * aqr[k];
+          wv[k] += bvv * avr[k];
+        }
+      }
+    return wf;
+  }
+  // HS_DENSE_PE: PromptEncoder.get_dense_pe (prompt_encoder.py:62-71,185-205), constant per config; on the host,
+  // since the device sinf/cosf may differ in the last bit
+  const std::vector<float>& G = in[0]->data;
+  std::vector<float> pe(static_cast<size_t>(s) * s * 256);
+  for (int y = 0; y < s; ++y)
+    for (int x = 0; x < s; ++x) {
+      const float cx = 2.0f * ((x + 0.5f) / s) - 1.0f, cy = 2.0f * ((y + 0.5f) / s) - 1.0f;
+      for (int k = 0; k < 128; ++k) {
+        const float a = 6.283185307179586f * (cx * G[k] + cy * G[128 + k]);
+        pe[(static_cast<size_t>(y) * s + x) * 256 + k] = sinf(a);
+        pe[(static_cast<size_t>(y) * s + x) * 256 + 128 + k] = cosf(a);
+      }
+    }
+  return pe;
+}
+
+// samroad_finalize_weights' state: the first failure wins, and its message is kept.
 struct Packer {
   samroad_ctx* h;
   bool ok = true;
   char msg[512] = "";
+  DeviceBuffer scratch;   // the fp32 values being packed
 
-  const HostTensor* get(const std::string& key, std::initializer_list<int64_t> shape) {
+  const HostTensor* get(const std::string& key, const std::vector<int64_t>& shape) {
     auto it = h->staged.find(key);
     if (it == h->staged.end()) {
       fail("missing state_dict key '%s'", key.c_str());
       return nullptr;
     }
     const HostTensor& t = it->second;
-    bool same = t.shape.size() == shape.size();
-    if (same) {
-      size_t i = 0;
-      for (auto d : shape) same = same && (t.shape[i++] == d);
-    }
-    if (!same) {
+    if (t.shape != shape) {
       std::string got;
       for (auto d : t.shape) got += std::to_string(d) + ",";
       std::string want;
@@ -180,75 +506,31 @@ struct Packer {
     vsnprintf(msg, sizeof(msg), fmt, ap);
     va_end(ap);
   }
-  template <typename T>
-  T* upload(const std::vector<T>& v) {
+  // one device buffer per region, with 256 bytes of tail slack
+  void* alloc(size_t bytes) {
     if (!ok) return nullptr;
     DeviceBuffer d;
-    if (d.reserve(v.size() * sizeof(T) + 256, "samroad_finalize_weights")) {
-      fail("cudaMalloc of %zu bytes for weights failed", v.size() * sizeof(T));
+    if (d.reserve(bytes + 256, "samroad_finalize_weights")) {
+      fail("cudaMalloc of %zu bytes for weights failed", bytes);
       return nullptr;
     }
-    T* p = d.as<T>();
+    void* p = d.get();
     h->weight_allocs.push_back(std::move(d));
-    if (cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) {
-      fail("cudaMemcpy of weights failed");
-      return nullptr;
-    }
     return p;
   }
-  float* f32(const std::string& key, std::initializer_list<int64_t> shape) {
-    const HostTensor* t = get(key, shape);
-    return t ? upload(t->data) : nullptr;
-  }
-  static std::vector<__half> to_half(const std::vector<float>& v) {
-    std::vector<__half> o(v.size());
-    for (size_t i = 0; i < v.size(); ++i) o[i] = __float2half_rn(v[i]);
-    return o;
-  }
-  // nn.Linear weight [out, in] is already the K-major [N, K] operand
-  __half* linear_w(const std::string& key, int64_t n, int64_t k) {
-    const HostTensor* t = get(key, {n, k});
-    return t ? upload(to_half(t->data)) : nullptr;
+  // uploads v into the scratch buffer and packs it into region r at dst, on the legacy default stream
+  void pack(const Region& r, const std::vector<float>& v, void* dst, int64_t at) {
+    if (!ok) return;
+    const size_t bytes = v.size() * sizeof(float);
+    if (grow(scratch, bytes, "samroad_finalize_weights") != 0) {
+      fail("%s", get_last_error());
+    } else if (cudaMemcpy(scratch.get(), v.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
+      fail("cudaMemcpy of weights failed");
+    } else if (pack_source(r, scratch.as<float>(), static_cast<int64_t>(v.size()), dst, at, nullptr) != 0) {
+      fail("%s", get_last_error());
+    }
   }
 };
-
-std::string fmt_key(const char* fmt, int i) {
-  char buf[256];
-  snprintf(buf, sizeof(buf), fmt, i);
-  return buf;
-}
-
-bool is_global_block(const SamRoadCfg& c, int i) {
-  for (int k = 0; k < 4; ++k)
-    if (c.global_attn_indexes[k] == i) return true;
-  return false;
-}
-
-// ConvTranspose2d(k=2,s=2) weight [Cin, Cout, 2, 2] -> GEMM operand [N = (d, co), K = ci] with
-// d = di*2 + dj, so that output column block d is sub-pixel (di,dj) (SURVEY.md §8a P7).
-std::vector<__half> pack_convT(const HostTensor& w, int cin, int cout) {
-  std::vector<__half> o(static_cast<size_t>(4) * cout * cin);
-  for (int ci = 0; ci < cin; ++ci)
-    for (int co = 0; co < cout; ++co)
-      for (int d = 0; d < 4; ++d)
-        o[(static_cast<size_t>(d) * cout + co) * cin + ci] =
-            __float2half_rn(w.data[(static_cast<size_t>(ci) * cout + co) * 4 + d]);
-  return o;
-}
-std::vector<float> tile4(const std::vector<float>& b) {
-  std::vector<float> o(b.size() * 4);
-  for (int d = 0; d < 4; ++d)
-    for (size_t i = 0; i < b.size(); ++i) o[d * b.size() + i] = b[i];
-  return o;
-}
-
-// Grows a workspace or staging buffer to `need` bytes.  The handle's three streams may still read the old
-// block, so the device is synchronised before it is replaced.
-int grow(DeviceBuffer& b, size_t need, const char* what) {
-  if (need <= b.capacity()) return 0;
-  if (b.get()) SRB_CUDA_OK(cudaDeviceSynchronize());
-  return b.reserve(need, what);
-}
 
 // ---- activation workspace layout for the encoder + decoder ------------------------------------------
 struct EncWs {
@@ -397,247 +679,46 @@ extern "C" int samroad_load_tensor(samroad_handle_t h, const char* key, const fl
 
 extern "C" int samroad_finalize_weights(samroad_handle_t h) {
   SRB_TRY(check_handle(h, false));
-  // drop previously packed weights (re-load after load_state_dict)
+  // drop previously packed weights (re-load after load_state_dict); until this call succeeds the handle has none
+  h->finalized = false;
   SRB_CUDA_OK(cudaDeviceSynchronize());
+  h->refresh_targets.clear();
   h->weight_allocs.clear();
-  h->blocks.clear();
 
   Packer P{h};
   const SamRoadCfg& c = h->cfg;
-  const int64_t D = h->D, s = h->s, hd = h->hd;
-
-  // ---- patch embed: [D,3,16,16] -> [D, 768] with k = ky*48 + kx*3 + c (matches im2col_patch16) ----
-  if (const HostTensor* w = P.get("image_encoder.patch_embed.proj.weight", {D, 3, 16, 16})) {
-    std::vector<__half> o(static_cast<size_t>(D) * 768);
-    for (int64_t n = 0; n < D; ++n)
-      for (int ch = 0; ch < 3; ++ch)
-        for (int ky = 0; ky < 16; ++ky)
-          for (int kx = 0; kx < 16; ++kx)
-            o[n * 768 + ky * 48 + kx * 3 + ch] =
-                __float2half_rn(w->data[((n * 3 + ch) * 16 + ky) * 16 + kx]);
-    h->pe_w = P.upload(o);
-  }
-  h->pe_b = P.f32("image_encoder.patch_embed.proj.bias", {D});
-  h->pos = P.f32("image_encoder.pos_embed", {1, s, s, D});
-
-  // ---- transformer blocks ----
-  h->blocks.resize(c.depth);
-  for (int i = 0; i < c.depth && P.ok; ++i) {
-    BlockW& b = h->blocks[i];
-    const bool glob = is_global_block(c, i);
+  h->blocks.assign(c.depth, BlockW{});
+  for (int i = 0; i < c.depth; ++i) {
     // A window block keeps its window size even when it exceeds the grid (s < 14, PATCH_SIZE < 224):
     // the s x s tokens are then padded to one window, whose pad tokens are softmax keys
     // (image_encoder.py:168-172), and the rel-pos tables have 2*window-1 rows.
-    b.win = glob ? static_cast<int>(s) : c.window_size;
-    const int64_t rel_rows = glob ? 2 * s - 1 : 2 * c.window_size - 1;
-    auto K = [&](const char* suffix) { return fmt_key("image_encoder.blocks.%d.", i) + suffix; };
-    b.ln1_g = P.f32(K("norm1.weight"), {D});
-    b.ln1_b = P.f32(K("norm1.bias"), {D});
-    b.ln2_g = P.f32(K("norm2.weight"), {D});
-    b.ln2_b = P.f32(K("norm2.bias"), {D});
-    // qkv (+ LoRA merge: qkv = xW^T + b ; q += B_q A_q x ; v += B_v A_v x   model.py:179-186)
-    if (const HostTensor* w = P.get(K("attn.qkv.weight"), {3 * D, D})) {
-      std::vector<float> wf = w->data;
-      if (c.lora_rank > 0) {
-        const int64_t r = c.lora_rank;
-        const HostTensor* aq = P.get(K("attn.qkv.linear_a_q.weight"), {r, D});
-        const HostTensor* bq = P.get(K("attn.qkv.linear_b_q.weight"), {D, r});
-        const HostTensor* av = P.get(K("attn.qkv.linear_a_v.weight"), {r, D});
-        const HostTensor* bv = P.get(K("attn.qkv.linear_b_v.weight"), {D, r});
-        if (aq && bq && av && bv) {
-          for (int64_t n = 0; n < D; ++n)
-            for (int64_t j = 0; j < r; ++j) {
-              const float bqv = bq->data[n * r + j], bvv = bv->data[n * r + j];
-              float* wq = &wf[n * D];
-              float* wv = &wf[(2 * D + n) * D];
-              const float* aqr = &aq->data[j * D];
-              const float* avr = &av->data[j * D];
-              for (int64_t k = 0; k < D; ++k) {
-                wq[k] += bqv * aqr[k];
-                wv[k] += bvv * avr[k];
-              }
-            }
-        }
-      }
-      b.qkv_w = P.upload(Packer::to_half(wf));
-    }
-    b.qkv_b = P.f32(K("attn.qkv.bias"), {3 * D});
-    b.proj_w = P.linear_w(K("attn.proj.weight"), D, D);
-    b.proj_b = P.f32(K("attn.proj.bias"), {D});
-    b.rel_h = P.f32(K("attn.rel_pos_h"), {rel_rows, hd});
-    b.rel_w = P.f32(K("attn.rel_pos_w"), {rel_rows, hd});
-    b.lin1_w = P.linear_w(K("mlp.lin1.weight"), 4 * D, D);
-    b.lin1_b = P.f32(K("mlp.lin1.bias"), {4 * D});
-    b.lin2_w = P.linear_w(K("mlp.lin2.weight"), D, 4 * D);
-    b.lin2_b = P.f32(K("mlp.lin2.bias"), {D});
-    if (!glob && c.window_size > 64)
-      P.fail("window_size=%d unsupported (at most 64)", c.window_size);
+    const bool glob = is_global_block(c, i);
+    h->blocks[i].win = glob ? h->s : c.window_size;
+    if (!glob && c.window_size > 64) P.fail("window_size=%d unsupported (at most 64)", c.window_size);
   }
-
-  // ---- neck (image_encoder.py:88-104) ----
-  if (const HostTensor* w = P.get("image_encoder.neck.0.weight", {256, D, 1, 1}))
-    h->neck0_w = P.upload(Packer::to_half(w->data));
-  h->neck1_g = P.f32("image_encoder.neck.1.weight", {256});
-  h->neck1_b = P.f32("image_encoder.neck.1.bias", {256});
-  if (const HostTensor* w = P.get("image_encoder.neck.2.weight", {256, 256, 3, 3})) {
-    std::vector<__half> o(static_cast<size_t>(256) * 2304);   // [n][tap*256 + c]
-    for (int n = 0; n < 256; ++n)
-      for (int ch = 0; ch < 256; ++ch)
-        for (int tap = 0; tap < 9; ++tap)
-          o[static_cast<size_t>(n) * 2304 + tap * 256 + ch] =
-              __float2half_rn(w->data[(static_cast<size_t>(n) * 256 + ch) * 9 + tap]);
-    h->neck2_w = P.upload(o);
-  }
-  h->neck3_g = P.f32("image_encoder.neck.3.weight", {256});
-  h->neck3_b = P.f32("image_encoder.neck.3.bias", {256});
-
-  if (!c.use_sam_decoder) {
-  // ---- naive map decoder (model.py:286-295) ----
-  if (const HostTensor* w = P.get("map_decoder.0.weight", {256, 128, 2, 2}))
-    h->dec1_w = P.upload(pack_convT(*w, 256, 128));
-  if (const HostTensor* b = P.get("map_decoder.0.bias", {128})) h->dec1_b = P.upload(tile4(b->data));
-  h->dec_ln_g = P.f32("map_decoder.1.weight", {128});
-  h->dec_ln_b = P.f32("map_decoder.1.bias", {128});
-  if (const HostTensor* w = P.get("map_decoder.3.weight", {128, 64, 2, 2}))
-    h->dec2_w = P.upload(pack_convT(*w, 128, 64));
-  if (const HostTensor* b = P.get("map_decoder.3.bias", {64})) h->dec2_b = P.upload(tile4(b->data));
-  if (const HostTensor* w = P.get("map_decoder.5.weight", {64, 32, 2, 2}))
-    h->dec3_w = P.upload(pack_convT(*w, 64, 32));
-  h->dec3_b = P.f32("map_decoder.5.bias", {32});
-  if (const HostTensor* w = P.get("map_decoder.7.weight", {32, 2, 2, 2})) {
-    std::vector<float> o(32 * 8);   // [ci][di*4 + dj*2 + co]
-    for (int ci = 0; ci < 32; ++ci)
-      for (int co = 0; co < 2; ++co)
-        for (int d = 0; d < 4; ++d) o[ci * 8 + d * 2 + co] = w->data[(ci * 2 + co) * 4 + d];
-    h->dec4_w = P.upload(o);
-  }
-  h->dec4_b = P.f32("map_decoder.7.bias", {2});
-
-  } else {
-    // ---- SAM mask decoder + null-prompt encoder (model.py:260-282) ----
-    SamDecoderWeights& S = h->sam;
-    const std::string md = "mask_decoder.", tr = "mask_decoder.transformer.";
-    if (const HostTensor* it = P.get(md + "iou_token.weight", {1, 256})) {
-      if (const HostTensor* mt = P.get(md + "mask_tokens.weight", {3, 256})) {
-        std::vector<float> tok(it->data);
-        tok.insert(tok.end(), mt->data.begin(), mt->data.end());
-        S.tokens = P.upload(tok);
-      }
+  packed_regions(h, [&](const Region& r, auto& field) {
+    std::vector<const HostTensor*> in;
+    for (const Source& src : r.src) in.push_back(P.get(src.key, src.shape));
+    void* dst = P.alloc(r.n * (packs_f16(r.pack) ? sizeof(__half) : sizeof(float)));
+    if (!dst) return;
+    field = static_cast<std::remove_reference_t<decltype(field)>>(dst);
+    if (r.refresh)
+      for (const Source& src : r.src) h->refresh_targets[src.key].push_back({r, dst, src});
+    if (r.host != HS_NONE) {
+      P.pack(r, host_values(h, r, in), dst, 0);
+    } else {
+      for (size_t i = 0; i < in.size(); ++i) P.pack(r, in[i]->data, dst, r.src[i].at);
     }
-    S.no_mask_embed = P.f32("prompt_encoder.no_mask_embed.weight", {1, 256});
-    if (const HostTensor* G = P.get("prompt_encoder.pe_layer.positional_encoding_gaussian_matrix", {2, 128})) {
-      // PromptEncoder.get_dense_pe (prompt_encoder.py:62-71,185-205): constant per config
-      std::vector<float> pe(static_cast<size_t>(s) * s * 256);
-      for (int y = 0; y < s; ++y)
-        for (int x = 0; x < s; ++x) {
-          const float cx = 2.0f * ((x + 0.5f) / s) - 1.0f, cy = 2.0f * ((y + 0.5f) / s) - 1.0f;
-          for (int k = 0; k < 128; ++k) {
-            const float a = 6.283185307179586f * (cx * G->data[k] + cy * G->data[128 + k]);
-            pe[(static_cast<size_t>(y) * s + x) * 256 + k] = sinf(a);
-            pe[(static_cast<size_t>(y) * s + x) * 256 + 128 + k] = cosf(a);
-          }
-        }
-      S.dense_pe = P.upload(pe);
-    }
-    auto attn = [&](const std::string& p, int64_t internal) {
-      SamAttnW a;
-      a.qw = P.f32(p + "q_proj.weight", {internal, 256}); a.qb = P.f32(p + "q_proj.bias", {internal});
-      a.kw = P.f32(p + "k_proj.weight", {internal, 256}); a.kb = P.f32(p + "k_proj.bias", {internal});
-      a.vw = P.f32(p + "v_proj.weight", {internal, 256}); a.vb = P.f32(p + "v_proj.bias", {internal});
-      a.ow = P.f32(p + "out_proj.weight", {256, internal}); a.ob = P.f32(p + "out_proj.bias", {256});
-      return a;
-    };
-    for (int l = 0; l < 2; ++l) {
-      const std::string p = tr + "layers." + std::to_string(l) + ".";
-      S.self_attn[l] = attn(p + "self_attn.", 256);
-      S.t2i[l] = attn(p + "cross_attn_token_to_image.", 128);
-      S.i2t[l] = attn(p + "cross_attn_image_to_token.", 128);
-      S.n1g[l] = P.f32(p + "norm1.weight", {256}); S.n1b[l] = P.f32(p + "norm1.bias", {256});
-      S.n2g[l] = P.f32(p + "norm2.weight", {256}); S.n2b[l] = P.f32(p + "norm2.bias", {256});
-      S.n3g[l] = P.f32(p + "norm3.weight", {256}); S.n3b[l] = P.f32(p + "norm3.bias", {256});
-      S.n4g[l] = P.f32(p + "norm4.weight", {256}); S.n4b[l] = P.f32(p + "norm4.bias", {256});
-      S.l1w[l] = P.f32(p + "mlp.lin1.weight", {2048, 256}); S.l1b[l] = P.f32(p + "mlp.lin1.bias", {2048});
-      S.l2w[l] = P.f32(p + "mlp.lin2.weight", {256, 2048}); S.l2b[l] = P.f32(p + "mlp.lin2.bias", {256});
-      S.t2i_kw16[l] = P.linear_w(p + "cross_attn_token_to_image.k_proj.weight", 128, 256);
-      S.t2i_vw16[l] = P.linear_w(p + "cross_attn_token_to_image.v_proj.weight", 128, 256);
-      S.i2t_qw16[l] = P.linear_w(p + "cross_attn_image_to_token.q_proj.weight", 128, 256);
-      S.i2t_ow16[l] = P.linear_w(p + "cross_attn_image_to_token.out_proj.weight", 256, 128);
-    }
-    S.final_attn = attn(tr + "final_attn_token_to_image.", 128);
-    S.t2i_kw16[2] = P.linear_w(tr + "final_attn_token_to_image.k_proj.weight", 128, 256);
-    S.t2i_vw16[2] = P.linear_w(tr + "final_attn_token_to_image.v_proj.weight", 128, 256);
-    S.nfg = P.f32(tr + "norm_final_attn.weight", {256}); S.nfb = P.f32(tr + "norm_final_attn.bias", {256});
-    for (int mi = 0; mi < 2; ++mi)
-      for (int j = 0; j < 3; ++j) {
-        const std::string k = md + "output_hypernetworks_mlps." + std::to_string(mi + 1) + ".layers." +
-                              std::to_string(j) + ".";
-        const int64_t out = j == 2 ? 32 : 256;
-        S.hw[mi][j] = P.f32(k + "weight", {out, 256});
-        S.hb[mi][j] = P.f32(k + "bias", {out});
-      }
-    if (const HostTensor* wt = P.get(md + "output_upscaling.0.weight", {256, 64, 2, 2}))
-      S.up1_w = P.upload(pack_convT(*wt, 256, 64));
-    if (const HostTensor* bt = P.get(md + "output_upscaling.0.bias", {64})) S.up1_b = P.upload(tile4(bt->data));
-    S.up1_g = P.f32(md + "output_upscaling.1.weight", {64});
-    S.up1_beta = P.f32(md + "output_upscaling.1.bias", {64});
-    if (const HostTensor* wt = P.get(md + "output_upscaling.3.weight", {64, 32, 2, 2}))
-      S.up2_w = P.upload(pack_convT(*wt, 64, 32));
-    if (const HostTensor* bt = P.get(md + "output_upscaling.3.bias", {32})) S.up2_b = P.upload(tile4(bt->data));
-    if (P.ok) {   // constant part of the decoder: layer-0 queries
-      float* q0 = P.upload(std::vector<float>(4 * 256, 0.f));
-      if (q0 && (sam_decoder_prepare(S, q0, nullptr) != 0 || cudaStreamSynchronize(nullptr) != cudaSuccess))
+  });
+  if (c.use_sam_decoder) {   // constant part of the decoder: layer-0 queries
+    if (float* q0 = static_cast<float*>(P.alloc(4 * 256 * sizeof(float)))) {
+      if (sam_decoder_prepare(h->sam, q0, nullptr) != 0 || cudaStreamSynchronize(nullptr) != cudaSuccess)
         P.fail("sam_decoder_prepare failed: %s", get_last_error());
-      S.q0 = q0;
+      h->sam.q0 = q0;
     }
   }
-
-  // ---- TopoNet (model.py:61-86) ----
-  h->tp_feat_w = P.linear_w("topo_net.feature_proj.weight", 128, 256);
-  h->tp_feat_b = P.f32("topo_net.feature_proj.bias", {128});
-  if (const HostTensor* w = P.get("topo_net.pair_proj.weight", {128, 258})) {
-    std::vector<__half> st(static_cast<size_t>(256) * 128);   // rows 0..127: Ws, 128..255: Wt
-    std::vector<float> off(128 * 2);
-    for (int n = 0; n < 128; ++n) {
-      for (int k = 0; k < 128; ++k) {
-        st[static_cast<size_t>(n) * 128 + k] = __float2half_rn(w->data[n * 258 + k]);
-        st[static_cast<size_t>(128 + n) * 128 + k] = __float2half_rn(w->data[n * 258 + 128 + k]);
-      }
-      off[n * 2 + 0] = w->data[n * 258 + 256];
-      off[n * 2 + 1] = w->data[n * 258 + 257];
-    }
-    h->tp_st_w = P.upload(st);
-    h->tp_off_w = P.upload(off);
-  }
-  h->tp_pair_b = P.f32("topo_net.pair_proj.bias", {128});
-  if (c.toponet_version != SAMROAD_TOPO_NO_TRANSFORMER) {
-    std::vector<__half> chunks(static_cast<size_t>(18) * 128 * 128);
-    for (int l = 0; l < 3 && P.ok; ++l) {
-      TopoLayerParams& t = h->tp_layers[l];
-      auto K = [&](const char* suffix) {
-        return fmt_key("topo_net.transformer_encoder.layers.%d.", l) + suffix;
-      };
-      const HostTensor* src[4] = {P.get(K("self_attn.in_proj_weight"), {384, 128}),
-                                  P.get(K("self_attn.out_proj.weight"), {128, 128}),
-                                  P.get(K("linear1.weight"), {128, 128}),
-                                  P.get(K("linear2.weight"), {128, 128})};
-      size_t off = static_cast<size_t>(l) * 6 * 128 * 128;
-      for (int i = 0; i < 4 && P.ok; ++i) {
-        for (size_t j = 0; j < src[i]->data.size(); ++j) chunks[off + j] = __float2half_rn(src[i]->data[j]);
-        off += src[i]->data.size();
-      }
-      t.in_b = P.f32(K("self_attn.in_proj_bias"), {384});
-      t.out_b = P.f32(K("self_attn.out_proj.bias"), {128});
-      t.l1_b = P.f32(K("linear1.bias"), {128});
-      t.l2_b = P.f32(K("linear2.bias"), {128});
-      t.n1_g = P.f32(K("norm1.weight"), {128});
-      t.n1_b = P.f32(K("norm1.bias"), {128});
-      t.n2_g = P.f32(K("norm2.weight"), {128});
-      t.n2_b = P.f32(K("norm2.bias"), {128});
-    }
-    h->tp_chunks = P.upload(chunks);
-  }
-  h->tp_out_w = P.f32("topo_net.output_proj.weight", {1, 128});
-  h->tp_out_b = P.f32("topo_net.output_proj.bias", {1});
+  const cudaError_t e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) P.fail("packing the weights failed: %s", cudaGetErrorString(e));
 
   if (!P.ok) {
     set_last_error("samroad_finalize_weights: %s", P.msg);
@@ -657,106 +738,23 @@ int samroad_handle_head_config(samroad_handle_t h, int* patch_size, int* toponet
   return 0;
 }
 
-// ---- device repack of one head tensor (samroad_update_tensor_device) ------------------------------------------
-namespace {
-
-enum RepackMode { RP_COPY, RP_CONVT, RP_TILE4, RP_DEC4, RP_PAIR_ST, RP_PAIR_OFF };
-
-// dst[i] = src[index(i)] for the packings of samroad_finalize_weights, fp16 (round to nearest even, as the host
-// pack) or fp32
-__global__ void repack_kernel(const float* __restrict__ src, int mode, int cin, int cout, long long n, float* d32,
-                              __half* d16) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  long long j = i;
-  switch (mode) {
-    case RP_CONVT: {   // o[(d*cout + co)*cin + ci] = w[(ci*cout + co)*4 + d]
-      const long long ci = i % cin, dc = i / cin, co = dc % cout, d = dc / cout;
-      j = (ci * cout + co) * 4 + d;
-      break;
-    }
-    case RP_TILE4: j = i % cout; break;
-    case RP_DEC4: {    // o[ci*8 + d*2 + co] = w[(ci*2 + co)*4 + d]
-      const long long ci = i / 8, d = (i % 8) / 2, co = i % 2;
-      j = (ci * 2 + co) * 4 + d;
-      break;
-    }
-    case RP_PAIR_ST: {   // rows 0..127: Ws, 128..255: Wt of pair_proj.weight [128, 258]
-      const long long r = i / 128, k = i % 128;
-      j = (r % 128) * 258 + (r / 128) * 128 + k;
-      break;
-    }
-    case RP_PAIR_OFF: j = (i / 2) * 258 + 256 + i % 2; break;
-    default: break;
-  }
-  const float v = src[j];
-  if (d16) d16[i] = __float2half_rn(v);
-  else d32[i] = v;
-}
-
-}  // namespace
-
 extern "C" int samroad_update_tensor_device(samroad_handle_t h, const char* key, const float* dev_data,
                                             const int64_t* shape, int ndim, void* stream) {
   SRB_TRY(check_handle(h, true));
   SRB_REQUIRE(key && dev_data && (shape || ndim == 0) && ndim >= 0 && ndim <= 8,
               "samroad_update_tensor_device: bad arguments");
   SRB_REQUIRE(!h->cfg.use_sam_decoder, "samroad_update_tensor_device: the SAM mask decoder is repacked on the host only");
-  const std::string k = key;
-  struct Target { int mode; int cin, cout; long long n; float* d32; __half* d16; };
-  std::vector<Target> tg;
-  std::vector<int64_t> want;
-  auto f32 = [&](const float* p, long long n) { tg.push_back({RP_COPY, 0, 0, n, const_cast<float*>(p), nullptr}); };
-  auto f16 = [&](const __half* p, long long n) { tg.push_back({RP_COPY, 0, 0, n, nullptr, const_cast<__half*>(p)}); };
-  if (k == "map_decoder.0.weight") { want = {256, 128, 2, 2}; tg.push_back({RP_CONVT, 256, 128, 4LL * 128 * 256, nullptr, h->dec1_w}); }
-  else if (k == "map_decoder.0.bias") { want = {128}; tg.push_back({RP_TILE4, 0, 128, 512, h->dec1_b, nullptr}); }
-  else if (k == "map_decoder.1.weight") { want = {128}; f32(h->dec_ln_g, 128); }
-  else if (k == "map_decoder.1.bias") { want = {128}; f32(h->dec_ln_b, 128); }
-  else if (k == "map_decoder.3.weight") { want = {128, 64, 2, 2}; tg.push_back({RP_CONVT, 128, 64, 4LL * 64 * 128, nullptr, h->dec2_w}); }
-  else if (k == "map_decoder.3.bias") { want = {64}; tg.push_back({RP_TILE4, 0, 64, 256, h->dec2_b, nullptr}); }
-  else if (k == "map_decoder.5.weight") { want = {64, 32, 2, 2}; tg.push_back({RP_CONVT, 64, 32, 4LL * 32 * 64, nullptr, h->dec3_w}); }
-  else if (k == "map_decoder.5.bias") { want = {32}; f32(h->dec3_b, 32); }
-  else if (k == "map_decoder.7.weight") { want = {32, 2, 2, 2}; tg.push_back({RP_DEC4, 0, 0, 256, h->dec4_w, nullptr}); }
-  else if (k == "map_decoder.7.bias") { want = {2}; f32(h->dec4_b, 2); }
-  else if (k == "topo_net.feature_proj.weight") { want = {128, 256}; f16(h->tp_feat_w, 128 * 256); }
-  else if (k == "topo_net.feature_proj.bias") { want = {128}; f32(h->tp_feat_b, 128); }
-  else if (k == "topo_net.pair_proj.weight") {
-    want = {128, 258};
-    tg.push_back({RP_PAIR_ST, 0, 0, 256 * 128, nullptr, h->tp_st_w});
-    tg.push_back({RP_PAIR_OFF, 0, 0, 256, h->tp_off_w, nullptr});
-  }
-  else if (k == "topo_net.pair_proj.bias") { want = {128}; f32(h->tp_pair_b, 128); }
-  else if (k == "topo_net.output_proj.weight") { want = {1, 128}; f32(h->tp_out_w, 128); }
-  else if (k == "topo_net.output_proj.bias") { want = {1}; f32(h->tp_out_b, 1); }
-  else if (h->cfg.toponet_version != SAMROAD_TOPO_NO_TRANSFORMER &&
-           k.rfind("topo_net.transformer_encoder.layers.", 0) == 0 && k.size() > 38 && k[37] == '.' &&
-           k[36] >= '0' && k[36] <= '2') {
-    const int l = k[36] - '0';
-    const std::string s = k.substr(38);
-    const TopoLayerParams& t = h->tp_layers[l];
-    const __half* chunk = h->tp_chunks + static_cast<size_t>(l) * 6 * 128 * 128;
-    if (s == "self_attn.in_proj_weight") { want = {384, 128}; f16(chunk, 384 * 128); }
-    else if (s == "self_attn.out_proj.weight") { want = {128, 128}; f16(chunk + 3 * 128 * 128, 128 * 128); }
-    else if (s == "linear1.weight") { want = {128, 128}; f16(chunk + 4 * 128 * 128, 128 * 128); }
-    else if (s == "linear2.weight") { want = {128, 128}; f16(chunk + 5 * 128 * 128, 128 * 128); }
-    else if (s == "self_attn.in_proj_bias") { want = {384}; f32(t.in_b, 384); }
-    else if (s == "self_attn.out_proj.bias") { want = {128}; f32(t.out_b, 128); }
-    else if (s == "linear1.bias") { want = {128}; f32(t.l1_b, 128); }
-    else if (s == "linear2.bias") { want = {128}; f32(t.l2_b, 128); }
-    else if (s == "norm1.weight") { want = {128}; f32(t.n1_g, 128); }
-    else if (s == "norm1.bias") { want = {128}; f32(t.n1_b, 128); }
-    else if (s == "norm2.weight") { want = {128}; f32(t.n2_g, 128); }
-    else if (s == "norm2.bias") { want = {128}; f32(t.n2_b, 128); }
-  }
-  SRB_REQUIRE(!tg.empty(), "samroad_update_tensor_device: '%s' is not a head tensor of this configuration", key);
-  bool same = static_cast<size_t>(ndim) == want.size();
-  for (int i = 0; same && i < ndim; ++i) same = shape[i] == want[i];
-  SRB_REQUIRE(same, "samroad_update_tensor_device: '%s' has the wrong shape", key);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  for (const Target& t : tg) {
-    SRB_LAUNCH(repack_kernel, static_cast<unsigned>((t.n + 255) / 256), 256, 0, st, dev_data, t.mode, t.cin, t.cout,
-               t.n, t.d32, t.d16);
-  }
+  const auto it = h->refresh_targets.find(key);
+  SRB_REQUIRE(it != h->refresh_targets.end(),
+              "samroad_update_tensor_device: '%s' is not a head tensor of this configuration", key);
+  const std::vector<RefreshTarget>& tg = it->second;
+  const std::vector<int64_t>& want = tg[0].src.shape;
+  SRB_REQUIRE(want == std::vector<int64_t>(shape, shape + ndim), "samroad_update_tensor_device: '%s' has the wrong shape",
+              key);
+  int64_t n = 1;
+  for (int64_t d : want) n *= d;
+  for (const RefreshTarget& t : tg)
+    SRB_TRY(pack_source(t.r, dev_data, n, t.dst, t.src.at, static_cast<cudaStream_t>(stream)));
   return 0;
 }
 
